@@ -12,7 +12,7 @@ CSRC = HERE / "csrc"
 LIBDIR = HERE / "lib"
 LIB = LIBDIR / "libb200audio.so"
 SOURCES = ["api.cu", "mel.cu", "snac.cu", "llama.cu", "tc_gemm.cu", "whisper.cu", "vocos.cu", "encodec.cu", "weights.cu", "speech_tokenizer.cu", "qwen3_sampler.cu"]
-NVCC_FLAGS = (["-DB2A_ATTN_TIMING"] if os.environ.get("B2A_ATTN_TIMING") else []) + [
+NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr",
 ]

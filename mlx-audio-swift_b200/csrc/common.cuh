@@ -165,23 +165,6 @@ static inline void launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
 #ifdef __CUDACC__
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-// L2 prefetch of a byte range, split over `n_workers` threads in 8 KB bulk requests (cp.async.bulk.prefetch.L2: a hint, no
-// completion tracking, no shared memory).  Used to keep HBM streaming the NEXT GEMM's weights while kernels that read little
-// (norms, attention, epilogue-only phases) run: the decode step is weight-streaming bound and the weights never depend on
-// activations.
-struct L2Prefetch {
-    const void* ptr;
-    long long bytes;
-};
-__device__ __forceinline__ void l2_prefetch(const L2Prefetch& pf, int worker, int n_workers) {
-    if (pf.ptr == nullptr) return;
-    constexpr long long CH = 8192;
-    const char* base = static_cast<const char*>(pf.ptr);
-    for (long long off = (long long)worker * CH; off < pf.bytes; off += (long long)n_workers * CH) {
-        const unsigned n = (unsigned)(pf.bytes - off < CH ? ((pf.bytes - off) & ~15ll) : CH);
-        if (n) asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(base + off), "r"(n) : "memory");
-    }
-}
 #endif
 
 }  // namespace b2a

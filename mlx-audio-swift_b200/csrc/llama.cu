@@ -107,12 +107,11 @@ constexpr int RN_THREADS = 1024, RN_MAXV = 8;
 __global__ void __launch_bounds__(RN_THREADS)
 add_rmsnorm_kernel(float* __restrict__ x, float* __restrict__ delta, const float* __restrict__ w,
                    bf16* __restrict__ xn, int H, float eps, float* __restrict__ trace, float* __restrict__ zero_ptr,
-                   int zero_n, int half, L2Prefetch pf, float* __restrict__ normed = nullptr, float* __restrict__ ss_out = nullptr,
+                   int zero_n, int half, float* __restrict__ normed = nullptr, float* __restrict__ ss_out = nullptr,
                    int ss_parts = 0) {
     __shared__ float red[RN_THREADS / 32];
     const int b = blockIdx.x, tid = threadIdx.x;
     pdl_trigger();
-    l2_prefetch(pf, b * RN_THREADS + tid, gridDim.x * RN_THREADS);
     pdl_wait();
     float* xr = x + (long long)b * H;
     float v[RN_MAXV];
@@ -239,19 +238,8 @@ gemv_bf16_kernel(const bf16* __restrict__ W, const bf16* __restrict__ xin, float
 
 // ------------------------------------------------------------------------------------------------
 // Decode attention (LlamaTTS.swift:235-266): RoPE on q/k, append k/v to the fp32 cache, softmax(qK^T)V.
-// grid = (kv heads, rows, key splits): split s owns keys [s*AT_CAP, (s+1)*AT_CAP); its K and V rows are
-// one contiguous block of the cache each, fetched with a single cp.async.bulk per matrix into shared memory
-// (one HBM round trip), the partial (max, sum, out) goes to a workspace and the last CTA of a (row, head)
-// to finish merges the partials (flash-decoding).
 // ------------------------------------------------------------------------------------------------
 constexpr int HD = 128, AT_THREADS = 256, MAXG = 8, AT_CAP = 64;   // AT_CAP * 4 == AT_THREADS
-
-#ifdef B2A_ATTN_TIMING
-__device__ long long g_attn_ts[8 * 4096];
-#define ATS(i) do { if (threadIdx.x == 0) g_attn_ts[(((long long)blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x) * 8 + (i)] = clock64(); } while (0)
-#else
-#define ATS(i) do {} while (0)
-#endif
 
 struct AttnArgs {
     const float* qkv;      // [B, (nq + 2 nkv) * 128] fp32
@@ -260,374 +248,25 @@ struct AttnArgs {
     float* kcache;         // this layer: [B][nkv][max_ctx][128] fp32
     float* vcache;
     bf16* out;             // [16, nq*128] hi/lo
-    float* part_o;         // [B][nkv][S][G][128]
-    float* part_ml;        // [B][nkv][S][G][2]
-    int* counters;         // [B][nkv], zero between launches
-    int nq, nkv, max_ctx, S;
+    int nq, nkv, max_ctx;
     float scale;
-    L2Prefetch pf;         // weights of a later GEMM, prefetched into L2 while attention (which reads little) runs
     const float* qnorm;    // nullable [128]: per-head RMSNorm gain applied to every q head BEFORE RoPE (Qwen3TTSTalker.swift:127-186)
-    const float* knorm;    // nullable [128]: same for the k head  (cluster kernel only)
+    const float* knorm;    // nullable [128]: same for the k head
     float qk_eps;
     int zero_qkv;          // fused-norm step: clear this (row, kv head)'s q | k | v slices after reading them, so that the next layer's
                            // stream-K QKV GEMM can add into the row (the stand-alone norm kernel that used to do it is gone)
 };
 
-template <int G>
-__global__ void __launch_bounds__(AT_THREADS)
-attn_decode_kernel(AttnArgs a) {
-    extern __shared__ __align__(16) uint8_t at_smem[];
-    float* sK = reinterpret_cast<float*>(at_smem);              // [AT_CAP][128]
-    float* sV = sK + AT_CAP * HD;                               // [AT_CAP][128]
-    float* sq = sV + AT_CAP * HD;                               // [G][128]
-    float* sc = sq + G * HD;                                    // [G][AT_CAP]
-    float* wpo = sc + G * AT_CAP;                               // [8 warps][G][128] warp-partial outputs
-    uint64_t* bar = reinterpret_cast<uint64_t*>(wpo + (AT_THREADS / 32) * G * HD);
-    __shared__ float red[AT_THREADS / 32][MAXG];
-    __shared__ int s_last;
-
-    const int h = blockIdx.x, b = blockIdx.y, s = blockIdx.z, tid = threadIdx.x;
-    ATS(0);
-    pdl_trigger();
-    l2_prefetch(a.pf, ((blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x) * AT_THREADS + tid,
-                gridDim.x * gridDim.y * gridDim.z * AT_THREADS);
-    // Everything that does not depend on this step's q|k|v runs BEFORE griddepcontrol.wait and overlaps with the
-    // tail of the QKV GEMM: pos[] is only written by the sampler (last kernel of the previous step's graph), the
-    // cache rows < pos by earlier steps.  So: position, RoPE angles, mbarrier, and the bulk K/V loads go first.
-    const int p = a.pos[b];
-    const bool row_ok = p >= 0 && p < a.max_ctx;
-    const int S_eff = row_ok ? p / AT_CAP + 1 : 0;
-    if (s >= S_eff) { pdl_wait(); return; }
-    const int t0 = s * AT_CAP, t1 = min(t0 + AT_CAP, p + 1), nk = t1 - t0;
-    const bool has_new = (s == S_eff - 1);                      // this split owns the new position p
-    const int n_load = has_new ? nk - 1 : nk;
-    const int qkv_ld = (a.nq + 2 * a.nkv) * HD;
-    const float* row = a.qkv + (long long)b * qkv_ld;
-    float* kc = a.kcache + (((long long)b * a.nkv + h) * a.max_ctx) * HD;
-    float* vc = a.vcache + (((long long)b * a.nkv + h) * a.max_ctx) * HD;
-
-    if (tid == 0) {
-        tc::mbar_init(bar, 1);
-        tc::fence_barrier_init();
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        if (n_load > 0) {
-            const uint32_t bytes = (uint32_t)n_load * HD * 4;
-            tc::mbar_arrive_expect_tx(bar, 2 * bytes);
-            asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                         ::"r"(tc::smem_u32(sK)), "l"(kc + (long long)t0 * HD), "r"(bytes), "r"(tc::smem_u32(bar)) : "memory");
-            asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                         ::"r"(tc::smem_u32(sV)), "l"(vc + (long long)t0 * HD), "r"(bytes), "r"(tc::smem_u32(bar)) : "memory");
-        } else {
-            tc::mbar_arrive(bar);
-        }
-    }
-    float sn = 0.f, cs = 1.f;
-    if (tid < HD / 2) sincosf((float)p / a.freqs[tid], &sn, &cs);   // MLXFast.RoPE(freqs:): angle = pos / freqs[i]
-    pdl_wait();
-    ATS(1);
-    if (tid < HD / 2) {  // non-traditional RoPE: pairs (i, i+64)
-        const int d = tid;
-        _Pragma("unroll") for (int g = 0; g < G; ++g) {
-            const float* q = row + (h * G + g) * HD;
-            const float x1 = q[d], x2 = q[d + HD / 2];
-            sq[g * HD + d] = x1 * cs - x2 * sn;
-            sq[g * HD + d + HD / 2] = x2 * cs + x1 * sn;
-        }
-        if (has_new) {
-            const float* k = row + (a.nq + h) * HD;
-            const float x1 = k[d], x2 = k[d + HD / 2];
-            const float k1 = x1 * cs - x2 * sn, k2 = x2 * cs + x1 * sn;
-            kc[(long long)p * HD + d] = k1;
-            kc[(long long)p * HD + d + HD / 2] = k2;
-            sK[(p - t0) * HD + d] = k1;
-            sK[(p - t0) * HD + d + HD / 2] = k2;
-        }
-    } else if (tid >= 128 && has_new) {
-        const int d = tid - 128;
-        const float v = row[(a.nq + a.nkv + h) * HD + d];
-        vc[(long long)p * HD + d] = v;
-        sV[(p - t0) * HD + d] = v;
-    }
-    __syncthreads();            // barrier init + q / new-row staging visible
-    ATS(2);
-    tc::mbar_wait(bar, 0);      // bulk-copied K and V have landed
-    ATS(3);
-
-    // Each warp owns 8 keys end to end (4 lanes per key): scores, a warp-local softmax (max / sum by shuffles) and
-    // its partial P*V; the 8 warp partials are merged through shared memory with ONE block barrier.
-    const int lane = tid & 31, warp = tid >> 5;
-    const int key = warp * 8 + (lane >> 2), part = lane & 3;
-    float sacc[G];
-    _Pragma("unroll") for (int g = 0; g < G; ++g) sacc[g] = 0.f;
-    if (key < nk) {
-        const float4* kr = reinterpret_cast<const float4*>(sK + key * HD);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-            const int d4 = part + 4 * ((j + key) & 7);     // rotated columns: every quarter-warp hits 8 distinct bank groups
-            const float4 kf = kr[d4];
-            _Pragma("unroll") for (int g = 0; g < G; ++g) {
-                const float4 qf = reinterpret_cast<const float4*>(sq + g * HD)[d4];
-                sacc[g] = fmaf(qf.x, kf.x, sacc[g]); sacc[g] = fmaf(qf.y, kf.y, sacc[g]);
-                sacc[g] = fmaf(qf.z, kf.z, sacc[g]); sacc[g] = fmaf(qf.w, kf.w, sacc[g]);
-            }
-        }
-    }
-    float pw[G], mw[G], lw[G];
-    _Pragma("unroll") for (int g = 0; g < G; ++g) {
-        float v = sacc[g];
-        v += __shfl_xor_sync(0xffffffffu, v, 1);
-        v += __shfl_xor_sync(0xffffffffu, v, 2);
-        const float sv = key < nk ? v * a.scale : -INFINITY;
-        float m = sv;
-        m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 4));
-        m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 8));
-        m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 16));
-        const float e = (m == -INFINITY) ? 0.f : __expf(sv - m);    // all 4 lanes of a key hold the same value
-        float l = part == 0 ? e : 0.f;
-        l = warp_sum(l);
-        pw[g] = e; mw[g] = m; lw[g] = l;
-    }
-    // warp-partial P*V: lane owns dims 4*lane .. 4*lane+3 (conflict-free float4 reads of a V row)
-    float4 o4[G];
-    _Pragma("unroll") for (int g = 0; g < G; ++g) o4[g] = make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-    for (int kk = 0; kk < 8; ++kk) {
-        const int t = warp * 8 + kk;
-        if (t < nk) {
-            const float4 v = reinterpret_cast<const float4*>(sV + t * HD)[lane];
-            _Pragma("unroll") for (int g = 0; g < G; ++g) {
-                const float pk = __shfl_sync(0xffffffffu, pw[g], kk * 4);
-                o4[g].x = fmaf(pk, v.x, o4[g].x); o4[g].y = fmaf(pk, v.y, o4[g].y);
-                o4[g].z = fmaf(pk, v.z, o4[g].z); o4[g].w = fmaf(pk, v.w, o4[g].w);
-            }
-        }
-    }
-    // spo doubles as the warp-partial buffer: [8 warps][G][128]; red / sc hold the warp (max, sum)
-    _Pragma("unroll") for (int g = 0; g < G; ++g) {
-        reinterpret_cast<float4*>(wpo + (warp * G + g) * HD)[lane] = o4[g];
-        if (lane == 0) { red[warp][g] = mw[g]; sc[g * AT_CAP + warp] = lw[g]; }
-    }
-    __syncthreads();
-    const long long pbase = (((long long)b * a.nkv + h) * a.S + s) * G;
-    if (tid < HD) {
-        _Pragma("unroll") for (int g = 0; g < G; ++g) {
-            float M = red[0][g];
-#pragma unroll
-            for (int w = 1; w < AT_THREADS / 32; ++w) M = fmaxf(M, red[w][g]);
-            float L = 0.f, O = 0.f;
-#pragma unroll
-            for (int w = 0; w < AT_THREADS / 32; ++w) {
-                const float sc_w = red[w][g] == -INFINITY ? 0.f : __expf(red[w][g] - M);
-                L = fmaf(sc[g * AT_CAP + w], sc_w, L);
-                O = fmaf(wpo[(w * G + g) * HD + tid], sc_w, O);
-            }
-            a.part_o[(pbase + g) * HD + tid] = O;
-            if (tid == 0) { a.part_ml[(pbase + g) * 2] = M; a.part_ml[(pbase + g) * 2 + 1] = L; }
-        }
-    }
-    ATS(4);
-    __threadfence();
-    __syncthreads();
-    if (tid == 0) s_last = (atomicAdd(&a.counters[b * a.nkv + h], 1) == S_eff - 1);
-    __syncthreads();
-    ATS(5);
-    if (!s_last) return;
-    __threadfence();
-    // merge the S_eff partials
-    if (tid < HD) {
-        const long long mbase = (((long long)b * a.nkv + h) * a.S) * G;
-        _Pragma("unroll") for (int g = 0; g < G; ++g) {
-            float M = -INFINITY;
-            for (int j = 0; j < S_eff; ++j) M = fmaxf(M, a.part_ml[(mbase + (long long)j * G + g) * 2]);
-            float L = 0.f, O = 0.f;
-            for (int j = 0; j < S_eff; ++j) {
-                const float wj = __expf(a.part_ml[(mbase + (long long)j * G + g) * 2] - M);
-                L = fmaf(a.part_ml[(mbase + (long long)j * G + g) * 2 + 1], wj, L);
-                O = fmaf(a.part_o[(mbase + (long long)j * G + g) * HD + tid], wj, O);
-            }
-            store_hilo(a.out, (long long)a.nq * HD, b, (h * G + g) * HD + tid, O / L);
-        }
-    }
-    if (tid == 0) a.counters[b * a.nkv + h] = 0;
-    ATS(6);
-}
-
-// ------------------------------------------------------------------------------------------------
-// Decode attention, one CTA per (kv head, row), looping over 64-key chunks with an online softmax (default).
-// The split-K kernel above pays three dependent global round trips after its compute (partials -> fence -> atomic ->
-// partial reads by the last CTA).  Here nothing leaves the SM:
-// chunks stream through an NB-deep ring of shared-memory buffers (one cp.async.bulk per matrix per chunk, up to NB chunks in
-// flight, the first NB issued BEFORE griddepcontrol.wait so they overlap the tail of the QKV GEMM), every warp keeps a
-// running (max, sum, P*V) for its 8 keys of each chunk, and the 8 warp states are merged once at the end.
-// ------------------------------------------------------------------------------------------------
-template <int G>
-__global__ void __launch_bounds__(AT_THREADS)
-attn_decode_loop_kernel(AttnArgs a, int NB) {
-    extern __shared__ __align__(16) uint8_t at_smem[];
-    float* sKV = reinterpret_cast<float*>(at_smem);             // [NB][2][AT_CAP][128]  (K then V of each ring slot)
-    float* sq = sKV + (size_t)NB * 2 * AT_CAP * HD;             // [G][128]
-    float* snew = sq + G * HD;                                  // [2][128] the new k / v row of this step
-    float* wpo = snew + 2 * HD;                                 // [8 warps][G][128] warp-partial outputs
-    uint64_t* bars = reinterpret_cast<uint64_t*>(wpo + (AT_THREADS / 32) * G * HD);   // [NB]
-    __shared__ float red_m[AT_THREADS / 32][MAXG], red_l[AT_THREADS / 32][MAXG];
-
-    const int h = blockIdx.x, b = blockIdx.y, tid = threadIdx.x;
-    pdl_trigger();
-    l2_prefetch(a.pf, (blockIdx.y * gridDim.x + blockIdx.x) * AT_THREADS + tid, gridDim.x * gridDim.y * AT_THREADS);
-    const int p = a.pos[b];                                     // written by the previous step's sampler only
-    if (!(p >= 0 && p < a.max_ctx)) { pdl_wait(); return; }
-    const int nch = p / AT_CAP + 1;
-    const int qkv_ld = (a.nq + 2 * a.nkv) * HD;
-    const float* row = a.qkv + (long long)b * qkv_ld;
-    float* kc = a.kcache + (((long long)b * a.nkv + h) * a.max_ctx) * HD;
-    float* vc = a.vcache + (((long long)b * a.nkv + h) * a.max_ctx) * HD;
-    // rows of chunk c already in the cache (the new position p is staged from this step's q|k|v instead)
-    auto issue = [&](int c) {
-        const int slot = c % NB;
-        const int n_load = (c < nch - 1) ? AT_CAP : p - c * AT_CAP;
-        float* dK = sKV + (size_t)slot * 2 * AT_CAP * HD;
-        if (n_load > 0) {
-            const uint32_t bytes = (uint32_t)n_load * HD * 4;
-            tc::mbar_arrive_expect_tx(&bars[slot], 2 * bytes);
-            asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                         ::"r"(tc::smem_u32(dK)), "l"(kc + (long long)c * AT_CAP * HD), "r"(bytes), "r"(tc::smem_u32(&bars[slot])) : "memory");
-            asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                         ::"r"(tc::smem_u32(dK + AT_CAP * HD)), "l"(vc + (long long)c * AT_CAP * HD), "r"(bytes), "r"(tc::smem_u32(&bars[slot])) : "memory");
-        } else {
-            tc::mbar_arrive(&bars[slot]);
-        }
-    };
-    if (tid == 0) {
-        for (int i = 0; i < NB; ++i) tc::mbar_init(&bars[i], 1);
-        tc::fence_barrier_init();
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        for (int c = 0; c < min(nch, NB); ++c) issue(c);
-    }
-    float sn = 0.f, cs = 1.f;
-    if (tid < HD / 2) sincosf((float)p / a.freqs[tid], &sn, &cs);   // MLXFast.RoPE(freqs:): angle = pos / freqs[i]
-    pdl_wait();
-    if (tid < HD / 2) {  // non-traditional RoPE: pairs (i, i+64)
-        const int d = tid;
-        _Pragma("unroll") for (int g = 0; g < G; ++g) {
-            const float* q = row + (h * G + g) * HD;
-            const float x1 = q[d], x2 = q[d + HD / 2];
-            sq[g * HD + d] = x1 * cs - x2 * sn;
-            sq[g * HD + d + HD / 2] = x2 * cs + x1 * sn;
-        }
-        const float* k = row + (a.nq + h) * HD;
-        const float x1 = k[d], x2 = k[d + HD / 2];
-        const float k1 = x1 * cs - x2 * sn, k2 = x2 * cs + x1 * sn;
-        kc[(long long)p * HD + d] = k1;
-        kc[(long long)p * HD + d + HD / 2] = k2;
-        snew[d] = k1;
-        snew[d + HD / 2] = k2;
-    } else if (tid >= 128) {
-        const int d = tid - 128;
-        const float v = row[(a.nq + a.nkv + h) * HD + d];
-        vc[(long long)p * HD + d] = v;
-        snew[HD + d] = v;
-    }
-    __syncthreads();            // barrier init + q / new-row staging visible
-
-    const int lane = tid & 31, warp = tid >> 5;
-    const int kslot = warp * 8 + (lane >> 2), part = lane & 3;
-    float m_run[G], l_run[G];
-    float4 o4[G];
-    _Pragma("unroll") for (int g = 0; g < G; ++g) { m_run[g] = -INFINITY; l_run[g] = 0.f; o4[g] = make_float4(0.f, 0.f, 0.f, 0.f); }
-
-    for (int c = 0; c < nch; ++c) {
-        const int slot = c % NB;
-        float* sK = sKV + (size_t)slot * 2 * AT_CAP * HD;
-        float* sV = sK + AT_CAP * HD;
-        const int t0 = c * AT_CAP, nk = min(AT_CAP, p + 1 - t0);
-        tc::mbar_wait(&bars[slot], (uint32_t)((c / NB) & 1));    // bulk-copied K and V of this chunk have landed
-        if (c == nch - 1) {                                      // splice in the new position (the bulk copy stopped before it)
-            if (tid < HD) sK[(p - t0) * HD + tid] = snew[tid];
-            else sV[(p - t0) * HD + tid - HD] = snew[tid];
-            __syncthreads();
-        }
-        float sacc[G];
-        _Pragma("unroll") for (int g = 0; g < G; ++g) sacc[g] = 0.f;
-        if (kslot < nk) {
-            const float4* kr = reinterpret_cast<const float4*>(sK + kslot * HD);
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                const int d4 = part + 4 * ((j + kslot) & 7);     // rotated columns: every quarter-warp hits 8 distinct bank groups
-                const float4 kf = kr[d4];
-                _Pragma("unroll") for (int g = 0; g < G; ++g) {
-                    const float4 qf = reinterpret_cast<const float4*>(sq + g * HD)[d4];
-                    sacc[g] = fmaf(qf.x, kf.x, sacc[g]); sacc[g] = fmaf(qf.y, kf.y, sacc[g]);
-                    sacc[g] = fmaf(qf.z, kf.z, sacc[g]); sacc[g] = fmaf(qf.w, kf.w, sacc[g]);
-                }
-            }
-        }
-        float pw[G];
-        _Pragma("unroll") for (int g = 0; g < G; ++g) {
-            float v = sacc[g];
-            v += __shfl_xor_sync(0xffffffffu, v, 1);
-            v += __shfl_xor_sync(0xffffffffu, v, 2);
-            const float sv = kslot < nk ? v * a.scale : -INFINITY;
-            float m = sv;
-            m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 4));
-            m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 8));
-            m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 16));
-            const float m_new = fmaxf(m_run[g], m);
-            const float rescale = (m_run[g] == -INFINITY) ? 0.f : __expf(m_run[g] - m_new);
-            const float e = (sv == -INFINITY) ? 0.f : __expf(sv - m_new);     // all 4 lanes of a key hold the same value
-            float l = part == 0 ? e : 0.f;
-            l = warp_sum(l);
-            l_run[g] = l_run[g] * rescale + l;
-            m_run[g] = m_new;
-            o4[g].x *= rescale; o4[g].y *= rescale; o4[g].z *= rescale; o4[g].w *= rescale;
-            pw[g] = e;
-        }
-        // warp-partial P*V: lane owns dims 4*lane .. 4*lane+3 (conflict-free float4 reads of a V row)
-#pragma unroll
-        for (int kk = 0; kk < 8; ++kk) {
-            const int t = warp * 8 + kk;
-            if (t < nk) {
-                const float4 v = reinterpret_cast<const float4*>(sV + t * HD)[lane];
-                _Pragma("unroll") for (int g = 0; g < G; ++g) {
-                    const float pk = __shfl_sync(0xffffffffu, pw[g], kk * 4);
-                    o4[g].x = fmaf(pk, v.x, o4[g].x); o4[g].y = fmaf(pk, v.y, o4[g].y);
-                    o4[g].z = fmaf(pk, v.z, o4[g].z); o4[g].w = fmaf(pk, v.w, o4[g].w);
-                }
-            }
-        }
-        if (c + NB < nch) {
-            __syncthreads();                                     // every warp is done with this slot
-            if (tid == 0) issue(c + NB);
-        }
-    }
-    // merge the 8 warp states
-    _Pragma("unroll") for (int g = 0; g < G; ++g) {
-        reinterpret_cast<float4*>(wpo + (warp * G + g) * HD)[lane] = o4[g];
-        if (lane == 0) { red_m[warp][g] = m_run[g]; red_l[warp][g] = l_run[g]; }
-    }
-    __syncthreads();
-    if (tid < HD) {
-        _Pragma("unroll") for (int g = 0; g < G; ++g) {
-            float M = red_m[0][g];
-#pragma unroll
-            for (int w = 1; w < AT_THREADS / 32; ++w) M = fmaxf(M, red_m[w][g]);
-            float L = 0.f, O = 0.f;
-#pragma unroll
-            for (int w = 0; w < AT_THREADS / 32; ++w) {
-                const float sc_w = red_m[w][g] == -INFINITY ? 0.f : __expf(red_m[w][g] - M);
-                L = fmaf(red_l[w][g], sc_w, L);
-                O = fmaf(wpo[(w * G + g) * HD + tid], sc_w, O);
-            }
-            store_hilo(a.out, (long long)a.nq * HD, b, (h * G + g) * HD + tid, O / L);
-        }
-    }
-}
-
-// Same, with the chunks of one (kv head, row) dealt alternately to the TWO CTAs of a thread-block cluster: 128 CTAs instead of
-// 64, so up to 2 x NB chunks (6 x 64 keys) are in flight before griddepcontrol.wait and the serial chunk count halves.  CTA 1
-// hands its (max, sum, P*V) state to CTA 0 through distributed shared memory; one cluster barrier, nothing goes through HBM.
+// One thread-block cluster of two CTAs per (kv head, row), grid (kv heads, rows, 2).  Keys 0..pos are cut into 64-key chunks
+// (AT_CAP) that are dealt alternately to the two CTAs: CTA r takes chunks r, r + 2, ...  Each CTA streams its chunks through an
+// NB-deep ring of shared-memory buffers, one cp.async.bulk per matrix per chunk; the first NB are issued BEFORE
+// griddepcontrol.wait, so up to 2 x NB chunks (6 x 64 keys) stream in under the tail of the QKV GEMM.  Every warp keeps a running
+// (max, sum, P*V) for its 8 keys of each chunk (online softmax) and the 8 warp states are merged once at the end.  CTA 1 hands its
+// merged state to CTA 0 through distributed shared memory: one cluster barrier, nothing goes through HBM.  `a` is __grid_constant__
+// for the reason given at tc_gemm_kernel.
 template <int G>
 __global__ void __cluster_dims__(1, 1, 2) __launch_bounds__(AT_THREADS)
-attn_decode_cluster_kernel(AttnArgs a, int NB) {
+attn_decode_cluster_kernel(const __grid_constant__ AttnArgs a, int NB) {
     namespace cgr = cooperative_groups;
     cgr::cluster_group cluster = cgr::this_cluster();
     const int rank = (int)cluster.block_rank();
@@ -643,7 +282,6 @@ attn_decode_cluster_kernel(AttnArgs a, int NB) {
 
     const int h = blockIdx.x, b = blockIdx.y, tid = threadIdx.x;
     pdl_trigger();
-    l2_prefetch(a.pf, ((blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x) * AT_THREADS + tid, gridDim.x * gridDim.y * gridDim.z * AT_THREADS);
     // pos[b] is read BEFORE griddepcontrol.wait so that the cached K / V chunks stream in under the QKV GEMM's tail.  Programmatic
     // launches chain (a kernel triggers its dependents at its first instruction, even while it is itself still waiting), so on a
     // small model -- every kernel of several layers resident at once -- this prologue can run before a kernel launched many
@@ -840,12 +478,6 @@ attn_decode_cluster_kernel(AttnArgs a, int NB) {
         }
     }
 }
-
-#ifdef B2A_ATTN_TIMING
-extern "C" int b2a_debug_attn_ts(long long* out, int n) {
-    return (int)cudaMemcpyFromSymbol(out, g_attn_ts, sizeof(long long) * n);
-}
-#endif
 
 // ------------------------------------------------------------------------------------------------
 // Batched prefill (LlamaTTS.swift:711 `self(inputIds, cache)` on the whole prompt): all B*L prompt tokens go
@@ -1305,13 +937,9 @@ struct b2a_tts {
     // activations: fp32 residual stream; GEMM inputs as [16, K] bf16 hi/lo pairs
     DBuf<float> x, y, qkv, logits, probs;
     DBuf<bf16> xn, attn, act;
-    // attention workspace (flash-decoding partials)
-    DBuf<float> part_o, part_ml;
-    DBuf<int> at_counters;
     DBuf<float> sk_ws;       // stream-K partial tiles of the decode GEMMs (qkv / o / down), see tc::Args::part_ws
     DBuf<unsigned> sk_cnt;
     int sk_slots = 0;
-    int at_splits = 1;
     // wgmma / TMA path
     bool use_tc = true;
     int num_sms = 132;
@@ -1338,7 +966,8 @@ struct b2a_tts {
     // fused-norm decode step (default on the wgmma path): o_proj / down_proj run as cluster split-K GEMMs whose leader CTA does the
     // residual add + the next norm's gain + hi/lo split + sum of squares; no stand-alone add_rmsnorm launches (tc_gemm.cuh)
     bool fused = false;
-    int fused_cluster = 5, fused_parts = 0;   // 5 CTAs per 128-row tile: 120 of 132 SMs for hidden 3072, one wave
+    static constexpr int fused_cluster = 5;   // 5 CTAs per 128-row tile: 120 of 132 SMs for hidden 3072, one wave
+    int fused_parts = 0;
     DBuf<float> ss_a, ss_b;          // [H / 128, 8] partial sums of squares: ss_a feeds the post-attention norm, ss_b the input norm
     StackSpec spec;                  // which keys / features this stack was built with
     const float* x_ext = nullptr;    // row N1: when set, a step starts from these embeddings [8, H] instead of embed(tokens)
@@ -1379,14 +1008,7 @@ struct b2a_tts {
         }
     }
 
-    template <int G>
-    static void attn_attr() {
-        B2A_CUDA(cudaFuncSetAttribute(attn_decode_kernel<G>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
-    }
-    template <int G>
-    static void attn_loop_attr() {
-        B2A_CUDA(cudaFuncSetAttribute(attn_decode_loop_kernel<G>, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));   // + 512 B static
-    }
+    // ring depth of attn_decode_cluster_kernel: as many 64-key K|V chunks as fit next to its other buffers, at most 3
     int attn_loop_bufs() const {
         const int G = cfg.num_attention_heads / cfg.num_key_value_heads;
         const size_t extra = (size_t)(G * HD + 2 * HD + (AT_THREADS / 32) * G * HD + G * HD + 2 * MAXG) * sizeof(float) + 64;
@@ -1396,52 +1018,19 @@ struct b2a_tts {
     static void attn_cluster_attr() {
         B2A_CUDA(cudaFuncSetAttribute(attn_decode_cluster_kernel<G>, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));
     }
-    bool attn_loop = true;     // B2A_ATTN=split selects the flash-decoding split kernel, =loop the single-CTA loop
-    bool attn_cluster = true;  // default: two-CTA cluster per (kv head, row)
     void attn_launch(const AttnArgs& aa, int B, cudaStream_t s) {
-        if (attn_loop && attn_cluster) {
-            const int G = aa.nq / aa.nkv, NB = attn_loop_bufs();
-            const size_t sm = (size_t)NB * 2 * AT_CAP * HD * sizeof(float) +
-                              (size_t)(G * HD + 2 * HD + (AT_THREADS / 32) * G * HD + G * HD + 2 * MAXG) * sizeof(float) + 64;
-            const dim3 g3(aa.nkv, B, 2);
-            switch (G) {
-                case 1: launch_pdl(attn_decode_cluster_kernel<1>, g3, dim3(AT_THREADS), sm, s, aa, NB); break;
-                case 2: launch_pdl(attn_decode_cluster_kernel<2>, g3, dim3(AT_THREADS), sm, s, aa, NB); break;
-                case 3: launch_pdl(attn_decode_cluster_kernel<3>, g3, dim3(AT_THREADS), sm, s, aa, NB); break;
-                case 4: launch_pdl(attn_decode_cluster_kernel<4>, g3, dim3(AT_THREADS), sm, s, aa, NB); break;
-                case 6: launch_pdl(attn_decode_cluster_kernel<6>, g3, dim3(AT_THREADS), sm, s, aa, NB); break;
-                default: launch_pdl(attn_decode_cluster_kernel<8>, g3, dim3(AT_THREADS), sm, s, aa, NB); break;
-            }
-            return;
+        const int G = aa.nq / aa.nkv, NB = attn_loop_bufs();
+        const size_t sm = (size_t)NB * 2 * AT_CAP * HD * sizeof(float) +
+                          (size_t)(G * HD + 2 * HD + (AT_THREADS / 32) * G * HD + G * HD + 2 * MAXG) * sizeof(float) + 64;
+        const dim3 g3(aa.nkv, B, 2);
+        switch (G) {
+            case 1: launch_pdl(attn_decode_cluster_kernel<1>, g3, dim3(AT_THREADS), sm, s, aa, NB); break;
+            case 2: launch_pdl(attn_decode_cluster_kernel<2>, g3, dim3(AT_THREADS), sm, s, aa, NB); break;
+            case 3: launch_pdl(attn_decode_cluster_kernel<3>, g3, dim3(AT_THREADS), sm, s, aa, NB); break;
+            case 4: launch_pdl(attn_decode_cluster_kernel<4>, g3, dim3(AT_THREADS), sm, s, aa, NB); break;
+            case 6: launch_pdl(attn_decode_cluster_kernel<6>, g3, dim3(AT_THREADS), sm, s, aa, NB); break;
+            default: launch_pdl(attn_decode_cluster_kernel<8>, g3, dim3(AT_THREADS), sm, s, aa, NB); break;
         }
-        if (attn_loop) {
-            const int G = aa.nq / aa.nkv, NB = attn_loop_bufs();
-            const size_t sm = (size_t)NB * 2 * AT_CAP * HD * sizeof(float) + (size_t)(G * HD + 2 * HD + (AT_THREADS / 32) * G * HD) * sizeof(float) + 64;
-            const dim3 g2(aa.nkv, B);
-            switch (G) {
-                case 1: launch_pdl(attn_decode_loop_kernel<1>, g2, dim3(AT_THREADS), sm, s, aa, NB); break;
-                case 2: launch_pdl(attn_decode_loop_kernel<2>, g2, dim3(AT_THREADS), sm, s, aa, NB); break;
-                case 3: launch_pdl(attn_decode_loop_kernel<3>, g2, dim3(AT_THREADS), sm, s, aa, NB); break;
-                case 4: launch_pdl(attn_decode_loop_kernel<4>, g2, dim3(AT_THREADS), sm, s, aa, NB); break;
-                case 6: launch_pdl(attn_decode_loop_kernel<6>, g2, dim3(AT_THREADS), sm, s, aa, NB); break;
-                default: launch_pdl(attn_decode_loop_kernel<8>, g2, dim3(AT_THREADS), sm, s, aa, NB); break;
-            }
-            return;
-        }
-        const dim3 grid(aa.nkv, B, aa.S);
-        const size_t sm = attn_smem_bytes();
-        switch (aa.nq / aa.nkv) {
-            case 1: launch_pdl(attn_decode_kernel<1>, grid, dim3(AT_THREADS), sm, s, aa); break;
-            case 2: launch_pdl(attn_decode_kernel<2>, grid, dim3(AT_THREADS), sm, s, aa); break;
-            case 3: launch_pdl(attn_decode_kernel<3>, grid, dim3(AT_THREADS), sm, s, aa); break;
-            case 4: launch_pdl(attn_decode_kernel<4>, grid, dim3(AT_THREADS), sm, s, aa); break;
-            case 6: launch_pdl(attn_decode_kernel<6>, grid, dim3(AT_THREADS), sm, s, aa); break;
-            default: launch_pdl(attn_decode_kernel<8>, grid, dim3(AT_THREADS), sm, s, aa); break;
-        }
-    }
-    size_t attn_smem_bytes() const {
-        const int G = cfg.num_attention_heads / cfg.num_key_value_heads;
-        return (size_t)(2 * AT_CAP * HD + G * HD + G * AT_CAP + (AT_THREADS / 32) * G * HD) * sizeof(float) + 16;
     }
 
     void check_config() {
@@ -1454,6 +1043,7 @@ struct b2a_tts {
             B2A_CHECK(g == 1 || g == 2 || g == 3 || g == 4 || g == 6 || g == 8, B2A_ERR_INVALID_INPUT,
                       "llama: unsupported GQA ratio (q heads per kv head must be 1, 2, 3, 4, 6 or 8)");
         }
+        B2A_CHECK(attn_loop_bufs() >= 1, B2A_ERR_INVALID_INPUT, "llama: GQA ratio too large for the attention tile");
         B2A_CHECK(c.max_batch >= 1 && c.max_batch <= 8, B2A_ERR_INVALID_INPUT, "llama: max_batch must be in 1..8");
         B2A_CHECK(c.max_context >= 8, B2A_ERR_INVALID_INPUT, "llama: max_context too small");
         require_device(device);
@@ -1487,33 +1077,17 @@ struct b2a_tts {
         B2A_CUDA(cudaMemset(tokens.p, 0, B * sizeof(int)));
         B2A_CUDA(cudaMemset(pos.p, 0, B * sizeof(int)));
         h_flag.alloc(16);
-        // attention workspace
-        const int G = nq / nkv;
-        at_splits = cdiv(c.max_context, AT_CAP);
-        part_o.alloc((size_t)B * nkv * at_splits * G * HD);
-        part_ml.alloc((size_t)B * nkv * at_splits * G * 2);
-        at_counters.alloc((size_t)B * nkv);
-        B2A_CUDA(cudaMemset(at_counters.p, 0, (size_t)B * nkv * sizeof(int)));
         // process-wide kernel attributes: always the same (largest) value, several handles may coexist
         gemv_attrs<1>(); gemv_attrs<2>(); gemv_attrs<4>(); gemv_attrs<8>();
-        B2A_CHECK(attn_smem_bytes() <= 220 * 1024, B2A_ERR_INVALID_INPUT, "llama: GQA ratio too large for the attention tile");
-        attn_attr<1>(); attn_attr<2>(); attn_attr<3>(); attn_attr<4>(); attn_attr<6>(); attn_attr<8>();
-        attn_loop_attr<1>(); attn_loop_attr<2>(); attn_loop_attr<3>(); attn_loop_attr<4>(); attn_loop_attr<6>(); attn_loop_attr<8>();
         attn_cluster_attr<1>(); attn_cluster_attr<2>(); attn_cluster_attr<3>(); attn_cluster_attr<4>(); attn_cluster_attr<6>(); attn_cluster_attr<8>();
-        { const char* e = getenv("B2A_ATTN"); attn_loop = !(e && std::string(e) == "split"); attn_cluster = !(e && std::string(e) == "loop"); }
-        if (spec.qk_norm) attn_loop = attn_cluster = true;   // only the cluster kernel applies the per-head q/k RMSNorm
-        {
-            const char* e = getenv("B2A_FUSED");
-            const char* cl = getenv("B2A_CLUSTER");
-            if (cl) fused_cluster = std::max(1, std::min(tc::SPLIT_MAX_CLUSTER, atoi(cl)));
-            fused_parts = H / tc::BM;
-            const char* g = getenv("B2A_GEMM");
-            const bool tc_ok = !(g && std::string(g) == "simt") && H % tc::BK == 0 && NQ % tc::BK == 0 && I % tc::BK == 0;
-            fused = !(e && std::string(e) == "0") && tc_ok && attn_loop && attn_cluster && H % tc::BM == 0 && fused_parts <= 64;
-            ss_a.alloc((size_t)64 * 8); ss_b.alloc((size_t)64 * 8);
-            B2A_CUDA(cudaMemset(ss_a.p, 0, 64 * 8 * sizeof(float)));
-            B2A_CUDA(cudaMemset(ss_b.p, 0, 64 * 8 * sizeof(float)));
-        }
+        // wgmma / TMA path: needs every GEMM K to be a multiple of 64; B2A_GEMM=simt forces the SIMT fallback
+        const char* env = getenv("B2A_GEMM");
+        use_tc = !(env && std::string(env) == "simt") && H % tc::BK == 0 && NQ % tc::BK == 0 && I % tc::BK == 0;
+        fused_parts = H / tc::BM;
+        fused = use_tc && H % tc::BM == 0 && fused_parts <= 64;
+        ss_a.alloc((size_t)64 * 8); ss_b.alloc((size_t)64 * 8);
+        B2A_CUDA(cudaMemset(ss_a.p, 0, 64 * 8 * sizeof(float)));
+        B2A_CUDA(cudaMemset(ss_b.p, 0, 64 * 8 * sizeof(float)));
         B2A_CUDA(cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, device));
         {   // stream-K workspace for the decode GEMMs that split K ranges across CTAs: qkv, o, down (BN = 16)
             const int ops[3][2] = {{NQ + 2 * NKV, H}, {H, NQ}, {H, I}};
@@ -1529,9 +1103,6 @@ struct b2a_tts {
             sk_cnt.alloc((size_t)std::max(1, mt_max));
             B2A_CUDA(cudaMemset(sk_cnt.p, 0, (size_t)std::max(1, mt_max) * sizeof(unsigned)));
         }
-        // wgmma / TMA path: needs every GEMM K to be a multiple of 64; B2A_GEMM=simt forces the SIMT fallback
-        const char* env = getenv("B2A_GEMM");
-        use_tc = !(env && std::string(env) == "simt") && H % tc::BK == 0 && NQ % tc::BK == 0 && I % tc::BK == 0;
         const char* envp = getenv("B2A_PREFILL");
         use_batched_prefill = !(envp && std::string(envp) == "step");
         if (use_tc) {
@@ -1541,12 +1112,9 @@ struct b2a_tts {
                 tm_o.push_back(tc::make_tmap_bf16(L.wo.p, H, NQ, tc::BM));
                 tm_gu.push_back(tc::make_tmap_bf16(L.wgu.p, 2 * I, H, tc::BM));
                 {   // decode step: when 128-row tiles would leave more than a quarter of the SMs idle (Qwen3-TTS: 6144 rows = 48 tiles), use
-                    // as many m-tiles as SMs (rows per tile a multiple of 8).  Orpheus (128 tiles on 132 SMs) keeps 128.  B2A_GU_ROWS overrides.
-                    static const int e_rows = getenv("B2A_GU_ROWS") ? atoi(getenv("B2A_GU_ROWS")) : 0;
-                    int rows = e_rows > 0 ? e_rows : (cdiv(2 * I, tc::BM) * 4 >= num_sms * 3 ? tc::BM : cdiv(cdiv(2 * I, num_sms), 8) * 8);
-                    rows = std::max(8, std::min(tc::BM, rows / 8 * 8));
-                    gu_tile_rows = rows;
-                    tm_gu_dec.push_back(tc::make_tmap_bf16(L.wgu.p, 2 * I, H, rows));
+                    // as many m-tiles as SMs (rows per tile a multiple of 8).  Orpheus (128 tiles on 132 SMs) keeps 128.
+                    gu_tile_rows = pick_tile_rows(2 * I, num_sms);
+                    tm_gu_dec.push_back(tc::make_tmap_bf16(L.wgu.p, 2 * I, H, gu_tile_rows));
                 }
                 tm_down.push_back(tc::make_tmap_bf16(L.wdown.p, H, I, tc::BM));
             }
@@ -1698,54 +1266,14 @@ struct b2a_tts {
     }
 
     // D[tokens, M] = X[tokens, K] * W[M, K]^T on the wgmma path (hi/lo activations, BN = 16)
-    // ---- L2 prefetch schedule (B2A_L2PF bit mask; see pf_of): which kernel prefetches which later GEMM's weights
-    enum : int { L2_NORM1 = 0, L2_QKV, L2_ATTN, L2_O, L2_NORM2, L2_GU, L2_DOWN };
-    int l2pf_mask = -1;
-    L2Prefetch pf_of(int site, int l) {
-        if (l2pf_mask < 0) {
-            const char* e = getenv("B2A_L2PF");
-            l2pf_mask = e ? (int)strtol(e, nullptr, 0) : L2PF_DEFAULT;
-        }
-        if (!use_tc || l < 0 || l >= cfg.num_hidden_layers) return L2Prefetch{nullptr, 0};
-        const long long H = cfg.hidden_size, I = cfg.intermediate_size, NQ = (long long)cfg.num_attention_heads * HD,
-                        NKV = (long long)cfg.num_key_value_heads * HD;
-        const long long b_qkv = (NQ + 2 * NKV) * H * 2, b_o = H * NQ * 2, b_gu = 2 * I * H * 2, b_down = H * I * 2;
-        LayerW& L = layers[l];
-        const bool last = l + 1 == cfg.num_hidden_layers;
-        switch (site) {
-            case L2_NORM1: if (l2pf_mask & 1) return L2Prefetch{L.wqkv.p, b_qkv}; break;                 // norm1 -> QKV
-            case L2_ATTN:
-                if ((l2pf_mask & 2) && (l2pf_mask & 4)) return L2Prefetch{L.wo.p, b_o};                   // attn -> O (GU by the O GEMM)
-                if (l2pf_mask & 2) {                                                                      // attn -> GU (first B2A_L2PF_GU_MB MB)
-                    static const long long cap = getenv("B2A_L2PF_GU_MB") ? atoll(getenv("B2A_L2PF_GU_MB")) << 20 : (1ll << 40);
-                    return L2Prefetch{L.wgu.p, std::min(b_gu, cap)};
-                }
-                if (l2pf_mask & 4) return L2Prefetch{L.wo.p, b_o};
-                break;
-            case L2_QKV: if (l2pf_mask & 8) return L2Prefetch{L.wo.p, b_o}; break;                        // QKV GEMM -> O
-            case L2_O: if (l2pf_mask & 16) return L2Prefetch{L.wgu.p, b_gu}; break;                       // O GEMM -> GU
-            case L2_NORM2: if (l2pf_mask & 32) return L2Prefetch{L.wdown.p, b_down}; break;               // norm2 -> DOWN
-            case L2_GU: if (l2pf_mask & 64) return L2Prefetch{L.wdown.p, b_down}; break;                  // GU GEMM -> DOWN
-            case L2_DOWN:
-                if (l2pf_mask & 128) return last ? L2Prefetch{lm_head, 64ll << 20} : L2Prefetch{layers[l + 1].wqkv.p, b_qkv};   // DOWN -> next QKV
-                break;
-        }
-        return L2Prefetch{nullptr, 0};
-    }
-    static constexpr int L2PF_DEFAULT = 0;
-
     void tc_gemm(const CUtensorMap& tmW, const CUtensorMap& tmX, int op, float* yout, bf16* actout, int B, int M, int K,
-                 cudaStream_t s, L2Prefetch pf = L2Prefetch{nullptr, 0}, const float* rstd_ss = nullptr) {
+                 cudaStream_t s, const float* rstd_ss = nullptr) {
         tc::Args a{};
-        a.pf_ptr = pf.ptr; a.pf_bytes = pf.bytes;
         a.rstd_ss = rstd_ss; a.rstd_parts = fused_parts; a.rstd_inv_h = 1.0f / (float)cfg.hidden_size; a.rstd_eps = cfg.rms_norm_eps;
         a.out_f32 = yout; a.out_bf16 = actout; a.M = M; a.N = B; a.K = K;
         a.m_tiles = cdiv(M, tc::BM); a.k_blocks = K / tc::BK;
         a.stages = 6;   // 6 x 18 KB ring + 10 KB staged accumulator = 119 KB: one GEMM CTA per SM.  5 stages (101 KB) let the next
                         // kernel's prefetching CTA co-reside, but measured slower on the H100 (Orpheus batch 8: 26.4x vs 28.3x real time)
-        { static const int e_all = getenv("B2A_STAGES") ? atoi(getenv("B2A_STAGES")) : 0, e_gu = getenv("B2A_STAGES_GU") ? atoi(getenv("B2A_STAGES_GU")) : 0;
-          if (e_all > 0) a.stages = e_all;
-          if (op == OP_GU && e_gu > 0) a.stages = e_gu; }
         a.hilo = 1;
         int ctas = num_sms;
         if (op == OP_GU) {
@@ -1770,19 +1298,19 @@ struct b2a_tts {
         LayerW* L = layer >= 0 ? &layers[layer] : nullptr;
         switch (op) {
             case OP_QKV:
-                if (use_tc) tc_gemm(tm_qkv[layer], tmx_xn, op, qkv.p, nullptr, B, NQ + 2 * NKV, H, s, pf_of(L2_QKV, layer));
+                if (use_tc) tc_gemm(tm_qkv[layer], tmx_xn, op, qkv.p, nullptr, B, NQ + 2 * NKV, H, s);
                 else gemv_nb(op, L->wqkv.p, xn.p, qkv.p, nullptr, NQ + 2 * NKV, H, s);
                 break;
             case OP_O:
-                if (use_tc) tc_gemm(tm_o[layer], tmx_attn, op, y.p, nullptr, B, H, NQ, s, pf_of(L2_O, layer));
+                if (use_tc) tc_gemm(tm_o[layer], tmx_attn, op, y.p, nullptr, B, H, NQ, s);
                 else gemv_nb(op, L->wo.p, attn.p, y.p, nullptr, H, NQ, s);
                 break;
             case OP_GU:
-                if (use_tc) tc_gemm(tm_gu_dec[layer], tmx_xn, op, nullptr, act.p, B, 2 * I, H, s, pf_of(L2_GU, layer));
+                if (use_tc) tc_gemm(tm_gu_dec[layer], tmx_xn, op, nullptr, act.p, B, 2 * I, H, s);
                 else gemv_nb(op, L->wgu.p, xn.p, nullptr, act.p, 2 * I, H, s);
                 break;
             case OP_DOWN:
-                if (use_tc) tc_gemm(tm_down[layer], tmx_act, op, y.p, nullptr, B, H, I, s, pf_of(L2_DOWN, layer));
+                if (use_tc) tc_gemm(tm_down[layer], tmx_act, op, y.p, nullptr, B, H, I, s);
                 else gemv_nb(op, L->wdown.p, act.p, y.p, nullptr, H, I, s);
                 break;
             default:
@@ -1792,17 +1320,10 @@ struct b2a_tts {
         }
     }
 
-    // timing ablation only (B2A_SKIP=norm|attn|gemm|qkv|o|gu|down, comma separated): skips launches, results invalid
-    static bool skip(const char* what) {
-        const char* e = getenv("B2A_SKIP");
-        return e && strstr(e, what) != nullptr;
-    }
-
     // o_proj / down_proj as a cluster split-K GEMM with the residual add and the next norm fused into the leader's epilogue
     void splitk_gemm(const CUtensorMap& tmW, const CUtensorMap& tmX, int M, int K, const float* gain, float* ss, int B, cudaStream_t s) {
         tc::SplitArgs a{};
         a.M = M; a.N = B; a.K = K; a.k_blocks = K / tc::BK; a.stages = 5;
-        { static const int e_sk = getenv("B2A_STAGES_SK") ? atoi(getenv("B2A_STAGES_SK")) : 0; if (e_sk > 0) a.stages = e_sk; }
         a.h = x.p; a.gain = gain; a.xn = xn.p; a.ss = ss;
         a.rstd_ss = nullptr; a.rstd_parts = 0; a.rstd_inv_h = 0.f; a.rstd_eps = 0.f;
         tc::launch_splitk(tmW, tmX, a, cdiv(M, tc::BM), std::max(1, std::min(fused_cluster, a.k_blocks)), s);
@@ -1816,17 +1337,16 @@ struct b2a_tts {
         if (x_ext) launch_pdl(ext_embed_kernel, dim3(B), dim3(256), 0, s, x_ext, x.p, y.p, H);
         else launch_pdl(embed_kernel, dim3(B), dim3(256), 0, s, tokens.p, embed.p, x.p, y.p, H, cfg.vocab_size);
         launch_pdl(add_rmsnorm_kernel, dim3(B), dim3(RN_THREADS), 0, s, x.p, (float*)nullptr, layers[0].ln1.p, xn.p, H, cfg.rms_norm_eps,
-                   (float*)nullptr, (float*)nullptr, 0, LO_ROW, L2Prefetch{nullptr, 0}, (float*)nullptr, ss_b.p, fused_parts);
+                   (float*)nullptr, (float*)nullptr, 0, LO_ROW, (float*)nullptr, ss_b.p, fused_parts);
         const size_t kv_layer = (size_t)cfg.max_batch * nkv * cfg.max_context * HD;
         for (int l = 0; l < L; ++l) {
             LayerW& Lw = layers[l];
-            tc_gemm(tm_qkv[l], tmx_xn, OP_QKV, qkv.p, nullptr, B, NQ + 2 * NKV, H, s, pf_of(L2_QKV, l), ss_b.p);
-            AttnArgs aa{qkv.p, pos.p, freqs.p, kcache.p + l * kv_layer, vcache.p + l * kv_layer, attn.p, part_o.p, part_ml.p,
-                        at_counters.p, nq, nkv, cfg.max_context, at_splits, 1.0f / sqrtf((float)HD), pf_of(L2_ATTN, l),
-                        spec.qk_norm ? Lw.qnorm.p : nullptr, spec.qk_norm ? Lw.knorm.p : nullptr, cfg.rms_norm_eps, 1};
+            tc_gemm(tm_qkv[l], tmx_xn, OP_QKV, qkv.p, nullptr, B, NQ + 2 * NKV, H, s, ss_b.p);
+            AttnArgs aa{qkv.p, pos.p, freqs.p, kcache.p + l * kv_layer, vcache.p + l * kv_layer, attn.p, nq, nkv, cfg.max_context,
+                        1.0f / sqrtf((float)HD), spec.qk_norm ? Lw.qnorm.p : nullptr, spec.qk_norm ? Lw.knorm.p : nullptr, cfg.rms_norm_eps, 1};
             attn_launch(aa, B, s);
             splitk_gemm(tm_o[l], tmx_attn, H, NQ, Lw.ln2.p, ss_a.p, B, s);
-            tc_gemm(tm_gu_dec[l], tmx_xn, OP_GU, nullptr, act.p, B, 2 * I, H, s, pf_of(L2_GU, l), ss_a.p);
+            tc_gemm(tm_gu_dec[l], tmx_xn, OP_GU, nullptr, act.p, B, 2 * I, H, s, ss_a.p);
             splitk_gemm(tm_down[l], tmx_act, H, I, l + 1 < L ? layers[l + 1].ln1.p : final_ln.p, ss_b.p, B, s);
         }
     }
@@ -1842,22 +1362,19 @@ struct b2a_tts {
         const size_t kv_layer = (size_t)cfg.max_batch * nkv * cfg.max_context * HD;
         for (int l = 0; l < cfg.num_hidden_layers; ++l) {
             LayerW& L = layers[l];
-            if (!skip("norm"))
             launch_pdl(add_rmsnorm_kernel, dim3(B), dim3(RN_THREADS), 0, s, x.p, l == 0 ? (float*)nullptr : y.p, L.ln1.p, xn.p, H,
                        cfg.rms_norm_eps, trace_on ? trace.p + (size_t)(2 * l) * 8 * H : (float*)nullptr, (float*)nullptr, 0, LO_ROW,
-                       pf_of(L2_NORM1, l), (float*)nullptr, (float*)nullptr, 0);
-            if (!skip("gemm") && !skip("qkv")) gemm(OP_QKV, l, B, s);
-            AttnArgs aa{qkv.p, pos.p, freqs.p, kcache.p + l * kv_layer, vcache.p + l * kv_layer, attn.p, part_o.p, part_ml.p,
-                        at_counters.p, nq, nkv, cfg.max_context, at_splits, 1.0f / sqrtf((float)HD), pf_of(L2_ATTN, l),
-                        spec.qk_norm ? L.qnorm.p : nullptr, spec.qk_norm ? L.knorm.p : nullptr, cfg.rms_norm_eps, 0};
-            if (!skip("attn")) attn_launch(aa, B, s);
-            if (!skip("gemm") && !skip("o_proj")) gemm(OP_O, l, B, s);
+                       (float*)nullptr, (float*)nullptr, 0);
+            gemm(OP_QKV, l, B, s);
+            AttnArgs aa{qkv.p, pos.p, freqs.p, kcache.p + l * kv_layer, vcache.p + l * kv_layer, attn.p, nq, nkv, cfg.max_context,
+                        1.0f / sqrtf((float)HD), spec.qk_norm ? L.qnorm.p : nullptr, spec.qk_norm ? L.knorm.p : nullptr, cfg.rms_norm_eps, 0};
+            attn_launch(aa, B, s);
+            gemm(OP_O, l, B, s);
             // also zeroes this row of q|k|v so the next layer's stream-K QKV GEMM can accumulate into it
-            if (!skip("norm"))
             launch_pdl(add_rmsnorm_kernel, dim3(B), dim3(RN_THREADS), 0, s, x.p, y.p, L.ln2.p, xn.p, H, cfg.rms_norm_eps,
-                       trace_on ? trace.p + (size_t)(2 * l + 1) * 8 * H : (float*)nullptr, qkv.p, QKV_N, LO_ROW, pf_of(L2_NORM2, l), (float*)nullptr, (float*)nullptr, 0);
-            if (!skip("gemm") && !skip("gate")) gemm(OP_GU, l, B, s);
-            if (!skip("gemm") && !skip("down")) gemm(OP_DOWN, l, B, s);
+                       trace_on ? trace.p + (size_t)(2 * l + 1) * 8 * H : (float*)nullptr, qkv.p, QKV_N, LO_ROW, (float*)nullptr, (float*)nullptr, 0);
+            gemm(OP_GU, l, B, s);
+            gemm(OP_DOWN, l, B, s);
         }
         (void)G;
     }
@@ -1871,24 +1388,23 @@ struct b2a_tts {
         }
         launch_pdl(add_rmsnorm_kernel, dim3(B), dim3(RN_THREADS), 0, s, x.p, y.p, final_ln.p, xn.p, cfg.hidden_size, cfg.rms_norm_eps,
                    trace_on ? trace.p + (size_t)(2 * cfg.num_hidden_layers) * 8 * cfg.hidden_size : (float*)nullptr, (float*)nullptr, 0, LO_ROW,
-                   L2Prefetch{nullptr, 0}, normed_out, (float*)nullptr, 0);
+                   normed_out, (float*)nullptr, 0);
     }
     void run_lm_head(int B, cudaStream_t s) {
         run_final_norm(B, s);
-        if (fused && !trace_on) tc_gemm(tm_lm, tmx_xn, OP_LM, logits.p, nullptr, B, cfg.vocab_size, cfg.hidden_size, s, L2Prefetch{nullptr, 0}, ss_b.p);
+        if (fused && !trace_on) tc_gemm(tm_lm, tmx_xn, OP_LM, logits.p, nullptr, B, cfg.vocab_size, cfg.hidden_size, s, ss_b.p);
         else gemm(OP_LM, -1, B, s);
     }
     // after prefill_batched's gather_last (x, y hold the last position un-added): always the stand-alone norm + plain GEMM
     void run_lm_head_after_prefill(int B, cudaStream_t s) {
         launch_pdl(add_rmsnorm_kernel, dim3(B), dim3(RN_THREADS), 0, s, x.p, y.p, final_ln.p, xn.p, cfg.hidden_size, cfg.rms_norm_eps,
-                   (float*)nullptr, (float*)nullptr, 0, LO_ROW, L2Prefetch{nullptr, 0}, (float*)nullptr, (float*)nullptr, 0);
+                   (float*)nullptr, (float*)nullptr, 0, LO_ROW, (float*)nullptr, (float*)nullptr, 0);
         gemm(OP_LM, -1, B, s);
     }
     // a head the caller owns (row N1: the code predictor's 15 lm heads): logits_out[b, :M] = W[M, H] * normed hidden
     void run_head(const CUtensorMap& tmW, const bf16* W, int M, float* logits_out, int B, cudaStream_t s, int tile_rows = 0) {
         head_rows_now = tile_rows;              // tmW's box rows (0: this stack's own lm_tile_rows)
-        if (use_tc) tc_gemm(tmW, tmx_xn, OP_LM, logits_out, nullptr, B, M, cfg.hidden_size, s, L2Prefetch{nullptr, 0},
-                            (fused && !trace_on) ? ss_b.p : nullptr);
+        if (use_tc) tc_gemm(tmW, tmx_xn, OP_LM, logits_out, nullptr, B, M, cfg.hidden_size, s, (fused && !trace_on) ? ss_b.p : nullptr);
         else gemv_nb(OP_LM, W, xn.p, logits_out, nullptr, M, cfg.hidden_size, s);
         head_rows_now = 0;
     }
@@ -1947,7 +1463,7 @@ struct b2a_tts {
         for (int l = 0; l < cfg.num_hidden_layers; ++l) {
             LayerW& Lw = layers[l];
             launch_pdl(add_rmsnorm_kernel, dim3(T), dim3(RN_THREADS), 0, s, xp.p, l == 0 ? (float*)nullptr : yp.p, Lw.ln1.p, xnp.p, H,
-                       cfg.rms_norm_eps, (float*)nullptr, (float*)nullptr, 0, PF_HALF, L2Prefetch{nullptr, 0}, (float*)nullptr, (float*)nullptr, 0);
+                       cfg.rms_norm_eps, (float*)nullptr, (float*)nullptr, 0, PF_HALF, (float*)nullptr, (float*)nullptr, 0);
             pf_gemm(tm_qkv[l], tmp_xn, tc::EPI_STORE, qkvp.p, nullptr, T, QKV_N, H, s);
             PrefillAttnArgs pa{qkvp.p, rope_tab.p, kcache.p + l * kv_layer, vcache.p + l * kv_layer, attnp.p, nq, nkv,
                                cfg.max_context, L, 1.0f / sqrtf((float)HD)};
@@ -1964,7 +1480,7 @@ struct b2a_tts {
             count_launch();
             pf_gemm(tm_o[l], tmp_attn, tc::EPI_STORE, yp.p, nullptr, T, H, NQ, s);
             launch_pdl(add_rmsnorm_kernel, dim3(T), dim3(RN_THREADS), 0, s, xp.p, yp.p, Lw.ln2.p, xnp.p, H, cfg.rms_norm_eps,
-                       (float*)nullptr, (float*)nullptr, 0, PF_HALF, L2Prefetch{nullptr, 0}, (float*)nullptr, (float*)nullptr, 0);
+                       (float*)nullptr, (float*)nullptr, 0, PF_HALF, (float*)nullptr, (float*)nullptr, 0);
             pf_gemm(tm_gu[l], tmp_xn, tc::EPI_SWIGLU, nullptr, actp.p, T, 2 * I, H, s);
             pf_gemm(tm_down[l], tmp_act, tc::EPI_STORE, yp.p, nullptr, T, H, I, s);
         }

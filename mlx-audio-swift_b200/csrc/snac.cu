@@ -623,7 +623,6 @@ struct b2a_snac {
     bool use_tc = true;      // wgmma / NLC path (B2A_SNAC=simt selects the fp32 CUDA-core path)
     int num_sms = 132;
     DBuf<float> xs, xs2;                 // NLC fp32 activations of the current stage (ping-pong for the fused units)
-    bool use_fused = true;               // fused ResidualUnit / NoiseBlock kernel for C <= 128 (B2A_SNAC_FUSED=0 disables)
     DBuf<__nv_bfloat16> hA, x2;          // hi/lo tiles: GEMM input of the stage / 2-tap im2col of the next transposed conv
     std::vector<DecBlock> blocks;
     DBuf<float> alpha_final;
@@ -758,8 +757,6 @@ struct b2a_snac {
             fused_attrs<64>(); fused_attrs<128>();
             B2A_CUDA(cudaFuncSetAttribute(rf::convt_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rf::convt_smem_bytes()));
             B2A_CUDA(cudaFuncSetAttribute(final_nlc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (FN_TT + 6) * FN_MAXC * (int)sizeof(float)));
-            const char* ef = getenv("B2A_SNAC_FUSED");
-            use_fused = !(ef && std::string(ef) == "0");
             pw0_tc.build(host_pw0, C, latent);
             size_t ip = 0;
             for (size_t i = 0; i < blocks.size(); ++i) {
@@ -810,15 +807,16 @@ struct b2a_snac {
         B2A_CUDA(cudaFuncSetAttribute(rf::ru_fused_kernel<rf::MODE_RU, 9, CC>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
         B2A_CUDA(cudaFuncSetAttribute(rf::ru_fused_kernel<rf::MODE_NOISE, 0, CC>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     }
+    // fused ResidualUnit / NoiseBlock kernels (snac_fused.cuh) for 64 or 128 channels; other widths run the unfused NLC kernels
     bool block_fused(const DecBlock& B) const {
-        bool ok = use_fused && (B.cout == 64 || B.cout == 128);
+        bool ok = B.cout == 64 || B.cout == 128;
         for (int u = 0; u < 3; ++u) ok = ok && (B.ru[u].dil == 1 || B.ru[u].dil == 3 || B.ru[u].dil == 9);
         return ok;
     }
     // Snake + transposed conv fused (snac_fused.cuh convt_fused_kernel): 128 input channels -> stride * C_out = 128 phase rows,
     // fed by a fused block (its fp32 output is the only copy)
     bool convt_fused_ok(size_t i) const {
-        if (!use_fused || i == 0 || i >= blocks.size()) return false;
+        if (i == 0 || i >= blocks.size()) return false;
         const DecBlock& B = blocks[i];
         return B.cin == 128 && B.stride * B.cout == 128 && block_fused(blocks[i - 1]) && block_fused(B);
     }

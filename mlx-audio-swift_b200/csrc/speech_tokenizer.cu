@@ -343,12 +343,8 @@ final_conv_kernel(const float* __restrict__ x, const float* __restrict__ st, con
 }
 
 // ----------------------------------------------------------------------------------------------- weights
-// k-blocks per accumulation segment of the implicit convolution (ic::Args::seg_kb); B2A_ST_SEG=0 restores one accumulator per tile
-static int seg_kb_default() {
-    static int v = -1;
-    if (v < 0) { const char* e = getenv("B2A_ST_SEG"); v = e ? std::max(0, atoi(e)) : 4; }
-    return v;
-}
+// k-blocks per accumulation segment of the implicit convolution (ic::Args::seg_kb)
+constexpr int SEG_KB = 4;
 
 struct IW {                       // implicit-conv weight: [M][taps][cblocks * 64] as bf16 hi / lo, K-major
     DBuf<bf16> hi, lo;
@@ -669,7 +665,7 @@ struct b2a_speech_tokenizer {
         a.t_tiles = cdiv(a.T, ic::HALF);
         a.bias = W.has_bias ? W.bias.p : nullptr;
         a.f16 = use_f16;
-        a.seg_kb = seg_kb_default();
+        a.seg_kb = SEG_KB;
         a.wscale = use_f16 ? W.rscale.p : nullptr;
         const CUtensorMap tb = make_tmap_planes(in, W.Cin, in_frames, a.B, use_f16);
         const long long tiles = (long long)a.B * a.t_tiles * a.m_tiles;
@@ -972,7 +968,7 @@ int32_t b2a_implicit_conv_test(const float* w, int32_t M, int32_t taps, int32_t 
         ic::Args a{};
         a.M = M; a.m_tiles = cdiv(M, tc::BM); a.taps = taps; a.cblocks = W.cblocks; a.dil = dil; a.shift0 = shift0;
         a.B = B; a.T = T; a.t_tiles = cdiv(T, ic::HALF); a.Cout = Cout; a.up = up; a.gelu = gelu; a.add = add; a.bias_twice_t0 = bias_twice_t0; a.Hout = Hout; a.f16 = fp16;
-        a.seg_kb = seg_kb_default();
+        a.seg_kb = SEG_KB;
         a.wscale = fp16 ? W.rscale.p : nullptr;
         if (bias) { dbias.upload(bias, Cout); a.bias = dbias.p; }
         if (gamma) { dgamma.upload(gamma, Cout); a.gamma = dgamma.p; }

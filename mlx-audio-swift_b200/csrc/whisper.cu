@@ -8,8 +8,8 @@
 // Every Linear / Conv is the wgmma "weights-as-A" GEMM (csrc/tc_gemm.cuh) on bf16 weights with bf16 hi/lo
 // activation pairs (fp32-activation accuracy): the conv stem through an im2col that writes the hi/lo tiles directly,
 // encoder layers with 64-token tiles, decoder steps with up to 16 rows in one 32-column tile.  Residual adds,
-// biases and GELU are GEMM epilogues.  Attention: a flash-style fp32 kernel for the 1500x1500 encoder maps and a
-// flash-decoding kernel (bulk async K/V loads, split over keys) for the decoder's self and cross attention.
+// biases and GELU are GEMM epilogues.  Attention: the wgmma flash-attention kernel (csrc/attn_tc.cuh, fp16 operands) for the
+// 1500x1500 encoder maps and a flash-decoding kernel (bulk async K/V loads, split over keys) for the decoder's self and cross attention.
 #include "common.cuh"
 #include "tc_gemm.cuh"
 #include "attn_tc.cuh"
@@ -174,107 +174,6 @@ __global__ void im2col3_kernel(const float* __restrict__ in, bf16* __restrict__ 
             if (ti >= 0 && ti < Tin) v = in[((long long)b * Tin + ti) * C + c];
         }
         store_hilo(out, Kp, tok, i, v, ENC_HALF);
-    }
-}
-
-// ------------------------------------------------------------------------------------------------
-// Encoder self-attention (bidirectional, WhisperLayers.swift:62-68): flash-style fp32, one CTA per
-// (64-query tile, head, clip); q|k|v come from the fused projection buffer [tokens, 3d].
-// ------------------------------------------------------------------------------------------------
-constexpr int FA_T = 64, FA_THREADS = 256, FA_LD = 68;
-__global__ void __launch_bounds__(FA_THREADS)
-mha_fwd_kernel(const float* __restrict__ qkv, bf16* __restrict__ out, int T, int d, float scale) {
-    extern __shared__ __align__(16) float fa_smem[];
-    float* Qs = fa_smem;                 // [64][64]
-    float* Kt = Qs + FA_T * HD;          // [64 d][68]  (transposed keys)
-    float* Vs = Kt + HD * FA_LD;         // [64 keys][64]
-    float* Ps = Vs + FA_T * HD;          // [64][68]
-    const int q0 = blockIdx.x * FA_T, h = blockIdx.y, b = blockIdx.z;
-    const int tid = threadIdx.x, ty = tid >> 4, tx = tid & 15;
-    const long long ld = 3LL * d;
-    const float* base = qkv + (long long)b * T * ld;
-
-    for (int i = tid; i < FA_T * HD; i += FA_THREADS) {
-        const int r = i >> 6, c = i & 63;
-        Qs[i] = (q0 + r < T) ? base[(long long)(q0 + r) * ld + h * HD + c] * scale : 0.f;
-    }
-    float m_i[4], l_i[4], o[4][4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-        m_i[i] = -INFINITY; l_i[i] = 0.f;
-#pragma unroll
-        for (int j = 0; j < 4; ++j) o[i][j] = 0.f;
-    }
-    for (int k0 = 0; k0 < T; k0 += FA_T) {
-        __syncthreads();
-        for (int i = tid; i < FA_T * HD; i += FA_THREADS) {
-            const int r = i >> 6, c = i & 63;      // key r, dim c
-            const bool ok = k0 + r < T;
-            const float* src = base + (long long)(k0 + r) * ld + h * HD + c;
-            Kt[c * FA_LD + r] = ok ? src[d] : 0.f;
-            Vs[r * HD + c] = ok ? src[2 * d] : 0.f;
-        }
-        __syncthreads();
-        float s[4][4];
-#pragma unroll
-        for (int i = 0; i < 4; ++i)
-#pragma unroll
-            for (int j = 0; j < 4; ++j) s[i][j] = 0.f;
-#pragma unroll 8
-        for (int dd = 0; dd < HD; ++dd) {
-            const float4 kf = *reinterpret_cast<const float4*>(&Kt[dd * FA_LD + 4 * tx]);
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                const float qv = Qs[(4 * ty + i) * HD + dd];
-                s[i][0] = fmaf(qv, kf.x, s[i][0]); s[i][1] = fmaf(qv, kf.y, s[i][1]);
-                s[i][2] = fmaf(qv, kf.z, s[i][2]); s[i][3] = fmaf(qv, kf.w, s[i][3]);
-            }
-        }
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-            float mx = -INFINITY;
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-                if (k0 + 4 * tx + j >= T) s[i][j] = -INFINITY;
-                mx = fmaxf(mx, s[i][j]);
-            }
-#pragma unroll
-            for (int off = 1; off < 16; off <<= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, off));
-            const float m_new = fmaxf(m_i[i], mx);
-            float rs = 0.f;
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-                const float p = s[i][j] == -INFINITY ? 0.f : __expf(s[i][j] - m_new);
-                Ps[(4 * ty + i) * FA_LD + 4 * tx + j] = p;
-                rs += p;
-            }
-#pragma unroll
-            for (int off = 1; off < 16; off <<= 1) rs += __shfl_xor_sync(0xffffffffu, rs, off);
-            const float alpha = m_i[i] == -INFINITY ? 0.f : __expf(m_i[i] - m_new);
-            l_i[i] = l_i[i] * alpha + rs;
-            m_i[i] = m_new;
-#pragma unroll
-            for (int j = 0; j < 4; ++j) o[i][j] *= alpha;
-        }
-        __syncthreads();
-#pragma unroll 8
-        for (int c = 0; c < FA_T; ++c) {
-            const float4 vf = *reinterpret_cast<const float4*>(&Vs[c * HD + 4 * tx]);
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                const float p = Ps[(4 * ty + i) * FA_LD + c];
-                o[i][0] = fmaf(p, vf.x, o[i][0]); o[i][1] = fmaf(p, vf.y, o[i][1]);
-                o[i][2] = fmaf(p, vf.z, o[i][2]); o[i][3] = fmaf(p, vf.w, o[i][3]);
-            }
-        }
-    }
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-        const int q = q0 + 4 * ty + i;
-        if (q >= T) continue;
-        const float inv = 1.0f / l_i[i];
-#pragma unroll
-        for (int j = 0; j < 4; ++j) store_hilo(out, d, (long long)b * T + q, h * HD + 4 * tx + j, o[i][j] * inv, ENC_HALF);
     }
 }
 
@@ -659,8 +558,6 @@ struct b2a_stt {
     DBuf<bf16> X1, X2, xne, attne, acte, enc_out;
     DBuf<__half> fa_q, fa_k, fa_vt;                  // attn_tc.cuh operands: [B*nh][Tp][64] x2, [B*nh][64][Tp]
     CUtensorMap tm_faq{}, tm_fak{}, tm_fav{};
-    bool split_residual_gemms = true;                // B2A_WH_SPLIT=0: whole-tile CTAs for the decoder's residual GEMMs
-    bool attn_tc = true;                             // B2A_WH_ATTN=simt: the fp32 CUDA-core flash kernel (kept as an independent implementation)
     static constexpr int FA_TP = 1536;               // 1500 keys padded to whole 128-key tiles
     CUtensorMap tmx_X1{}, tmx_X2{}, tmx_xne{}, tmx_attne{}, tmx_acte{}, tmx_encout{};
     // caches
@@ -701,8 +598,7 @@ struct b2a_stt {
     // A decode-step GEMM that cannot split K (bias / GELU epilogue) runs on M / 128 CTAs -- 12, 4 and 16 for q|k|v, the cross query and
     // fc1 of Whisper-base.  Tiles of fewer weight rows (a multiple of 8) spread the same rows over up to one CTA per SM.
     void make_step_map(Lin& L) {
-        static const bool off = getenv("B2A_WH_ROWS") && atoi(getenv("B2A_WH_ROWS")) == 128;
-        if (off || cdiv(L.M, tc::BM) * 4 >= num_sms * 3) return;
+        if (cdiv(L.M, tc::BM) * 4 >= num_sms * 3) return;
         L.step_rows = std::max(8, std::min(tc::BM, cdiv(cdiv(L.M, num_sms), 8) * 8));
         L.tm_step = tc::make_tmap_bf16(L.w.p, L.M, L.K, L.step_rows);
     }
@@ -720,7 +616,6 @@ struct b2a_stt {
         B2A_CUDA(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
         B2A_CUDA(cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, device));
         tc::set_attributes();
-        B2A_CUDA(cudaFuncSetAttribute(mha_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
     }
 
     int k1p() const { return cdiv(3 * cfg.num_mel_bins, 64) * 64; }
@@ -925,7 +820,7 @@ struct b2a_stt {
         a.epi_full = epi; a.epi_partial = -1; a.bias = bias; a.act = act;
         a.lo_rows = epi == tc::EPI_STORE_BF16 ? DEC_HALF : 0;
         int ctas = std::min(num_sms, a.m_tiles);
-        if (epi == tc::EPI_ADD && act == tc::ACT_NONE && split_residual_gemms) {
+        if (epi == tc::EPI_ADD && act == tc::ACT_NONE) {
             // out-proj / cross out-proj / fc2 add into the residual stream: their (m_tile, k_block) units can be dealt to many CTAs
             // (stream-K), a tile's partials summed in slot order and added into x.  M = 512 gives only 4 whole-tile CTAs otherwise,
             // each streaming its K range alone.
@@ -938,7 +833,7 @@ struct b2a_stt {
         tc::launch<32>(tmW, tmX, a, ctas, 1, s);
     }
     void gemm_step(const Lin& L, const CUtensorMap& tmX, int epi, int act, float* of32, bf16* obf16, int B, cudaStream_t s) {
-        const bool whole = !(epi == tc::EPI_ADD && act == tc::ACT_NONE && split_residual_gemms);
+        const bool whole = !(epi == tc::EPI_ADD && act == tc::ACT_NONE);
         if (whole && L.step_rows > 0) gemm_step(L.tm_step, L.M, L.K, L.has_bias ? L.b.p : nullptr, tmX, epi, act, of32, obf16, B, s, L.step_rows);
         else gemm_step(L.tm, L.M, L.K, L.has_bias ? L.b.p : nullptr, tmX, epi, act, of32, obf16, B, s);
     }
@@ -977,10 +872,6 @@ struct b2a_stt {
         tmx_acte = tc::make_tmap_bf16(acte.p, 2 * T2p, c.encoder_ffn_dim, 128);
         tmx_encout = tc::make_tmap_bf16(enc_out.p, 2 * T2p, D, 128);
         {
-            const char* e = getenv("B2A_WH_ATTN");
-            attn_tc = !(e && std::string(e) == "simt");
-            const char* sp = getenv("B2A_WH_SPLIT");
-            split_residual_gemms = !(sp && std::string(sp) == "0");
             const int nh = c.encoder_attention_heads;
             const size_t n = (size_t)B * nh * FA_TP * HD;
             fa_q.alloc(n); fa_k.alloc(n); fa_vt.alloc(n);
@@ -1007,21 +898,15 @@ struct b2a_stt {
         im2col3_kernel<<<(unsigned)T2, 256, 0, s>>>(h1.p, X2.p, 3000, 1500, D, 3 * D, 2);
         count_launch();
         gemm_big(conv2, tmx_X2, tc::EPI_STORE, tc::ACT_GELU, xe.p, nullptr, T2, s);
-        const size_t fa_sm = (size_t)(FA_T * HD + HD * FA_LD + FA_T * HD + FA_T * FA_LD) * sizeof(float);
         for (int l = 0; l < c.encoder_layers; ++l) {
             EncLayer& L = enc[l];
             ln(L.ln1, xe.p, xne.p, T2, ENC_HALF, l == 0 ? enc_pos.p : nullptr, 1500, s);     // + positions (:150)
             gemm_big(L.qkv, tmx_xne, tc::EPI_STORE, tc::ACT_NONE, qkve.p, nullptr, T2, s);
-            if (attn_tc) {
-                // wgmma attention (attn_tc.cuh): pack q | k | v as fp16 operands, then one CTA per (128-query tile, head, clip)
-                fa::pack_qkv_f16_kernel<<<dim3(FA_TP / 64, B, nh), 256, 0, s>>>(qkve.p, fa_q.p, fa_k.p, fa_vt.p, 1500, FA_TP, nh, 1.0f / sqrtf((float)HD));
-                fa::Args fa_args{attne.p, 1500, FA_TP, nh, D, ENC_HALF};
-                fa::mha_tc_kernel<<<dim3(FA_TP / fa::BQ, nh, B), fa::FA_THREADS, fa::FA_SMEM_BYTES, s>>>(tm_faq, tm_fak, tm_fav, fa_args);
-                count_launch(2);
-            } else {
-                mha_fwd_kernel<<<dim3(cdiv(1500, FA_T), nh, B), FA_THREADS, fa_sm, s>>>(qkve.p, attne.p, 1500, D, 1.0f / sqrtf((float)HD));
-                count_launch();
-            }
+            // wgmma attention (attn_tc.cuh): pack q | k | v as fp16 operands, then one CTA per (128-query tile, head, clip)
+            fa::pack_qkv_f16_kernel<<<dim3(FA_TP / 64, B, nh), 256, 0, s>>>(qkve.p, fa_q.p, fa_k.p, fa_vt.p, 1500, FA_TP, nh, 1.0f / sqrtf((float)HD));
+            fa::Args fa_args{attne.p, 1500, FA_TP, nh, D, ENC_HALF};
+            fa::mha_tc_kernel<<<dim3(FA_TP / fa::BQ, nh, B), fa::FA_THREADS, fa::FA_SMEM_BYTES, s>>>(tm_faq, tm_fak, tm_fav, fa_args);
+            count_launch(2);
             gemm_big(L.o, tmx_attne, tc::EPI_ADD, tc::ACT_NONE, xe.p, nullptr, T2, s);
             ln(L.ln2, xe.p, xne.p, T2, ENC_HALF, nullptr, 1, s);
             gemm_big(L.fc1, tmx_xne, tc::EPI_STORE_BF16, tc::ACT_GELU, nullptr, acte.p, T2, s);

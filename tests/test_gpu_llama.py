@@ -154,7 +154,7 @@ def test_end_to_end_tokens_to_waveform_and_errors(b2a):
     assert all(len(t) <= 5 for t in toks3)
 
 
-def test_simt_fallback_matches_tcgen05_path(b2a, tiny, monkeypatch):
+def test_simt_fallback_matches_wgmma_path(b2a, tiny, monkeypatch):
     """B2A_GEMM=simt selects the CUDA-core GEMV fallback (same hi/lo numerics): both paths agree to fp32 noise."""
     cfg, W, m = tiny
     ids = np.random.default_rng(17).integers(0, 2048, size=(3, 9)).astype(np.int32)
@@ -169,7 +169,8 @@ def test_simt_fallback_matches_tcgen05_path(b2a, tiny, monkeypatch):
 
 
 def test_long_context_attention_splits(b2a):
-    """Context beyond one 144-key attention split (flash-decoding merge) against the oracle."""
+    """Context over many 64-key attention chunks against the oracle: positions on both sides of chunk boundaries, where the
+    chunks alternate between the two CTAs of the cluster and their softmax states are merged."""
     cfg = ol.LlamaConfig(hidden_size=128, num_hidden_layers=1, intermediate_size=256, num_attention_heads=3,
                          num_key_value_heads=1, head_dim=128, vocab_size=512)
     W = ol.init_weights(cfg, 5, std=0.1)
@@ -177,7 +178,7 @@ def test_long_context_attention_splits(b2a):
     ids = np.random.default_rng(1).integers(0, 512, size=(2, 330)).astype(np.int32)
     lg = m(ids)
     ref = ol.LlamaOracle(cfg, W, round_acts=False).forward(torch.as_tensor(ids)).numpy()
-    for pos in (0, 143, 144, 145, 287, 288, 329):
+    for pos in (0, 63, 64, 65, 127, 128, 143, 144, 145, 191, 192, 255, 256, 287, 288, 329):
         assert rel_err(lg[:, pos], ref[:, pos]) < 1e-4, pos
 
 

@@ -125,7 +125,7 @@ def bench_speech_tokenizer():
     ms = (time.perf_counter() - t0) / n * 1e3                    # every streaming_step ends synchronised (waveform copied to the host)
     print(json.dumps({"stage": "speech_tokenizer_decode", "workload": f"{B} rows x {frames} code frames in {chunk}-frame streaming chunks -> {B} x {frames * 1920 / 24000:.1f} s",
                       "ms": ms, "x_realtime": B * frames * 1920 / 24000 / (ms * 1e-3),
-                      "operands": "fp16 pairs" if os.environ.get("B2A_ST_FP16", "1") != "0" else "bf16 pairs", "seg_kb": os.environ.get("B2A_ST_SEG", "default")}))
+                      "operands": "fp16 pairs" if os.environ.get("B2A_ST_FP16", "1") != "0" else "bf16 pairs"}))
 
 
 if __name__ == "__main__":

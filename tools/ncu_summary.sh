@@ -10,5 +10,5 @@ cap() {  # name, kernel regex, skip, count, command...
   wc -c gpurun_out/ncu_$name.csv
 }
 cap snac 'ru_fused|conv_gemm|final_nlc|dw7' 37 37 python tools/profile_snac.py 8 1024
-cap whisper 'mha_fwd|mel_log|tc_gemm_kernel<128>|layernorm' 30 12 python tools/profile_whisper.py 16 2
+cap whisper 'mha_tc|mel_log|tc_gemm_kernel<128>|layernorm' 30 12 python tools/profile_whisper.py 16 2
 cap step 'tc_gemm|add_rmsnorm|attn_decode' 210 8 python tools/profile_step.py 320 3
