@@ -62,6 +62,28 @@ int32_t b2a_qwen3_sample_test(const float* logits, int32_t batch, int32_t vocab,
 int32_t b2a_implicit_conv_test(const float* w, int32_t M, int32_t taps, int32_t Cin, const float* x, int32_t B, int32_t Ttot, int32_t T,
                                int32_t dil, int32_t shift0, int32_t up, const float* bias, const float* gamma, int32_t gelu, int32_t add,
                                int32_t bias_twice_t0, const float* sa, const float* sb, int32_t Hout, int32_t fp16, float* xo, float* hl_out);
+/* tests/test_gpu_tc_gemm.py: one launch of tc_gemm_kernel<bn> (csrc/tc_gemm.cuh) on DEVICE pointers: out[N, M] = X[N, K] W[M, K]^T
+ * through epilogue epi (0 store fp32, 2 SwiGLU bf16 [., M/2], 3 store bf16, 4 add into the caller's fp32 out), bias (nullable [M]),
+ * act (1 = exact-erf GELU), tile_rows (0 = 128 weight rows per m-tile), lo_rows != 0 (bf16 outputs as hi/lo rows in X's tile layout)
+ * and rstd_ss (nullable [rstd_parts, 8]: columns scaled by rsqrt(sum / K + rstd_eps), bn = 16 only).  hilo != 0: X is
+ * cdiv(N, bn/2) tiles of bn rows, hi rows then lo rows.  split != 0: stream-K over ctas CTAs (store / add only, no GELU).
+ * stages = 0: the deepest ring that fits.  Unsupported combinations return B2A_ERR_INVALID_INPUT.
+ *   b2a_tc_gemm_test: the same with no bias, activation, tile_rows or norm scale, the deepest ring, and hi/lo rows for the bf16
+ *       epilogues of hi/lo inputs.                                                                                         */
+int32_t b2a_tc_gemm_epilogue_test(const void* W, const void* X, void* out, int32_t M, int32_t N, int32_t K, int32_t bn, int32_t epi,
+                                  int32_t split, int32_t hilo, int32_t ctas, const float* bias, int32_t act, int32_t tile_rows,
+                                  int32_t lo_rows, const float* rstd_ss, int32_t rstd_parts, float rstd_eps, int32_t stages, void* stream);
+int32_t b2a_tc_gemm_test(const void* W, const void* X, void* out, int32_t M, int32_t N, int32_t K, int32_t bn, int32_t epi,
+                         int32_t split, int32_t hilo, int32_t ctas, void* stream);
+/* tests/test_gpu_splitk_norm.py: one launch of the cluster split-K GEMM (tc_gemm_splitk_kernel) on DEVICE pointers: W [M, K] bf16,
+ * X [16, K] bf16 (hi rows 0..7, lo rows 8..15); for t < N: h[t] += W x[t] (h [8, M] fp32, in place), xn[t] / xn[8 + t] = hi / lo of
+ * h[t] * gain (xn [16, M] bf16), ss[m_tile, t] = sum of h[t]^2 over the tile's rows (ss [cdiv(M, 128), 8]; 0 for t >= N).     */
+int32_t b2a_tc_gemm_splitk_test(const void* W, const void* X, float* h, const float* gain, void* xn, float* ss, int32_t M, int32_t N,
+                                int32_t K, int32_t cluster, int32_t stages, void* stream);
+/* tests/test_gpu_encoder_attention.py: the Whisper encoder attention (csrc/attn_tc.cuh, pack_qkv_f16_kernel + mha_tc_kernel) on a
+ * DEVICE qkv [B * T, 3 * nh * 64] fp32; out [2 * 64 * cdiv(B * T, 64), nh * 64] bf16: token t = b * T + i at hi row
+ * (t / 64) * 128 + t % 64, lo row = hi row + 64.  Rows of tokens >= B * T are not written.                                  */
+int32_t b2a_mha_tc_test(const float* qkv, void* out, int32_t B, int32_t T, int32_t nh, void* stream);
 
 #ifdef __cplusplus
 }

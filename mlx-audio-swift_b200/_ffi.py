@@ -205,6 +205,11 @@ SIGNATURES = {
                                          C.c_int32, _P, C.c_int32, C.c_uint64, C.c_int32, _P, _P]),
     "b2a_implicit_conv_test": (C.c_int32, [_P, C.c_int32, C.c_int32, C.c_int32, _P, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                           _P, _P, C.c_int32, C.c_int32, C.c_int32, _P, _P, C.c_int32, C.c_int32, _P, _P]),
+    "b2a_tc_gemm_test": (C.c_int32, [_P, _P, _P] + [C.c_int32] * 8 + [_P]),
+    "b2a_tc_gemm_epilogue_test": (C.c_int32, [_P, _P, _P] + [C.c_int32] * 8 + [_P, C.c_int32, C.c_int32, C.c_int32, _P, C.c_int32,
+                                                                             C.c_float, C.c_int32, _P]),
+    "b2a_tc_gemm_splitk_test": (C.c_int32, [_P, _P, _P, _P, _P, _P] + [C.c_int32] * 5 + [_P]),
+    "b2a_mha_tc_test": (C.c_int32, [_P, _P, C.c_int32, C.c_int32, C.c_int32, _P]),
     "b2a_speech_tokenizer_debug_stage": (C.c_int32, [_P, C.c_int32, _P, C.c_int64, _P]),
     "b2a_speech_tokenizer_debug_layout": (C.c_int32, [_P, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _P, C.c_int64, _P, _P, _P]),
     "b2a_encodec_create": (C.c_int32, [C.c_int32, C.POINTER(EncodecConfig), C.POINTER(Tensor), C.c_int32, C.POINTER(_P)]),

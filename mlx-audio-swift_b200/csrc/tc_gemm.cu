@@ -84,27 +84,51 @@ void set_attributes() {
 }  // namespace tc
 }  // namespace b2a
 
-// Standalone entry used by tests/test_gpu_tc_gemm.py: out[N, M] = X[N, K] * W[M, K]^T through the wgmma path.
-// All pointers are DEVICE pointers.  epi: 0 store fp32, 2 SwiGLU (bf16 out [N(+lo), M/2]), 3 store bf16;
-// split != 0 allows stream-K partial tiles (summed in a fixed order and added into the zero-initialised fp32 output).
-extern "C" int32_t b2a_tc_gemm_test(const void* W, const void* X, void* out, int32_t M, int32_t N, int32_t K, int32_t bn,
-                                    int32_t epi, int32_t split, int32_t hilo, int32_t ctas, void* stream) {
+// Standalone entries (include/b200audio_internal.h): one launch of tc_gemm_kernel / tc_gemm_splitk_kernel on DEVICE pointers,
+// with the epilogue options the engines' call sites use.
+
+// out[N, M] = X[N, K] * W[M, K]^T through tc_gemm_kernel<bn>.  hilo: X holds cdiv(N, bn / 2) tiles of bn rows (hi rows, then lo rows).
+// split != 0 lets CTAs own partial K ranges (stream-K): epi must then be a store into the zeroed or an add into the caller's fp32 out.
+extern "C" int32_t b2a_tc_gemm_epilogue_test(const void* W, const void* X, void* out, int32_t M, int32_t N, int32_t K, int32_t bn,
+                                             int32_t epi, int32_t split, int32_t hilo, int32_t ctas, const float* bias, int32_t act,
+                                             int32_t tile_rows, int32_t lo_rows, const float* rstd_ss, int32_t rstd_parts,
+                                             float rstd_eps, int32_t stages, void* stream) {
     using namespace b2a;
     using namespace b2a::tc;
     return guarded([&] {
-        B2A_CHECK(W && X && out && (bn == 16 || bn == 32 || bn == 128) && K % BK == 0, B2A_ERR_INVALID_INPUT, "b2a_tc_gemm_test: bad argument");
+        B2A_CHECK(W && X && out && (bn == 16 || bn == 32 || bn == 128) && K % BK == 0 && M > 0 && N > 0 && ctas > 0, B2A_ERR_INVALID_INPUT,
+                  "b2a_tc_gemm_epilogue_test: bad argument");
+        B2A_CHECK(epi == EPI_STORE || epi == EPI_SWIGLU || epi == EPI_STORE_BF16 || epi == EPI_ADD, B2A_ERR_INVALID_INPUT,
+                  "b2a_tc_gemm_epilogue_test: unknown epilogue");
+        B2A_CHECK(act == ACT_NONE || act == ACT_GELU, B2A_ERR_INVALID_INPUT, "b2a_tc_gemm_epilogue_test: unknown activation");
+        B2A_CHECK(!split || epi == EPI_STORE || epi == EPI_ADD, B2A_ERR_INVALID_INPUT,
+                  "b2a_tc_gemm_epilogue_test: stream-K partial tiles are summed into fp32 outputs only");
+        B2A_CHECK(!split || act == ACT_NONE, B2A_ERR_INVALID_INPUT, "b2a_tc_gemm_epilogue_test: GELU of a partial K range is not the GELU of the sum");
+        B2A_CHECK(!split || tile_rows == 0, B2A_ERR_INVALID_INPUT, "b2a_tc_gemm_epilogue_test: tile_rows is a whole-tile option");
+        B2A_CHECK(tile_rows == 0 || (tile_rows % 8 == 0 && tile_rows >= 8 && tile_rows <= BM), B2A_ERR_INVALID_INPUT,
+                  "b2a_tc_gemm_epilogue_test: tile_rows must be a multiple of 8 in [8, 128]");
+        B2A_CHECK(!lo_rows || (hilo && (epi == EPI_SWIGLU || epi == EPI_STORE_BF16)), B2A_ERR_INVALID_INPUT,
+                  "b2a_tc_gemm_epilogue_test: hi/lo outputs need hi/lo inputs and a bf16 epilogue");
+        B2A_CHECK(epi != EPI_SWIGLU || M % 2 == 0, B2A_ERR_INVALID_INPUT, "b2a_tc_gemm_epilogue_test: SwiGLU needs (gate, up) row pairs");
+        B2A_CHECK(!rstd_ss || (bn == 16 && hilo && N <= 8 && rstd_parts >= 1), B2A_ERR_INVALID_INPUT,
+                  "b2a_tc_gemm_epilogue_test: the fused RMSNorm scale is a BN = 16 hi/lo option");
         require_device(0);
         set_attributes();
-        const int x_rows = hilo ? bn : N;
-        CUtensorMap ta = make_tmap_bf16(W, M, K, BM), tb = make_tmap_bf16(X, x_rows, K, bn);
+        const int n_tiles = hilo ? cdiv(N, bn / 2) : cdiv(N, bn);
+        B2A_CHECK(n_tiles <= 65535, B2A_ERR_INVALID_INPUT, "b2a_tc_gemm_epilogue_test: too many tokens");
+        const int x_rows = hilo ? n_tiles * bn : N;
+        const int TR = tile_rows > 0 ? tile_rows : BM;
+        CUtensorMap ta = make_tmap_bf16(W, M, K, TR), tb = make_tmap_bf16(X, x_rows, K, bn);
         Args a{};
         a.out_f32 = (float*)out; a.out_bf16 = (__nv_bfloat16*)out; a.M = M; a.N = N; a.K = K;
         a.ldo = epi == EPI_SWIGLU ? M / 2 : M;
-        a.m_tiles = cdiv(M, BM); a.k_blocks = K / BK;
-        a.stages = bn == 16 ? Smem<16>::max_stages() : bn == 32 ? Smem<32>::max_stages() : Smem<128>::max_stages();
+        a.tile_rows = tile_rows; a.m_tiles = cdiv(M, TR); a.k_blocks = K / BK;
+        const int max_st = bn == 16 ? Smem<16>::max_stages() : bn == 32 ? Smem<32>::max_stages() : Smem<128>::max_stages();
+        a.stages = stages > 0 ? stages : max_st;
         a.epi_full = epi; a.epi_partial = split ? EPI_PARTIAL : -1; a.hilo = hilo;
-        a.lo_rows = (hilo && epi != EPI_STORE) ? bn / 2 : 0;
-        const int n_tiles = hilo ? 1 : cdiv(N, bn);
+        a.bias = bias; a.act = act;
+        a.lo_rows = lo_rows ? bn / 2 : 0;
+        a.rstd_ss = rstd_ss; a.rstd_parts = rstd_parts; a.rstd_inv_h = 1.0f / (float)K; a.rstd_eps = rstd_eps;
         DBuf<float> ws;
         DBuf<unsigned> cnt;
         if (split) {
@@ -117,6 +141,37 @@ extern "C" int32_t b2a_tc_gemm_test(const void* W, const void* X, void* out, int
         if (bn == 16) launch<16>(ta, tb, a, ctas, n_tiles, (cudaStream_t)stream);
         else if (bn == 32) launch<32>(ta, tb, a, ctas, n_tiles, (cudaStream_t)stream);
         else launch<128>(ta, tb, a, ctas, n_tiles, (cudaStream_t)stream);
+        B2A_CUDA(cudaGetLastError());
+        B2A_CUDA(cudaStreamSynchronize((cudaStream_t)stream));
+    });
+}
+
+// The plain GEMM with no bias, activation, tile_rows or norm scale and the deepest ring; bf16 epilogues of hi/lo inputs write hi/lo rows.
+extern "C" int32_t b2a_tc_gemm_test(const void* W, const void* X, void* out, int32_t M, int32_t N, int32_t K, int32_t bn,
+                                    int32_t epi, int32_t split, int32_t hilo, int32_t ctas, void* stream) {
+    const int32_t lo_rows = hilo && (epi == b2a::tc::EPI_SWIGLU || epi == b2a::tc::EPI_STORE_BF16);
+    return b2a_tc_gemm_epilogue_test(W, X, out, M, N, K, bn, epi, split, hilo, ctas, nullptr, b2a::tc::ACT_NONE, 0, lo_rows, nullptr, 0,
+                                     0.f, 0, stream);
+}
+
+// The decode step's o_proj / down_proj GEMM: h[t] += W * (x_hi[t] + x_lo[t]) for t < N, then xn = hi / lo of h * gain and
+// ss[m_tile, t] = sum over the tile's rows of h^2, one cluster of `cluster` CTAs per 128-row tile.
+extern "C" int32_t b2a_tc_gemm_splitk_test(const void* W, const void* X, float* h, const float* gain, void* xn, float* ss, int32_t M,
+                                           int32_t N, int32_t K, int32_t cluster, int32_t stages, void* stream) {
+    using namespace b2a;
+    using namespace b2a::tc;
+    return guarded([&] {
+        B2A_CHECK(W && X && h && gain && xn && ss && M > 0 && M % 8 == 0 && K > 0 && K % BK == 0 && N >= 1 && N <= 8 && stages >= 1,
+                  B2A_ERR_INVALID_INPUT, "b2a_tc_gemm_splitk_test: bad argument");
+        B2A_CHECK(cluster >= 1 && cluster <= SPLIT_MAX_CLUSTER && cluster <= K / BK, B2A_ERR_INVALID_INPUT,
+                  "b2a_tc_gemm_splitk_test: cluster must be in [1, min(8, K / 64)]");
+        require_device(0);
+        set_attributes();
+        CUtensorMap ta = make_tmap_bf16(W, M, K, BM), tb = make_tmap_bf16(X, 16, K, 16);
+        SplitArgs a{};
+        a.M = M; a.N = N; a.K = K; a.k_blocks = K / BK; a.stages = stages;
+        a.h = h; a.gain = gain; a.xn = (__nv_bfloat16*)xn; a.ss = ss;
+        launch_splitk(ta, tb, a, cdiv(M, BM), cluster, (cudaStream_t)stream);
         B2A_CUDA(cudaGetLastError());
         B2A_CUDA(cudaStreamSynchronize((cudaStream_t)stream));
     });

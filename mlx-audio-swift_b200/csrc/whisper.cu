@@ -1376,3 +1376,28 @@ int32_t b2a_stt_session_tokens(b2a_stt_session* s, int32_t which, int32_t window
 void b2a_stt_session_destroy(b2a_stt_session* s) { delete s; }
 
 }  // extern "C"
+
+// The encoder attention on its own (include/b200audio_internal.h): pack_qkv_f16_kernel + mha_tc_kernel on a DEVICE fp32
+// qkv [B * T, 3 * nh * 64] (q | k | v), written to `out` as the encoder's hi/lo bf16 tiles of 64 tokens, [2 * 64 * cdiv(B * T, 64), nh * 64].
+extern "C" int32_t b2a_mha_tc_test(const float* qkv, void* out, int32_t B, int32_t T, int32_t nh, void* stream) {
+    using namespace b2a;
+    return guarded([&] {
+        B2A_CHECK(qkv && out && B >= 1 && T >= 1 && nh >= 1, B2A_ERR_INVALID_INPUT, "b2a_mha_tc_test: bad argument");
+        require_device(0);
+        const cudaStream_t s = (cudaStream_t)stream;
+        const int Tp = cdiv(T, fa::BQ) * fa::BQ;
+        const size_t n = (size_t)B * nh * Tp * HD;
+        DBuf<__half> q, k, vt;
+        q.alloc(n); k.alloc(n); vt.alloc(n);
+        const CUtensorMap tq = tc::make_tmap_f16_3d(q.p, HD, Tp, (long long)B * nh, 64, fa::BQ);
+        const CUtensorMap tk = tc::make_tmap_f16_3d(k.p, HD, Tp, (long long)B * nh, 64, fa::BKV);
+        const CUtensorMap tv = tc::make_tmap_f16_3d(vt.p, Tp, HD, (long long)B * nh, 64, 64);
+        B2A_CUDA(cudaFuncSetAttribute(fa::mha_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fa::FA_SMEM_BYTES));
+        fa::pack_qkv_f16_kernel<<<dim3(Tp / 64, B, nh), 256, 0, s>>>(qkv, q.p, k.p, vt.p, T, Tp, nh, 1.0f / sqrtf((float)HD));
+        const fa::Args args{(__nv_bfloat16*)out, T, Tp, nh, nh * HD, ENC_HALF};
+        fa::mha_tc_kernel<<<dim3(Tp / fa::BQ, nh, B), fa::FA_THREADS, fa::FA_SMEM_BYTES, s>>>(tq, tk, tv, args);
+        count_launch(2);
+        B2A_CUDA(cudaGetLastError());
+        B2A_CUDA(cudaStreamSynchronize(s));
+    });
+}

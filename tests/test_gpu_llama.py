@@ -182,11 +182,43 @@ def test_long_context_attention_splits(b2a):
         assert rel_err(lg[:, pos], ref[:, pos]) < 1e-4, pos
 
 
-@pytest.mark.parametrize("B,L", [(3, 37), (8, 64), (1, 2), (2, 128)])
-def test_batched_prefill_matches_stepwise_and_oracle(b2a, tiny, monkeypatch, B, L):
-    """The tensor-core batched prompt pass (64-token hi/lo tiles + causal prompt attention) must give the same greedy
-    continuation as replaying the decode step per position, and as the oracle."""
-    cfg, W, _ = tiny
+# every other GQA ratio the engine accepts (q heads per kv head 1, 2, 3, 4, 6, 8; 3 is the test above), and hidden 192
+LONG_CONTEXT_HEADS = [(128, 1, 1), (128, 2, 1), (128, 4, 1), (128, 6, 1), (128, 8, 1), (128, 8, 2), (192, 4, 1)]
+
+
+@pytest.mark.parametrize("hidden,nq,nkv", LONG_CONTEXT_HEADS, ids=[f"h{h}-q{q}-kv{k}" for h, q, k in LONG_CONTEXT_HEADS])
+def test_long_context_attention_every_gqa_ratio(b2a, hidden, nq, nkv):
+    """test_long_context_attention_splits for the other GQA ratios.  330 positions (more than one prompt tile of 128) go through the
+    decode step one position at a time, so each runs attn_decode_cluster_kernel<G>; at G = 8 the K/V ring is 2 chunks deep and
+    wraps many times.  Hidden 192 is not a multiple of 128, which selects the unfused step (stand-alone RMSNorm kernels, stream-K
+    o_proj / down_proj)."""
+    cfg = ol.LlamaConfig(hidden_size=hidden, num_hidden_layers=1, intermediate_size=256, num_attention_heads=nq,
+                         num_key_value_heads=nkv, head_dim=128, vocab_size=512)
+    W = ol.init_weights(cfg, 5, std=0.1)
+    m = b2a.LlamaTTSModel(hf_config(cfg), W, max_batch=2, max_context=400)
+    ids = np.random.default_rng(1).integers(0, 512, size=(2, 330)).astype(np.int32)
+    lg = m(ids)
+    ref = ol.LlamaOracle(cfg, W, round_acts=False).forward(torch.as_tensor(ids)).numpy()
+    for pos in (0, 63, 64, 65, 127, 128, 143, 144, 145, 191, 192, 255, 256, 287, 288, 329):
+        assert rel_err(lg[:, pos], ref[:, pos]) < 1e-4, pos
+
+
+# (B, L, q heads, kv heads).  The batched prompt pass runs when its attention tile fits: 1024 L + 16384 G bytes <= 220 KB, so
+# L <= 128 up to G = 4, L <= 124 at G = 6 and L <= 92 at G = 8.  Every case here takes it; the model built under B2A_PREFILL=step
+# replays the decode step (attn_decode_cluster_kernel<G>) instead.
+PREFILL_CASES = [pytest.param(3, 37, 2, 1, id="3-37"), pytest.param(8, 64, 2, 1, id="8-64"), pytest.param(1, 2, 2, 1, id="1-2"),
+                 pytest.param(2, 128, 2, 1, id="2-128"), pytest.param(2, 50, 1, 1, id="g1-2-50"), pytest.param(3, 37, 3, 1, id="g3-3-37"),
+                 pytest.param(2, 100, 4, 1, id="g4-2-100"), pytest.param(2, 124, 6, 1, id="g6-2-124"),
+                 pytest.param(3, 92, 8, 1, id="g8-3-92")]
+
+
+@pytest.mark.parametrize("B,L,nq,nkv", PREFILL_CASES)
+def test_batched_prefill_matches_stepwise_and_oracle(b2a, monkeypatch, B, L, nq, nkv):
+    """The tensor-core batched prompt pass (64-token hi/lo tiles + causal prompt attention, prefill_attn_kernel<G>) must give the
+    same greedy continuation as replaying the decode step per position, and as the oracle; then the KV cache it left must be
+    what the decode step expects: one more position fed to both models gives the same logits as each other and as the oracle."""
+    cfg = ol.LlamaConfig(**{**TINY, "num_attention_heads": nq, "num_key_value_heads": nkv})
+    W = ol.init_weights(cfg, 1234, std=0.08)
     ids = np.random.default_rng(100 + L).integers(0, 2048, size=(B, L)).astype(np.int32)
     P = b2a.GenerateParameters(max_tokens=12, temperature=0.0, top_p=1.0, repetition_penalty=1.0, repetition_context_size=0)
     m_b = b2a.LlamaTTSModel(hf_config(cfg), W, max_batch=8, max_context=192)
@@ -198,8 +230,15 @@ def test_batched_prefill_matches_stepwise_and_oracle(b2a, tiny, monkeypatch, B, 
     assert a == s
     ref = ol.generate_tokens(ol.LlamaOracle(cfg, W, False), ids, 12, temperature=0.0, rep_penalty=1.0, rep_context=0)
     assert a == ref
-    # after a batched prefill the KV cache must be what the decode path expects: continue with forward_logits
+    # the cache now holds the prompt and the first 11 generated tokens: feed the 12th.  The two caches were written by different
+    # GEMMs (prompt tiles of 64 tokens vs the fused decode step), so they agree to fp32 rounding: 1.6e-5 at most on an H100.
     nxt = np.asarray([[t[-1]] for t in a], dtype=np.int32)
+    lb, ls = m_b(nxt, reset_cache=False), m_s(nxt, reset_cache=False)
+    assert rel_err(lb, ls) < 4e-5, rel_err(lb, ls)
+    full = np.concatenate([ids, np.asarray(a, dtype=np.int32)], axis=1)
+    ref_lg = ol.LlamaOracle(cfg, W, False).forward(torch.as_tensor(full)).numpy()[:, -1:]
+    assert rel_err(lb, ref_lg) < 1e-4, rel_err(lb, ref_lg)
+    assert rel_err(ls, ref_lg) < 1e-4, rel_err(ls, ref_lg)
 
 
 def test_streamed_audio_chunks_match_the_one_shot_waveform(b2a):
