@@ -84,6 +84,34 @@ int32_t b2a_tc_gemm_splitk_test(const void* W, const void* X, float* h, const fl
  * DEVICE qkv [B * T, 3 * nh * 64] fp32; out [2 * 64 * cdiv(B * T, 64), nh * 64] bf16: token t = b * T + i at hi row
  * (t / 64) * 128 + t % 64, lo row = hi row + 64.  Rows of tokens >= B * T are not written.                                  */
 int32_t b2a_mha_tc_test(const float* qkv, void* out, int32_t B, int32_t T, int32_t nh, void* stream);
+/* tests/test_gpu_conv_gemm.py: one launch of the codec conv GEMM (cg::conv_gemm_kernel, csrc/conv_gemm.cuh, as snac.cu compiles it):
+ * acc[n, m] = W[m, :] . X[n, :] for the host fp32 weight w [M, K] (split into bf16 hi/lo like the engines' weights) and the DEVICE
+ * activations X, 2 * pad64(N) rows of 64-token hi/lo tiles (hi rows, then lo rows) by K.  Then v = gamma * GELU(acc + bias) (each
+ * optional) through epilogue epi: 0 E_STORE_HILO (Snake(alpha) of v as hi/lo into hl; dual: token b*T + t to row b*(T+1) + t,
+ * columns [0, M), and to row b*(T+1) + t + 1, columns [M, 2M)), 1 E_CONVT (row m = r*Cout + co of input token b*(Tin+1) + q to
+ * output token b*T + q*stride + r - pad, kept when inside [0, T), into x and optionally hl), 2 E_NOISE (x += noise[n] * v; noise
+ * null: the seeded N(0, 1) draw for token n), 3 E_ADD (x += v), 4 E_ADD_HILO (x += v, then as E_STORE_HILO), 5 E_STORE_F32 (x = v).
+ * x [., ldx] fp32 and hl [., ldh] bf16 hi/lo tiles are DEVICE pointers.  Combinations no engine launches return B2A_ERR_INVALID_INPUT.
+ * ctas = 0: min(SM count, work tiles), as the engines launch it.                                                           */
+int32_t b2a_conv_gemm_test(const float* w, int32_t M, int32_t K, const void* X, int32_t N, int32_t epi, const float* bias,
+                           const float* alpha, const float* gamma, int32_t gelu, float* x, int32_t ldx, void* hl, int32_t ldh,
+                           int32_t dual, int32_t T, int32_t Cout, int32_t stride, int32_t pad, int32_t Tin, const float* noise,
+                           uint64_t seed, int32_t ctas, void* stream);
+/* tests/test_gpu_snac_fused.py: one launch of the fused SNAC unit (rf::ru_fused_kernel, csrc/snac_fused.cuh) on DEVICE fp32
+ * x, y [B * T, C], C = 64 or 128.  mode 0 (ResidualUnit, dil 1, 3 or 9): y = x + W Snake(a_mid, dwconv7_dil(Snake(a_in, x)) + dw_b)
+ * + pw_bias; mode 1 (NoiseBlock, dil 0): y = x + noise[b*T + t] * (W x), noise null: the seeded N(0, 1) draw for token b*T + t.
+ * pw_w: host fp32 [C, C].  hl (with a_next): Snake(a_next, y) as hi/lo tiles of the next transposed conv's 2-tap im2col, ld 2C,
+ * laid out as conv GEMM dual outputs.  dw_w [C, 7], dw_b, a_in, a_mid, pw_bias [C], a_next [C] are DEVICE pointers (biases nullable).
+ * ctas = 0: the engine's CTA count.                                                                                        */
+int32_t b2a_snac_unit_test(int32_t mode, int32_t C, int32_t dil, const float* x, float* y, int32_t B, int32_t T, const float* dw_w,
+                           const float* dw_b, const float* a_in, const float* a_mid, const float* pw_w, const float* pw_bias,
+                           const float* noise, uint64_t seed, void* hl, const float* a_next, int32_t ctas, void* stream);
+/* tests/test_gpu_snac_fused.py: one launch of the fused Snake + transposed conv (rf::convt_fused_kernel) on DEVICE fp32
+ * x [B * Tin, 128] -> y [B * Tin * stride, cout]: y = conv_transpose1d(Snake(alpha, x), w, bias, stride, padding ceil(stride / 2)),
+ * w the host fp32 weight in torch layout [128, cout, 2 * stride].  Only (stride, cout) = (2, 64) and (1, 128).  ctas = 0: the
+ * engine's CTA count.                                                                                                      */
+int32_t b2a_snac_convt_test(const float* x, float* y, const float* alpha, const float* bias, const float* w, int32_t B, int32_t Tin,
+                            int32_t stride, int32_t cout, int32_t ctas, void* stream);
 
 #ifdef __cplusplus
 }

@@ -210,6 +210,10 @@ SIGNATURES = {
                                                                              C.c_float, C.c_int32, _P]),
     "b2a_tc_gemm_splitk_test": (C.c_int32, [_P, _P, _P, _P, _P, _P] + [C.c_int32] * 5 + [_P]),
     "b2a_mha_tc_test": (C.c_int32, [_P, _P, C.c_int32, C.c_int32, C.c_int32, _P]),
+    "b2a_conv_gemm_test": (C.c_int32, [_P, C.c_int32, C.c_int32, _P, C.c_int32, C.c_int32, _P, _P, _P, C.c_int32, _P, C.c_int32, _P,
+                                       C.c_int32] + [C.c_int32] * 6 + [_P, C.c_uint64, C.c_int32, _P]),
+    "b2a_snac_unit_test": (C.c_int32, [C.c_int32] * 3 + [_P, _P, C.c_int32, C.c_int32] + [_P] * 6 + [_P, C.c_uint64, _P, _P, C.c_int32, _P]),
+    "b2a_snac_convt_test": (C.c_int32, [_P] * 5 + [C.c_int32] * 5 + [_P]),
     "b2a_speech_tokenizer_debug_stage": (C.c_int32, [_P, C.c_int32, _P, C.c_int64, _P]),
     "b2a_speech_tokenizer_debug_layout": (C.c_int32, [_P, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _P, C.c_int64, _P, _P, _P]),
     "b2a_encodec_create": (C.c_int32, [C.c_int32, C.POINTER(EncodecConfig), C.POINTER(Tensor), C.c_int32, C.POINTER(_P)]),

@@ -597,6 +597,33 @@ static std::vector<float> fold_wn(const TensorTable& tt, const std::string& pref
     return v;
 }
 
+// transposed-conv weight wt [cin, 2s, cout] (kernel 2s, stride s) -> GEMM rows A[(co*s + r), (tap*cin + ci)] = wt[ci, r + tap*s, co]
+static std::vector<float> convt_gemm_rows(const std::vector<float>& wt, int cin, int cout, int s) {
+    const int k = 2 * s;
+    std::vector<float> A((size_t)cout * s * 2 * cin);
+    for (int co = 0; co < cout; ++co)
+        for (int r = 0; r < s; ++r)
+            for (int tap = 0; tap < 2; ++tap)
+                for (int ci = 0; ci < cin; ++ci)
+                    A[((size_t)(co * s + r)) * (2 * cin) + tap * cin + ci] = wt[((size_t)ci * k + (r + tap * s)) * cout + co];
+    return A;
+}
+// the same rows phase-major (m = r*cout + co) for the tensor-core operand, so a warp's 32 lanes write 32 consecutive channels
+static std::vector<float> convt_phase_major(const std::vector<float>& A, int cin, int cout, int s) {
+    std::vector<float> At((size_t)cout * s * 2 * cin);
+    for (int co = 0; co < cout; ++co)
+        for (int r = 0; r < s; ++r)
+            memcpy(&At[((size_t)r * cout + co) * 2 * cin], &A[((size_t)co * s + r) * 2 * cin], (size_t)2 * cin * sizeof(float));
+    return At;
+}
+// [64, 64] -> [128, 128] = [W 0; 0 W]: the weight operand of the fused C = 64 kernel (two 64-token sub-tiles per MMA)
+static std::vector<float> block_diag2(const std::vector<float>& w) {
+    std::vector<float> d((size_t)128 * 128, 0.f);
+    for (int r = 0; r < 64; ++r)
+        for (int c2 = 0; c2 < 64; ++c2) { d[(size_t)r * 128 + c2] = w[(size_t)r * 64 + c2]; d[(size_t)(r + 64) * 128 + 64 + c2] = w[(size_t)r * 64 + c2]; }
+    return d;
+}
+
 static void load_bias(const TensorTable& tt, const std::string& prefix, int n, ConvW& c) {
     if (tt.find(prefix + ".bias")) {
         std::vector<float> b = tt.f32(prefix + ".bias", n);
@@ -692,21 +719,9 @@ struct b2a_snac {
             B.alpha.upload(a.data(), a.size());
             const int s = B.stride, k = 2 * s;
             std::vector<float> wt = fold_wn(tt, b + "1", B.cin, k, B.cout, false);  // [ci, k, co]
-            std::vector<float> A((size_t)B.cout * s * 2 * B.cin);
-            for (int co = 0; co < B.cout; ++co)
-                for (int r = 0; r < s; ++r)
-                    for (int tap = 0; tap < 2; ++tap)
-                        for (int ci = 0; ci < B.cin; ++ci)
-                            A[((size_t)(co * s + r)) * (2 * B.cin) + tap * B.cin + ci] =
-                                wt[((size_t)ci * k + (r + tap * s)) * B.cout + co];
+            std::vector<float> A = convt_gemm_rows(wt, B.cin, B.cout, s);
             B.ct.w.upload(A.data(), A.size());
-            {   // tensor-core operand: rows phase-major (m = r*cout + co) so a warp's 32 lanes write 32 consecutive channels
-                std::vector<float> At((size_t)B.cout * s * 2 * B.cin);
-                for (int co = 0; co < B.cout; ++co)
-                    for (int r = 0; r < s; ++r)
-                        memcpy(&At[((size_t)r * B.cout + co) * 2 * B.cin], &A[((size_t)co * s + r) * 2 * B.cin], (size_t)2 * B.cin * sizeof(float));
-                host_ct.push_back(At);
-            }
+            host_ct.push_back(convt_phase_major(A, B.cin, B.cout, s));
             load_bias(tt, b + "1", B.cout, B.ct);
             int j = 2;
             B.has_noise = c.noise != 0;
@@ -763,15 +778,9 @@ struct b2a_snac {
                 DecBlock& B = blocks[i];
                 B.ct_tc.build(host_ct[i], B.cout * B.stride, 2 * B.cin);
                 B.noise_tc.build(host_noise[i], B.cout, B.cout);
-                auto blockdiag = [&](const std::vector<float>& w) {       // [64, 64] -> [128, 128] = [W 0; 0 W]
-                    std::vector<float> d((size_t)128 * 128, 0.f);
-                    for (int r = 0; r < 64; ++r)
-                        for (int c2 = 0; c2 < 64; ++c2) { d[(size_t)r * 128 + c2] = w[(size_t)r * 64 + c2]; d[(size_t)(r + 64) * 128 + 64 + c2] = w[(size_t)r * 64 + c2]; }
-                    return d;
-                };
-                if (B.cout == 64) B.noise_bd.build(blockdiag(host_noise[i]), 128, 128);
+                if (B.cout == 64) B.noise_bd.build(block_diag2(host_noise[i]), 128, 128);
                 for (int u = 0; u < 3; ++u) {
-                    if (B.cout == 64) B.ru[u].pw_bd.build(blockdiag(host_pw[ip]), 128, 128);
+                    if (B.cout == 64) B.ru[u].pw_bd.build(block_diag2(host_pw[ip]), 128, 128);
                     B.ru[u].pw_tc.build(host_pw[ip++], B.cout, B.cout);
                 }
             }
@@ -782,12 +791,14 @@ struct b2a_snac {
     std::vector<std::vector<float>> host_ct, host_noise, host_pw;
 
     // ---- tensor-core / NLC decode --------------------------------------------------------------------------
-    void cgemm(const TcW& W, const __nv_bfloat16* X, long long x_rows, cg::Args a, cudaStream_t s) {
+    void cgemm(const TcW& W, const __nv_bfloat16* X, long long x_rows, cg::Args a, cudaStream_t s) { launch_cgemm(W, X, x_rows, a, num_sms, s); }
+    // min(max_ctas, work items) CTAs (the engine passes the SM count)
+    static void launch_cgemm(const TcW& W, const __nv_bfloat16* X, long long x_rows, cg::Args a, long long max_ctas, cudaStream_t s) {
         a.M = W.M; a.K = W.K;
         a.m_tiles = cdiv(W.M, tc::BM); a.k_blocks = W.K / tc::BK; a.n_tiles = cdiv(a.N, cg::HALF);
         const CUtensorMap tb = tc::make_tmap_bf16(X, x_rows, W.K, 128);
         const long long tiles = (long long)a.n_tiles * a.m_tiles;
-        launch_pdl(cg::conv_gemm_kernel, dim3((unsigned)std::min<long long>(num_sms, tiles)), dim3(cg::CG_THREADS), cg::SMEM_BYTES, s,
+        launch_pdl(cg::conv_gemm_kernel, dim3((unsigned)std::min<long long>(max_ctas, tiles)), dim3(cg::CG_THREADS), cg::SMEM_BYTES, s,
                    W.th, W.tl, tb, a);
     }
     void dw_nlc(const ConvW& W, const float* xin, __nv_bfloat16* out, const float* a_in, const float* a_out, int batch, int T, int C,
@@ -821,7 +832,7 @@ struct b2a_snac {
         return B.cin == 128 && B.stride * B.cout == 128 && block_fused(blocks[i - 1]) && block_fused(B);
     }
     template <int CC>
-    void fused_c(const TcW& W, const rf::Args& a, dim3 g, size_t sm, cudaStream_t s) {
+    static void fused_c(const TcW& W, const rf::Args& a, dim3 g, size_t sm, cudaStream_t s) {
         const dim3 bl(rf::THREADS);
         if (a.mode == rf::MODE_NOISE) launch_pdl(rf::ru_fused_kernel<rf::MODE_NOISE, 0, CC>, g, bl, sm, s, W.th, W.tl, a);
         else if (a.dil == 1) launch_pdl(rf::ru_fused_kernel<rf::MODE_RU, 1, CC>, g, bl, sm, s, W.th, W.tl, a);
@@ -829,14 +840,21 @@ struct b2a_snac {
         else launch_pdl(rf::ru_fused_kernel<rf::MODE_RU, 9, CC>, g, bl, sm, s, W.th, W.tl, a);
     }
     // W: the [128, 128] operand (the layer's own weights for C = 128, the block-diagonal copy for C = 64)
-    void fused(const TcW& W, rf::Args a, int batch, long long T, cudaStream_t s) {
+    void fused(const TcW& W, rf::Args a, int batch, long long T, cudaStream_t s) { launch_fused(W, a, batch, T, num_sms, s); }
+    static void launch_fused(const TcW& W, rf::Args a, int batch, long long T, long long max_ctas, cudaStream_t s) {
         a.B = batch; a.T = (int)T;
         const int tile_tokens = a.C == 64 ? 2 * rf::TOK : rf::TOK;
         a.tiles_per_utt = cdiv(T, tile_tokens); a.n_tiles = (long long)batch * a.tiles_per_utt;
-        const long long ctas = std::min<long long>(num_sms, (a.n_tiles + rf::TEAMS - 1) / rf::TEAMS);
+        const long long ctas = std::min<long long>(max_ctas, (a.n_tiles + rf::TEAMS - 1) / rf::TEAMS);
         const size_t sm = rf::smem_bytes(a.dil, a.mode);
         if (a.C == 64) fused_c<64>(W, a, dim3((unsigned)ctas), sm, s);
         else fused_c<128>(W, a, dim3((unsigned)ctas), sm, s);
+    }
+    // Snake + transposed conv of the last block (convt_fused_ok); a.x .. a.pad set by the caller
+    static void launch_convt(const TcW& W, rf::ConvtArgs a, long long max_ctas, cudaStream_t s) {
+        a.tiles_per_utt = cdiv(a.Tin + 1, rf::TOK); a.n_tiles = (long long)a.B * a.tiles_per_utt;
+        const long long ctas = std::min<long long>(max_ctas, (a.n_tiles + rf::TEAMS - 1) / rf::TEAMS);
+        launch_pdl(rf::convt_fused_kernel, dim3((unsigned)ctas), dim3(rf::THREADS), rf::convt_smem_bytes(), s, W.th, W.tl, a);
     }
 
     void decode_dev_tc(const int* const* d_codes_in, int batch, long long T, const float* const* d_noise_in, int noise_mode,
@@ -879,9 +897,7 @@ struct b2a_snac {
                 rf::ConvtArgs a{};
                 a.x = xs.p; a.y = xs2.p; a.alpha = B.alpha.p; a.bias = B.ct.has_bias ? B.ct.bias.p : nullptr;
                 a.Tin = (int)t; a.T = (int)tout; a.B = batch; a.stride = B.stride; a.cout = B.cout; a.pad = B.pad;
-                a.tiles_per_utt = cdiv(t + 1, rf::TOK); a.n_tiles = (long long)batch * a.tiles_per_utt;
-                const long long ctas = std::min<long long>(num_sms, (a.n_tiles + rf::TEAMS - 1) / rf::TEAMS);
-                launch_pdl(rf::convt_fused_kernel, dim3((unsigned)ctas), dim3(rf::THREADS), rf::convt_smem_bytes(), s, B.ct_tc.th, B.ct_tc.tl, a);
+                launch_convt(B.ct_tc, a, num_sms, s);
                 std::swap(xs.p, xs2.p); std::swap(xs.n, xs2.n);
             } else {   // transposed conv: tokens (b, q), q = 0..t ; rows m = r*cout + co ; scatter to t_out = q*s + r - pad
                 cg::Args a{};
@@ -1154,3 +1170,110 @@ int32_t b2a_snac_quantize(b2a_snac* h, const float* z, int32_t batch, int64_t T,
 void b2a_snac_destroy(b2a_snac* h) { delete h; }
 
 }  // extern "C"
+
+// Single-kernel entries (include/b200audio_internal.h): one launch of the conv GEMM, of a fused ResidualUnit / NoiseBlock or of the
+// fused Snake + transposed conv, through the engine's launch code.  Activations are DEVICE pointers; the weights are host fp32 and
+// take the constructor's path (the same layout helpers, then TcW::build's hi/lo split).  ctas = 0: the engine's CTA count.
+static long long hook_ctas(int32_t ctas) {
+    if (ctas > 0) return ctas;
+    int n = 0;
+    B2A_CUDA(cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, 0));
+    return n;
+}
+
+extern "C" int32_t b2a_conv_gemm_test(const float* w, int32_t M, int32_t K, const void* X, int32_t N, int32_t epi, const float* bias,
+                                      const float* alpha, const float* gamma, int32_t gelu, float* x, int32_t ldx, void* hl, int32_t ldh,
+                                      int32_t dual, int32_t T, int32_t Cout, int32_t stride, int32_t pad, int32_t Tin, const float* noise,
+                                      uint64_t seed, int32_t ctas, void* stream) {
+    return guarded([&] {
+        B2A_CHECK(w && X && M > 0 && K > 0 && K % tc::BK == 0 && N > 0 && ctas >= 0 && (gelu == 0 || gelu == 1) && (dual == 0 || dual == 1),
+                  B2A_ERR_INVALID_INPUT, "b2a_conv_gemm_test: bad argument");
+        B2A_CHECK(epi >= cg::E_STORE_HILO && epi <= cg::E_STORE_F32, B2A_ERR_INVALID_INPUT, "b2a_conv_gemm_test: unknown epilogue");
+        const bool hilo_out = epi == cg::E_STORE_HILO || epi == cg::E_ADD_HILO;
+        B2A_CHECK(epi == cg::E_STORE_HILO ? !x : (x && ldx >= (epi == cg::E_CONVT ? Cout : M)), B2A_ERR_INVALID_INPUT,
+                  "b2a_conv_gemm_test: every epilogue but cg::E_STORE_HILO writes the fp32 x (ldx >= its columns)");
+        B2A_CHECK(hilo_out ? hl != nullptr : (!hl || epi == cg::E_CONVT), B2A_ERR_INVALID_INPUT,
+                  "b2a_conv_gemm_test: hl is the output of cg::E_STORE_HILO / cg::E_ADD_HILO and the optional copy of cg::E_CONVT");
+        B2A_CHECK(!hl || ldh >= (dual ? 2 * M : epi == cg::E_CONVT ? Cout : M), B2A_ERR_INVALID_INPUT, "b2a_conv_gemm_test: ldh too small");
+        B2A_CHECK(!alpha || hilo_out, B2A_ERR_INVALID_INPUT, "b2a_conv_gemm_test: Snake applies to the hi/lo outputs only");
+        B2A_CHECK(!dual || (hilo_out && T >= 1 && N % T == 0), B2A_ERR_INVALID_INPUT,
+                  "b2a_conv_gemm_test: the 2-tap im2col (dual) is a hi/lo output of whole utterances of T tokens");
+        B2A_CHECK(epi != cg::E_ADD_HILO || dual, B2A_ERR_INVALID_INPUT, "b2a_conv_gemm_test: cg::E_ADD_HILO feeds the next transposed conv (dual)");
+        B2A_CHECK(!gelu || epi == cg::E_STORE_HILO, B2A_ERR_INVALID_INPUT, "b2a_conv_gemm_test: GELU is the Vocos pwconv1 epilogue (cg::E_STORE_HILO)");
+        B2A_CHECK(!gamma || epi == cg::E_ADD, B2A_ERR_INVALID_INPUT, "b2a_conv_gemm_test: gamma is the ConvNeXt residual add (cg::E_ADD)");
+        B2A_CHECK(epi == cg::E_NOISE ? !bias : (!noise && seed == 0), B2A_ERR_INVALID_INPUT,
+                  "b2a_conv_gemm_test: noise / seed belong to cg::E_NOISE, whose linear has no bias");
+        B2A_CHECK(epi != cg::E_CONVT || (Cout > 0 && stride >= 1 && M == stride * Cout && pad >= 0 && Tin >= 1 && N % (Tin + 1) == 0 &&
+                                     T == Tin * stride),
+                  B2A_ERR_INVALID_INPUT, "b2a_conv_gemm_test: cg::E_CONVT needs M = stride * Cout, N = B * (Tin + 1) and T = Tin * stride");
+        require_device(0);
+        B2A_CUDA(cudaFuncSetAttribute(cg::conv_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cg::SMEM_BYTES));
+        TcW W;
+        W.build(std::vector<float>(w, w + (size_t)M * K), M, K);
+        cg::Args a{};
+        a.N = N; a.epi = epi; a.bias = bias; a.alpha = alpha; a.gamma = gamma; a.gelu = gelu; a.x = x; a.ldx = ldx;
+        a.hl = (__nv_bfloat16*)hl; a.ldh = ldh; a.dual = dual; a.T = T; a.Cout = Cout; a.stride = stride; a.pad = pad; a.Tin = Tin;
+        a.noise = noise; a.seed = seed;
+        const cudaStream_t s = (cudaStream_t)stream;
+        b2a_snac::launch_cgemm(W, (const __nv_bfloat16*)X, 2 * b2a_snac::pad64(N), a, hook_ctas(ctas), s);
+        B2A_CUDA(cudaGetLastError());
+        B2A_CUDA(cudaStreamSynchronize(s));
+    });
+}
+
+extern "C" int32_t b2a_snac_unit_test(int32_t mode, int32_t C, int32_t dil, const float* x, float* y, int32_t B, int32_t T,
+                                      const float* dw_w, const float* dw_b, const float* a_in, const float* a_mid, const float* pw_w,
+                                      const float* pw_bias, const float* noise, uint64_t seed, void* hl, const float* a_next, int32_t ctas,
+                                      void* stream) {
+    return guarded([&] {
+        B2A_CHECK(x && y && x != y && pw_w && (C == 64 || C == 128) && B >= 1 && T >= 1 && (long long)B * T < (1ll << 31) - 64 && ctas >= 0,
+                  B2A_ERR_INVALID_INPUT, "b2a_snac_unit_test: bad argument");
+        if (mode == rf::MODE_RU)
+            B2A_CHECK((dil == 1 || dil == 3 || dil == 9) && dw_w && a_in && a_mid && !noise && seed == 0, B2A_ERR_INVALID_INPUT,
+                      "b2a_snac_unit_test: a ResidualUnit takes dil 1, 3 or 9, the depthwise weight and both Snake alphas, and no noise");
+        else
+            B2A_CHECK(mode == rf::MODE_NOISE && dil == 0 && !dw_w && !dw_b && !a_in && !a_mid && !pw_bias && !hl, B2A_ERR_INVALID_INPUT,
+                      "b2a_snac_unit_test: a NoiseBlock is x + noise * (W x): no depthwise conv, bias or hi/lo copy");
+        B2A_CHECK(!hl == !a_next, B2A_ERR_INVALID_INPUT, "b2a_snac_unit_test: the hi/lo copy is Snake(a_next) of y");
+        require_device(0);
+        b2a_snac::fused_attrs<64>();
+        b2a_snac::fused_attrs<128>();
+        std::vector<float> pw(pw_w, pw_w + (size_t)C * C);
+        TcW W;                                              // the [128, 128] operand: W itself (C = 128) or [W 0; 0 W] (C = 64)
+        W.build(C == 64 ? block_diag2(pw) : pw, 128, 128);
+        rf::Args a{};
+        a.x = x; a.y = y; a.C = C; a.mode = mode; a.dil = dil; a.dw_w = dw_w; a.dw_b = dw_b; a.a_in = a_in; a.a_mid = a_mid;
+        a.pw_bias = pw_bias; a.noise = noise; a.seed = seed; a.hl = (__nv_bfloat16*)hl; a.a_next = a_next;
+        const cudaStream_t s = (cudaStream_t)stream;
+        b2a_snac::launch_fused(W, a, B, T, hook_ctas(ctas), s);
+        B2A_CUDA(cudaGetLastError());
+        B2A_CUDA(cudaStreamSynchronize(s));
+    });
+}
+
+extern "C" int32_t b2a_snac_convt_test(const float* x, float* y, const float* alpha, const float* bias, const float* w, int32_t B,
+                                       int32_t Tin, int32_t stride, int32_t cout, int32_t ctas, void* stream) {
+    return guarded([&] {
+        constexpr int CIN = 128;
+        B2A_CHECK(x && y && alpha && w && B >= 1 && Tin >= 1 && ctas >= 0 && (long long)B * Tin * stride < (1ll << 31) - 64,
+                  B2A_ERR_INVALID_INPUT, "b2a_snac_convt_test: bad argument");
+        B2A_CHECK((stride == 2 && cout == 64) || (stride == 1 && cout == 128), B2A_ERR_INVALID_INPUT,
+                  "b2a_snac_convt_test: the fused transposed conv maps 128 channels to stride * cout = 128 phase rows");
+        require_device(0);
+        B2A_CUDA(cudaFuncSetAttribute(rf::convt_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rf::convt_smem_bytes()));
+        const int k = 2 * stride;
+        std::vector<float> wt((size_t)CIN * k * cout);      // torch [ci, co, k] -> the checkpoint's [ci, k, co]
+        for (int ci = 0; ci < CIN; ++ci)
+            for (int co = 0; co < cout; ++co)
+                for (int j = 0; j < k; ++j) wt[((size_t)ci * k + j) * cout + co] = w[((size_t)ci * cout + co) * k + j];
+        TcW W;
+        W.build(convt_phase_major(convt_gemm_rows(wt, CIN, cout, stride), CIN, cout, stride), stride * cout, 2 * CIN);
+        rf::ConvtArgs a{};
+        a.x = x; a.y = y; a.alpha = alpha; a.bias = bias;
+        a.Tin = Tin; a.T = Tin * stride; a.B = B; a.stride = stride; a.cout = cout; a.pad = (stride + 1) / 2;    // DecBlock::pad
+        const cudaStream_t s = (cudaStream_t)stream;
+        b2a_snac::launch_convt(W, a, hook_ctas(ctas), s);
+        B2A_CUDA(cudaGetLastError());
+        B2A_CUDA(cudaStreamSynchronize(s));
+    });
+}
