@@ -114,6 +114,7 @@ void b2a_logmel_destroy(b2a_logmel* h);
  *   decode(_ codes:) :127-131 / decodeAudio :199 -> b2a_snac_decode
  *   quantizer(z) (ResidualVectorQuantize.callAsFunction, SNAC/VQ.swift:150-163), the
  *   encode-side code search                      -> b2a_snac_quantize
+ *   encode(_ audioData:) :120-125 / encodeAudio :197-199 -> b2a_snac_encode (preprocess -> Encoder -> quantizer)
  * codes[i] is [B, T_i] int32 with T_i = t_latent / vq_strides[i]; wave is [B, 1, t_latent*hop].
  * noise[i] (nullable array of nullable pointers) is the [B, 1, T] Gaussian draw of decoder
  * block i's NoiseBlock (Layers.swift:263-279); NULL = draw on device from `seed`
@@ -149,6 +150,18 @@ int32_t b2a_snac_decode_dev(b2a_snac* h, const int32_t* const* d_codes, int32_t 
 /* z [B, latent_dim, T] float32 -> codes[i] [B, T/stride_i] int32 (+ optional z_q [B, latent, T]) */
 int32_t b2a_snac_quantize(b2a_snac* h, const float* z, int32_t batch, int64_t t_latent,
                           int32_t* const* codes, float* z_q);
+/* SNAC.encode (SNACDecoder.swift:86-105,120-125): wave [B, 1, n_samples] float32 is zero right-padded to a multiple of
+ * hop * lcm(vq_strides) (2048 for the 24 kHz model), run through the encoder (Layers.swift:236-259,319-360) and the residual
+ * quantizer; codes[i] [B, t_latent / vq_strides[i]] int32 with t_latent = b2a_snac_encoded_length(h, n_samples).
+ * Needs the checkpoint's encoder.* tensors (a decoder-only handle returns B2A_ERR_MODEL_NOT_INITIALIZED); empty audio is
+ * B2A_ERR_AUDIO_ENCODING_FAILED; an encoder geometry the device path does not run (a stride < 2, latent_dim other than
+ * encoder_dim * 2^len(encoder_rates), batch * padded samples >= 2^31) is B2A_ERR_INVALID_INPUT.  Deterministic: the same
+ * input gives the same codes, and a batch gives the codes of its clips encoded one by one. */
+int64_t b2a_snac_encoded_length(const b2a_snac* h, int64_t n_samples); /* 0 without encoder weights */
+int32_t b2a_snac_encode(b2a_snac* h, const float* wave, int32_t batch, int64_t n_samples, int32_t* const* codes);
+/* the same on DEVICE pointers, enqueued on `stream` (no host synchronisation) */
+int32_t b2a_snac_encode_dev(b2a_snac* h, const float* d_wave, int32_t batch, int64_t n_samples, int32_t* const* d_codes,
+                            void* stream);
 void b2a_snac_destroy(b2a_snac* h);
 
 /* ------------------------------------------------------------------ Orpheus / Llama TTS
@@ -211,6 +224,14 @@ int32_t b2a_tts_create(int32_t device, const b2a_llama_config* cfg, const b2a_te
 /* [SOH] ids [EOT, EOH], left-padded with 128263 to the longest prompt; out is [B, max_len+3] */
 int32_t b2a_tts_prepare_input_ids(const int32_t* const* prompt_ids, const int32_t* lens, int32_t batch,
                                   int32_t* out, int32_t* out_len);
+/* prepareInputIds with refAudio / refText (voice cloning, :446-553): every row is
+ *   [128263 padding] [SOH] ref_text_ids [EOT, EOH] [128261, SOS] ref_code_list + 128266 [EOS, 128262] [SOH] prompt [EOT, EOH],
+ * the padding in front to the longest prompt.  ref_code_list is the 7-token interleaved reference (b2a_tts_interleave of the
+ * reference clip's b2a_snac_encode codes, values in [0, 7 * 4096)); ref_text_ids is the tokenised transcript (may be empty).
+ * out NULL: only *out_len.  B2A_ERR_INVALID_INPUT for null arguments, ref_code_len % 7 != 0 or a code out of range. */
+int32_t b2a_tts_prepare_input_ids_ref(const int32_t* const* prompt_ids, const int32_t* lens, int32_t batch,
+                                      const int32_t* ref_text_ids, int32_t ref_text_len, const int32_t* ref_code_list,
+                                      int32_t ref_code_len, int32_t* out, int32_t* out_len);
 /* One forward over ids [B, L] appended at the cache's current offset (reset_cache != 0 clears
  * it first); logits_out [B, L, vocab] float32 (host). */
 int32_t b2a_tts_forward_logits(b2a_tts* h, const int32_t* ids, int32_t batch, int32_t len,

@@ -112,6 +112,9 @@ int32_t b2a_snac_unit_test(int32_t mode, int32_t C, int32_t dil, const float* x,
  * engine's CTA count.                                                                                                      */
 int32_t b2a_snac_convt_test(const float* x, float* y, const float* alpha, const float* bias, const float* w, int32_t B, int32_t Tin,
                             int32_t stride, int32_t cout, int32_t ctas, void* stream);
+/* tests/test_gpu_snac_encode.py: the SNAC encoder's latent before the code search (what b2a_snac_encode quantizes) on HOST data:
+ * wave [B, n_samples] -> z [B, latent, t_latent] float32, t_latent as b2a_snac_encoded_length gives it.  Errors as b2a_snac_encode. */
+int32_t b2a_snac_encode_latent_test(b2a_snac* h, const float* wave, int32_t batch, int64_t n_samples, float* z);
 
 #ifdef __cplusplus
 }

@@ -160,6 +160,10 @@ SIGNATURES = {
     "b2a_snac_decode": (C.c_int32, [_P, C.POINTER(_P), C.c_int32, C.c_int64, C.POINTER(_P), C.c_int32, C.c_uint64, _P]),
     "b2a_snac_decode_dev": (C.c_int32, [_P, C.POINTER(_P), C.c_int32, C.c_int64, C.POINTER(_P), C.c_int32, C.c_uint64, _P, _P]),
     "b2a_snac_quantize": (C.c_int32, [_P, _P, C.c_int32, C.c_int64, C.POINTER(_P), _P]),
+    "b2a_snac_encoded_length": (C.c_int64, [_P, C.c_int64]),
+    "b2a_snac_encode": (C.c_int32, [_P, _P, C.c_int32, C.c_int64, C.POINTER(_P)]),
+    "b2a_snac_encode_dev": (C.c_int32, [_P, _P, C.c_int32, C.c_int64, C.POINTER(_P), _P]),
+    "b2a_snac_encode_latent_test": (C.c_int32, [_P, _P, C.c_int32, C.c_int64, _P]),
     "b2a_snac_destroy": (None, [_P]),
     "b2a_tts_create": (C.c_int32, [C.c_int32, C.POINTER(LlamaConfig), C.POINTER(Tensor), C.c_int32, _P, C.POINTER(_P)]),
     "b2a_tts_debug_trace": (C.c_int32, [_P, C.c_int32, C.c_int32, _P]),
@@ -170,6 +174,7 @@ SIGNATURES = {
     "b2a_tts_time_steps": (C.c_int32, [_P, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_float)]),
     "b2a_snac_stream": (C.c_void_p, [_P]),
     "b2a_tts_prepare_input_ids": (C.c_int32, [C.POINTER(_P), _P, C.c_int32, _P, C.POINTER(C.c_int32)]),
+    "b2a_tts_prepare_input_ids_ref": (C.c_int32, [C.POINTER(_P), _P, C.c_int32, _P, C.c_int32, _P, C.c_int32, _P, C.POINTER(C.c_int32)]),
     "b2a_tts_forward_logits": (C.c_int32, [_P, _P, C.c_int32, C.c_int32, C.c_int32, _P]),
     "b2a_tts_generate": (C.c_int32, [_P, _P, C.c_int32, C.c_int32, C.POINTER(GenParams), _P, _P, _P, C.c_int64, _P,
                                      C.POINTER(GenInfo), TOKEN_CB, _P]),

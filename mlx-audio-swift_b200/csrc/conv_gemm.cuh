@@ -46,7 +46,9 @@ struct Args {
     int ldh;
     int dual;                 // hi/lo output is the 2-tap im2col of the next transposed conv:
                               //   token (b, t) -> row b*(T+1)+t cols [m], and row b*(T+1)+t+1 cols [M + m]
-    int T;                    // tokens per utterance on the OUTPUT side of this GEMM (for dual / noise / convT)
+    int T;                    // tokens per utterance on the OUTPUT side of this GEMM (for dual / noise / convT / frames)
+    int fs, fpad;             // fs > 0: the hi/lo output is the 2-frame im2col of a strided conv (kernel 2 fs, stride fs, left
+                              //   pad fpad) over utterances of T tokens, laid out by put_frames (replaces dual)
     // E_CONVT: rows m = r*Cout + co; input token n = b*(Tin+1) + q  ->  t_out = q*stride + r - pad
     int Cout, stride, pad, Tin;
     // E_NOISE: x = x + noise[b, t] * acc      (NoiseBlock, Layers.swift:271-278)
@@ -85,6 +87,16 @@ __device__ __forceinline__ void put_hilo(__nv_bfloat16* base, long long ld, long
     const long long r = (tok / HALF) * BN + (tok % HALF);
     base[r * ld + col] = hi;
     base[(r + HALF) * ld + col] = __float2bfloat16_rn(v - __bfloat162float(hi));
+}
+// Input of a strided conv (kernel 2 fs, stride fs, left pad fpad < fs) over utterances of T tokens (T % fs == 0) as a 2-tap GEMM
+// operand: the zero-padded sequence is cut into frames of fs tokens x C channels; output token q reads frames q and q + 1, so row
+// b (T / fs + 1) + q holds frame q in columns [0, fs C) and frame q + 1 in [fs C, 2 fs C) (row q = T / fs is computed and dropped).
+// Token (b, t) is padded position p = t + fpad of frame f = p / fs: it lands in row f (first half) and in row f - 1 (second half).
+__device__ __forceinline__ void put_frames(__nv_bfloat16* hl, int fs, int fpad, int C, int T, long long b, int t, int c, float v) {
+    const int p = t + fpad, f = p / fs, col = (p - f * fs) * C + c;
+    const long long ld = 2ll * fs * C, row = b * (T / fs + 1) + f;
+    put_hilo(hl, ld, row, col, v);
+    if (f > 0) put_hilo(hl, ld, row - 1, (long long)fs * C + col, v);
 }
 
 static __global__ void __launch_bounds__(CG_THREADS, 1)
@@ -218,7 +230,10 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                     if (a.epi == E_ADD) continue;
                 }
                 if (a.alpha) val = snake_inv(val, al, inv_al);
-                if (a.dual) {
+                if (a.fs) {
+                    const long long b = n / a.T;
+                    put_frames(a.hl, a.fs, a.fpad, a.M, a.T, b, (int)(n - b * a.T), m, val);
+                } else if (a.dual) {
                     const long long b = n / a.T, tt = n - b * a.T;
                     const long long row = b * (a.T + 1) + tt;
                     put_hilo(a.hl, a.ldh, row, m, val);

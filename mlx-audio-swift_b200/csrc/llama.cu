@@ -30,6 +30,7 @@ typedef __nv_bfloat16 bf16;
 constexpr int TOK_START_OF_HUMAN = 128259, TOK_END_OF_HUMAN = 128260, TOK_END_OF_TEXT = 128009;
 constexpr int TOK_START_OF_SPEECH = 128257, TOK_END_OF_SPEECH = 128258, TOK_PAD = 128263;
 constexpr int TOK_AUDIO_OFFSET = 128266;
+constexpr int TOK_AUDIO_START = 128261, TOK_AUDIO_END = 128262;        // LlamaTTS.swift:27-28
 
 __device__ __forceinline__ float bf16_round(float x) { return __bfloat162float(__float2bfloat16_rn(x)); }
 __device__ __forceinline__ float bf_lo(unsigned u) { return __uint_as_float(u << 16); }
@@ -1894,6 +1895,46 @@ int32_t b2a_tts_prepare_input_ids(const int32_t* const* prompt_ids, const int32_
             int32_t* r = out + (size_t)b * (mx + 3);
             int j = 0;
             for (; j < mx - lens[b]; ++j) r[j] = TOK_PAD;
+            r[j++] = TOK_START_OF_HUMAN;
+            for (int i = 0; i < lens[b]; ++i) r[j++] = prompt_ids[b][i];
+            r[j++] = TOK_END_OF_TEXT;
+            r[j++] = TOK_END_OF_HUMAN;
+        }
+    });
+}
+
+int32_t b2a_tts_prepare_input_ids_ref(const int32_t* const* prompt_ids, const int32_t* lens, int32_t batch, const int32_t* ref_text_ids,
+                                      int32_t ref_text_len, const int32_t* ref_code_list, int32_t ref_code_len, int32_t* out,
+                                      int32_t* out_len) {
+    return guarded([&] {
+        B2A_CHECK(prompt_ids && lens && out_len && batch > 0 && ref_text_len >= 0 && ref_code_len >= 0 && (ref_text_ids || ref_text_len == 0) &&
+                      (ref_code_list || ref_code_len == 0),
+                  B2A_ERR_INVALID_INPUT, "b2a_tts_prepare_input_ids_ref: null argument");
+        B2A_CHECK(ref_code_len % 7 == 0, B2A_ERR_INVALID_INPUT, "b2a_tts_prepare_input_ids_ref: ref_code_len must be a multiple of 7");
+        for (int i = 0; i < ref_code_len; ++i)
+            B2A_CHECK(ref_code_list[i] >= 0 && ref_code_list[i] < 7 * 4096, B2A_ERR_INVALID_INPUT,
+                      "b2a_tts_prepare_input_ids_ref: reference code out of range [0, 7 * 4096)");
+        int mx = 0;
+        for (int b = 0; b < batch; ++b) {
+            B2A_CHECK(lens[b] >= 0 && (prompt_ids[b] || lens[b] == 0), B2A_ERR_INVALID_INPUT, "b2a_tts_prepare_input_ids_ref: bad prompt");
+            mx = std::max(mx, lens[b]);
+        }
+        const int ref = 1 + ref_text_len + 2 + 2 + ref_code_len + 2;        // LlamaTTS.swift:520-527
+        *out_len = mx + ref + 3;
+        if (!out) return;
+        for (int b = 0; b < batch; ++b) {   // LlamaTTS.swift:499-543: padding, reference block, prompt
+            int32_t* r = out + (size_t)b * (mx + ref + 3);
+            int j = 0;
+            for (; j < mx - lens[b]; ++j) r[j] = TOK_PAD;
+            r[j++] = TOK_START_OF_HUMAN;
+            for (int i = 0; i < ref_text_len; ++i) r[j++] = ref_text_ids[i];
+            r[j++] = TOK_END_OF_TEXT;
+            r[j++] = TOK_END_OF_HUMAN;
+            r[j++] = TOK_AUDIO_START;
+            r[j++] = TOK_START_OF_SPEECH;
+            for (int i = 0; i < ref_code_len; ++i) r[j++] = ref_code_list[i] + TOK_AUDIO_OFFSET;
+            r[j++] = TOK_END_OF_SPEECH;
+            r[j++] = TOK_AUDIO_END;
             r[j++] = TOK_START_OF_HUMAN;
             for (int i = 0; i < lens[b]; ++i) r[j++] = prompt_ids[b][i];
             r[j++] = TOK_END_OF_TEXT;

@@ -1,7 +1,8 @@
-// SNAC codec decode + RVQ code search for sm_90a.  Replaces (reference paths):
+// SNAC codec decode, encode + RVQ code search for sm_90a.  Replaces (reference paths):
 //   Sources/MLXAudioCodecs/SNAC/VQ.swift:14-20,47-120,150-191    (RVQ lookup / code search)
 //   Sources/MLXAudioCodecs/SNAC/Layers.swift:44-50,54-183,202-232,263-315,364-421 (decoder)
 //   Sources/MLXAudioCodecs/SNAC/SNACDecoder.swift:127-131          (SNAC.decode)
+//   Sources/MLXAudioCodecs/SNAC/Layers.swift:236-259,319-360, SNACDecoder.swift:86-105,120-125 (encoder, SNAC.encode; DESIGN.md §3.2b)
 //
 // HBM layout: activations float32 [B, C, T] (time contiguous -> every load/store is coalesced
 // along T); two ping-pong buffers sized for the widest stage.  Weight-norm (g*v/||v||) is folded
@@ -20,6 +21,7 @@
 #include <algorithm>
 #include <cmath>
 #include <cstdlib>
+#include <numeric>
 
 namespace b2a {
 
@@ -476,6 +478,70 @@ __global__ void x2_zero_edges_kernel(__nv_bfloat16* __restrict__ x2, int T, int 
     }
 }
 
+// ---- encoder (Layers.swift:236-259, 319-360) -------------------------------------------------------------------------------
+// stem WNConv1d(1 -> C, k7, pad 3) on the raw waveform, zero right-padded from n to T samples: y[b*T + t, c], C % 4 == 0 (channels
+// past the model width have zero weights and bias, so they stay 0).  One thread = one token x 4 channels (float4 store).
+__global__ void enc_stem_kernel(const float* __restrict__ wave, float* __restrict__ y, const float* __restrict__ w /*[C,7]*/,
+                                const float* __restrict__ bias, int B, long long n, int T, int C) {
+    const int cq = C >> 2;
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= (long long)B * T * cq) return;
+    const long long tok = i / cq;
+    const int c = (int)(i - tok * cq) * 4;
+    const int b = (int)(tok / T), t = (int)(tok - (long long)b * T);
+    const float* x = wave + (long long)b * n;
+    float xv[7];
+#pragma unroll
+    for (int k = 0; k < 7; ++k) { const long long s = (long long)t + k - 3; xv[k] = (s >= 0 && s < n) ? x[s] : 0.f; }
+    float o[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+        float acc = bias[c + j];
+#pragma unroll
+        for (int k = 0; k < 7; ++k) acc = fmaf(w[(c + j) * 7 + k], xv[k], acc);
+        o[j] = acc;
+    }
+    *reinterpret_cast<float4*>(y + tok * C + c) = make_float4(o[0], o[1], o[2], o[3]);
+}
+
+// zero the padding positions of the strided conv's 2-frame im2col (conv_gemm.cuh put_frames), which no producer writes: frame 0
+// positions [0, pad), frame T/s positions [pad, s) (rows T/s and T/s - 1), and the second half of the dropped row T/s
+__global__ void frames_zero_edges_kernel(__nv_bfloat16* __restrict__ hl, int T, int s, int pad, int C) {
+    const long long tout = T / s, r0 = (long long)blockIdx.x * (tout + 1), rl = r0 + tout;
+    const long long ld = 2ll * s * C, sc = (long long)s * C;
+    const __nv_bfloat16 z = __float2bfloat16_rn(0.f);
+    auto zero = [&](long long row, long long c0, long long c1) {
+        const long long h = (row / 64) * 128 + (row % 64);
+        for (long long c = c0 + threadIdx.x; c < c1; c += blockDim.x) { hl[h * ld + c] = z; hl[(h + 64) * ld + c] = z; }
+    };
+    zero(r0, 0, (long long)pad * C);
+    zero(rl, (long long)pad * C, ld);
+    zero(rl - 1, sc + (long long)pad * C, ld);
+}
+
+// final depthwise WNConv1d(C -> C, k7, pad 3, groups C) from NLC x [B*T, ld] (ld >= C: the last strided conv's padded width) to the
+// quantizer's fp32 z [B, C, T]: 32 tokens x 32 channels per CTA, staged (with the 3-token halo) in shared memory so that both the
+// load and the store are coalesced
+__global__ void __launch_bounds__(256)
+enc_final_dw_kernel(const float* __restrict__ x, float* __restrict__ z, const float* __restrict__ w /*[C,7]*/,
+                    const float* __restrict__ bias, int T, int C, int ld) {
+    __shared__ float s[38][33];
+    const int t0 = blockIdx.x * 32, c0 = blockIdx.y * 32, b = blockIdx.z;
+    for (int i = threadIdx.y * 32 + threadIdx.x; i < 38 * 32; i += 256) {
+        const int r = i >> 5, c = i & 31, t = t0 + r - 3;
+        s[r][c] = (t >= 0 && t < T && c0 + c < C) ? x[((long long)b * T + t) * ld + c0 + c] : 0.f;
+    }
+    __syncthreads();
+    const int t = t0 + threadIdx.x;
+    if (t >= T) return;
+    for (int c = threadIdx.y; c < 32 && c0 + c < C; c += 8) {
+        float acc = bias[c0 + c];
+#pragma unroll
+        for (int k = 0; k < 7; ++k) acc = fmaf(w[(c0 + c) * 7 + k], s[threadIdx.x + k][c], acc);
+        z[((long long)b * C + c0 + c) * T + t] = acc;
+    }
+}
+
 // final Snake -> conv k7 (C -> 1) -> tanh in NLC (Layers.swift:411-415), C == 64.
 // 256 tokens per CTA; the Snake'd tile (+3 halo rows each side) is staged in shared memory.  Thread (tg, cg) owns 8 consecutive
 // tokens x 8 channels (two float4 column groups {4cg..4cg+3} and {32+4cg..}, so a quarter-warp's LDS.128 covers 128 contiguous
@@ -583,6 +649,25 @@ struct DecBlock {
     ResUnit ru[3];
 };
 
+// encoder block (Layers.swift:236-259) at its padded width cp: three ResidualUnits, Snake, strided conv cp -> cp_out
+struct EncBlock {
+    int c, cp, cout, cp_out, stride, pad;
+    ResUnit ru[3];
+    DBuf<float> alpha;   // Snake before the strided conv
+    TcW down;            // [cp_out, 2 * stride * cp]: A[co, j * cp + ci] = w[co, j, ci]  (kernel position j < 2 stride)
+    ConvW down_b;        // bias only
+};
+// channel width the encoder runs a C-channel stage at: the fused unit's 64 / 128 up to 128, else the conv GEMM's multiple of 64.
+// The extra channels carry exact zeros (weights and biases 0, Snake alpha 1).
+static int enc_padded(int c) { return c <= 64 ? 64 : c <= 128 ? 128 : (c + 63) / 64 * 64; }
+// [rows, cols] -> [prow, pcol] with zeros (and `fill` for 1-D vectors) outside
+static std::vector<float> pad2(const std::vector<float>& v, int rows, int cols, int prow, int pcol, float fill = 0.f) {
+    std::vector<float> o((size_t)prow * pcol, fill);
+    for (int r = 0; r < rows; ++r)
+        for (int c = 0; c < cols; ++c) o[(size_t)r * pcol + c] = v[(size_t)r * cols + c];
+    return o;
+}
+
 static std::vector<float> fold_wn(const TensorTable& tt, const std::string& prefix, int d0, int d1, int d2, bool eps) {
     // weight = g * v / (||v||_{dims 1,2} (+ 1e-12))   Layers.swift:102-103 (eps) / :166 (no eps)
     std::vector<float> v = tt.f32(prefix + ".weight_v", (int64_t)d0 * d1 * d2);
@@ -656,8 +741,14 @@ struct b2a_snac {
     ConvW final_conv;
     int final_c = 0;
     float final_bias = 0.f;
+    // encoder (only when the checkpoint has encoder.* keys)
+    bool has_enc = false;
+    std::string enc_error = "SNAC encode: the checkpoint has no encoder weights";
+    int enc_hop = 1;
+    ConvW enc_stem, enc_final;           // [cp0, 7] / [latent, 7] + bias
+    std::vector<EncBlock> eblocks;
     // workspaces
-    DBuf<float> bufX, bufY, d_wave, d_noise[8], d_ze, d_en, d_e2, d_zq;
+    DBuf<float> bufX, bufY, d_wave, d_noise[8], d_ze, d_en, d_e2, d_zq, d_zenc, d_ewave;
     DBuf<int> d_codes[8], d_idx;
 
     ~b2a_snac() { if (stream) cudaStreamDestroy(stream); }
@@ -786,6 +877,75 @@ struct b2a_snac {
             }
         }
         host_pw0.clear(); host_ct.clear(); host_noise.clear(); host_pw.clear();
+        if (tt.find("encoder.block.layers.0.weight_v")) {
+            // a malformed encoder leaves a working decoder: encode then reports why (B2A_ERR_MODEL_NOT_INITIALIZED)
+            try { load_encoder(tt); has_enc = true; }
+            catch (const Error& e) { eblocks.clear(); enc_error = std::string("SNAC encode: encoder weights unusable: ") + e.what(); }
+            B2A_CUDA(cudaGetLastError());
+        }
+    }
+
+    // encoder weights at padded widths (Layers.swift:236-259, 319-360; keys encoder.block.layers.*)
+    void load_encoder(const TensorTable& tt) {
+        const std::string p = "encoder.block.layers.";
+        const int n = cfg.n_encoder_rates;
+        B2A_CHECK(n >= 1 && n <= 8 && cfg.encoder_dim >= 1, B2A_ERR_INVALID_INPUT, "encoder_dim / encoder_rates");
+        int c = cfg.encoder_dim;
+        {
+            const int cp = enc_padded(c);
+            std::vector<float> w = pad2(fold_wn(tt, p + "0", c, 7, 1, true), c, 7, cp, 7);
+            std::vector<float> b = pad2(tt.f32(p + "0.bias", c), 1, c, 1, cp);
+            enc_stem.w.upload(w.data(), w.size());
+            enc_stem.bias.upload(b.data(), b.size());
+        }
+        B2A_CUDA(cudaFuncSetAttribute(cg::conv_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cg::SMEM_BYTES));
+        B2A_CUDA(cudaFuncSetAttribute(dw7_nlc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
+        fused_attrs<64>(); fused_attrs<128>();
+        eblocks.resize(n);
+        enc_hop = 1;
+        for (int i = 0; i < n; ++i, c *= 2) {
+            EncBlock& E = eblocks[i];
+            E.c = c; E.cp = enc_padded(c); E.cout = 2 * c; E.cp_out = enc_padded(2 * c);
+            E.stride = cfg.encoder_rates[i]; E.pad = (E.stride + 1) / 2;      // Int(ceil(stride / 2)), Layers.swift:251
+            B2A_CHECK(E.stride >= 1, B2A_ERR_INVALID_INPUT, "encoder stride");
+            enc_hop *= E.stride;
+            const std::string b = p + std::to_string(i + 1) + ".block.layers.";
+            const int dils[3] = {1, 3, 9};
+            for (int u = 0; u < 3; ++u) {
+                ResUnit& R = E.ru[u];
+                R.dil = dils[u];
+                const std::string r = b + std::to_string(u) + ".block.layers.";
+                std::vector<float> a0 = pad2(tt.f32(r + "0.alpha", c), 1, c, 1, E.cp, 1.f), a2 = pad2(tt.f32(r + "2.alpha", c), 1, c, 1, E.cp, 1.f);
+                R.a0.upload(a0.data(), a0.size());
+                R.a2.upload(a2.data(), a2.size());
+                std::vector<float> wd = pad2(fold_wn(tt, r + "1", c, 7, 1, true), c, 7, E.cp, 7);
+                R.dw.w.upload(wd.data(), wd.size());
+                std::vector<float> bd = pad2(tt.f32(r + "1.bias", c), 1, c, 1, E.cp);
+                R.dw.bias.upload(bd.data(), bd.size()); R.dw.has_bias = true;
+                std::vector<float> wp = pad2(fold_wn(tt, r + "3", c, 1, c, true), c, c, E.cp, E.cp);
+                R.pw_tc.build(wp, E.cp, E.cp);
+                if (E.cp == 64) R.pw_bd.build(block_diag2(wp), 128, 128);
+                std::vector<float> bp = pad2(tt.f32(r + "3.bias", c), 1, c, 1, E.cp);
+                R.pw.bias.upload(bp.data(), bp.size()); R.pw.has_bias = true;
+            }
+            std::vector<float> a = pad2(tt.f32(b + "3.alpha", c), 1, c, 1, E.cp, 1.f);
+            E.alpha.upload(a.data(), a.size());
+            const int k = 2 * E.stride;
+            std::vector<float> wt = fold_wn(tt, b + "4", E.cout, k, c, true);        // [co, j, ci]
+            std::vector<float> A((size_t)E.cp_out * k * E.cp, 0.f);
+            for (int co = 0; co < E.cout; ++co)
+                for (int j = 0; j < k; ++j)
+                    for (int ci = 0; ci < c; ++ci) A[(size_t)co * k * E.cp + (size_t)j * E.cp + ci] = wt[((size_t)co * k + j) * c + ci];
+            E.down.build(A, E.cp_out, k * E.cp);
+            std::vector<float> bb = pad2(tt.f32(b + "4.bias", E.cout), 1, E.cout, 1, E.cp_out);
+            E.down_b.bias.upload(bb.data(), bb.size()); E.down_b.has_bias = true;
+        }
+        const std::string f = p + std::to_string(n + 1);
+        std::vector<float> w = fold_wn(tt, f, c, 7, 1, true);                            // depthwise [C, 7, 1]
+        enc_final.w.upload(w.data(), w.size());
+        std::vector<float> b = tt.f32(f + ".bias", c);
+        enc_final.bias.upload(b.data(), b.size()); enc_final.has_bias = true;
+        B2A_CUDA(cudaStreamSynchronize(stream));
     }
     std::vector<float> host_pw0;
     std::vector<std::vector<float>> host_ct, host_noise, host_pw;
@@ -1056,6 +1216,122 @@ struct b2a_snac {
         B2A_CUDA(cudaGetLastError());
     }
 
+    // ---- encode (SNACDecoder.swift:86-105,120-125) ----------------------------------------------------------------------------
+    // padded length: a multiple of hop * lcm(vq_strides) (SNACDecoder.swift:86-100)
+    long long enc_pad_multiple() const {
+        long long l = 1;
+        for (auto& L : levels) l = std::lcm(l, (long long)L.stride);
+        return (long long)enc_hop * l;
+    }
+    long long encoded_length(long long n) const {
+        const long long m = enc_pad_multiple();
+        return (n + m - 1) / m * m / enc_hop;
+    }
+    // throws unless the handle can encode `batch` clips of n samples
+    void enc_check(int batch, long long n) const {
+        B2A_CHECK(batch > 0 && n > 0, B2A_ERR_AUDIO_ENCODING_FAILED, "snac encode: empty audio");
+        B2A_CHECK(has_enc, B2A_ERR_MODEL_NOT_INITIALIZED, enc_error);
+        for (auto& L : levels) B2A_CHECK(L.win.p, B2A_ERR_MODEL_NOT_INITIALIZED, "snac encode: quantizer in_proj weights were not provided");
+        B2A_CHECK(cfg.encoder_dim << cfg.n_encoder_rates == latent, B2A_ERR_INVALID_INPUT,
+                  "snac encode: latent_dim must be encoder_dim * 2^len(encoder_rates)");
+        for (auto& E : eblocks) B2A_CHECK(E.stride >= 2, B2A_ERR_INVALID_INPUT, "snac encode: encoder strides must be >= 2");
+        const long long np = encoded_length(n) * enc_hop;
+        B2A_CHECK((long long)batch * np < (1ll << 31) - 64, B2A_ERR_INVALID_INPUT, "snac encode: batch * padded samples must be < 2^31");
+    }
+    // stages at the fused unit's widths; the others run dw7_nlc_kernel + the conv GEMM through the hi/lo operand hA
+    static bool enc_fused(const EncBlock& E) { return E.cp == 64 || E.cp == 128; }
+    // d_wave [B, n] -> z [B, latent, T_lat] fp32 NCT in d_zenc (returned); channels-last fp32 stream + bf16 hi/lo GEMM operands
+    float* encode_latent_dev(const float* d_wave_in, int batch, long long n, cudaStream_t s) {
+        const long long tl = encoded_length(n), T0 = tl * enc_hop;
+        size_t max_x = (size_t)batch * tl * latent, max_h = 0, max_x2 = 0;
+        {
+            long long t = T0;
+            for (auto& E : eblocks) {
+                max_x = std::max<size_t>(max_x, (size_t)batch * t * E.cp);
+                if (!enc_fused(E)) max_h = std::max<size_t>(max_h, (size_t)(2 * pad64((long long)batch * t)) * E.cp);   // dw7 -> GEMM operand
+                t /= E.stride;
+                max_x2 = std::max<size_t>(max_x2, (size_t)(2 * pad64((long long)batch * (t + 1))) * 2 * E.stride * E.cp);
+                max_x = std::max<size_t>(max_x, (size_t)batch * t * E.cp_out);
+            }
+        }
+        xs.alloc(max_x); xs2.alloc(max_x); hA.alloc(max_h); x2.alloc(max_x2);
+        d_zenc.alloc((size_t)batch * latent * tl);
+        {
+            const int cp0 = eblocks[0].cp;
+            const long long nthr = (long long)batch * T0 * (cp0 / 4);
+            enc_stem_kernel<<<(unsigned)((nthr + 255) / 256), 256, 0, s>>>(d_wave_in, xs.p, enc_stem.w.p, enc_stem.bias.p, batch, n, (int)T0, cp0);
+            count_launch();
+        }
+        long long t = T0;
+        for (size_t i = 0; i < eblocks.size(); ++i) {
+            EncBlock& E = eblocks[i];
+            const long long tout = t / E.stride, ntok = (long long)batch * t;
+            if (enc_fused(E)) {
+                // fused ResidualUnits, fp32 in -> fp32 out (ping-pong xs <-> xs2); the last one also writes Snake(alpha) of its
+                // output into the strided conv's 2-frame im2col
+                for (int u = 0; u < 3; ++u) {
+                    ResUnit& R = E.ru[u];
+                    rf::Args a{};
+                    a.x = xs.p; a.y = xs2.p; a.C = E.cp; a.mode = rf::MODE_RU; a.dil = R.dil;
+                    a.dw_w = R.dw.w.p; a.dw_b = R.dw.bias.p; a.a_in = R.a0.p; a.a_mid = R.a2.p; a.pw_bias = R.pw.bias.p;
+                    if (u == 2) { a.hl = x2.p; a.a_next = E.alpha.p; a.fs = E.stride; a.fpad = E.pad; }
+                    fused(E.cp == 64 ? R.pw_bd : R.pw_tc, a, batch, t, s);
+                    std::swap(xs.p, xs2.p); std::swap(xs.n, xs2.n);
+                }
+            } else {
+                for (int u = 0; u < 3; ++u) {
+                    ResUnit& R = E.ru[u];
+                    dw_nlc(R.dw, xs.p, hA.p, R.a0.p, R.a2.p, batch, (int)t, E.cp, R.dil, s);
+                    cg::Args a{};
+                    a.N = (int)ntok; a.bias = R.pw.bias.p; a.x = xs.p; a.ldx = E.cp; a.T = (int)t;
+                    if (u == 2) { a.epi = cg::E_ADD_HILO; a.alpha = E.alpha.p; a.hl = x2.p; a.fs = E.stride; a.fpad = E.pad; }
+                    else a.epi = cg::E_ADD;
+                    cgemm(R.pw_tc, hA.p, 2 * pad64(ntok), a, s);
+                }
+            }
+            // after the units (it writes other positions of x2): a plain launch between the last fused unit and the strided conv's
+            // GEMM, whose TMA producer reads x2 without waiting on the programmatic dependency
+            frames_zero_edges_kernel<<<batch, 256, 0, s>>>(x2.p, (int)t, E.stride, E.pad, E.cp);
+            count_launch();
+            {   // strided conv = 2-tap GEMM over the frames: token (b, q), q = 0..tout (q = tout dropped) -> fp32 [B*tout, cp_out] + bias
+                cg::Args a{};
+                a.N = (int)(batch * (tout + 1)); a.epi = cg::E_CONVT; a.bias = E.down_b.bias.p;
+                a.x = xs.p; a.ldx = E.cp_out; a.T = (int)tout; a.Cout = E.cp_out; a.stride = 1; a.pad = 0; a.Tin = (int)tout;
+                cgemm(E.down, x2.p, 2 * pad64((long long)batch * (tout + 1)), a, s);
+            }
+            t = tout;
+        }
+        enc_final_dw_kernel<<<dim3(cdiv(t, 32), cdiv(latent, 32), batch), dim3(32, 8), 0, s>>>(xs.p, d_zenc.p, enc_final.w.p, enc_final.bias.p,
+                                                                                             (int)t, latent, eblocks.back().cp_out);
+        count_launch();
+        B2A_CUDA(cudaGetLastError());
+        return d_zenc.p;
+    }
+    // residual VQ (VQ.swift:47-120,150-163) of d_res = z [B, latent, T] fp32 on the device (left holding the final residual):
+    // codes of level i -> d_codes_out[i] [B, T / stride_i]; z_q accumulated into d_zq_out when non-null
+    void quantize_dev(float* d_res, int batch, long long T, int* const* d_codes_out, float* d_zq_out, cudaStream_t s) {
+        const int C = latent, D = cfg.codebook_dim;
+        if (d_zq_out) B2A_CUDA(cudaMemsetAsync(d_zq_out, 0, (size_t)batch * C * T * sizeof(float), s));
+        for (size_t i = 0; i < levels.size(); ++i) {
+            auto& L = levels[i];
+            const int Ts = (int)(T / L.stride), N = batch * Ts;
+            d_ze.alloc((size_t)N * D);
+            vq_inproj_kernel<<<dim3(cdiv(Ts, 64), batch), 64, 0, s>>>(d_res, L.win.p, L.bin.p, d_ze.p, C, (int)T, L.stride, D);
+            count_launch();
+            nearest(d_ze.p, N, d_codes_out[i], L, s);
+            RvqArgs ra{};
+            ra.n_levels = 1; ra.D = D; ra.C = C; ra.T = (int)T; ra.codebook_size = cfg.codebook_size;
+            ra.lv[0] = RvqLevel{d_codes_out[i], L.codebook.p, L.wout.p, L.bout.p, L.stride};
+            if (d_zq_out) {
+                rvq_lookup_kernel<<<dim3(cdiv(T, 256), C, batch), 256, 0, s>>>(ra, d_zq_out, 1.f, 1.f);    // zQ += zQ_i
+                count_launch();
+            }
+            rvq_lookup_kernel<<<dim3(cdiv(T, 256), C, batch), 256, 0, s>>>(ra, d_res, 1.f, -1.f);         // residual -= zQ_i
+            count_launch();
+        }
+        B2A_CUDA(cudaGetLastError());
+    }
+
     void nearest(const float* d_enc, int N, int* d_out_idx, const Level& L, cudaStream_t s) {
         const int D = cfg.codebook_dim;
         d_en.alloc((size_t)N * D);
@@ -1136,32 +1412,62 @@ int32_t b2a_snac_quantize(b2a_snac* h, const float* z, int32_t batch, int64_t T,
             B2A_CHECK(T % L.stride == 0, B2A_ERR_AUDIO_ENCODING_FAILED, "b2a_snac_quantize: T must be a multiple of every vq stride");
             B2A_CHECK(L.win.p, B2A_ERR_MODEL_NOT_INITIALIZED, "b2a_snac_quantize: in_proj weights were not provided");
         }
+        for (size_t i = 0; i < h->levels.size(); ++i) B2A_CHECK(codes[i], B2A_ERR_INVALID_INPUT, "b2a_snac_quantize: null code output");
         B2A_CUDA(cudaSetDevice(h->device));
         cudaStream_t s = h->stream;
-        const int C = h->latent, D = h->cfg.codebook_dim;
-        const size_t n = (size_t)batch * C * T;
+        const size_t n = (size_t)batch * h->latent * T;
         h->bufX.alloc(n);   // residual
-        h->d_zq.alloc(n);
         B2A_CUDA(cudaMemcpyAsync(h->bufX.p, z, n * sizeof(float), cudaMemcpyHostToDevice, s));
-        B2A_CUDA(cudaMemsetAsync(h->d_zq.p, 0, n * sizeof(float), s));
+        if (z_q) h->d_zq.alloc(n);
+        int* dc[8];
         for (size_t i = 0; i < h->levels.size(); ++i) {
-            auto& L = h->levels[i];
-            const int Ts = (int)(T / L.stride), N = batch * Ts;
-            h->d_ze.alloc((size_t)N * D);
-            h->d_idx.alloc(N);
-            vq_inproj_kernel<<<dim3(cdiv(Ts, 64), batch), 64, 0, s>>>(h->bufX.p, L.win.p, L.bin.p, h->d_ze.p, C, (int)T, L.stride, D);
-            count_launch();
-            h->nearest(h->d_ze.p, N, h->d_idx.p, L, s);
-            RvqArgs ra{};
-            ra.n_levels = 1; ra.D = D; ra.C = C; ra.T = (int)T; ra.codebook_size = h->cfg.codebook_size;
-            ra.lv[0] = RvqLevel{h->d_idx.p, L.codebook.p, L.wout.p, L.bout.p, L.stride};
-            rvq_lookup_kernel<<<dim3(cdiv(T, 256), C, batch), 256, 0, s>>>(ra, h->d_zq.p, 1.f, 1.f);    // zQ += zQ_i
-            rvq_lookup_kernel<<<dim3(cdiv(T, 256), C, batch), 256, 0, s>>>(ra, h->bufX.p, 1.f, -1.f);   // residual -= zQ_i
-            count_launch(2);
-            B2A_CHECK(codes[i], B2A_ERR_INVALID_INPUT, "b2a_snac_quantize: null code output");
-            B2A_CUDA(cudaMemcpyAsync(codes[i], h->d_idx.p, (size_t)N * sizeof(int), cudaMemcpyDeviceToHost, s));
+            h->d_codes[i].alloc((size_t)batch * (T / h->levels[i].stride));
+            dc[i] = h->d_codes[i].p;
         }
+        h->quantize_dev(h->bufX.p, batch, T, dc, z_q ? h->d_zq.p : nullptr, s);
+        for (size_t i = 0; i < h->levels.size(); ++i)
+            B2A_CUDA(cudaMemcpyAsync(codes[i], dc[i], (size_t)batch * (T / h->levels[i].stride) * sizeof(int), cudaMemcpyDeviceToHost, s));
         if (z_q) B2A_CUDA(cudaMemcpyAsync(z_q, h->d_zq.p, n * sizeof(float), cudaMemcpyDeviceToHost, s));
+        B2A_CUDA(cudaStreamSynchronize(s));
+        B2A_CUDA(cudaGetLastError());
+    });
+}
+
+int64_t b2a_snac_encoded_length(const b2a_snac* h, int64_t n_samples) {
+    return h && h->has_enc && n_samples > 0 ? h->encoded_length(n_samples) : 0;
+}
+
+int32_t b2a_snac_encode_dev(b2a_snac* h, const float* d_wave, int32_t batch, int64_t n_samples, int32_t* const* d_codes, void* stream) {
+    return guarded([&] {
+        B2A_CHECK(h && d_wave && d_codes, B2A_ERR_INVALID_INPUT, "b2a_snac_encode_dev: null argument");
+        h->enc_check(batch, n_samples);
+        for (size_t i = 0; i < h->levels.size(); ++i) B2A_CHECK(d_codes[i], B2A_ERR_INVALID_INPUT, "b2a_snac_encode_dev: null code output");
+        B2A_CUDA(cudaSetDevice(h->device));
+        const cudaStream_t s = (cudaStream_t)stream;
+        float* z = h->encode_latent_dev(d_wave, batch, n_samples, s);
+        h->quantize_dev(z, batch, h->encoded_length(n_samples), d_codes, nullptr, s);
+    });
+}
+
+int32_t b2a_snac_encode(b2a_snac* h, const float* wave, int32_t batch, int64_t n_samples, int32_t* const* codes) {
+    return guarded([&] {
+        B2A_CHECK(h && wave && codes, B2A_ERR_INVALID_INPUT, "b2a_snac_encode: null argument");
+        h->enc_check(batch, n_samples);
+        for (size_t i = 0; i < h->levels.size(); ++i) B2A_CHECK(codes[i], B2A_ERR_INVALID_INPUT, "b2a_snac_encode: null code output");
+        B2A_CUDA(cudaSetDevice(h->device));
+        cudaStream_t s = h->stream;
+        const long long tl = h->encoded_length(n_samples);
+        h->d_ewave.alloc((size_t)batch * n_samples);
+        B2A_CUDA(cudaMemcpyAsync(h->d_ewave.p, wave, (size_t)batch * n_samples * sizeof(float), cudaMemcpyHostToDevice, s));
+        int* dc[8];
+        for (size_t i = 0; i < h->levels.size(); ++i) {
+            h->d_codes[i].alloc((size_t)batch * (tl / h->levels[i].stride));
+            dc[i] = h->d_codes[i].p;
+        }
+        float* z = h->encode_latent_dev(h->d_ewave.p, batch, n_samples, s);
+        h->quantize_dev(z, batch, tl, dc, nullptr, s);
+        for (size_t i = 0; i < h->levels.size(); ++i)
+            B2A_CUDA(cudaMemcpyAsync(codes[i], dc[i], (size_t)batch * (tl / h->levels[i].stride) * sizeof(int), cudaMemcpyDeviceToHost, s));
         B2A_CUDA(cudaStreamSynchronize(s));
         B2A_CUDA(cudaGetLastError());
     });
@@ -1275,5 +1581,21 @@ extern "C" int32_t b2a_snac_convt_test(const float* x, float* y, const float* al
         b2a_snac::launch_convt(W, a, hook_ctas(ctas), s);
         B2A_CUDA(cudaGetLastError());
         B2A_CUDA(cudaStreamSynchronize(s));
+    });
+}
+
+// The device encoder's latent (before the code search) on HOST data: wave [B, n] -> z [B, latent, b2a_snac_encoded_length(n)].
+extern "C" int32_t b2a_snac_encode_latent_test(b2a_snac* h, const float* wave, int32_t batch, int64_t n_samples, float* z) {
+    return guarded([&] {
+        B2A_CHECK(h && wave && z, B2A_ERR_INVALID_INPUT, "b2a_snac_encode_latent_test: null argument");
+        h->enc_check(batch, n_samples);
+        B2A_CUDA(cudaSetDevice(h->device));
+        cudaStream_t s = h->stream;
+        h->d_ewave.alloc((size_t)batch * n_samples);
+        B2A_CUDA(cudaMemcpyAsync(h->d_ewave.p, wave, (size_t)batch * n_samples * sizeof(float), cudaMemcpyHostToDevice, s));
+        const float* dz = h->encode_latent_dev(h->d_ewave.p, batch, n_samples, s);
+        B2A_CUDA(cudaMemcpyAsync(z, dz, (size_t)batch * h->latent * h->encoded_length(n_samples) * sizeof(float), cudaMemcpyDeviceToHost, s));
+        B2A_CUDA(cudaStreamSynchronize(s));
+        B2A_CUDA(cudaGetLastError());
     });
 }

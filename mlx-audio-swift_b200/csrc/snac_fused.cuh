@@ -42,6 +42,7 @@ struct Args {
     unsigned long long seed;
     __nv_bfloat16* hl;         // optional: Snake(a_next) of y as the next block's 2-tap im2col (conv_gemm.cuh "dual"), ld = 2*C
     const float* a_next;
+    int fs, fpad;              // fs > 0: hl is instead the 2-frame im2col of the encoder's strided conv (conv_gemm.cuh put_frames)
     int tiles_per_utt;
     long long n_tiles;
 };
@@ -258,9 +259,13 @@ ru_fused_kernel(const __grid_constant__ CUtensorMap tmWh, const __grid_constant_
                     a.y[erow * C + ech] = val;
                     if (a.hl) {
                         const float sv = cg::snake(val, an);
-                        const long long row = (long long)b * (a.T + 1) + etok;
-                        cg::put_hilo(a.hl, 2 * C, row, ech, sv);
-                        cg::put_hilo(a.hl, 2 * C, row + 1, C + ech, sv);
+                        if (a.fs) {
+                            cg::put_frames(a.hl, a.fs, a.fpad, C, a.T, b, etok, ech, sv);
+                        } else {
+                            const long long row = (long long)b * (a.T + 1) + etok;
+                            cg::put_hilo(a.hl, 2 * C, row, ech, sv);
+                            cg::put_hilo(a.hl, 2 * C, row + 1, C + ech, sv);
+                        }
                     }
                 }
             }

@@ -131,17 +131,39 @@ class LlamaTTSModel:
 
     # -- token plumbing -------------------------------------------------------------------------
     @staticmethod
-    def prepare_input_ids(prompt_token_ids: Sequence[Sequence[int]]) -> Tuple[np.ndarray, np.ndarray]:
-        """prepareInputIds (:446-553) on already-tokenised prompts."""
+    def prepare_input_ids(prompt_token_ids: Sequence[Sequence[int]], ref_code_list: Optional[Sequence[int]] = None,
+                          ref_text_ids: Optional[Sequence[int]] = None) -> Tuple[np.ndarray, np.ndarray]:
+        """prepareInputIds (:446-553) on already-tokenised prompts.  With both `ref_code_list` (the 7-token interleaved codes
+        of a reference clip, `encode_audio_to_code_list`) and `ref_text_ids` (its tokenised transcript) every row gets the
+        voice-cloning reference block between its padding and its prompt; with either missing the prompts are framed alone."""
         B = len(prompt_token_ids)
         rows = [np.ascontiguousarray(p, dtype=np.int32) for p in prompt_token_ids]
         lens = np.asarray([len(r) for r in rows], dtype=np.int32)
         pp = (C.c_void_p * B)(*[r.ctypes.data for r in rows])
         n = C.c_int32(0)
-        _ffi.check(_ffi.lib().b2a_tts_prepare_input_ids(pp, _ffi.ptr(lens), B, None, C.byref(n)))
+        if ref_code_list is None or ref_text_ids is None:
+            fn, extra = _ffi.lib().b2a_tts_prepare_input_ids, ()
+        else:
+            rc = np.ascontiguousarray(ref_code_list, dtype=np.int32).reshape(-1)
+            rt = np.ascontiguousarray(ref_text_ids, dtype=np.int32).reshape(-1)
+            fn, extra = _ffi.lib().b2a_tts_prepare_input_ids_ref, (_ffi.ptr(rt), len(rt), _ffi.ptr(rc), len(rc))
+        _ffi.check(fn(pp, _ffi.ptr(lens), B, *extra, None, C.byref(n)))
         out = np.empty((B, n.value), dtype=np.int32)
-        _ffi.check(_ffi.lib().b2a_tts_prepare_input_ids(pp, _ffi.ptr(lens), B, _ffi.ptr(out), C.byref(n)))
+        _ffi.check(fn(pp, _ffi.ptr(lens), B, *extra, _ffi.ptr(out), C.byref(n)))
         return out, out != PAD_TOKEN
+
+    def encode_audio_to_code_list(self, audio) -> List[int]:
+        """llamaEncodeAudioToCodes (:72-98): a 1-D reference clip at 24 kHz -> SNAC codes on the device -> 7-token interleave."""
+        if self._snac_model is None:
+            raise _ffi.AudioGenerationError(_ffi.ERR_MODEL_NOT_INITIALIZED, "SNAC model not loaded")
+        codes = self._snac_model.encode(np.asarray(audio, dtype=np.float32).reshape(1, 1, -1))
+        return self.code_list_from_codes(codes)
+
+    def _prompt_ids(self, prompt_token_ids, ref_audio, ref_text_ids):
+        # cloning applies only when both the reference audio and its transcript are given (:456)
+        if ref_audio is not None and ref_text_ids is not None:
+            return self.prepare_input_ids([list(prompt_token_ids)], self.encode_audio_to_code_list(ref_audio), ref_text_ids)[0]
+        return self.prepare_input_ids([list(prompt_token_ids)])[0]
 
     @staticmethod
     def parse_output(input_ids) -> List[List[int]]:
@@ -222,11 +244,13 @@ class LlamaTTSModel:
         return AudioGenerationInfo(info.prompt_token_count, info.generation_token_count, info.prefill_time,
                                    info.generate_time, info.tokens_per_second, info.peak_memory_gb, info.codec_time)
 
-    def generate(self, prompt_token_ids: Sequence[int], parameters: Optional[GenerateParameters] = None) -> np.ndarray:
-        """generate(text:voice:...) (:658-765) for ONE utterance, after tokenisation: returns the 1-D waveform."""
+    def generate(self, prompt_token_ids: Sequence[int], parameters: Optional[GenerateParameters] = None, ref_audio=None,
+                 ref_text_ids: Optional[Sequence[int]] = None) -> np.ndarray:
+        """generate(text:voice:refAudio:refText:...) (:658-765) for ONE utterance, after tokenisation: returns the 1-D waveform.
+        `ref_audio` (1-D, 24 kHz) with `ref_text_ids` clones the reference voice (prepareInputIds, :446-553)."""
         if self._snac_model is None:
             raise _ffi.AudioGenerationError(_ffi.ERR_MODEL_NOT_INITIALIZED, "SNAC model not loaded")
-        ids, _ = self.prepare_input_ids([list(prompt_token_ids)])
+        ids = self._prompt_ids(prompt_token_ids, ref_audio, ref_text_ids)
         _, waves, _ = self.generate_batch(ids, parameters)
         return waves[0]
 
@@ -260,14 +284,16 @@ class LlamaTTSModel:
         return [toks[b, :ntok[b]].tolist() for b in range(B)], chunks, gi
 
     def generate_stream(self, prompt_token_ids: Sequence[int], parameters: Optional[GenerateParameters] = None,
-                        streaming_interval: Optional[float] = None) -> Iterator:
+                        streaming_interval: Optional[float] = None, ref_audio=None,
+                        ref_text_ids: Optional[Sequence[int]] = None) -> Iterator:
         """generateStream (:777-913): yields ('token', id)..., ('info', AudioGenerationInfo), ('audio', waveform).  With
         streaming_interval = None the audio comes once, at the end, as the reference's Orpheus does (the protocol's default overload
         ignores the interval for such models, Generation.swift:119-137); with a float (seconds) ('audio', chunk) events are produced
-        every round(interval * 24000 / 2048) frames while tokens are still being generated (row N2)."""
+        every round(interval * 24000 / 2048) frames while tokens are still being generated (row N2).  `ref_audio` with
+        `ref_text_ids` clones the reference voice, as in generate."""
         if self._snac_model is None:
             raise _ffi.AudioGenerationError(_ffi.ERR_MODEL_NOT_INITIALIZED, "SNAC model not loaded")
-        ids, _ = self.prepare_input_ids([list(prompt_token_ids)])
+        ids = self._prompt_ids(prompt_token_ids, ref_audio, ref_text_ids)
         if streaming_interval is not None:
             events = []
             fpc = max(1, int(round(streaming_interval * 24000.0 / 2048.0)))
@@ -284,9 +310,10 @@ class LlamaTTSModel:
         yield ("audio", waves[0])
 
     def generate_samples_stream(self, prompt_token_ids: Sequence[int], parameters: Optional[GenerateParameters] = None,
-                                streaming_interval: Optional[float] = None) -> Iterator[np.ndarray]:
+                                streaming_interval: Optional[float] = None, ref_audio=None,
+                                ref_text_ids: Optional[Sequence[int]] = None) -> Iterator[np.ndarray]:
         """generateSamplesStream (Generation.swift:52-74): only the .audio events of generateStream, as sample arrays."""
-        for kind, value in self.generate_stream(prompt_token_ids, parameters, streaming_interval):
+        for kind, value in self.generate_stream(prompt_token_ids, parameters, streaming_interval, ref_audio, ref_text_ids):
             if kind == "audio" and value is not None:
                 yield value
 

@@ -1,5 +1,5 @@
 """Host-side mirror of `SNAC` (Sources/MLXAudioCodecs/SNAC/SNACDecoder.swift:12-204) behind the
-AudioCodecModel protocol (Sources/MLXAudioCodecs/AudioCodecModel.swift:4-27), over the C ABI."""
+AudioCodecModel protocol (encode and decode) (Sources/MLXAudioCodecs/AudioCodecModel.swift:4-27), over the C ABI."""
 from __future__ import annotations
 
 import ctypes as C
@@ -44,9 +44,11 @@ class SNAC:
     @staticmethod
     def random_init_weights(seed: int = 1234, latent: int = 768, decoder_dim: int = 1024,
                             decoder_rates: Sequence[int] = (8, 8, 4, 2), vq_strides: Sequence[int] = (4, 2, 1),
-                            codebook_size: int = 4096, codebook_dim: int = 8) -> Dict[str, np.ndarray]:
+                            codebook_size: int = 4096, codebook_dim: int = 8, encoder: bool = False, encoder_dim: int = 48,
+                            encoder_rates: Sequence[int] = (2, 4, 8, 8)) -> Dict[str, np.ndarray]:
         """Random-init snac_24khz-shaped weights (benchmarks): conv v ~ U(+-1/sqrt(fan_in)) as
-        Layers.swift:81-86, g = ||v||, zero biases, Snake alpha = 1."""
+        Layers.swift:81-86, g = ||v||, zero biases, Snake alpha = 1.  encoder=True appends the encoder's
+        weights (drawn after everything else, so the decoder / quantizer weights do not change)."""
         rng = np.random.default_rng(seed)
         w: Dict[str, np.ndarray] = {}
 
@@ -83,6 +85,21 @@ class SNAC:
         cf = decoder_dim // 2 ** len(decoder_rates)
         w[f"{p}.{li}.alpha"] = np.ones((1, cf, 1), dtype=np.float32)
         wn(f"{p}.{li + 1}", (1, 7, cf), cf * 7, 1)
+        if encoder:
+            p, d = "encoder.block.layers", encoder_dim
+            wn(f"{p}.0", (d, 7, 1), 7, d)
+            for i, s in enumerate(encoder_rates):
+                b = f"{p}.{i + 1}.block.layers"
+                for j in range(3):
+                    r = f"{b}.{j}.block.layers"
+                    w[f"{r}.0.alpha"] = np.ones((1, d, 1), dtype=np.float32)
+                    wn(f"{r}.1", (d, 7, 1), 7, d)
+                    w[f"{r}.2.alpha"] = np.ones((1, d, 1), dtype=np.float32)
+                    wn(f"{r}.3", (d, 1, d), d, d)
+                w[f"{b}.3.alpha"] = np.ones((1, d, 1), dtype=np.float32)
+                wn(f"{b}.4", (2 * d, 2 * s, d), 2 * s * d, 2 * d)
+                d *= 2
+            wn(f"{p}.{len(encoder_rates) + 1}", (d, 7, 1), 7, d)
         return w
 
     # -- loading (SNACDecoder.swift:135-189) ------------------------------------------------------
@@ -136,10 +153,31 @@ class SNAC:
     def decode_audio(self, codes):            # AudioDecoderModel.decodeAudio (:199)
         return self.decode(codes)
 
+    @staticmethod
+    def _check_dev(t, dtype: str, shape, what: str) -> None:
+        # the library reads / writes exactly these extents through raw device pointers: anything else is an input error, not a fault
+        import torch
+        ok = (isinstance(t, torch.Tensor) and t.is_cuda and t.dtype == getattr(torch, dtype) and t.is_contiguous()
+              and tuple(t.shape) == tuple(shape))
+        if not ok:
+            got = tuple(t.shape) if hasattr(t, "shape") else type(t).__name__
+            raise _ffi.AudioGenerationError(_ffi.ERR_INVALID_INPUT, f"{what}: expected a contiguous CUDA {dtype} tensor {tuple(shape)}, got {got}")
+
+    def _check_code_list(self, d_codes, B: int, T: int) -> None:
+        if len(d_codes) != self.n_codebooks:
+            raise _ffi.AudioGenerationError(_ffi.ERR_INVALID_INPUT, f"expected {self.n_codebooks} code layers")
+        for i, (c, s) in enumerate(zip(d_codes, self.vq_strides)):
+            self._check_dev(c, "int32", (B, T // s), f"code layer {i}")
+
     def decode_dev(self, d_codes, d_wave, zero_noise: bool = False, seed: int = 0, stream: int = 0) -> None:
         """Device-resident decode: torch CUDA int32 tensors [B, T_i] -> d_wave [B, 1, T*hop]."""
+        if len(d_codes) != self.n_codebooks or d_codes[0].dim() != 2:
+            raise _ffi.AudioGenerationError(_ffi.ERR_INVALID_INPUT, f"expected {self.n_codebooks} code layers [B, T_i]")
         B = d_codes[0].shape[0]
         T = d_codes[0].shape[1] * self.vq_strides[0]
+        self._check_code_list(d_codes, B, T)
+        n_out = B * T * self.hop_length          # any contiguous layout of [B, 1, T*hop], as before
+        self._check_dev(d_wave, "float32", tuple(d_wave.shape) if getattr(d_wave, "numel", lambda: -1)() == n_out else (B, 1, T * self.hop_length), "d_wave")
         cp = (C.c_void_p * len(d_codes))(*[c.data_ptr() for c in d_codes])
         _ffi.check(_ffi.lib().b2a_snac_decode_dev(self._h, cp, B, T, None, int(zero_noise), seed, _ffi.ptr(d_wave),
                                                   C.c_void_p(stream)))
@@ -153,6 +191,45 @@ class SNAC:
         zq = np.empty_like(z)
         _ffi.check(_ffi.lib().b2a_snac_quantize(self._h, _ffi.ptr(z), B, T, cp, _ffi.ptr(zq)))
         return zq, codes
+
+    def encoded_length(self, n_samples: int) -> int:
+        """Latent steps of an n-sample clip after preprocess's padding (SNACDecoder.swift:86-105); 0 without encoder weights."""
+        return int(_ffi.lib().b2a_snac_encoded_length(self._h, n_samples))
+
+    def encode(self, wave) -> List[np.ndarray]:
+        """SNAC.encode (:120-125): waveform [B, 1, n] (or [B, n]) float -> [codes_i [B, t_latent / stride_i] int32]."""
+        w = np.ascontiguousarray(wave, dtype=np.float32)
+        if w.ndim == 3:
+            if w.shape[1] != 1:
+                raise _ffi.AudioGenerationError(_ffi.ERR_INVALID_INPUT, "SNAC encodes mono audio [B, 1, n]")
+            w = w[:, 0]
+        if w.ndim != 2:
+            raise _ffi.AudioGenerationError(_ffi.ERR_INVALID_INPUT, "expected a waveform [B, 1, n]")
+        B, n = w.shape
+        w = np.ascontiguousarray(w)
+        T = self.encoded_length(n)
+        codes = [np.empty((B, T // s), dtype=np.int32) for s in self.vq_strides]
+        cp = (C.c_void_p * len(codes))(*[c.ctypes.data for c in codes])
+        _ffi.check(_ffi.lib().b2a_snac_encode(self._h, _ffi.ptr(w), B, n, cp))
+        return codes
+
+    def encode_audio(self, wave) -> List[np.ndarray]:        # AudioCodecModel.encodeAudio (:197-199)
+        return self.encode(wave)
+
+    def encode_dev(self, d_wave, d_codes, stream: int = 0) -> None:
+        """Device-resident encode: torch CUDA float32 d_wave [B, 1, n] (or [B, n]) -> int32 tensors d_codes[i]
+        [B, encoded_length(n) / stride_i], enqueued on `stream`."""
+        if d_wave.dim() not in (2, 3):
+            raise _ffi.AudioGenerationError(_ffi.ERR_INVALID_INPUT, "expected a waveform [B, 1, n]")
+        B, n = d_wave.shape[0], d_wave.shape[-1]
+        self._check_dev(d_wave, "float32", (B, 1, n) if d_wave.dim() == 3 else (B, n), "d_wave")
+        T = self.encoded_length(n)
+        if len(d_codes) != self.n_codebooks:
+            raise _ffi.AudioGenerationError(_ffi.ERR_INVALID_INPUT, f"expected {self.n_codebooks} code layers")
+        if T > 0:          # T == 0: no encoder weights or no samples -- the library reports which
+            self._check_code_list(d_codes, B, T)
+        cp = (C.c_void_p * len(d_codes))(*[c.data_ptr() for c in d_codes])
+        _ffi.check(_ffi.lib().b2a_snac_encode_dev(self._h, _ffi.ptr(d_wave), B, n, cp, C.c_void_p(stream)))
 
     def __del__(self):
         try:

@@ -4,7 +4,12 @@ tokenizer or checkpoint here).  The reference's Orpheus emits its audio once, at
 whole generation; with --stream (row N2, b2a_tts_generate_stream) audio chunks are decoded by SNAC while tokens are still being
 generated and TTFB is the latency of the first .audio event, as the CLI measures it (App.swift:155-170, streamingInterval 0.32 s).
 
-    python tools/tts_benchmark.py [--batch 1] [--prompt 64] [--max-tokens 512] [--model-dir DIR] [--stream] [--interval 0.32]"""
+With --ref-seconds S every row carries a voice-cloning reference block (prepareInputIds with refAudio / refText, LlamaTTS.swift:446-553):
+a synthetic S-second clip encoded by SNAC on the device and a 16-token stand-in transcript.  The encode runs before the timed call;
+prompts longer than 128 tokens take the token-by-token prefill.
+
+    python tools/tts_benchmark.py [--batch 1] [--prompt 64] [--max-tokens 512] [--model-dir DIR] [--stream] [--interval 0.32]
+                                  [--ref-seconds S]"""
 import argparse
 import sys
 import time
@@ -23,13 +28,28 @@ ap.add_argument("--max-tokens", type=int, default=512)
 ap.add_argument("--model-dir", default=None, help="checkpoint directory (config.json + *.safetensors); default: random init")
 ap.add_argument("--stream", action="store_true", help="chunked audio emission during generation (TTFB = first audio chunk)")
 ap.add_argument("--interval", type=float, default=0.32, help="streaming interval in seconds (App.swift:137)")
+ap.add_argument("--ref-seconds", type=float, default=0.0, help="voice-cloning prompt with a synthetic reference clip of S seconds")
 a = ap.parse_args()
-codec = m.SNAC(weights=m.SNAC.random_init_weights(1234))
+codec = m.SNAC(weights=m.SNAC.random_init_weights(1234, encoder=a.ref_seconds > 0))
+ref_len = 0
+if a.ref_seconds > 0:
+    n_ref = int(a.ref_seconds * 24000)
+    ref_len = 7 * codec.encoded_length(n_ref) // 4 + 16 + 9            # codes + transcript + the block's framing tokens
+ctx = a.prompt + ref_len + a.max_tokens + 16
 if a.model_dir:
-    tts = m.LlamaTTSModel.from_model_directory(a.model_dir, snac=codec, max_batch=a.batch, max_context=a.prompt + a.max_tokens + 16)
+    tts = m.LlamaTTSModel.from_model_directory(a.model_dir, snac=codec, max_batch=a.batch, max_context=ctx)
 else:
-    tts = m.LlamaTTSModel.random_init(ORPHEUS, snac=codec, max_batch=a.batch, max_context=a.prompt + a.max_tokens + 16)
+    tts = m.LlamaTTSModel.random_init(ORPHEUS, snac=codec, max_batch=a.batch, max_context=ctx)
 ids = make_prompts(0)[:a.batch, :a.prompt]
+if a.ref_seconds > 0:
+    t = np.arange(n_ref) / 24000.0
+    clip = (0.5 * np.sin(2 * np.pi * 220.0 * t) + 0.1 * np.random.default_rng(0).standard_normal(n_ref)).astype(np.float32)
+    ref_text = make_prompts(1)[0, 1:17].tolist()
+    # the untruncated make_prompts rows are [SOH] body [EOT, EOH, SOS]: a body of prompt - 4 tokens keeps the framed prompt at --prompt
+    body = [r[1:-3][:max(a.prompt - 4, 1)].tolist() for r in make_prompts(0)[:a.batch]]
+    ids, _ = tts.prepare_input_ids(body, tts.encode_audio_to_code_list(clip), ref_text)
+    ids = np.concatenate([ids, np.full((ids.shape[0], 1), 128257, dtype=np.int32)], axis=1)
+    print(f"Cloning prompt: {a.ref_seconds:g}s reference -> {ids.shape[1]} tokens per row")
 P = m.GenerateParameters(max_tokens=a.max_tokens, temperature=0.6, top_p=0.8, repetition_penalty=1.3, repetition_context_size=20,
                          mask_eos=True, wrap_codes=True)
 tts.generate_batch(ids, P)                       # warm-up (graph capture, allocations)
