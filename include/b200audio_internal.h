@@ -84,7 +84,7 @@ int32_t b2a_tc_gemm_splitk_test(const void* W, const void* X, float* h, const fl
  * DEVICE qkv [B * T, 3 * nh * 64] fp32; out [2 * 64 * cdiv(B * T, 64), nh * 64] bf16: token t = b * T + i at hi row
  * (t / 64) * 128 + t % 64, lo row = hi row + 64.  Rows of tokens >= B * T are not written.                                  */
 int32_t b2a_mha_tc_test(const float* qkv, void* out, int32_t B, int32_t T, int32_t nh, void* stream);
-/* tests/test_gpu_conv_gemm.py: one launch of the codec conv GEMM (cg::conv_gemm_kernel, csrc/conv_gemm.cuh, as snac.cu compiles it):
+/* tests/test_gpu_conv_gemm.py: one launch of the codec conv GEMM (cg::conv_gemm_kernel, csrc/conv_gemm.cu, through the launch SNAC and Vocos use):
  * acc[n, m] = W[m, :] . X[n, :] for the host fp32 weight w [M, K] (split into bf16 hi/lo like the engines' weights) and the DEVICE
  * activations X, 2 * pad64(N) rows of 64-token hi/lo tiles (hi rows, then lo rows) by K.  Then v = gamma * GELU(acc + bias) (each
  * optional) through epilogue epi: 0 E_STORE_HILO (Snake(alpha) of v as hi/lo into hl; dual: token b*T + t to row b*(T+1) + t,

@@ -1,5 +1,5 @@
-// Shared host-side plumbing for libb200audio: status codes, error text, launch counting,
-// device buffers.  sm_90a only; no CPU fallback anywhere.
+// Shared plumbing for libb200audio: status codes, error text, launch counting, device buffers, and the small device
+// helpers every engine uses (warp / block sums, range-reduced sin).  sm_90a only; no CPU fallback anywhere.
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -165,6 +165,33 @@ static inline void launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
 #ifdef __CUDACC__
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
+
+__device__ __forceinline__ float warp_sum(float v) {
+#pragma unroll
+    for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    return v;
+}
+// sum over a CTA of THREADS threads; red holds THREADS / 32 floats
+template <int THREADS>
+__device__ __forceinline__ float block_sum(float v, float* red) {
+    v = warp_sum(v);
+    __syncthreads();
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+    __syncthreads();
+    float t = 0.f;
+#pragma unroll
+    for (int i = 0; i < THREADS / 32; ++i) t += red[i];
+    return t;
+}
+
+// sin with an explicit two-term 2*pi range reduction + MUFU.SIN: |error| < 5e-7 for |x| < 1e4 (the libdevice sinf slow
+// path costs ~40 dependent instructions per call and made every Snake epilogue issue bound)
+__device__ __forceinline__ float fast_sin(float x) {
+    const float k = rintf(x * 0.15915494309189535f);
+    float r = fmaf(k, -6.28318548202514648f, x);
+    r = fmaf(k, 1.7484555e-7f, r);
+    return __sinf(r);
+}
 #endif
 
 }  // namespace b2a

@@ -8,7 +8,10 @@
 // bias, Snake, residual add, NoiseBlock, the transposed-conv phase scatter, and the hi/lo re-split that feeds the
 // next GEMM (optionally written twice, shifted by one token, which is the im2col the 2-tap transposed conv needs).
 #pragma once
+#include "common.cuh"
 #include "tc_gemm.cuh"
+
+#include <vector>
 
 namespace b2a {
 namespace cg {
@@ -56,23 +59,17 @@ struct Args {
     unsigned long long seed;
 };
 
-// sin with an explicit two-term 2*pi range reduction + MUFU.SIN: |error| < 5e-7 for |x| < 1e4 (the libdevice sinf slow
-// path costs ~40 dependent instructions per call and made every Snake epilogue issue bound)
-__device__ __forceinline__ float fast_sin(float x) {
-    const float k = rintf(x * 0.15915494309189535f);
-    float r = fmaf(k, -6.28318548202514648f, x);
-    r = fmaf(k, 1.7484555e-7f, r);
-    return __sinf(r);
-}
+// Snake (Layers.swift:44-50): v + 1/(alpha + 1e-9) * sin(alpha v)^2
 __device__ __forceinline__ float snake(float v, float al) {
     const float s = fast_sin(al * v);
     return v + (1.0f / (al + 1e-9f)) * s * s;
 }
-// same with the per-channel 1 / (alpha + 1e-9) computed once by the caller
+// same with the per-channel 1 / (alpha + 1e-9) computed once by the caller; the fma rounds differently from snake()
 __device__ __forceinline__ float snake_inv(float v, float al, float inv) {
     const float s = fast_sin(al * v);
     return fmaf(inv * s, s, v);
 }
+// counter-based N(0,1) for the NoiseBlock: splitmix64 -> two uniforms -> Box-Muller (MLXRandom.normal stand-in)
 __device__ __forceinline__ float gauss(unsigned long long seed, unsigned long long idx) {
     unsigned long long z = seed + 0x9E3779B97F4A7C15ull * (idx + 1);
     z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
@@ -82,12 +79,6 @@ __device__ __forceinline__ float gauss(unsigned long long seed, unsigned long lo
     const float u2 = (unsigned)((z >> 8) & 0xFFFFFF) * (1.0f / 16777216.0f);
     return sqrtf(-2.0f * logf(u1)) * cospif(2.0f * u2);
 }
-__device__ __forceinline__ void put_hilo(__nv_bfloat16* base, long long ld, long long tok, long long col, float v) {
-    const __nv_bfloat16 hi = __float2bfloat16_rn(v);
-    const long long r = (tok / HALF) * BN + (tok % HALF);
-    base[r * ld + col] = hi;
-    base[(r + HALF) * ld + col] = __float2bfloat16_rn(v - __bfloat162float(hi));
-}
 // Input of a strided conv (kernel 2 fs, stride fs, left pad fpad < fs) over utterances of T tokens (T % fs == 0) as a 2-tap GEMM
 // operand: the zero-padded sequence is cut into frames of fs tokens x C channels; output token q reads frames q and q + 1, so row
 // b (T / fs + 1) + q holds frame q in columns [0, fs C) and frame q + 1 in [fs C, 2 fs C) (row q = T / fs is computed and dropped).
@@ -95,156 +86,22 @@ __device__ __forceinline__ void put_hilo(__nv_bfloat16* base, long long ld, long
 __device__ __forceinline__ void put_frames(__nv_bfloat16* hl, int fs, int fpad, int C, int T, long long b, int t, int c, float v) {
     const int p = t + fpad, f = p / fs, col = (p - f * fs) * C + c;
     const long long ld = 2ll * fs * C, row = b * (T / fs + 1) + f;
-    put_hilo(hl, ld, row, col, v);
-    if (f > 0) put_hilo(hl, ld, row - 1, (long long)fs * C + col, v);
+    store_hilo(hl, ld, row, col, v, HALF);
+    if (f > 0) store_hilo(hl, ld, row - 1, (long long)fs * C + col, v, HALF);
 }
 
-static __global__ void __launch_bounds__(CG_THREADS, 1)
-conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmA2,
-                 const __grid_constant__ CUtensorMap tmB, Args a) {
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    float* sacc = reinterpret_cast<float*>(smem + (size_t)STAGES * STAGE);                     // [128][ACC_LD]
-    uint8_t* zero_w = reinterpret_cast<uint8_t*>(sacc + (size_t)BM * ACC_LD);                  // [64][64] bf16 zeros (1024-aligned)
-    uint64_t* full = reinterpret_cast<uint64_t*>(zero_w + ZERO_BYTES);
-    uint64_t* empty = full + STAGES;
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+// ----------------------------------------------------------------------------------------------- host (conv_gemm.cu)
+// fp32 weight matrix [M, K] as two bf16 K-major operands (hi + lo) with their TMA maps
+struct TcW {
+    DBuf<__nv_bfloat16> hi, lo;
+    CUtensorMap th{}, tl{};
+    int M = 0, K = 0;
+    void build(const std::vector<float>& W, int M_, int K_);
+};
 
-    if (threadIdx.x == 0) {
-        tma_prefetch_desc(&tmA); tma_prefetch_desc(&tmA2); tma_prefetch_desc(&tmB);
-        for (int i = 0; i < STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], EPI_WARPS); }
-        fence_barrier_init();
-    }
-    for (int i = threadIdx.x; i < ZERO_BYTES / 16; i += blockDim.x) reinterpret_cast<uint4*>(zero_w)[i] = make_uint4(0, 0, 0, 0);
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");       // generic-proxy stores -> visible to the tensor core
-    __syncthreads();
-    const long long tiles = (long long)a.n_tiles * a.m_tiles;   // tile id = n_tile * m_tiles + m_tile, dealt round-robin
-
-    if (warp == EPI_WARPS) {
-        if (lane == 0) {
-            int stage = 0; uint32_t phase = 0;
-            for (long long t = blockIdx.x; t < tiles; t += gridDim.x) {
-                const int nt = (int)(t / a.m_tiles), mt = (int)(t - (long long)nt * a.m_tiles);
-                for (int kb = 0; kb < a.k_blocks; ++kb) {
-                    mbar_wait(&empty[stage], phase ^ 1);
-                    uint8_t* s0 = smem + (size_t)stage * STAGE;
-                    mbar_arrive_expect_tx(&full[stage], STAGE);
-                    tma_load_2d(s0, &tmA, &full[stage], kb * BK, mt * BM);
-                    tma_load_2d(s0 + A_BYTES, &tmA2, &full[stage], kb * BK, mt * BM);
-                    tma_load_2d(s0 + 2 * A_BYTES, &tmB, &full[stage], kb * BK, nt * BN);
-                    if (++stage == STAGES) { stage = 0; phase ^= 1; }
-                }
-            }
-        }
-    } else {
-        const int q = warp & 3, c0 = (warp >> 2) * 16;
-        const int wg = warp >> 2, row_blk = wg & 1, col_blk = wg >> 1;   // this warpgroup's 64 x 64 block of the accumulator
-        const float* arow = sacc + (size_t)(q * 32 + lane) * ACC_LD;
-        const uint64_t zero_desc = make_smem_desc(smem_u32(zero_w));
-        int stage = 0; uint32_t phase = 0;
-        float acc[32];
-#pragma unroll
-        for (int i = 0; i < 32; ++i) acc[i] = 0.f;
-        // acc = Wh * X  over this block (+ Wl * Xh for the hi columns), k-blocks [kb0, kb1); then staged in sacc
-        auto mma_block = [&](int kb0, int kb1) {
-            for (int kb = kb0; kb < kb1; ++kb) {
-                mbar_wait(&full[stage], phase);
-                const uint32_t s0 = smem_u32(smem + (size_t)stage * STAGE);
-                const uint64_t ad = make_smem_desc(s0 + (uint32_t)(row_blk * 64 * 128)), a2d = col_blk == 0 ? make_smem_desc(s0 + A_BYTES + (uint32_t)(row_blk * 64 * 128)) : zero_desc;
-                const uint64_t bd = make_smem_desc(s0 + 2 * A_BYTES + (uint32_t)(col_blk * 64 * 128));
-                wg_fence();
-#pragma unroll
-                for (int k = 0; k < BK / UMMA_K; ++k) {
-                    const uint64_t off = (uint64_t)(2 * k);
-                    wgmma_bf16_n64(acc, ad + off, bd + off, (kb == kb0 && k == 0) ? 0u : 1u);     // Wh * [Xh; Xl]
-                    wgmma_bf16_n64(acc, a2d + (col_blk == 0 ? off : 0), bd + off, 1u);        // Wl * Xh -> columns [0, 64) (else + 0)
-                }
-                wg_commit();
-                wg_wait0();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&empty[stage]);
-                if (++stage == STAGES) { stage = 0; phase ^= 1; }
-            }
-            wg_fence_operand(acc);
-            named_sync(1, 32 * EPI_WARPS);                        // the previous epilogue has read sacc
-            store_frag<64>(sacc, ACC_LD, acc, row_blk * 64, col_blk * 64);
-            named_sync(1, 32 * EPI_WARPS);
-        };
-        const bool rmw = a.epi == E_NOISE || a.epi == E_ADD || a.epi == E_ADD_HILO;
-        for (long long t = blockIdx.x; t < tiles; t += gridDim.x) {
-            const int nt = (int)(t / a.m_tiles), mt = (int)(t - (long long)nt * a.m_tiles);
-            const int m = mt * BM + q * 32 + lane;
-            const bool m_ok = m < a.M;
-            float bias = 0.f, al = 0.f, gm = 1.f;
-            int co = m, r = 0;
-            if (a.epi == E_CONVT) { r = m / a.Cout; co = m - r * a.Cout; }
-            if (m_ok) {
-                if (a.bias) bias = a.bias[co];
-                if (a.alpha) al = a.alpha[m];
-                if (a.gamma) gm = a.gamma[m];
-            }
-            const float inv_al = 1.0f / (al + 1e-9f);
-            const long long n_first = (long long)nt * HALF + c0;
-            // everything that does not depend on the accumulator is fetched BEFORE waiting for the MMA: the residual /
-            // read-modify-write operand (16 independent loads) and the NoiseBlock noise (one value per token: lane j computes
-            // or loads token j, broadcast by shuffle below)
-            float xv[16];
-            if (rmw) {
-#pragma unroll
-                for (int j = 0; j < 16; ++j) xv[j] = (m_ok && n_first + j < a.N) ? a.x[(n_first + j) * a.ldx + m] : 0.f;
-            }
-            float nz_lane = 0.f;
-            if (a.epi == E_NOISE) {
-                const long long n = n_first + (lane & 15);
-                if (n < a.N) nz_lane = a.noise ? a.noise[n] : gauss(a.seed, (unsigned long long)n);
-            }
-            mma_block(0, a.k_blocks);
-            float v[16], w[16];
-            ld_acc16(arow + c0, v);
-            ld_acc16(arow + c0 + HALF, w);
-#pragma unroll
-            for (int j = 0; j < 16; ++j) {
-                const long long n = n_first + j;      // token (row of X)
-                const float nz = a.epi == E_NOISE ? __shfl_sync(0xffffffffu, nz_lane, j) : 0.f;
-                if (n >= a.N || !m_ok) continue;
-                float val = v[j] + w[j] + bias;
-                if (a.gelu) val = 0.5f * val * (1.0f + erff(val * 0.70710678118654752f));
-                val *= gm;
-                if (a.epi == E_STORE_F32) { a.x[n * a.ldx + m] = val; continue; }
-                if (a.epi == E_CONVT) {
-                    const int b = (int)(n / (a.Tin + 1)), qq = (int)(n - (long long)b * (a.Tin + 1));
-                    const int to = qq * a.stride + r - a.pad;
-                    if (to < 0 || to >= a.T) continue;
-                    const long long tok = (long long)b * a.T + to;
-                    a.x[tok * a.ldx + co] = val;
-                    if (a.hl) put_hilo(a.hl, a.ldh, tok, co, val);
-                    continue;
-                }
-                if (a.epi == E_NOISE) {
-                    a.x[n * a.ldx + m] = xv[j] + nz * val;
-                    continue;
-                }
-                if (rmw) {
-                    val += xv[j];
-                    a.x[n * a.ldx + m] = val;
-                    if (a.epi == E_ADD) continue;
-                }
-                if (a.alpha) val = snake_inv(val, al, inv_al);
-                if (a.fs) {
-                    const long long b = n / a.T;
-                    put_frames(a.hl, a.fs, a.fpad, a.M, a.T, b, (int)(n - b * a.T), m, val);
-                } else if (a.dual) {
-                    const long long b = n / a.T, tt = n - b * a.T;
-                    const long long row = b * (a.T + 1) + tt;
-                    put_hilo(a.hl, a.ldh, row, m, val);
-                    put_hilo(a.hl, a.ldh, row + 1, a.M + m, val);
-                } else {
-                    put_hilo(a.hl, a.ldh, n, m, val);
-                }
-            }
-        }
-    }
-}
+// D = W * X^T with the epilogue `a` (a.M, a.K and the tile counts are set here): X is the hi/lo activation matrix of x_rows rows
+// and W.K columns; min(max_ctas, work items) persistent CTAs
+void launch(const TcW& W, const __nv_bfloat16* X, long long x_rows, Args a, long long max_ctas, cudaStream_t s);
 
 }  // namespace cg
 }  // namespace b2a

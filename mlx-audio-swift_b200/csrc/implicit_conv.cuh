@@ -17,6 +17,7 @@
 // kernel, the taps run over input frames q - (n - 1) .. q, and the epilogue writes output frame q * stride + rho
 // ("pixel shuffle"); the reference's trim of (k - stride) frames on the right falls out of the causal form.
 #pragma once
+#include "common.cuh"
 #include "tc_gemm.cuh"
 
 #include <cuda_fp16.h>
@@ -69,13 +70,6 @@ __device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* map, u
         "cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
         ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
         : "memory");
-}
-// sin with a two-term 2*pi range reduction + MUFU.SIN (see conv_gemm.cuh)
-__device__ __forceinline__ float fast_sin(float x) {
-    const float k = rintf(x * 0.15915494309189535f);
-    float r = fmaf(k, -6.28318548202514648f, x);
-    r = fmaf(k, 1.7484555e-7f, r);
-    return __sinf(r);
 }
 // v -> hi + lo in the operand format, stored as raw 16-bit words at idx and plane + idx
 __device__ __forceinline__ void put_hilo16(uint16_t* base, long long plane, long long idx, float v, int f16) {

@@ -43,12 +43,6 @@ __device__ __forceinline__ uint4 ldg_stream(const uint4* p) {
     return r;
 }
 
-__device__ __forceinline__ float warp_sum(float v) {
-#pragma unroll
-    for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
-}
-
 // ------------------------------------------------------------------------------------------------
 // embed + RMSNorm
 // ------------------------------------------------------------------------------------------------
@@ -91,15 +85,6 @@ __global__ void finalize_norm_kernel(const float* __restrict__ x, const float* _
 }
 
 constexpr int LO_ROW = 8;   // activation matrices are [16, K] bf16: row b = hi(x_b), row 8 + b = lo(x_b) = bf16(x_b - hi)
-
-// token t of a [tokens, K] activation matrix lives in rows  hi = (t / half) * 2 * half + t % half,  lo = hi + half
-// (half = 8 for the decode step's [16, K] matrices, 64 for the prefill's 128-row TMA tiles)
-__device__ __forceinline__ void store_hilo(bf16* base, long long ld, int t, long long i, float v, int half = LO_ROW) {
-    const bf16 hi = __float2bfloat16_rn(v);
-    const long long r = (long long)(t / half) * 2 * half + (t % half);
-    base[r * ld + i] = hi;
-    base[(r + half) * ld + i] = __float2bfloat16_rn(v - __bfloat162float(hi));
-}
 
 // x += delta (optional, delta is zeroed afterwards);  xn = hi/lo split of  x * rsqrt(mean(x^2) + eps) * w
 // One 1024-thread CTA per row, the row lives in registers (H <= 8192).  Also zeroes `zero_ptr[b, :zero_n]`
@@ -144,7 +129,7 @@ add_rmsnorm_kernel(float* __restrict__ x, float* __restrict__ delta, const float
         const int i = tid + j * RN_THREADS;
         if (i < H) {
             const float o = v[j] * r * w[i];
-            store_hilo(xn, H, b, i, o, half);
+            tc::store_hilo(xn, H, b, i, o, half);
             if (normed) normed[(long long)b * H + i] = o;     // the fp32 normalised row (the talker's hidden state, row N1)
         }
     }
@@ -231,7 +216,7 @@ gemv_bf16_kernel(const bf16* __restrict__ W, const bf16* __restrict__ xin, float
 #pragma unroll
                     for (int b = 0; b < NB; ++b) {
                         const float g = acc[r][b], u = acc[r + 1][b];
-                        store_hilo(act, N / 2, b, (row0 + r) / 2, g / (1.0f + __expf(-g)) * u);
+                        tc::store_hilo(act, N / 2, b, (row0 + r) / 2, g / (1.0f + __expf(-g)) * u, LO_ROW);
                     }
         }
     }
@@ -475,7 +460,7 @@ attn_decode_cluster_kernel(const __grid_constant__ AttnArgs a, int NB) {
             const float M = fmaxf(Ms[g], M1);
             const float w0 = Ms[g] == -INFINITY ? 0.f : __expf(Ms[g] - M), w1 = M1 == -INFINITY ? 0.f : __expf(M1 - M);
             const float L = Ls[g] * w0 + L1 * w1, O = Os[g] * w0 + O1 * w1;
-            store_hilo(a.out, (long long)a.nq * HD, b, (h * G + g) * HD + tid, O / L);
+            tc::store_hilo(a.out, (long long)a.nq * HD, b, (h * G + g) * HD + tid, O / L, LO_ROW);
         }
     }
 }
@@ -604,10 +589,10 @@ prefill_attn_kernel(PrefillAttnArgs a) {
         const int tok = b * a.L + qpos;
         const long long col = (long long)(h * G + g) * HD + lane * 4;
         const long long ldo = (long long)a.nq * HD;
-        store_hilo(a.out, ldo, tok, col + 0, o.x * inv, PF_HALF);
-        store_hilo(a.out, ldo, tok, col + 1, o.y * inv, PF_HALF);
-        store_hilo(a.out, ldo, tok, col + 2, o.z * inv, PF_HALF);
-        store_hilo(a.out, ldo, tok, col + 3, o.w * inv, PF_HALF);
+        tc::store_hilo(a.out, ldo, tok, col + 0, o.x * inv, PF_HALF);
+        tc::store_hilo(a.out, ldo, tok, col + 1, o.y * inv, PF_HALF);
+        tc::store_hilo(a.out, ldo, tok, col + 2, o.z * inv, PF_HALF);
+        tc::store_hilo(a.out, ldo, tok, col + 3, o.w * inv, PF_HALF);
     }
 }
 
@@ -645,26 +630,6 @@ struct SampleArgs {
     unsigned long long seed;
     int mask_eos;
 };
-
-__device__ __forceinline__ float block_sum_1024(float v, float* sred) {
-    v = warp_sum(v);
-    __syncthreads();
-    if ((threadIdx.x & 31) == 0) sred[threadIdx.x >> 5] = v;
-    __syncthreads();
-    float t = 0.f;
-#pragma unroll
-    for (int i = 0; i < SM_WARPS; ++i) t += sred[i];
-    return t;
-}
-
-__device__ __forceinline__ float uniform01(unsigned long long seed, unsigned long long a, unsigned long long b,
-                                           unsigned long long c) {
-    unsigned long long z = seed + 0x9E3779B97F4A7C15ull * (a * 1000003ull + b * 131ull + c + 1ull);
-    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
-    z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
-    z ^= z >> 31;
-    return (float)(z >> 40) * (1.0f / 16777216.0f);
-}
 
 // Logits processors + sampler (deterministic for a given seed, no atomics):
 //   RepetitionContext.process -> EOS mask (bench only) -> argmax | TopPSampler.
@@ -2350,8 +2315,7 @@ struct b2a_qwen3_talker {
         {
             q3s::Args a = sampler_args(p, true, 0);
             a.tokens = codes.p; a.tokens_stride = G();
-            q3s::sample_kernel<<<B, q3s::THREADS, 0, s>>>(a);
-            count_launch();
+            q3s::launch(a, B, s);
         }
         // 2. code predictor: position 0 = the talker's hidden state, position 1 = codec_embed(c0) -> head 0 -> c1, then
         //    position k + 1 = predictor_embed_{k-1}(c_k) -> head k -> c_{k+1}
@@ -2365,8 +2329,7 @@ struct b2a_qwen3_talker {
             pred->run_head(tm_cp_head[k], cp_head[k].p, cfg.cp_vocab_size, pred->logits.p, B, s, cp_head_rows);
             q3s::Args a = sampler_args(p, false, k + 1);
             a.tokens = codes.p + (k + 1); a.tokens_stride = G();
-            q3s::sample_kernel<<<B, q3s::THREADS, 0, s>>>(a);
-            count_launch();
+            q3s::launch(a, B, s);
         }
         // 3. feedback + bookkeeping
         Q3Feedback f{codec_emb.p, cfg.vocab_size, cp_emb_ptrs.p, cfg.cp_vocab_size, codes.p, trailing.p, n_trailing.p, nmax, pad.p, x_in.p,

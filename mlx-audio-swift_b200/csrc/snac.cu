@@ -25,25 +25,6 @@
 
 namespace b2a {
 
-__device__ __forceinline__ float snake_fi(float x, float alpha, float inv) {      // 1 / (alpha + 1e-9) hoisted by the caller
-    const float ax = alpha * x;
-    const float k = rintf(ax * 0.15915494309189535f);
-    float r = fmaf(k, -6.28318548202514648f, ax);
-    r = fmaf(k, 1.7484555e-7f, r);
-    const float s = __sinf(r);
-    return fmaf(inv * s, s, x);
-}
-__device__ __forceinline__ float snake_f(float x, float alpha) {
-    // Layers.swift:44-50: x + 1/(alpha + 1e-9) * sin(alpha*x)^2
-    // explicit 2*pi range reduction + MUFU.SIN (|error| < 5e-7): libdevice sinf is ~40 dependent instructions per call
-    const float ax = alpha * x;
-    const float k = rintf(ax * 0.15915494309189535f);
-    float r = fmaf(k, -6.28318548202514648f, ax);
-    r = fmaf(k, 1.7484555e-7f, r);
-    const float s = __sinf(r);
-    return x + (1.0f / (alpha + 1e-9f)) * s * s;
-}
-
 // ------------------------------------------------------------------------------------------------
 // RVQ lookup: z[b,c,t] (+)= bias_i[c] + sum_d Wout_i[c,d] * codebook_i[codes_i[b, t/s_i], d]
 // (VectorQuantize.decodeCode + outProj + repeat-interleave, VQ.swift:88-94,165-191)
@@ -98,7 +79,7 @@ dwconv7_kernel(const float* __restrict__ in, float* __restrict__ out, const floa
     for (int i = threadIdx.x; i < DW_TT + 2 * halo; i += DW_THREADS) {
         const int t = t0 + i - halo;
         float v = 0.f;
-        if (t >= 0 && t < T) { v = x[t]; if (alpha_in) v = snake_f(v, ai); }
+        if (t >= 0 && t < T) { v = x[t]; if (alpha_in) v = cg::snake(v, ai); }
         s[i] = v;
     }
     __syncthreads();
@@ -114,7 +95,7 @@ dwconv7_kernel(const float* __restrict__ in, float* __restrict__ out, const floa
         float acc = bv;
 #pragma unroll
         for (int k = 0; k < 7; ++k) acc = fmaf(wk[k], s[i + k * dil], acc);
-        y[t] = alpha_out ? snake_f(acc, ao) : acc;
+        y[t] = alpha_out ? cg::snake(acc, ao) : acc;
     }
 }
 
@@ -139,17 +120,6 @@ struct GemmArgs {
     unsigned long long seed;
     int noise_layer;
 };
-
-__device__ __forceinline__ float gauss_from_counter(unsigned long long seed, unsigned long long idx) {
-    // counter-based N(0,1): splitmix64 -> two uniforms -> Box-Muller (MLXRandom.normal stand-in)
-    unsigned long long z = seed + 0x9E3779B97F4A7C15ull * (idx + 1);
-    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
-    z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
-    z ^= z >> 31;
-    const float u1 = ((unsigned)(z >> 40) + 1.0f) * (1.0f / 16777217.0f);
-    const float u2 = (unsigned)((z >> 8) & 0xFFFFFF) * (1.0f / 16777216.0f);
-    return sqrtf(-2.0f * logf(u1)) * cospif(2.0f * u2);
-}
 
 template <int EPI>
 __global__ void __launch_bounds__(G_THREADS)
@@ -227,7 +197,7 @@ gemm_f32_kernel(GemmArgs g) {
                 const int t = n * g.stride + r - g.pad;
                 if (t < 0 || t >= g.Tout) continue;
                 if (g.bias) v += g.bias[co];
-                if (g.alpha_out) v = snake_f(v, g.alpha_out[co]);
+                if (g.alpha_out) v = cg::snake(v, g.alpha_out[co]);
                 g.Y[((long long)b * g.Cout + co) * g.Tout + t] = v;
             } else {
                 const long long o = ((long long)b * g.Cout + m) * g.Tout + n;
@@ -236,11 +206,11 @@ gemm_f32_kernel(GemmArgs g) {
                 if (EPI == EPI_NOISE) {
                     // NoiseBlock (Layers.swift:271-278): x + noise[b,0,t] * (W x)
                     const float nz = g.noise ? g.noise[(long long)b * g.Tout + n]
-                                             : gauss_from_counter(g.seed + 0x1000193ull * (g.noise_layer + 1),
-                                                                  (unsigned long long)b * g.Tout + n);
+                                             : cg::gauss(g.seed + 0x1000193ull * (g.noise_layer + 1),
+                                                         (unsigned long long)b * g.Tout + n);
                     v = g.res[o] + nz * v;
                 }
-                if (g.alpha_out) v = snake_f(v, g.alpha_out[m]);
+                if (g.alpha_out) v = cg::snake(v, g.alpha_out[m]);
                 g.Y[o] = v;
             }
         }
@@ -363,13 +333,6 @@ nearest_code_kernel(const float* __restrict__ en, const float* __restrict__ e2, 
 // Channels-last (NLC) tensor-core path: activations fp32 [B*T, C] plus bf16 hi/lo copies in 64-token tiles that
 // the conv GEMM (conv_gemm.cuh) reads through TMA.  The kernels below are the non-GEMM pieces.
 // ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void put_hilo_nlc(__nv_bfloat16* base, long long ld, long long tok, long long col, float v) {
-    const __nv_bfloat16 hi = __float2bfloat16_rn(v);
-    const long long r = (tok / 64) * 128 + (tok % 64);
-    base[r * ld + col] = hi;
-    base[(r + 64) * ld + col] = __float2bfloat16_rn(v - __bfloat162float(hi));
-}
-
 // z[b*T + t, c] = sum_i (bias_i[c] + Wout_i[c,:] . codebook_i[codes_i[b, t/s_i], :])      (VQ.swift:165-191)
 __global__ void rvq_lookup_nlc_kernel(RvqArgs a, float* __restrict__ out) {
     const long long tok = blockIdx.x;                  // b*T + t
@@ -418,8 +381,8 @@ dw7_nlc_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ out, con
                 v = *reinterpret_cast<const float4*>(xb + (long long)t * C + c0 + c);
                 if (alpha_in) {
                     const float4 al = *reinterpret_cast<const float4*>(alpha_in + c0 + c);
-                    v.x = snake_fi(v.x, al.x, 1.0f / (al.x + 1e-9f)); v.y = snake_fi(v.y, al.y, 1.0f / (al.y + 1e-9f));
-                    v.z = snake_fi(v.z, al.z, 1.0f / (al.z + 1e-9f)); v.w = snake_fi(v.w, al.w, 1.0f / (al.w + 1e-9f));
+                    v.x = cg::snake_inv(v.x, al.x, 1.0f / (al.x + 1e-9f)); v.y = cg::snake_inv(v.y, al.y, 1.0f / (al.y + 1e-9f));
+                    v.z = cg::snake_inv(v.z, al.z, 1.0f / (al.z + 1e-9f)); v.w = cg::snake_inv(v.w, al.w, 1.0f / (al.w + 1e-9f));
                 }
             }
             *reinterpret_cast<float4*>(dsm + (size_t)r * CT + c) = v;
@@ -431,7 +394,7 @@ dw7_nlc_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ out, con
             float v = 0.f;
             if (t >= 0 && t < T && c0 + c < C) {
                 v = xb[(long long)t * C + c0 + c];
-                if (alpha_in) v = snake_f(v, alpha_in[c0 + c]);
+                if (alpha_in) v = cg::snake(v, alpha_in[c0 + c]);
             }
             dsm[i] = v;
         }
@@ -455,7 +418,7 @@ dw7_nlc_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ out, con
             const float2 xv = *reinterpret_cast<const float2*>(dsm + (size_t)(tt + k * dil) * CT + c);
             va = fmaf(wa[k], xv.x, va); vb = fmaf(wb[k], xv.y, vb);
         }
-        if (alpha_out) { va = snake_fi(va, aoa, ioa); vb = snake_fi(vb, aob, iob); }
+        if (alpha_out) { va = cg::snake_inv(va, aoa, ioa); vb = cg::snake_inv(vb, aob, iob); }
         const long long tok = (long long)b * T + t;
         const long long r = (tok / 64) * 128 + (tok % 64);
         const __nv_bfloat162 hi = __floats2bfloat162_rn(va, vb);
@@ -563,7 +526,7 @@ final_nlc_kernel(const float* __restrict__ x, float* __restrict__ wave, const fl
             float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
             if (t >= 0 && t < T) {
                 v = *reinterpret_cast<const float4*>(xb + (long long)t * FN_MAXC + c);
-                v.x = snake_fi(v.x, al.x, iv.x); v.y = snake_fi(v.y, al.y, iv.y); v.z = snake_fi(v.z, al.z, iv.z); v.w = snake_fi(v.w, al.w, iv.w);
+                v.x = cg::snake_inv(v.x, al.x, iv.x); v.y = cg::snake_inv(v.y, al.y, iv.y); v.z = cg::snake_inv(v.z, al.z, iv.z); v.w = cg::snake_inv(v.w, al.w, iv.w);
             }
             *reinterpret_cast<float4*>(fsm + r * FN_MAXC + c) = v;
         }
@@ -618,25 +581,7 @@ struct ConvW {       // folded weights on the device
     bool has_bias = false;
 };
 
-// fp32 weight matrix [M, K] as two bf16 K-major operands (hi + lo) with their TMA maps
-struct TcW {
-    DBuf<__nv_bfloat16> hi, lo;
-    CUtensorMap th{}, tl{};
-    int M = 0, K = 0;
-    void build(const std::vector<float>& W, int M_, int K_) {
-        M = M_; K = K_;
-        std::vector<__nv_bfloat16> h((size_t)M * K), l((size_t)M * K);
-        for (size_t i = 0; i < h.size(); ++i) {
-            h[i] = __float2bfloat16_rn(W[i]);
-            l[i] = __float2bfloat16_rn(W[i] - __bfloat162float(h[i]));
-        }
-        hi.upload(h.data(), h.size());
-        lo.upload(l.data(), l.size());
-        B2A_CUDA(cudaDeviceSynchronize());
-        th = tc::make_tmap_bf16(hi.p, M, K, tc::BM);
-        tl = tc::make_tmap_bf16(lo.p, M, K, tc::BM);
-    }
-};
+using cg::TcW;
 
 struct ResUnit { DBuf<float> a0, a2; ConvW dw, pw; TcW pw_tc, pw_bd; int dil; };   // pw_bd: [W 0; 0 W] for the fused C = 64 kernel
 struct DecBlock {
@@ -858,7 +803,6 @@ struct b2a_snac {
         for (auto& B : blocks) shapes_ok = shapes_ok && B.cin % 64 == 0 && B.cout % 64 == 0;
         use_tc = shapes_ok && !(env && std::string(env) == "simt");
         if (use_tc) {
-            B2A_CUDA(cudaFuncSetAttribute(cg::conv_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cg::SMEM_BYTES));
             B2A_CUDA(cudaFuncSetAttribute(dw7_nlc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
             fused_attrs<64>(); fused_attrs<128>();
             B2A_CUDA(cudaFuncSetAttribute(rf::convt_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rf::convt_smem_bytes()));
@@ -898,7 +842,6 @@ struct b2a_snac {
             enc_stem.w.upload(w.data(), w.size());
             enc_stem.bias.upload(b.data(), b.size());
         }
-        B2A_CUDA(cudaFuncSetAttribute(cg::conv_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cg::SMEM_BYTES));
         B2A_CUDA(cudaFuncSetAttribute(dw7_nlc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
         fused_attrs<64>(); fused_attrs<128>();
         eblocks.resize(n);
@@ -951,16 +894,6 @@ struct b2a_snac {
     std::vector<std::vector<float>> host_ct, host_noise, host_pw;
 
     // ---- tensor-core / NLC decode --------------------------------------------------------------------------
-    void cgemm(const TcW& W, const __nv_bfloat16* X, long long x_rows, cg::Args a, cudaStream_t s) { launch_cgemm(W, X, x_rows, a, num_sms, s); }
-    // min(max_ctas, work items) CTAs (the engine passes the SM count)
-    static void launch_cgemm(const TcW& W, const __nv_bfloat16* X, long long x_rows, cg::Args a, long long max_ctas, cudaStream_t s) {
-        a.M = W.M; a.K = W.K;
-        a.m_tiles = cdiv(W.M, tc::BM); a.k_blocks = W.K / tc::BK; a.n_tiles = cdiv(a.N, cg::HALF);
-        const CUtensorMap tb = tc::make_tmap_bf16(X, x_rows, W.K, 128);
-        const long long tiles = (long long)a.n_tiles * a.m_tiles;
-        launch_pdl(cg::conv_gemm_kernel, dim3((unsigned)std::min<long long>(max_ctas, tiles)), dim3(cg::CG_THREADS), cg::SMEM_BYTES, s,
-                   W.th, W.tl, tb, a);
-    }
     void dw_nlc(const ConvW& W, const float* xin, __nv_bfloat16* out, const float* a_in, const float* a_out, int batch, int T, int C,
                 int dil, cudaStream_t s) {
         const int CT = std::min(C, 64);
@@ -1046,7 +979,7 @@ struct b2a_snac {
             cg::Args a{};
             a.N = (int)(batch * T); a.epi = cg::E_STORE_HILO; a.bias = pw0.has_bias ? pw0.bias.p : nullptr; a.alpha = blocks[0].alpha.p;
             a.hl = x2.p; a.ldh = 2 * C; a.dual = 1; a.T = (int)T;
-            cgemm(pw0_tc, hA.p, 2 * pad64((long long)batch * T), a, s);
+            cg::launch(pw0_tc, hA.p, 2 * pad64((long long)batch * T), a, num_sms, s);
         }
         long long t = T;
         for (size_t i = 0; i < blocks.size(); ++i) {
@@ -1065,7 +998,7 @@ struct b2a_snac {
                 a.x = xs.p; a.ldx = B.cout; a.hl = block_fused(B) ? nullptr : hA.p;     // the fused units read fp32 only
                 a.ldh = B.cout; a.T = (int)tout; a.Cout = B.cout; a.stride = B.stride;
                 a.pad = B.pad; a.Tin = (int)t;
-                cgemm(B.ct_tc, x2.p, 2 * pad64((long long)batch * (t + 1)), a, s);
+                cg::launch(B.ct_tc, x2.p, 2 * pad64((long long)batch * (t + 1)), a, num_sms, s);
             }
             const float* nz = d_noise_in ? d_noise_in[i] : nullptr;
             const bool fz = block_fused(B);
@@ -1101,7 +1034,7 @@ struct b2a_snac {
                 cg::Args a{};
                 a.N = (int)ntok; a.epi = cg::E_NOISE; a.x = xs.p; a.ldx = B.cout; a.noise = nz;
                 a.seed = seed + 0x1000193ull * (i + 1); a.T = (int)tout;
-                cgemm(B.noise_tc, hA.p, 2 * pad64(ntok), a, s);
+                cg::launch(B.noise_tc, hA.p, 2 * pad64(ntok), a, num_sms, s);
             }
             for (int u = 0; u < 3; ++u) {
                 ResUnit& R = B.ru[u];
@@ -1115,7 +1048,7 @@ struct b2a_snac {
                 } else {
                     a.epi = cg::E_ADD;
                 }
-                cgemm(R.pw_tc, hA.p, 2 * pad64(ntok), a, s);
+                cg::launch(R.pw_tc, hA.p, 2 * pad64(ntok), a, num_sms, s);
             }
             t = tout;
         }
@@ -1286,7 +1219,7 @@ struct b2a_snac {
                     a.N = (int)ntok; a.bias = R.pw.bias.p; a.x = xs.p; a.ldx = E.cp; a.T = (int)t;
                     if (u == 2) { a.epi = cg::E_ADD_HILO; a.alpha = E.alpha.p; a.hl = x2.p; a.fs = E.stride; a.fpad = E.pad; }
                     else a.epi = cg::E_ADD;
-                    cgemm(R.pw_tc, hA.p, 2 * pad64(ntok), a, s);
+                    cg::launch(R.pw_tc, hA.p, 2 * pad64(ntok), a, num_sms, s);
                 }
             }
             // after the units (it writes other positions of x2): a plain launch between the last fused unit and the strided conv's
@@ -1297,7 +1230,7 @@ struct b2a_snac {
                 cg::Args a{};
                 a.N = (int)(batch * (tout + 1)); a.epi = cg::E_CONVT; a.bias = E.down_b.bias.p;
                 a.x = xs.p; a.ldx = E.cp_out; a.T = (int)tout; a.Cout = E.cp_out; a.stride = 1; a.pad = 0; a.Tin = (int)tout;
-                cgemm(E.down, x2.p, 2 * pad64((long long)batch * (tout + 1)), a, s);
+                cg::launch(E.down, x2.p, 2 * pad64((long long)batch * (tout + 1)), a, num_sms, s);
             }
             t = tout;
         }
@@ -1513,7 +1446,6 @@ extern "C" int32_t b2a_conv_gemm_test(const float* w, int32_t M, int32_t K, cons
                                      T == Tin * stride),
                   B2A_ERR_INVALID_INPUT, "b2a_conv_gemm_test: cg::E_CONVT needs M = stride * Cout, N = B * (Tin + 1) and T = Tin * stride");
         require_device(0);
-        B2A_CUDA(cudaFuncSetAttribute(cg::conv_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cg::SMEM_BYTES));
         TcW W;
         W.build(std::vector<float>(w, w + (size_t)M * K), M, K);
         cg::Args a{};
@@ -1521,7 +1453,7 @@ extern "C" int32_t b2a_conv_gemm_test(const float* w, int32_t M, int32_t K, cons
         a.hl = (__nv_bfloat16*)hl; a.ldh = ldh; a.dual = dual; a.T = T; a.Cout = Cout; a.stride = stride; a.pad = pad; a.Tin = Tin;
         a.noise = noise; a.seed = seed;
         const cudaStream_t s = (cudaStream_t)stream;
-        b2a_snac::launch_cgemm(W, (const __nv_bfloat16*)X, 2 * b2a_snac::pad64(N), a, hook_ctas(ctas), s);
+        cg::launch(W, (const __nv_bfloat16*)X, 2 * b2a_snac::pad64(N), a, hook_ctas(ctas), s);
         B2A_CUDA(cudaGetLastError());
         B2A_CUDA(cudaStreamSynchronize(s));
     });

@@ -63,12 +63,6 @@ __device__ __forceinline__ uint32_t sw128(int row, int col) {
     return (uint32_t)(row * 128 + ((((col >> 3) ^ (row & 7)) << 4) | ((col & 7) << 1)));
 }
 
-// Snake with the per-channel 1 / (alpha + 1e-9) hoisted out of the element loops
-__device__ __forceinline__ float snake_pre(float v, float al, float inv) {
-    const float sn = cg::fast_sin(al * v);
-    return fmaf(inv * sn, sn, v);
-}
-
 // MODE_RU: DIL in {1, 3, 9}; MODE_NOISE: DIL = 0.  The input rows of the NEXT (tile, k-block) unit are prefetched into
 // registers (P float4 per thread) before the current unit's depthwise conv / MMA / epilogue, so their latency is hidden.
 template <int MODE, int DIL, int C>
@@ -142,8 +136,8 @@ ru_fused_kernel(const __grid_constant__ CUtensorMap tmWh, const __grid_constant_
             for (int p = 0; p < P; ++p) {
                 if (ld_r + p * 16 < ROWS) {
                     float4 v = R[p];
-                    v.x = snake_pre(v.x, al.x, iv.x); v.y = snake_pre(v.y, al.y, iv.y);
-                    v.z = snake_pre(v.z, al.z, iv.z); v.w = snake_pre(v.w, al.w, iv.w);
+                    v.x = cg::snake_inv(v.x, al.x, iv.x); v.y = cg::snake_inv(v.y, al.y, iv.y);
+                    v.z = cg::snake_inv(v.z, al.z, iv.z); v.w = cg::snake_inv(v.w, al.w, iv.w);
                     *reinterpret_cast<float4*>(S + (ld_r + p * 16) * BK + ld_c) = v;
                 }
             }
@@ -189,7 +183,7 @@ ru_fused_kernel(const __grid_constant__ CUtensorMap tmWh, const __grid_constant_
                     const float2 xv = *reinterpret_cast<const float2*>(Sp + (j + k * DIL) * BK);
                     va = fmaf(wa[k], xv.x, va); vb = fmaf(wb[k], xv.y, vb);
                 }
-                va = snake_pre(va, ama, ima); vb = snake_pre(vb, amb, imb);
+                va = cg::snake_inv(va, ama, ima); vb = cg::snake_inv(vb, amb, imb);
                 if (j >= nv) { va = 0.f; vb = 0.f; }
                 const __nv_bfloat162 hi = __floats2bfloat162_rn(va, vb);
                 const __nv_bfloat162 lo = __floats2bfloat162_rn(va - __low2float(hi), vb - __high2float(hi));
@@ -263,8 +257,8 @@ ru_fused_kernel(const __grid_constant__ CUtensorMap tmWh, const __grid_constant_
                             cg::put_frames(a.hl, a.fs, a.fpad, C, a.T, b, etok, ech, sv);
                         } else {
                             const long long row = (long long)b * (a.T + 1) + etok;
-                            cg::put_hilo(a.hl, 2 * C, row, ech, sv);
-                            cg::put_hilo(a.hl, 2 * C, row + 1, C + ech, sv);
+                            store_hilo(a.hl, 2 * C, row, ech, sv, cg::HALF);
+                            store_hilo(a.hl, 2 * C, row + 1, C + ech, sv, cg::HALF);
                         }
                     }
                 }
@@ -358,8 +352,8 @@ convt_fused_kernel(const __grid_constant__ CUtensorMap tmWh, const __grid_consta
             for (int p = 0; p < P; ++p) {
                 const int r = ld_r + p * 16;
                 float4 v = R[p];
-                v.x = snake_pre(v.x, al.x, iv.x); v.y = snake_pre(v.y, al.y, iv.y);
-                v.z = snake_pre(v.z, al.z, iv.z); v.w = snake_pre(v.w, al.w, iv.w);
+                v.x = cg::snake_inv(v.x, al.x, iv.x); v.y = cg::snake_inv(v.y, al.y, iv.y);
+                v.z = cg::snake_inv(v.z, al.z, iv.z); v.w = cg::snake_inv(v.w, al.w, iv.w);
                 const __nv_bfloat162 h0 = __floats2bfloat162_rn(v.x, v.y), h1 = __floats2bfloat162_rn(v.z, v.w);
                 const __nv_bfloat162 l0 = __floats2bfloat162_rn(v.x - __low2float(h0), v.y - __high2float(h0));
                 const __nv_bfloat162 l1 = __floats2bfloat162_rn(v.z - __low2float(h1), v.w - __high2float(h1));

@@ -29,48 +29,6 @@ namespace st {
 
 typedef __nv_bfloat16 bf16;
 
-// ----------------------------------------------------------------------------------------------- tensor maps
-static tc::EncodeTiledFn encode_fn() {
-    static tc::EncodeTiledFn fn = nullptr;
-    if (!fn) {
-        void* p = nullptr;
-        cudaDriverEntryPointQueryResult q;
-        B2A_CUDA(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q));
-        B2A_CHECK(p && q == cudaDriverEntryPointSuccess, B2A_ERR_CUDA, "cuTensorMapEncodeTiled is not available in this driver");
-        fn = (tc::EncodeTiledFn)p;
-    }
-    return fn;
-}
-
-// planar hi/lo activations [2][B][Ttot][C] bf16 -> rank-4 map {C, Ttot, B, 2}, box {64, 64, 1, 2}, 128-byte swizzle
-static CUtensorMap make_tmap_planes(const bf16* base, int C, long long Ttot, int B, int f16) {
-    B2A_CHECK(C % 8 == 0 && ((uintptr_t)base & 15) == 0 && Ttot >= 1 && B >= 1, B2A_ERR_INVALID_INPUT,
-              "TMA: activation planes must be 16-byte aligned with channels % 8 == 0");
-    CUtensorMap m;
-    const cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)Ttot, (cuuint64_t)B, 2};
-    const cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)Ttot * C * 2, (cuuint64_t)B * Ttot * C * 2};
-    const cuuint32_t box[4] = {(cuuint32_t)tc::BK, (cuuint32_t)ic::HALF, 1, 2};
-    const cuuint32_t estr[4] = {1, 1, 1, 1};
-    const CUresult r = encode_fn()(&m, f16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<bf16*>(base), dims, strides, box, estr,
-                                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    B2A_CHECK(r == CUDA_SUCCESS, B2A_ERR_CUDA, "cuTensorMapEncodeTiled (rank 4) failed (" + std::to_string((int)r) + ")");
-    return m;
-}
-
-// weights [rows, cols] 16-bit row-major, {64, 128} box, 128-byte swizzle (tc::make_tmap_bf16 with a selectable element type)
-static CUtensorMap make_tmap_w16(const void* base, long long rows, long long cols, int f16) {
-    B2A_CHECK(cols % 8 == 0 && ((uintptr_t)base & 15) == 0, B2A_ERR_INVALID_INPUT, "TMA: tensor must be 16-byte aligned with cols % 8 == 0");
-    CUtensorMap m;
-    const cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-    const cuuint64_t strides[1] = {(cuuint64_t)cols * 2};
-    const cuuint32_t box[2] = {(cuuint32_t)tc::BK, (cuuint32_t)tc::BM};
-    const cuuint32_t estr[2] = {1, 1};
-    const CUresult r = encode_fn()(&m, f16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr,
-                                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    B2A_CHECK(r == CUDA_SUCCESS, B2A_ERR_CUDA, "cuTensorMapEncodeTiled failed (" + std::to_string((int)r) + ")");
-    return m;
-}
 // host-side hi / lo split in the operand format, as raw 16-bit words
 static inline void split16(float v, int f16, uint16_t& hi, uint16_t& lo) {
     if (f16) {
@@ -89,22 +47,6 @@ static inline float join16(uint16_t hi, uint16_t lo, int f16) {
 }
 
 // ----------------------------------------------------------------------------------------------- SIMT kernels
-__device__ __forceinline__ float wsum(float v) {
-#pragma unroll
-    for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
-}
-template <int THREADS>
-__device__ __forceinline__ float block_sum(float v, float* red) {
-    v = wsum(v);
-    __syncthreads();
-    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
-    __syncthreads();
-    float t = 0.f;
-#pragma unroll
-    for (int i = 0; i < THREADS / 32; ++i) t += red[i];
-    return t;
-}
 __device__ __forceinline__ void put_planes(bf16* base, long long plane, long long idx, float v, int f16) {
     ic::put_hilo16(reinterpret_cast<uint16_t*>(base), plane, idx, v, f16);
 }
@@ -200,7 +142,7 @@ attn_kernel(const float* __restrict__ qkv, const float* __restrict__ Kc, const f
             s[u] = d0;
         }
 #pragma unroll
-        for (int u = 0; u < 4; ++u) s[u] = wsum(s[u]);
+        for (int u = 0; u < 4; ++u) s[u] = warp_sum(s[u]);
         float mx = m;
 #pragma unroll
         for (int u = 0; u < 4; ++u) if (p0 + u < nkeys) mx = fmaxf(mx, s[u]);
@@ -388,8 +330,8 @@ struct IW {                       // implicit-conv weight: [M][taps][cblocks * 6
         hi.upload(reinterpret_cast<const bf16*>(h.data()), h.size());
         lo.upload(reinterpret_cast<const bf16*>(l.data()), l.size());
         B2A_CUDA(cudaDeviceSynchronize());
-        th = make_tmap_w16(hi.p, M, (long long)K, f16);
-        tl = make_tmap_w16(lo.p, M, (long long)K, f16);
+        th = tc::make_tmap_bf16(hi.p, M, (long long)K, tc::BM, f16);
+        tl = tc::make_tmap_bf16(lo.p, M, (long long)K, tc::BM, f16);
     }
     void set_bias(const std::vector<float>& b) { bias.upload(b.data(), b.size()); has_bias = true; B2A_CUDA(cudaDeviceSynchronize()); }
 };
@@ -667,7 +609,7 @@ struct b2a_speech_tokenizer {
         a.f16 = use_f16;
         a.seg_kb = SEG_KB;
         a.wscale = use_f16 ? W.rscale.p : nullptr;
-        const CUtensorMap tb = make_tmap_planes(in, W.Cin, in_frames, a.B, use_f16);
+        const CUtensorMap tb = tc::make_tmap_planes(in, W.Cin, in_frames, a.B, ic::HALF, use_f16);
         const long long tiles = (long long)a.B * a.t_tiles * a.m_tiles;
         launch_pdl(a.f16 ? ic::implicit_conv_kernel<1> : ic::implicit_conv_kernel<0>, dim3((unsigned)std::min<long long>(num_sms, tiles)), dim3(ic::IC_THREADS), ic::SMEM_BYTES, s,
                    W.th, W.tl, tb, a);
@@ -976,7 +918,7 @@ int32_t b2a_implicit_conv_test(const float* w, int32_t M, int32_t taps, int32_t 
         if (xo) { dxo.upload(xo, no); a.xo = dxo.p; }
         if (hl_out) { dh.alloc(2 * nh); B2A_CUDA(cudaMemset(dh.p, 0, 2 * nh * sizeof(bf16))); a.hl = dh.p; }
         B2A_CUDA(cudaDeviceSynchronize());
-        const CUtensorMap tb = make_tmap_planes(dx.p, Cin, Ttot, B, fp16);
+        const CUtensorMap tb = tc::make_tmap_planes(dx.p, Cin, Ttot, B, ic::HALF, fp16);
         const long long tiles = (long long)B * a.t_tiles * a.m_tiles;
         launch_pdl(a.f16 ? ic::implicit_conv_kernel<1> : ic::implicit_conv_kernel<0>, dim3((unsigned)std::min<long long>(num_sms, tiles)), dim3(ic::IC_THREADS), ic::SMEM_BYTES, (cudaStream_t)0,
                    W.th, W.tl, tb, a);

@@ -7,6 +7,10 @@
 namespace b2a {
 namespace tc {
 
+typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
+                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
+                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+
 static EncodeTiledFn encode_fn() {
     static EncodeTiledFn fn = nullptr;
     if (!fn) {
@@ -19,14 +23,16 @@ static EncodeTiledFn encode_fn() {
     return fn;
 }
 
-CUtensorMap make_tmap_bf16(const void* base, long long rows, long long cols, int box_rows) {
+static CUtensorMapDataType type16(int f16) { return f16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16; }
+
+CUtensorMap make_tmap_bf16(const void* base, long long rows, long long cols, int box_rows, int f16) {
     B2A_CHECK(cols % 8 == 0 && ((uintptr_t)base & 15) == 0, B2A_ERR_INVALID_INPUT, "TMA: tensor must be 16-byte aligned with cols % 8 == 0");
     CUtensorMap m;
     const cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
     const cuuint64_t strides[1] = {(cuuint64_t)cols * 2};
     const cuuint32_t box[2] = {(cuuint32_t)BK, (cuuint32_t)box_rows};
     const cuuint32_t estr[2] = {1, 1};
-    const CUresult r = encode_fn()(&m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr,
+    const CUresult r = encode_fn()(&m, type16(f16), 2, const_cast<void*>(base), dims, strides, box, estr,
                                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     B2A_CHECK(r == CUDA_SUCCESS, B2A_ERR_CUDA, "cuTensorMapEncodeTiled failed (" + std::to_string((int)r) + ")");
@@ -45,6 +51,22 @@ CUtensorMap make_tmap_f16_3d(const void* base, long long d0, long long d1, long 
                                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     B2A_CHECK(r == CUDA_SUCCESS, B2A_ERR_CUDA, "cuTensorMapEncodeTiled (3-D fp16) failed (" + std::to_string((int)r) + ")");
+    return m;
+}
+
+// the operand of implicit_conv.cuh: one box is 64 channels of box_frames frames, hi plane then lo plane
+CUtensorMap make_tmap_planes(const void* base, int C, long long Ttot, int B, int box_frames, int f16) {
+    B2A_CHECK(C % 8 == 0 && ((uintptr_t)base & 15) == 0 && Ttot >= 1 && B >= 1, B2A_ERR_INVALID_INPUT,
+              "TMA: activation planes must be 16-byte aligned with channels % 8 == 0");
+    CUtensorMap m;
+    const cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)Ttot, (cuuint64_t)B, 2};
+    const cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)Ttot * C * 2, (cuuint64_t)B * Ttot * C * 2};
+    const cuuint32_t box[4] = {(cuuint32_t)BK, (cuuint32_t)box_frames, 1, 2};
+    const cuuint32_t estr[4] = {1, 1, 1, 1};
+    const CUresult r = encode_fn()(&m, type16(f16), 4, const_cast<void*>(base), dims, strides, box, estr,
+                                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    B2A_CHECK(r == CUDA_SUCCESS, B2A_ERR_CUDA, "cuTensorMapEncodeTiled (rank 4) failed (" + std::to_string((int)r) + ")");
     return m;
 }
 

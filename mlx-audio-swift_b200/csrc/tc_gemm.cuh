@@ -202,6 +202,17 @@ __device__ __forceinline__ void ld_acc16(const float* p, float* v) {
 }
 __device__ __forceinline__ void named_sync(int id, int threads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory"); }
 
+// Activation v of token t, column col, as the hi/lo pair the B operand is read in: hi = bf16(v) in row (t / half) * 2 half + t % half,
+// lo = bf16(v - hi) in the row `half` below (half = tokens per tile: 8 / 16 for the decode steps, 64 for 128-row tiles).  I is the
+// caller's token index type (int or long long): the division is done in it.
+template <class I>
+__device__ __forceinline__ void store_hilo(__nv_bfloat16* base, long long ld, I t, long long col, float v, int half) {
+    const __nv_bfloat16 hi = __float2bfloat16_rn(v);
+    const long long r = (long long)(t / half) * 2 * half + (t % half);
+    base[r * ld + col] = hi;
+    base[(r + half) * ld + col] = __float2bfloat16_rn(v - __bfloat162float(hi));
+}
+
 // Consumer warps per CTA (wgmma + epilogue), followed by one TMA producer warp.  The 128-column tile (prefill / Whisper encoder: 64
 // tokens as hi/lo pairs) is split over four warpgroups (two 64-row blocks x two 64-column halves) so that the epilogue, which adds,
 // activates and stores 128 x 128 values per tile, is spread over 16 warps; the narrow decode tiles need one warpgroup.
@@ -696,13 +707,11 @@ tc_gemm_splitk_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
 #endif  // B2A_TC_GEMM_IMPL
 
 // ----------------------------------------------------------------------------------------------- host
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-// 2-D bf16 row-major [rows, cols] tensor map with a {64, box_rows} box and 128-byte swizzle
-CUtensorMap make_tmap_bf16(const void* base, long long rows, long long cols, int box_rows);
+// 2-D bf16 (f16 != 0: fp16) row-major [rows, cols] tensor map with a {64, box_rows} box and 128-byte swizzle
+CUtensorMap make_tmap_bf16(const void* base, long long rows, long long cols, int box_rows, int f16 = 0);
 CUtensorMap make_tmap_f16_3d(const void* base, long long d0, long long d1, long long d2, int b0, int b1);
+// planar hi/lo activations [2][B][Ttot][C], bf16 (f16 != 0: fp16) -> rank-4 map {C, Ttot, B, 2}, box {64, box_frames, 1, 2}, 128-byte swizzle
+CUtensorMap make_tmap_planes(const void* base, int C, long long Ttot, int B, int box_frames, int f16);
 
 template <int BN>
 void launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const Args& a, int ctas, int n_tiles, cudaStream_t s);

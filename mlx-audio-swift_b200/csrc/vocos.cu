@@ -19,18 +19,6 @@ namespace vc {
 
 typedef __nv_bfloat16 bf16;
 
-__device__ __forceinline__ void put_hilo(bf16* base, long long ld, long long tok, long long col, float v) {
-    const bf16 hi = __float2bfloat16_rn(v);
-    const long long r = (tok / 64) * 128 + (tok % 64);
-    base[r * ld + col] = hi;
-    base[(r + 64) * ld + col] = __float2bfloat16_rn(v - __bfloat162float(hi));
-}
-__device__ __forceinline__ float wsum(float v) {
-#pragma unroll
-    for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
-}
-
 // k-tap im2col along time (zero padded, "same"): out row (b, t) = [x[t-k/2] | ... | x[t+k/2]] as hi/lo, Kp >= k*C
 __global__ void im2colk_kernel(const float* __restrict__ in, bf16* __restrict__ out, int L, int C, int k, int Kp) {
     const long long tok = blockIdx.x;
@@ -42,21 +30,8 @@ __global__ void im2colk_kernel(const float* __restrict__ in, bf16* __restrict__ 
             const int ti = t + kk - k / 2;
             if (ti >= 0 && ti < L) v = in[((long long)b * L + ti) * C + c];
         }
-        put_hilo(out, Kp, tok, i, v);
+        tc::store_hilo(out, Kp, tok, i, v, cg::HALF);
     }
-}
-
-// block reduce helpers for one row per CTA
-template <int THREADS>
-__device__ __forceinline__ float block_sum(float v, float* red) {
-    v = wsum(v);
-    __syncthreads();
-    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
-    __syncthreads();
-    float t = 0.f;
-#pragma unroll
-    for (int i = 0; i < THREADS / 32; ++i) t += red[i];
-    return t;
 }
 
 // (optional depthwise conv k over time) -> LayerNorm(eps) over channels.  One CTA per token, one thread per channel slot.
@@ -105,7 +80,7 @@ dw_layernorm_kernel(const float* __restrict__ x, const float* __restrict__ dw_w 
         if (c < C) {
             const float o = (v[j] - mean) * r * ln_w[c] + ln_b[c];
             if (out_f32) out_f32[tok * C + c] = o;
-            if (out_hl) put_hilo(out_hl, C, tok, c, o);
+            if (out_hl) tc::store_hilo(out_hl, C, tok, c, o, cg::HALF);
         }
     }
 }
@@ -135,7 +110,7 @@ __global__ void spec_kernel(const float* __restrict__ h, bf16* __restrict__ out,
             sincosf(h[tok * 2 * half + half + kq], &sn, &cs);
             v = mag * (i < half ? cs : sn);
         }
-        put_hilo(out, Kp, tok, i, v);
+        tc::store_hilo(out, Kp, tok, i, v, cg::HALF);
     }
 }
 
@@ -157,29 +132,9 @@ __global__ void ola_kernel(const float* __restrict__ frames /*[B*L, n_fft] alrea
     wave[(long long)b * out_len + tp] = ws != 0.f ? acc / ws : acc;
 }
 
-struct TcW {
-    DBuf<bf16> hi, lo;
-    DBuf<float> bias;
-    CUtensorMap th{}, tl{};
-    int M = 0, K = 0;
-    bool has_bias = false;
-    void build(const std::vector<float>& W, int M_, int K_) {
-        M = M_; K = K_;
-        std::vector<bf16> h((size_t)M * K), l((size_t)M * K);
-        for (size_t i = 0; i < h.size(); ++i) {
-            h[i] = __float2bfloat16_rn(W[i]);
-            l[i] = __float2bfloat16_rn(W[i] - __bfloat162float(h[i]));
-        }
-        hi.upload(h.data(), h.size());
-        lo.upload(l.data(), l.size());
-        B2A_CUDA(cudaDeviceSynchronize());
-        th = tc::make_tmap_bf16(hi.p, M, K, tc::BM);
-        tl = tc::make_tmap_bf16(lo.p, M, K, tc::BM);
-    }
-    void set_bias(const std::vector<float>& b) { bias.upload(b.data(), b.size()); has_bias = true; B2A_CUDA(cudaDeviceSynchronize()); }
-};
+using cg::TcW;
 
-struct Block { DBuf<float> dw_w, dw_b, ln_w, ln_b, gamma; TcW pw1, pw2; };
+struct Block { DBuf<float> dw_w, dw_b, ln_w, ln_b, gamma, pw1_b, pw2_b; TcW pw1, pw2; };
 
 }  // namespace vc
 }  // namespace b2a
@@ -193,6 +148,7 @@ struct b2a_vocos {
     cudaStream_t stream = nullptr;
     int num_sms = 132, kp_embed = 0, kp_spec = 0;
     TcW embed, head, idft;
+    DBuf<float> embed_b, head_b;
     DBuf<float> n0_w, n0_b, nf_w, nf_b, win;
     DBuf<float> ada_w, ada_b, ada_out, cond;     // AdaLayerNorm: [2][1 + layers][dim][E] / [2][1 + layers][dim]; per-call [2][1 + layers][B][dim]
     std::vector<Block> blocks;
@@ -212,17 +168,16 @@ struct b2a_vocos {
         require_device(dev);
         B2A_CUDA(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
         B2A_CUDA(cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, device));
-        B2A_CUDA(cudaFuncSetAttribute(cg::conv_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cg::SMEM_BYTES));
         const int D = c.dim, I = c.intermediate_dim, Cin = c.input_channels, k = c.input_kernel_size, N = c.n_fft, half = N / 2 + 1;
+        auto up = [&](DBuf<float>& d, const std::string& name, int n) { std::vector<float> v = tt.f32(name, n); d.upload(v.data(), n); };
         // embed conv: MLX weight [out, k, in] is already [out, k*in + i]; pad K to a multiple of 64
         kp_embed = (int)pad64((long long)k * Cin);
         {
             std::vector<float> w = tt.f32("backbone.embed.weight", (int64_t)D * k * Cin), wp((size_t)D * kp_embed, 0.f);
             for (int o = 0; o < D; ++o) memcpy(&wp[(size_t)o * kp_embed], &w[(size_t)o * k * Cin], (size_t)k * Cin * sizeof(float));
             embed.build(wp, D, kp_embed);
-            embed.set_bias(tt.f32("backbone.embed.bias", D));
+            up(embed_b, "backbone.embed.bias", D);
         }
-        auto up = [&](DBuf<float>& d, const std::string& name, int n) { std::vector<float> v = tt.f32(name, n); d.upload(v.data(), n); };
         const int E = c.adanorm_num_embeddings, norms = 1 + c.num_layers;
         std::vector<float> aw, ab;
         if (E > 0) { aw.resize((size_t)2 * norms * D * E); ab.resize((size_t)2 * norms * D); }
@@ -245,13 +200,13 @@ struct b2a_vocos {
             up(B.dw_b, p + "dwconv.bias", D);
             if (E > 0) ada(1 + l, p + "norm.");
             else { up(B.ln_w, p + "norm.weight", D); up(B.ln_b, p + "norm.bias", D); }
-            B.pw1.build(tt.f32(p + "pwconv1.weight", (int64_t)I * D), I, D); B.pw1.set_bias(tt.f32(p + "pwconv1.bias", I));
-            B.pw2.build(tt.f32(p + "pwconv2.weight", (int64_t)D * I), D, I); B.pw2.set_bias(tt.f32(p + "pwconv2.bias", D));
+            B.pw1.build(tt.f32(p + "pwconv1.weight", (int64_t)I * D), I, D); up(B.pw1_b, p + "pwconv1.bias", I);
+            B.pw2.build(tt.f32(p + "pwconv2.weight", (int64_t)D * I), D, I); up(B.pw2_b, p + "pwconv2.bias", D);
             if (tt.find(p + "gamma")) up(B.gamma, p + "gamma", D);
         }
         if (E > 0) { ada_w.upload(aw.data(), aw.size()); ada_b.upload(ab.data(), ab.size()); B2A_CUDA(cudaDeviceSynchronize()); }
         head.build(tt.f32("head.out.weight", (int64_t)(N + 2) * D), N + 2, D);
-        head.set_bias(tt.f32("head.out.bias", N + 2));
+        up(head_b, "head.out.bias", N + 2);
         // windowed inverse real DFT as a matrix: frame[j] = w[j]/N * (Re0 + (-1)^j Re_{N/2} + 2 sum_k (Re_k cos - Im_k sin))
         kp_spec = (int)pad64(2 * half);
         {
@@ -268,16 +223,6 @@ struct b2a_vocos {
             win.upload(wv.data(), N);
         }
         B2A_CUDA(cudaDeviceSynchronize());
-    }
-
-    void cgemm(const TcW& W, const bf16* X, long long x_rows, cg::Args a, cudaStream_t s) {
-        a.M = W.M; a.K = W.K;
-        a.m_tiles = cdiv(W.M, tc::BM); a.k_blocks = W.K / tc::BK; a.n_tiles = cdiv(a.N, cg::HALF);
-        a.bias = W.has_bias ? W.bias.p : nullptr;
-        const CUtensorMap tb = tc::make_tmap_bf16(X, x_rows, W.K, 128);
-        const long long tiles = (long long)a.n_tiles * a.m_tiles;
-        launch_pdl(cg::conv_gemm_kernel, dim3((unsigned)std::min<long long>(num_sms, tiles)), dim3(cg::CG_THREADS), cg::SMEM_BYTES, s,
-                   W.th, W.tl, tb, a);
     }
 
     long long out_len(int L) const { return (long long)(L - 1) * cfg.hop_length; }
@@ -312,8 +257,8 @@ struct b2a_vocos {
         im2colk_kernel<<<(unsigned)T, 256, 0, s>>>(d_feats, xa.p, L, cfg.input_channels, cfg.input_kernel_size, kp_embed);
         count_launch();
         {
-            cg::Args a{}; a.N = (int)T; a.epi = cg::E_STORE_F32; a.x = spec.p; a.ldx = D;      // spec doubles as scratch [T, D]
-            cgemm(embed, xa.p, 2 * Tp, a, s);
+            cg::Args a{}; a.N = (int)T; a.epi = cg::E_STORE_F32; a.bias = embed_b.p; a.x = spec.p; a.ldx = D;      // spec doubles as scratch [T, D]
+            cg::launch(embed, xa.p, 2 * Tp, a, num_sms, s);
         }
         dw_layernorm_kernel<<<(unsigned)T, DL_THREADS, 0, s>>>(spec.p, nullptr, nullptr, g0, b0, h.p, nullptr, L, D, 1, 1e-6f, bs);
         count_launch();
@@ -323,22 +268,22 @@ struct b2a_vocos {
             dw_layernorm_kernel<<<(unsigned)T, DL_THREADS, 0, s>>>(h.p, Bk.dw_w.p, Bk.dw_b.p, gain(li, Bk.ln_w.p), shift(li, Bk.ln_b.p), nullptr, xa.p, L, D,
                                                                    cfg.dw_kernel_size, 1e-6f, bs);
             count_launch();
-            cg::Args a1{}; a1.N = (int)T; a1.epi = cg::E_STORE_HILO; a1.gelu = 1; a1.hl = xb.p; a1.ldh = I; a1.T = L;
-            cgemm(Bk.pw1, xa.p, 2 * Tp, a1, s);
-            cg::Args a2{}; a2.N = (int)T; a2.epi = cg::E_ADD; a2.x = h.p; a2.ldx = D; a2.gamma = Bk.gamma.p;      // h += gamma * pw2(...)
-            cgemm(Bk.pw2, xb.p, 2 * Tp, a2, s);
+            cg::Args a1{}; a1.N = (int)T; a1.epi = cg::E_STORE_HILO; a1.bias = Bk.pw1_b.p; a1.gelu = 1; a1.hl = xb.p; a1.ldh = I; a1.T = L;
+            cg::launch(Bk.pw1, xa.p, 2 * Tp, a1, num_sms, s);
+            cg::Args a2{}; a2.N = (int)T; a2.epi = cg::E_ADD; a2.bias = Bk.pw2_b.p; a2.x = h.p; a2.ldx = D; a2.gamma = Bk.gamma.p;      // h += gamma * pw2(...)
+            cg::launch(Bk.pw2, xb.p, 2 * Tp, a2, num_sms, s);
         }
         dw_layernorm_kernel<<<(unsigned)T, DL_THREADS, 0, s>>>(h.p, nullptr, nullptr, nf_w.p, nf_b.p, nullptr, xa.p, L, D, 1, 1e-6f);
         count_launch();
         {
-            cg::Args a{}; a.N = (int)T; a.epi = cg::E_STORE_F32; a.x = spec.p; a.ldx = N + 2;
-            cgemm(head, xa.p, 2 * Tp, a, s);
+            cg::Args a{}; a.N = (int)T; a.epi = cg::E_STORE_F32; a.bias = head_b.p; a.x = spec.p; a.ldx = N + 2;
+            cg::launch(head, xa.p, 2 * Tp, a, num_sms, s);
         }
         spec_kernel<<<(unsigned)T, 256, 0, s>>>(spec.p, xb.p, N / 2 + 1, kp_spec);
         count_launch();
         {
             cg::Args a{}; a.N = (int)T; a.epi = cg::E_STORE_F32; a.x = frames.p; a.ldx = N;
-            cgemm(idft, xb.p, 2 * Tp, a, s);
+            cg::launch(idft, xb.p, 2 * Tp, a, num_sms, s);
         }
         const int ol = (int)out_len(L);
         ola_kernel<<<dim3(cdiv(ol, 256), B), 256, 0, s>>>(frames.p, win.p, d_wave, L, N, cfg.hop_length, ol);

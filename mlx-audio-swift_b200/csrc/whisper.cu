@@ -29,19 +29,6 @@ constexpr int HD = 64;               // every Whisper size uses 64-dim heads
 constexpr int ENC_HALF = 64;         // tokens per 128-row tile (encoder / prompt side)
 constexpr int DEC_HALF = 16;         // decoder step: up to 16 rows as hi/lo in a 32-row tile
 
-__device__ __forceinline__ float wsum(float v) {
-#pragma unroll
-    for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
-}
-// token t -> hi row (t / half) * 2 * half + t % half, lo row = hi + half   (layout the TMA B-operand tiles expect)
-__device__ __forceinline__ void store_hilo(bf16* base, long long ld, long long t, long long i, float v, int half) {
-    const bf16 hi = __float2bfloat16_rn(v);
-    const long long r = (t / half) * 2 * half + (t % half);
-    base[r * ld + i] = hi;
-    base[(r + half) * ld + i] = __float2bfloat16_rn(v - __bfloat162float(hi));
-}
-
 // ------------------------------------------------------------------------------------------------
 // LayerNorm (eps 1e-5, biased variance) -> bf16 hi/lo.  Optionally first adds a table row
 // (encoder positional embedding, WhisperLayers.swift:150) into the residual stream.
@@ -69,7 +56,7 @@ layernorm_hilo_kernel(float* __restrict__ x, const float* __restrict__ w, const 
         v[j] = val;
         s += val;
     }
-    s = wsum(s);
+    s = warp_sum(s);
     if ((tid & 31) == 0) red[tid >> 5] = s;
     __syncthreads();
     float mean = 0.f;
@@ -83,7 +70,7 @@ layernorm_hilo_kernel(float* __restrict__ x, const float* __restrict__ w, const 
         const int i = tid + j * LN_THREADS;
         if (i < d) { const float c = v[j] - mean; q += c * c; }
     }
-    q = wsum(q);
+    q = warp_sum(q);
     if ((tid & 31) == 0) red[tid >> 5] = q;
     __syncthreads();
     float var = 0.f;
@@ -93,7 +80,7 @@ layernorm_hilo_kernel(float* __restrict__ x, const float* __restrict__ w, const 
 #pragma unroll
     for (int j = 0; j < LN_MAXV; ++j) {
         const int i = tid + j * LN_THREADS;
-        if (i < d) store_hilo(out, d, row, i, (v[j] - mean) * r * w[i] + b[i], half);
+        if (i < d) tc::store_hilo(out, d, row, i, (v[j] - mean) * r * w[i] + b[i], half);
     }
 }
 
@@ -124,7 +111,7 @@ layernorm_hilo_rows_kernel(float* __restrict__ x, const float* __restrict__ w, c
             s += (t.x + t.y) + (t.z + t.w);
         }
     }
-    s = wsum(s);
+    s = warp_sum(s);
     const float mean = s / (float)d;
     float q = 0.f;
 #pragma unroll
@@ -134,7 +121,7 @@ layernorm_hilo_rows_kernel(float* __restrict__ x, const float* __restrict__ w, c
             q += (c0 * c0 + c1 * c1) + (c2 * c2 + c3 * c3);
         }
     }
-    q = wsum(q);
+    q = warp_sum(q);
     const float r = rsqrtf(q / (float)d + 1e-5f);
     const long long orow = (row / half) * 2 * half + (row % half);
     uint2* oh = reinterpret_cast<uint2*>(out + orow * d);
@@ -173,7 +160,7 @@ __global__ void im2col3_kernel(const float* __restrict__ in, bf16* __restrict__ 
             const int ti = t * stride + k - 1;
             if (ti >= 0 && ti < Tin) v = in[((long long)b * Tin + ti) * C + c];
         }
-        store_hilo(out, Kp, tok, i, v, ENC_HALF);
+        tc::store_hilo(out, Kp, tok, i, v, ENC_HALF);
     }
 }
 
@@ -332,7 +319,7 @@ mha_decode_kernel(DecAttnArgs a) {
     __syncthreads();
     const float e = (key < nk && part == 0) ? __expf(sval - stat[0]) : 0.f;
     if (key < nk && part == 0) sc[key] = e;
-    const float es = wsum(e);
+    const float es = warp_sum(e);
     __syncthreads();
     if ((tid & 31) == 0) red[tid >> 5] = es;
     __syncthreads();
@@ -374,7 +361,7 @@ mha_decode_kernel(DecAttnArgs a) {
             L = fmaf(a.part_ml[(mb + j) * 2 + 1], wj, L);
             O = fmaf(a.part_o[(mb + j) * HD + tid], wj, O);
         }
-        store_hilo(a.out, a.d, b, h * HD + tid, O / L, DEC_HALF);
+        tc::store_hilo(a.out, a.d, (long long)b, h * HD + tid, O / L, DEC_HALF);
     }
     if (tid == 0) a.counters[b * a.nh + h] = 0;
 }

@@ -1,4 +1,4 @@
-"""The codec conv GEMM (cg::conv_gemm_kernel, csrc/conv_gemm.cuh) in isolation through b2a_conv_gemm_test, one case per engine
+"""The codec conv GEMM (cg::conv_gemm_kernel, csrc/conv_gemm.cu) in isolation through b2a_conv_gemm_test, one case per engine
 call site at that call site's shapes, against float64.
 
 The kernel multiplies the fp32 weight, split into bf16 hi + lo, by fp32 activations given as bf16 hi/lo tiles, and drops the
