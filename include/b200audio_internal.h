@@ -37,6 +37,11 @@ int32_t b2a_qwen3_talker_set_bench_flags(b2a_qwen3_talker* h, int32_t mask_eos);
  *   b2a_tts_debug_trace : enable != 0 makes later b2a_tts_forward_logits calls record the residual stream at every RMSNorm
  *       input; out (nullable) receives the record of the last traced position as [2*layers+1, batch, hidden] float32.        */
 int32_t b2a_tts_debug_trace(b2a_tts* h, int32_t enable, int32_t batch, float* out);
+/* Host-only (no device needed): dynamic shared-memory bytes per CTA of the fused decode step's kernels as the engine launches
+ * them -- out[0] the decode GEMM (tc_gemm_kernel<16>), out[1] the cluster split-K GEMM, out[2] the attention kernel for `gqa`
+ * q heads per kv head (1, 2, 3, 4, 6 or 8; its 512 static bytes are not included).  tests/test_gpu_step_coresidency.py checks
+ * that neighbouring kernels of the step fit on one SM together.                                                              */
+int32_t b2a_debug_step_smem(int32_t gqa, int32_t* out);
 
 /* Host-only (no device needed): the GEMM weight matrix the implicit convolution reads for an MLX-layout [out, k, in] weight --
  * stride 0: causal conv, rows = out, taps = k; stride > 0: transposed conv with k = n * stride, rows = stride * out

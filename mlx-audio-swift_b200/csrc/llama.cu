@@ -226,6 +226,14 @@ gemv_bf16_kernel(const bf16* __restrict__ W, const bf16* __restrict__ xin, float
 // Decode attention (LlamaTTS.swift:235-266): RoPE on q/k, append k/v to the fp32 cache, softmax(qK^T)V.
 // ------------------------------------------------------------------------------------------------
 constexpr int HD = 128, AT_THREADS = 256, MAXG = 8, AT_CAP = 64;   // AT_CAP * 4 == AT_THREADS
+constexpr int AT_SLOTS = 3;                                         // ring slots of attn_decode_cluster_kernel, one 64 x 128 fp32 matrix each
+// Dynamic shared memory of attn_decode_cluster_kernel<G>: the ring (96 KB), q, the new k | v row, the peer's merged state, barriers.
+// 102 528 bytes at G = 3 and 107 648 at G = 8 (plus 512 static): one CTA fits beside a decode GEMM CTA (121 088) or a split-K CTA
+// (109 056) on an SM.  The 8 warp-partial outputs ([8][G][128] fp32) are written over ring slot 0 once the last chunk is consumed.
+constexpr size_t attn_smem_bytes(int G) {
+    return ((size_t)AT_SLOTS * AT_CAP * HD + (size_t)G * HD + 2 * HD + (size_t)G * HD + 2 * MAXG) * sizeof(float) + 64;
+}
+static_assert((AT_THREADS / 32) * MAXG * HD <= AT_CAP * HD, "the warp-partial outputs must fit in one ring slot");
 
 struct AttnArgs {
     const float* qkv;      // [B, (nq + 2 nkv) * 128] fp32
@@ -244,26 +252,28 @@ struct AttnArgs {
 };
 
 // One thread-block cluster of two CTAs per (kv head, row), grid (kv heads, rows, 2).  Keys 0..pos are cut into 64-key chunks
-// (AT_CAP) that are dealt alternately to the two CTAs: CTA r takes chunks r, r + 2, ...  Each CTA streams its chunks through an
-// NB-deep ring of shared-memory buffers, one cp.async.bulk per matrix per chunk; the first NB are issued BEFORE
-// griddepcontrol.wait, so up to 2 x NB chunks (6 x 64 keys) stream in under the tail of the QKV GEMM.  Every warp keeps a running
+// (AT_CAP) that are dealt alternately to the two CTAs: CTA r takes chunks r, r + 2, ...  Each CTA streams the matrices of its chunks
+// in the order K_0, V_0, K_1, V_1, ... through a ring of AT_SLOTS one-matrix slots, one cp.async.bulk and one mbarrier per matrix:
+// the score pass waits for the K slot only, the P*V pass for the V slot, and a slot is refilled as soon as every warp has left it.
+// The first three (K_0, V_0, K_1) are issued BEFORE griddepcontrol.wait; the ring is kept to 96 KB so that this CTA can be resident,
+// and those copies in flight, while the QKV GEMM's CTA on the same SM is still in its main loop.  Every warp keeps a running
 // (max, sum, P*V) for its 8 keys of each chunk (online softmax) and the 8 warp states are merged once at the end.  CTA 1 hands its
 // merged state to CTA 0 through distributed shared memory: one cluster barrier, nothing goes through HBM.  `a` is __grid_constant__
 // for the reason given at tc_gemm_kernel.
 template <int G>
 __global__ void __cluster_dims__(1, 1, 2) __launch_bounds__(AT_THREADS)
-attn_decode_cluster_kernel(const __grid_constant__ AttnArgs a, int NB) {
+attn_decode_cluster_kernel(const __grid_constant__ AttnArgs a) {
     namespace cgr = cooperative_groups;
     cgr::cluster_group cluster = cgr::this_cluster();
     const int rank = (int)cluster.block_rank();
     extern __shared__ __align__(16) uint8_t at_smem[];
-    float* sKV = reinterpret_cast<float*>(at_smem);             // [NB][2][AT_CAP][128]  (K then V of each ring slot)
-    float* sq = sKV + (size_t)NB * 2 * AT_CAP * HD;             // [G][128]
+    float* sKV = reinterpret_cast<float*>(at_smem);             // [AT_SLOTS][AT_CAP][128]: matrix j of this CTA in slot j % AT_SLOTS
+    float* wpo = sKV;                                           // [8 warps][G][128] warp-partial outputs, over slot 0 after the loop
+    float* sq = sKV + (size_t)AT_SLOTS * AT_CAP * HD;           // [G][128]
     float* snew = sq + G * HD;                                  // [2][128] the new k / v row of this step
-    float* wpo = snew + 2 * HD;                                 // [8 warps][G][128] warp-partial outputs
-    float* xo = wpo + (AT_THREADS / 32) * G * HD;               // [G][128] + [2][G]: the peer CTA's merged state (written remotely)
+    float* xo = snew + 2 * HD;                                  // [G][128] + [2][G]: the peer CTA's merged state (written remotely)
     float* xml = xo + G * HD;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(xml + 2 * MAXG);   // [NB]
+    uint64_t* bars = reinterpret_cast<uint64_t*>(xml + 2 * MAXG);   // [AT_SLOTS]
     __shared__ float red_m[AT_THREADS / 32][MAXG], red_l[AT_THREADS / 32][MAXG];
 
     const int h = blockIdx.x, b = blockIdx.y, tid = threadIdx.x;
@@ -283,27 +293,27 @@ attn_decode_cluster_kernel(const __grid_constant__ AttnArgs a, int NB) {
     const float* row = a.qkv + (long long)b * qkv_ld;
     float* kc = a.kcache + (((long long)b * a.nkv + h) * a.max_ctx) * HD;
     float* vc = a.vcache + (((long long)b * a.nkv + h) * a.max_ctx) * HD;
-    // rows of chunk c already in the cache (the new position p is staged from this step's q|k|v instead)
-    auto issue = [&](int i) {
-        const int slot = i % NB, c = rank + 2 * i;
+    // matrix j of this CTA: K (j even) or V (j odd) of its chunk j / 2; the rows already in the cache are copied (the new position p
+    // is staged from this step's q|k|v instead)
+    const int n_mat = 2 * n_my;
+    auto issue = [&](int j) {
+        const int slot = j % AT_SLOTS, c = rank + 2 * (j >> 1);
         const int n_load = (c < nch - 1) ? AT_CAP : p - c * AT_CAP;
-        float* dK = sKV + (size_t)slot * 2 * AT_CAP * HD;
         if (n_load > 0) {
             const uint32_t bytes = (uint32_t)n_load * HD * 4;
-            tc::mbar_arrive_expect_tx(&bars[slot], 2 * bytes);
+            tc::mbar_arrive_expect_tx(&bars[slot], bytes);
             asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                         ::"r"(tc::smem_u32(dK)), "l"(kc + (long long)c * AT_CAP * HD), "r"(bytes), "r"(tc::smem_u32(&bars[slot])) : "memory");
-            asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                         ::"r"(tc::smem_u32(dK + AT_CAP * HD)), "l"(vc + (long long)c * AT_CAP * HD), "r"(bytes), "r"(tc::smem_u32(&bars[slot])) : "memory");
+                         ::"r"(tc::smem_u32(sKV + (size_t)slot * AT_CAP * HD)), "l"(((j & 1) ? vc : kc) + (long long)c * AT_CAP * HD), "r"(bytes),
+                           "r"(tc::smem_u32(&bars[slot])) : "memory");
         } else {
             tc::mbar_arrive(&bars[slot]);
         }
     };
     if (tid == 0) {
-        for (int i = 0; i < NB; ++i) tc::mbar_init(&bars[i], 1);
+        for (int i = 0; i < AT_SLOTS; ++i) tc::mbar_init(&bars[i], 1);
         tc::fence_barrier_init();
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        for (int i = 0; i < min(n_my, NB); ++i) issue(i);
+        for (int j = 0; j < min(n_mat, AT_SLOTS); ++j) issue(j);
     }
     float sn = 0.f, cs = 1.f;
     if (tid < HD / 2) sincosf((float)p / a.freqs[tid], &sn, &cs);   // MLXFast.RoPE(freqs:): angle = pos / freqs[i]
@@ -311,8 +321,8 @@ attn_decode_cluster_kernel(const __grid_constant__ AttnArgs a, int NB) {
     const float* qsrc = row + (long long)h * G * HD;            // this kv head's G query heads, contiguous
     const float* ksrc = row + (a.nq + h) * HD;
     if (a.qnorm) {
-        // per-head RMSNorm of q and k before RoPE: x * rsqrt(mean(x^2) + eps) * w, one warp per 128-vector, staged in the
-        // (not yet used) warp-partial output area
+        // per-head RMSNorm of q and k before RoPE: x * rsqrt(mean(x^2) + eps) * w, one warp per 128-vector, staged where RoPE will
+        // leave the rotated vector (sq, snew): the thread that rotates the pair (d, d + 64) reads both before it writes either
         for (int vec = tid >> 5; vec < G + 1; vec += AT_THREADS / 32) {
             const float* src = vec < G ? qsrc + vec * HD : ksrc;
             const float* w = vec < G ? a.qnorm : a.knorm;
@@ -320,11 +330,12 @@ attn_decode_cluster_kernel(const __grid_constant__ AttnArgs a, int NB) {
             const float ss = warp_sum(x.x * x.x + x.y * x.y + x.z * x.z + x.w * x.w);
             const float r = rsqrtf(ss * (1.0f / HD) + a.qk_eps);
             const float4 g4 = reinterpret_cast<const float4*>(w)[tid & 31];
-            reinterpret_cast<float4*>(wpo + vec * HD)[tid & 31] = make_float4(x.x * r * g4.x, x.y * r * g4.y, x.z * r * g4.z, x.w * r * g4.w);
+            reinterpret_cast<float4*>(vec < G ? sq + vec * HD : snew)[tid & 31] =
+                make_float4(x.x * r * g4.x, x.y * r * g4.y, x.z * r * g4.z, x.w * r * g4.w);
         }
         __syncthreads();
-        qsrc = wpo;
-        ksrc = wpo + G * HD;
+        qsrc = sq;
+        ksrc = snew;
     }
     if (tid < HD / 2) {  // non-traditional RoPE: pairs (i, i+64)
         const int d = tid;
@@ -355,14 +366,13 @@ attn_decode_cluster_kernel(const __grid_constant__ AttnArgs a, int NB) {
     _Pragma("unroll") for (int g = 0; g < G; ++g) { m_run[g] = -INFINITY; l_run[g] = 0.f; o4[g] = make_float4(0.f, 0.f, 0.f, 0.f); }
 
     for (int i = 0; i < n_my; ++i) {
-        const int slot = i % NB, c = rank + 2 * i;
-        float* sK = sKV + (size_t)slot * 2 * AT_CAP * HD;
-        float* sV = sK + AT_CAP * HD;
+        const int jk = 2 * i, jv = 2 * i + 1, c = rank + 2 * i;
+        float* sK = sKV + (size_t)(jk % AT_SLOTS) * AT_CAP * HD;
+        float* sV = sKV + (size_t)(jv % AT_SLOTS) * AT_CAP * HD;
         const int t0 = c * AT_CAP, nk = min(AT_CAP, p + 1 - t0);
-        tc::mbar_wait(&bars[slot], (uint32_t)((i / NB) & 1));    // bulk-copied K and V of this chunk have landed
+        tc::mbar_wait(&bars[jk % AT_SLOTS], (uint32_t)((jk / AT_SLOTS) & 1));    // the bulk-copied K rows of this chunk have landed
         if (c == nch - 1) {                                      // splice in the new position (the bulk copy stopped before it)
             if (tid < HD) sK[(p - t0) * HD + tid] = snew[tid];
-            else sV[(p - t0) * HD + tid - HD] = snew[tid];
             __syncthreads();
         }
         float sacc[G];
@@ -379,6 +389,10 @@ attn_decode_cluster_kernel(const __grid_constant__ AttnArgs a, int NB) {
                     sacc[g] = fmaf(qf.z, kf.z, sacc[g]); sacc[g] = fmaf(qf.w, kf.w, sacc[g]);
                 }
             }
+        }
+        if (jk + AT_SLOTS < n_mat) {
+            __syncthreads();                                     // every warp has left the K slot: the next chunk's V goes there
+            if (tid == 0) issue(jk + AT_SLOTS);
         }
         float pw[G];
         _Pragma("unroll") for (int g = 0; g < G; ++g) {
@@ -400,6 +414,11 @@ attn_decode_cluster_kernel(const __grid_constant__ AttnArgs a, int NB) {
             o4[g].x *= rescale; o4[g].y *= rescale; o4[g].z *= rescale; o4[g].w *= rescale;
             pw[g] = e;
         }
+        tc::mbar_wait(&bars[jv % AT_SLOTS], (uint32_t)((jv / AT_SLOTS) & 1));    // ... and its V rows
+        if (c == nch - 1) {
+            if (tid >= HD) sV[(p - t0) * HD + tid - HD] = snew[tid];
+            __syncthreads();
+        }
         // warp-partial P*V: lane owns dims 4*lane .. 4*lane+3 (conflict-free float4 reads of a V row)
 #pragma unroll
         for (int kk = 0; kk < 8; ++kk) {
@@ -413,11 +432,12 @@ attn_decode_cluster_kernel(const __grid_constant__ AttnArgs a, int NB) {
                 }
             }
         }
-        if (i + NB < n_my) {
-            __syncthreads();                                     // every warp is done with this slot
-            if (tid == 0) issue(i + NB);
+        if (jv + AT_SLOTS < n_mat) {
+            __syncthreads();                                     // every warp has left the V slot: the K after next goes there
+            if (tid == 0) issue(jv + AT_SLOTS);
         }
     }
+    __syncthreads();            // every copy has landed and every warp has left the ring: slot 0 now holds the warp-partial outputs
     // merge the 8 warp states
     _Pragma("unroll") for (int g = 0; g < G; ++g) {
         reinterpret_cast<float4*>(wpo + (warp * G + g) * HD)[lane] = o4[g];
@@ -933,6 +953,9 @@ struct b2a_tts {
     // residual add + the next norm's gain + hi/lo split + sum of squares; no stand-alone add_rmsnorm launches (tc_gemm.cuh)
     bool fused = false;
     static constexpr int fused_cluster = 5;   // 5 CTAs per 128-row tile: 120 of 132 SMs for hidden 3072, one wave
+    // ring depths of the decode step's GEMMs.  With them tc::Smem<16>::bytes, tc::SmemSplit::bytes and attn_smem_bytes() are sized so
+    // that any two kernels that follow each other in the fused step fit on one SM together (b2a_debug_step_smem reports the three)
+    static constexpr int gemm_stages = 6, splitk_stages = 5;
     int fused_parts = 0;
     DBuf<float> ss_a, ss_b;          // [H / 128, 8] partial sums of squares: ss_a feeds the post-attention norm, ss_b the input norm
     StackSpec spec;                  // which keys / features this stack was built with
@@ -974,28 +997,23 @@ struct b2a_tts {
         }
     }
 
-    // ring depth of attn_decode_cluster_kernel: as many 64-key K|V chunks as fit next to its other buffers, at most 3
-    int attn_loop_bufs() const {
-        const int G = cfg.num_attention_heads / cfg.num_key_value_heads;
-        const size_t extra = (size_t)(G * HD + 2 * HD + (AT_THREADS / 32) * G * HD + G * HD + 2 * MAXG) * sizeof(float) + 64;
-        return (int)std::min<size_t>(3, (226 * 1024 - extra) / ((size_t)2 * AT_CAP * HD * sizeof(float)));
-    }
     template <int G>
     static void attn_cluster_attr() {
-        B2A_CUDA(cudaFuncSetAttribute(attn_decode_cluster_kernel<G>, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));
+        B2A_CUDA(cudaFuncSetAttribute(attn_decode_cluster_kernel<G>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)attn_smem_bytes(G)));
+        // it shares an SM with a GEMM CTA of the step (see tc::set_attributes)
+        B2A_CUDA(cudaFuncSetAttribute(attn_decode_cluster_kernel<G>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
     }
     void attn_launch(const AttnArgs& aa, int B, cudaStream_t s) {
-        const int G = aa.nq / aa.nkv, NB = attn_loop_bufs();
-        const size_t sm = (size_t)NB * 2 * AT_CAP * HD * sizeof(float) +
-                          (size_t)(G * HD + 2 * HD + (AT_THREADS / 32) * G * HD + G * HD + 2 * MAXG) * sizeof(float) + 64;
+        const int G = aa.nq / aa.nkv;
+        const size_t sm = attn_smem_bytes(G);
         const dim3 g3(aa.nkv, B, 2);
         switch (G) {
-            case 1: launch_pdl(attn_decode_cluster_kernel<1>, g3, dim3(AT_THREADS), sm, s, aa, NB); break;
-            case 2: launch_pdl(attn_decode_cluster_kernel<2>, g3, dim3(AT_THREADS), sm, s, aa, NB); break;
-            case 3: launch_pdl(attn_decode_cluster_kernel<3>, g3, dim3(AT_THREADS), sm, s, aa, NB); break;
-            case 4: launch_pdl(attn_decode_cluster_kernel<4>, g3, dim3(AT_THREADS), sm, s, aa, NB); break;
-            case 6: launch_pdl(attn_decode_cluster_kernel<6>, g3, dim3(AT_THREADS), sm, s, aa, NB); break;
-            default: launch_pdl(attn_decode_cluster_kernel<8>, g3, dim3(AT_THREADS), sm, s, aa, NB); break;
+            case 1: launch_pdl(attn_decode_cluster_kernel<1>, g3, dim3(AT_THREADS), sm, s, aa); break;
+            case 2: launch_pdl(attn_decode_cluster_kernel<2>, g3, dim3(AT_THREADS), sm, s, aa); break;
+            case 3: launch_pdl(attn_decode_cluster_kernel<3>, g3, dim3(AT_THREADS), sm, s, aa); break;
+            case 4: launch_pdl(attn_decode_cluster_kernel<4>, g3, dim3(AT_THREADS), sm, s, aa); break;
+            case 6: launch_pdl(attn_decode_cluster_kernel<6>, g3, dim3(AT_THREADS), sm, s, aa); break;
+            default: launch_pdl(attn_decode_cluster_kernel<8>, g3, dim3(AT_THREADS), sm, s, aa); break;
         }
     }
 
@@ -1009,7 +1027,6 @@ struct b2a_tts {
             B2A_CHECK(g == 1 || g == 2 || g == 3 || g == 4 || g == 6 || g == 8, B2A_ERR_INVALID_INPUT,
                       "llama: unsupported GQA ratio (q heads per kv head must be 1, 2, 3, 4, 6 or 8)");
         }
-        B2A_CHECK(attn_loop_bufs() >= 1, B2A_ERR_INVALID_INPUT, "llama: GQA ratio too large for the attention tile");
         B2A_CHECK(c.max_batch >= 1 && c.max_batch <= 8, B2A_ERR_INVALID_INPUT, "llama: max_batch must be in 1..8");
         B2A_CHECK(c.max_context >= 8, B2A_ERR_INVALID_INPUT, "llama: max_context too small");
         require_device(device);
@@ -1238,8 +1255,7 @@ struct b2a_tts {
         a.rstd_ss = rstd_ss; a.rstd_parts = fused_parts; a.rstd_inv_h = 1.0f / (float)cfg.hidden_size; a.rstd_eps = cfg.rms_norm_eps;
         a.out_f32 = yout; a.out_bf16 = actout; a.M = M; a.N = B; a.K = K;
         a.m_tiles = cdiv(M, tc::BM); a.k_blocks = K / tc::BK;
-        a.stages = 6;   // 6 x 18 KB ring + 10 KB staged accumulator = 119 KB: one GEMM CTA per SM.  5 stages (101 KB) let the next
-                        // kernel's prefetching CTA co-reside, but measured slower on the H100 (Orpheus batch 8: 26.4x vs 28.3x real time)
+        a.stages = gemm_stages;
         a.hilo = 1;
         int ctas = num_sms;
         if (op == OP_GU) {
@@ -1289,7 +1305,7 @@ struct b2a_tts {
     // o_proj / down_proj as a cluster split-K GEMM with the residual add and the next norm fused into the leader's epilogue
     void splitk_gemm(const CUtensorMap& tmW, const CUtensorMap& tmX, int M, int K, const float* gain, float* ss, int B, cudaStream_t s) {
         tc::SplitArgs a{};
-        a.M = M; a.N = B; a.K = K; a.k_blocks = K / tc::BK; a.stages = 5;
+        a.M = M; a.N = B; a.K = K; a.k_blocks = K / tc::BK; a.stages = splitk_stages;
         a.h = x.p; a.gain = gain; a.xn = xn.p; a.ss = ss;
         a.rstd_ss = nullptr; a.rstd_parts = 0; a.rstd_inv_h = 0.f; a.rstd_eps = 0.f;
         tc::launch_splitk(tmW, tmX, a, cdiv(M, tc::BM), std::max(1, std::min(fused_cluster, a.k_blocks)), s);
@@ -1910,6 +1926,16 @@ int32_t b2a_tts_prepare_input_ids_ref(const int32_t* const* prompt_ids, const in
 
 // Debug / parity hook: residual stream seen by every RMSNorm (2 per layer + final) for the LAST position of
 // the last b2a_tts_forward_logits call made while tracing was enabled; out is [2*layers+1, batch, hidden].
+int32_t b2a_debug_step_smem(int32_t gqa, int32_t* out) {
+    return guarded([&] {
+        B2A_CHECK(out && (gqa == 1 || gqa == 2 || gqa == 3 || gqa == 4 || gqa == 6 || gqa == 8), B2A_ERR_INVALID_INPUT,
+                  "b2a_debug_step_smem: q heads per kv head must be 1, 2, 3, 4, 6 or 8");
+        out[0] = (int32_t)tc::Smem<16>::bytes(b2a_tts::gemm_stages);
+        out[1] = (int32_t)tc::SmemSplit::bytes(b2a_tts::splitk_stages, b2a_tts::fused_cluster);
+        out[2] = (int32_t)attn_smem_bytes(gqa);
+    });
+}
+
 int32_t b2a_tts_debug_trace(b2a_tts* h, int32_t enable, int32_t batch, float* out) {
     return guarded([&] {
         B2A_CHECK(h, B2A_ERR_INVALID_INPUT, "b2a_tts_debug_trace: null handle");

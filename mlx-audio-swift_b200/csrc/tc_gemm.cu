@@ -99,6 +99,10 @@ void launch_splitk(const CUtensorMap& tmA, const CUtensorMap& tmB, const SplitAr
 void set_attributes() {
     B2A_CUDA(cudaFuncSetAttribute(tc_gemm_splitk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     B2A_CUDA(cudaFuncSetAttribute(tc_gemm_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    // the decode-step kernels are sized to share an SM with their neighbours in the step (Smem / SmemSplit): ask for the largest
+    // shared-memory carve-out, or an SM configured for one kernel's footprint alone cannot take the next kernel's CTA beside it
+    B2A_CUDA(cudaFuncSetAttribute(tc_gemm_splitk_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+    B2A_CUDA(cudaFuncSetAttribute(tc_gemm_kernel<16>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
     B2A_CUDA(cudaFuncSetAttribute(tc_gemm_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     B2A_CUDA(cudaFuncSetAttribute(tc_gemm_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
 }

@@ -226,13 +226,21 @@ struct Cfg {
     static constexpr int NTHREADS = 32 * EPI_WARPS + 32;
 };
 
+// Dynamic shared memory of tc_gemm_kernel<BN>: the ring, the staged accumulator, 256 bytes of barriers.  The decode step runs BN = 16
+// with 6 stages: 6 x 18 432 + 10 240 + 256 = 121 088 bytes, which leaves room on the SM (233 472 bytes, 1 KB of it reserved per
+// resident CTA) for one CTA of either neighbour in the step, the split-K GEMM or the attention kernel, so that the neighbour's
+// prefetch-before-griddepcontrol.wait runs under this kernel's main loop and vice versa.
 template <int BN>
 struct Smem {
     static constexpr int A_BYTES = BM * BK * 2, B_BYTES = BN * BK * 2, STAGE = A_BYTES + B_BYTES;
     static constexpr int ACC_BYTES = BM * Cfg<BN>::LD * 4;
-    static int max_stages() { return (227 * 1024 - 1024 - 256 - ACC_BYTES) / STAGE; }
-    static size_t bytes(int stages) { return 1024 + (size_t)stages * STAGE + ACC_BYTES + 256; }
+    static int max_stages() { return (226 * 1024 - 256 - ACC_BYTES) / STAGE; }   // 1 KB under the 227 KB a CTA may have
+    static size_t bytes(int stages) { return (size_t)stages * STAGE + ACC_BYTES + 256; }
 };
+// The tile bases must be 1024-byte aligned (make_smem_desc): the dynamic array is declared so, and the kernels check it once.
+__device__ __forceinline__ void check_smem_base(const void* base) {
+    if (threadIdx.x == 0 && (smem_u32(base) & 1023u)) __trap();
+}
 
 // `a` is __grid_constant__: the kernel reads its fields from kernel-parameter memory where they are used.  Without it nvcc 12.9 may
 // copy the whole struct into registers at entry (decode GEMM, BN = 16: 106 registers instead of 92 and ~15% more instructions).
@@ -241,8 +249,7 @@ __global__ void __launch_bounds__(Cfg<BN>::NTHREADS, Cfg<BN>::EPI_WARPS > 4 ? 1 
 tc_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ Args a) {
     using S = Smem<BN>;
     using C = Cfg<BN>;
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+    extern __shared__ __align__(1024) uint8_t smem[];
     float* sacc = reinterpret_cast<float*>(smem + (size_t)a.stages * S::STAGE);            // [128][LD] staged accumulator
     uint64_t* full = reinterpret_cast<uint64_t*>(smem + (size_t)a.stages * S::STAGE + S::ACC_BYTES);
     uint64_t* empty = full + a.stages;
@@ -254,6 +261,7 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     const uint32_t stage_tx = (uint32_t)(TR * BK * 2 + S::B_BYTES);     // bytes the two TMA loads of a stage deliver
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");   // PDL: let the next kernel's prologue start
 
+    check_smem_base(smem);
     if (threadIdx.x == 0) {
         tma_prefetch_desc(&tmA);
         tma_prefetch_desc(&tmB);
@@ -547,11 +555,16 @@ __device__ __forceinline__ void st_cluster_f4(uint32_t addr, float a, float b, f
 }
 
 constexpr int SPLIT_MAX_CLUSTER = 8;
+// Dynamic shared memory of tc_gemm_splitk_kernel: the ring, the peers' partials (written remotely while the leader may still be
+// streaming, so they have a buffer of their own), 512 bytes of barriers and reduction scratch.  A CTA streams ONE tile, so its ring
+// is idle once the main loop ends and the 128 x 16 accumulator is staged in ring stage 0.  The decode step runs 5 stages in clusters
+// of 5: 5 x 18 432 + 4 x 4096 + 512 = 109 056 bytes; with tc_gemm_kernel<16>'s 121 088 and 1 KB reserved per CTA that is
+// 232 192 of an SM's 233 472 bytes.
 struct SmemSplit {
     static constexpr int STAGE = Smem<16>::STAGE;
     static constexpr int PART_BYTES = BM * 8 * 4;                      // one CTA's 128 x 8 fp32 partial
-    static constexpr int ACC_BYTES = Smem<16>::ACC_BYTES;              // this CTA's staged 128 x 16 accumulator
-    static size_t bytes(int stages, int cluster) { return 1024 + (size_t)stages * STAGE + (size_t)(cluster - 1) * PART_BYTES + ACC_BYTES + 512; }
+    static_assert(Smem<16>::ACC_BYTES <= STAGE, "the staged accumulator lives in ring stage 0");
+    static size_t bytes(int stages, int cluster) { return (size_t)stages * STAGE + (size_t)(cluster - 1) * PART_BYTES + 512; }
 };
 
 #ifdef B2A_TC_GEMM_IMPL   // the kernel body lives in tc_gemm.cu only (a non-template __global__ cannot be defined in every translation unit)
@@ -559,12 +572,11 @@ __global__ void __launch_bounds__(THREADS, 2)
 tc_gemm_splitk_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, SplitArgs a) {
     using S = Smem<16>;
     constexpr int BN = 16;
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+    extern __shared__ __align__(1024) uint8_t smem[];
     const uint32_t C = cluster_nctarank(), rank = cluster_ctarank();
     float* part = reinterpret_cast<float*>(smem + (size_t)a.stages * S::STAGE);                 // [C - 1][128][8]
-    float* sacc = part + (size_t)(C - 1) * BM * 8;                                               // [128][LD]
-    uint64_t* full = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(sacc) + SmemSplit::ACC_BYTES);
+    float* sacc = reinterpret_cast<float*>(smem);                                                // [128][LD], over ring stage 0
+    uint64_t* full = reinterpret_cast<uint64_t*>(part + (size_t)(C - 1) * BM * 8);
     uint64_t* empty = full + a.stages;
     float* s_red = reinterpret_cast<float*>(empty + a.stages);                                   // [4][8] + [8]
 
@@ -573,6 +585,7 @@ tc_gemm_splitk_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
     const int kb0 = (int)((long long)a.k_blocks * rank / C), kb1 = (int)((long long)a.k_blocks * (rank + 1) / C);
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
 
+    check_smem_base(smem);
     if (threadIdx.x == 0) {
         tma_prefetch_desc(&tmA);
         tma_prefetch_desc(&tmB);
@@ -640,6 +653,7 @@ tc_gemm_splitk_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
             if (lane == 0) mbar_arrive(&empty[stage]);
             if (++stage == a.stages) { stage = 0; phase ^= 1; }
         }
+        named_sync(3, 128);                                      // every warp's last wgmma has read the ring: stage 0 is free
 #pragma unroll
         for (int rb = 0; rb < 2; ++rb) {
             wg_fence_operand(d[rb]);
