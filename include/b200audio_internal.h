@@ -89,6 +89,16 @@ int32_t b2a_tc_gemm_splitk_test(const void* W, const void* X, float* h, const fl
  * DEVICE qkv [B * T, 3 * nh * 64] fp32; out [2 * 64 * cdiv(B * T, 64), nh * 64] bf16: token t = b * T + i at hi row
  * (t / 64) * 128 + t % 64, lo row = hi row + 64.  Rows of tokens >= B * T are not written.                                  */
 int32_t b2a_mha_tc_test(const float* qkv, void* out, int32_t B, int32_t T, int32_t nh, void* stream);
+/* tests/test_gpu_whisper_decode_attention.py: one Whisper decoder-step attention launch (mha_decode_kernel, csrc/whisper.cu) with the
+ * engine's grid (nh, B, S), all pointers DEVICE.  self_attn != 0: q is the fused q|k|v row [B, 3 * nh * 64] (query, new key, new
+ * value), kcache / vcache fp32 [B][nh][max_t][64]; row b with 0 <= pos[b] < max_t writes its new key / value at pos[b] and attends
+ * to positions 0..pos[b] in S = cdiv(max_t, 64) splits.  self_attn == 0: kv [B * max_t, 2 * nh * 64] fp32 (k | v projection of
+ * the encoder states) is first relaid into the fp16 caches kcache / vcache [B][nh][max_t][64], then q [B, nh * 64] attends to all
+ * max_t keys in S = cdiv(max_t, 128) splits.  Rows with pos[b] < 0 are skipped.  out [32, nh * 64] bf16: hi row b, lo row b + 16.
+ * Workspace: part_o [B * nh * S * 64], part_ml [B * nh * S * 2], counters [B * nh] int, zero on entry and left zero.             */
+int32_t b2a_wh_decode_attn_test(int32_t self_attn, const float* q, const float* kv, const int32_t* pos, void* kcache, void* vcache,
+                                void* out, float* part_o, float* part_ml, int32_t* counters, int32_t B, int32_t nh, int32_t max_t,
+                                void* stream);
 /* tests/test_gpu_conv_gemm.py: one launch of the codec conv GEMM (cg::conv_gemm_kernel, csrc/conv_gemm.cu, through the launch SNAC and Vocos use):
  * acc[n, m] = W[m, :] . X[n, :] for the host fp32 weight w [M, K] (split into bf16 hi/lo like the engines' weights) and the DEVICE
  * activations X, 2 * pad64(N) rows of 64-token hi/lo tiles (hi rows, then lo rows) by K.  Then v = gamma * GELU(acc + bias) (each

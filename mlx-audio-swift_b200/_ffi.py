@@ -216,6 +216,7 @@ SIGNATURES = {
                                                                              C.c_float, C.c_int32, _P]),
     "b2a_tc_gemm_splitk_test": (C.c_int32, [_P, _P, _P, _P, _P, _P] + [C.c_int32] * 5 + [_P]),
     "b2a_mha_tc_test": (C.c_int32, [_P, _P, C.c_int32, C.c_int32, C.c_int32, _P]),
+    "b2a_wh_decode_attn_test": (C.c_int32, [C.c_int32, _P, _P, _P, _P, _P, _P, _P, _P, _P, C.c_int32, C.c_int32, C.c_int32, _P]),
     "b2a_conv_gemm_test": (C.c_int32, [_P, C.c_int32, C.c_int32, _P, C.c_int32, C.c_int32, _P, _P, _P, C.c_int32, _P, C.c_int32, _P,
                                        C.c_int32] + [C.c_int32] * 6 + [_P, C.c_uint64, C.c_int32, _P]),
     "b2a_snac_unit_test": (C.c_int32, [C.c_int32] * 3 + [_P, _P, C.c_int32, C.c_int32] + [_P] * 6 + [_P, C.c_uint64, _P, _P, C.c_int32, _P]),

@@ -1388,3 +1388,33 @@ extern "C" int32_t b2a_mha_tc_test(const float* qkv, void* out, int32_t B, int32
         B2A_CUDA(cudaStreamSynchronize(s));
     });
 }
+
+// The decoder-step attention on its own (include/b200audio_internal.h): mha_decode_kernel with the grid and launch of
+// b2a_stt::dec_attn, on DEVICE caches and workspace the caller owns; cross-attention runs kv_relayout_kernel first, as encode_dev does.
+extern "C" int32_t b2a_wh_decode_attn_test(int32_t self_attn, const float* q, const float* kv, const int32_t* pos, void* kcache,
+                                           void* vcache, void* out, float* part_o, float* part_ml, int32_t* counters, int32_t B,
+                                           int32_t nh, int32_t max_t, void* stream) {
+    using namespace b2a;
+    return guarded([&] {
+        B2A_CHECK(q && pos && kcache && vcache && out && part_o && part_ml && counters && (self_attn || kv) && B >= 1 && B <= DEC_HALF &&
+                      nh >= 1 && max_t >= 1, B2A_ERR_INVALID_INPUT, "b2a_wh_decode_attn_test: bad argument");
+        require_device(0);
+        const cudaStream_t s = (cudaStream_t)stream;
+        const int d = nh * HD;
+        if (self_attn) {
+            const int S = cdiv(max_t, DA_CAP);
+            const DecAttnArgs a{q, q, pos, kcache, vcache, (bf16*)out, part_o, part_ml, counters, 3 * d, 0, d, 2 * d, nh, max_t, 0, S, d,
+                                1.0f / sqrtf((float)HD)};
+            launch_pdl(mha_decode_kernel<true>, dim3(nh, B, S), dim3(2 * DA_CAP), 0, s, a);
+        } else {
+            kv_relayout_kernel<<<(unsigned)((long long)B * max_t), 256, 0, s>>>(kv, (__half*)kcache, (__half*)vcache, max_t, d, nh);
+            count_launch();
+            const int S = cdiv(max_t, DA_CAP_CROSS);
+            const DecAttnArgs a{q, nullptr, pos, kcache, vcache, (bf16*)out, part_o, part_ml, counters, d, 0, 0, 0, nh, max_t, max_t, S, d,
+                                1.0f / sqrtf((float)HD)};
+            launch_pdl(mha_decode_kernel<false>, dim3(nh, B, S), dim3(2 * DA_CAP_CROSS), 0, s, a);
+        }
+        B2A_CUDA(cudaGetLastError());
+        B2A_CUDA(cudaStreamSynchronize(s));
+    });
+}
