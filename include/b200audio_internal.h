@@ -85,6 +85,18 @@ int32_t b2a_tc_gemm_test(const void* W, const void* X, void* out, int32_t M, int
  * h[t] * gain (xn [16, M] bf16), ss[m_tile, t] = sum of h[t]^2 over the tile's rows (ss [cdiv(M, 128), 8]; 0 for t >= N).     */
 int32_t b2a_tc_gemm_splitk_test(const void* W, const void* X, float* h, const float* gain, void* xn, float* ss, int32_t M, int32_t N,
                                 int32_t K, int32_t cluster, int32_t stages, void* stream);
+/* tests/test_gpu_splitk_store.py: the same kernel in the store mode of the decode step's q|k|v projection: for t < N,
+ * out[t] = rstd[t] * W (x_hi[t] + x_lo[t]) (out [8, M] fp32, DEVICE; rows t >= N untouched), rstd[t] = rsqrt(sum_p rstd_ss[p, t] / K
+ * + rstd_eps) for a DEVICE rstd_ss [rstd_parts, 8], or 1 when rstd_ss is null.  sk_ctas > 0: the k-blocks of a tile are cut as the
+ * stream-K GEMM over sk_ctas CTAs cuts them (cluster >= the most pieces of a tile), and out is bit-identical to that GEMM's;
+ * sk_ctas = 0: evenly over the cluster.                                                                                      */
+int32_t b2a_tc_gemm_splitk_store_test(const void* W, const void* X, float* out, const float* rstd_ss, int32_t rstd_parts, float rstd_eps,
+                                      int32_t M, int32_t N, int32_t K, int32_t cluster, int32_t sk_ctas, int32_t stages, void* stream);
+/* Needs a device: how the fused decode step launches its q|k|v GEMM for m_tiles 128-row tiles of k_blocks 64-wide k-blocks on
+ * device 0.  out[0] = the split-K cluster size (0: the stream-K GEMM runs), out[1] = its dynamic shared-memory bytes per CTA,
+ * out[2] = the clusters of that size and footprint the device holds at once, out[3] = the stream-K CTA count whose cut the split-K
+ * launch reproduces, out[4] = the most pieces that cut gives one tile (0 in out[1..2] when out[0] = 0).                     */
+int32_t b2a_debug_qkv_split(int32_t m_tiles, int32_t k_blocks, int32_t* out);
 /* tests/test_gpu_encoder_attention.py: the Whisper encoder attention (csrc/attn_tc.cuh, pack_qkv_f16_kernel + mha_tc_kernel) on a
  * DEVICE qkv [B * T, 3 * nh * 64] fp32; out [2 * 64 * cdiv(B * T, 64), nh * 64] bf16: token t = b * T + i at hi row
  * (t / 64) * 128 + t % 64, lo row = hi row + 64.  Rows of tokens >= B * T are not written.                                  */

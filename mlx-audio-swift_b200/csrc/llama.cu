@@ -87,14 +87,12 @@ __global__ void finalize_norm_kernel(const float* __restrict__ x, const float* _
 constexpr int LO_ROW = 8;   // activation matrices are [16, K] bf16: row b = hi(x_b), row 8 + b = lo(x_b) = bf16(x_b - hi)
 
 // x += delta (optional, delta is zeroed afterwards);  xn = hi/lo split of  x * rsqrt(mean(x^2) + eps) * w
-// One 1024-thread CTA per row, the row lives in registers (H <= 8192).  Also zeroes `zero_ptr[b, :zero_n]`
-// (the fp32 q|k|v row, so the next stream-K GEMM can add its partial sums into it).
+// One 1024-thread CTA per row, the row lives in registers (H <= 8192).
 constexpr int RN_THREADS = 1024, RN_MAXV = 8;
 __global__ void __launch_bounds__(RN_THREADS)
 add_rmsnorm_kernel(float* __restrict__ x, float* __restrict__ delta, const float* __restrict__ w,
-                   bf16* __restrict__ xn, int H, float eps, float* __restrict__ trace, float* __restrict__ zero_ptr,
-                   int zero_n, int half, float* __restrict__ normed = nullptr, float* __restrict__ ss_out = nullptr,
-                   int ss_parts = 0) {
+                   bf16* __restrict__ xn, int H, float eps, float* __restrict__ trace, int half,
+                   float* __restrict__ normed = nullptr, float* __restrict__ ss_out = nullptr, int ss_parts = 0) {
     __shared__ float red[RN_THREADS / 32];
     const int b = blockIdx.x, tid = threadIdx.x;
     pdl_trigger();
@@ -133,8 +131,6 @@ add_rmsnorm_kernel(float* __restrict__ x, float* __restrict__ delta, const float
             if (normed) normed[(long long)b * H + i] = o;     // the fp32 normalised row (the talker's hidden state, row N1)
         }
     }
-    if (zero_ptr)
-        for (int i = tid; i < zero_n; i += RN_THREADS) zero_ptr[(long long)b * zero_n + i] = 0.f;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -247,8 +243,6 @@ struct AttnArgs {
     const float* qnorm;    // nullable [128]: per-head RMSNorm gain applied to every q head BEFORE RoPE (Qwen3TTSTalker.swift:127-186)
     const float* knorm;    // nullable [128]: same for the k head
     float qk_eps;
-    int zero_qkv;          // fused-norm step: clear this (row, kv head)'s q | k | v slices after reading them, so that the next layer's
-                           // stream-K QKV GEMM can add into the row (the stand-alone norm kernel that used to do it is gone)
 };
 
 // One thread-block cluster of two CTAs per (kv head, row), grid (kv heads, rows, 2).  Keys 0..pos are cut into 64-key chunks
@@ -469,11 +463,6 @@ attn_decode_cluster_kernel(const __grid_constant__ AttnArgs a) {
         }
     }
     cluster.sync();
-    if (a.zero_qkv && rank == 0) {
-        float* wrow = const_cast<float*>(row);
-        for (int i = tid; i < G * HD; i += AT_THREADS) wrow[(long long)h * G * HD + i] = 0.f;
-        if (tid < HD) { wrow[(a.nq + h) * HD + tid] = 0.f; wrow[(a.nq + a.nkv + h) * HD + tid] = 0.f; }
-    }
     if (rank == 0 && tid < HD) {
         _Pragma("unroll") for (int g = 0; g < G; ++g) {
             const float M1 = xml[g], L1 = xml[MAXG + g], O1 = xo[g * HD + tid];
@@ -950,9 +939,12 @@ struct b2a_tts {
     HBuf<int> h_flag;
     cudaEvent_t ev_poll[2] = {nullptr, nullptr};   // the generate loop's pipelined "rows still active" polls
     // fused-norm decode step (default on the wgmma path): o_proj / down_proj run as cluster split-K GEMMs whose leader CTA does the
-    // residual add + the next norm's gain + hi/lo split + sum of squares; no stand-alone add_rmsnorm launches (tc_gemm.cuh)
+    // residual add + the next norm's gain + hi/lo split + sum of squares; no stand-alone add_rmsnorm launches (tc_gemm.cuh).  q|k|v runs
+    // on the same kernel in store mode (qkv_gemm)
     bool fused = false;
     static constexpr int fused_cluster = 5;   // 5 CTAs per 128-row tile: 120 of 132 SMs for hidden 3072, one wave
+    int qkv_cluster = 0;                      // CTAs per 128-row tile of the q|k|v split-K GEMM (pick_qkv_cluster); 0: stream-K
+    int qkv_sk_ctas = 0;                      // the stream-K CTA count whose cut of the k-blocks that GEMM reproduces
     // ring depths of the decode step's GEMMs.  With them tc::Smem<16>::bytes, tc::SmemSplit::bytes and attn_smem_bytes() are sized so
     // that any two kernels that follow each other in the fused step fit on one SM together (b2a_debug_step_smem reports the three)
     static constexpr int gemm_stages = 6, splitk_stages = 5;
@@ -1090,6 +1082,9 @@ struct b2a_tts {
         use_batched_prefill = !(envp && std::string(envp) == "step");
         if (use_tc) {
             tc::set_attributes();
+            if (fused) {
+                qkv_cluster = pick_qkv_cluster(cdiv(NQ + 2 * NKV, tc::BM), H / tc::BK, num_sms, &qkv_sk_ctas);
+            }
             for (auto& L : layers) {
                 tm_qkv.push_back(tc::make_tmap_bf16(L.wqkv.p, NQ + 2 * NKV, H, tc::BM));
                 tm_o.push_back(tc::make_tmap_bf16(L.wo.p, H, NQ, tc::BM));
@@ -1266,7 +1261,7 @@ struct b2a_tts {
             a.ldo = M; a.epi_full = tc::EPI_STORE; a.epi_partial = -1; a.lo_rows = 0;
             a.tile_rows = head_rows_now > 0 ? head_rows_now : lm_tile_rows; a.m_tiles = cdiv(M, a.tile_rows);
             ctas = std::min(num_sms, a.m_tiles);
-        } else {   // qkv / o / down: stream-K, partial tiles summed in slot order into the zeroed fp32 output
+        } else {   // qkv / o / down: stream-K, partial tiles summed in slot order and stored into the fp32 output
             a.ldo = M; a.epi_full = tc::EPI_STORE; a.epi_partial = tc::EPI_PARTIAL; a.lo_rows = 0;
             ctas = (int)std::min<long long>(num_sms, (long long)a.m_tiles * a.k_blocks);
             a.part_ws = sk_ws.p; a.part_cnt = sk_cnt.p; a.part_slots = sk_slots;
@@ -1310,22 +1305,44 @@ struct b2a_tts {
         a.rstd_ss = nullptr; a.rstd_parts = 0; a.rstd_inv_h = 0.f; a.rstd_eps = 0.f;
         tc::launch_splitk(tmW, tmX, a, cdiv(M, tc::BM), std::max(1, std::min(fused_cluster, a.k_blocks)), s);
     }
-    // The fused-norm step: embed -> raw norm -> L x [qkv gemm (rstd in the epilogue) -> attention (clears q|k|v) -> o split-K (+ residual,
-    // norm 2) -> gate/up gemm (rstd, SwiGLU) -> down split-K (+ residual, next layer's norm 1 / the final norm)].  Leaves the residual
+    // q|k|v projection of the fused step: q|k|v[t] = rstd[t] * Wqkv xn[t] (the input norm's scale from ss_b), stored, in clusters of
+    // qkv_cluster CTAs that compute exactly what the stream-K GEMM computes (tc::SplitArgs::sk_ctas); that GEMM itself when the
+    // clusters do not fit in one wave
+    void qkv_gemm(int layer, int B, cudaStream_t s) {
+        const int H = cfg.hidden_size, M = (cfg.num_attention_heads + 2 * cfg.num_key_value_heads) * HD;
+        if (qkv_cluster < 1) { tc_gemm(tm_qkv[layer], tmx_xn, OP_QKV, qkv.p, nullptr, B, M, H, s, ss_b.p); return; }
+        tc::SplitArgs a{};
+        a.M = M; a.N = B; a.K = H; a.k_blocks = H / tc::BK; a.stages = splitk_stages; a.sk_ctas = qkv_sk_ctas;
+        a.out = qkv.p;
+        a.rstd_ss = ss_b.p; a.rstd_parts = fused_parts; a.rstd_inv_h = 1.0f / (float)H; a.rstd_eps = cfg.rms_norm_eps;
+        tc::launch_splitk(tm_qkv[layer], tmx_xn, a, cdiv(M, tc::BM), qkv_cluster, s);
+    }
+    // The q|k|v split-K launch cuts each tile's k-blocks where the stream-K GEMM over *sk_ctas = min(SMs, units) CTAs cuts them (so
+    // its output is bit-identical), one CTA per piece: the cluster size is the most pieces of any tile (tc::stream_k_slots).  It is
+    // used when that is at most 8 and all m_tiles clusters are resident at once (cudaOccupancyMaxActiveClusters at the launch's own
+    // shared-memory footprint); 0 otherwise (the stream-K GEMM runs).  Needs tc::set_attributes().
+    static int pick_qkv_cluster(int m_tiles, int k_blocks, int sms, int* sk_ctas) {
+        *sk_ctas = (int)std::min<long long>(sms, (long long)m_tiles * k_blocks);
+        const int c = tc::stream_k_slots(m_tiles, k_blocks, *sk_ctas);
+        if (c > tc::SPLIT_MAX_CLUSTER) return 0;
+        return m_tiles <= tc::splitk_active_clusters(c, tc::SmemSplit::bytes(splitk_stages, c)) ? c : 0;
+    }
+    // The fused-norm step: embed -> raw norm -> L x [qkv gemm (rstd in the epilogue) -> attention -> o split-K (+ residual, norm 2)
+    // -> gate/up gemm (rstd, SwiGLU) -> down split-K (+ residual, next layer's norm 1 / the final norm)].  Leaves the residual
     // stream in x, xn = hi/lo of x * final_norm_gain and its sums of squares in ss_b: the lm head GEMM applies rstd itself.
     void run_layers_fused(int B, cudaStream_t s) {
         const int H = cfg.hidden_size, I = cfg.intermediate_size, nq = cfg.num_attention_heads, nkv = cfg.num_key_value_heads;
-        const int NQ = nq * HD, NKV = nkv * HD, L = cfg.num_hidden_layers;
+        const int NQ = nq * HD, L = cfg.num_hidden_layers;
         if (x_ext) launch_pdl(ext_embed_kernel, dim3(B), dim3(256), 0, s, x_ext, x.p, y.p, H);
         else launch_pdl(embed_kernel, dim3(B), dim3(256), 0, s, tokens.p, embed.p, x.p, y.p, H, cfg.vocab_size);
         launch_pdl(add_rmsnorm_kernel, dim3(B), dim3(RN_THREADS), 0, s, x.p, (float*)nullptr, layers[0].ln1.p, xn.p, H, cfg.rms_norm_eps,
-                   (float*)nullptr, (float*)nullptr, 0, LO_ROW, (float*)nullptr, ss_b.p, fused_parts);
+                   (float*)nullptr, LO_ROW, (float*)nullptr, ss_b.p, fused_parts);
         const size_t kv_layer = (size_t)cfg.max_batch * nkv * cfg.max_context * HD;
         for (int l = 0; l < L; ++l) {
             LayerW& Lw = layers[l];
-            tc_gemm(tm_qkv[l], tmx_xn, OP_QKV, qkv.p, nullptr, B, NQ + 2 * NKV, H, s, ss_b.p);
+            qkv_gemm(l, B, s);
             AttnArgs aa{qkv.p, pos.p, freqs.p, kcache.p + l * kv_layer, vcache.p + l * kv_layer, attn.p, nq, nkv, cfg.max_context,
-                        1.0f / sqrtf((float)HD), spec.qk_norm ? Lw.qnorm.p : nullptr, spec.qk_norm ? Lw.knorm.p : nullptr, cfg.rms_norm_eps, 1};
+                        1.0f / sqrtf((float)HD), spec.qk_norm ? Lw.qnorm.p : nullptr, spec.qk_norm ? Lw.knorm.p : nullptr, cfg.rms_norm_eps};
             attn_launch(aa, B, s);
             splitk_gemm(tm_o[l], tmx_attn, H, NQ, Lw.ln2.p, ss_a.p, B, s);
             tc_gemm(tm_gu_dec[l], tmx_xn, OP_GU, nullptr, act.p, B, 2 * I, H, s, ss_a.p);
@@ -1338,23 +1355,22 @@ struct b2a_tts {
     void run_layers(int B, cudaStream_t s) {
         if (fused && !trace_on) { run_layers_fused(B, s); return; }
         const int H = cfg.hidden_size, nq = cfg.num_attention_heads, nkv = cfg.num_key_value_heads;
-        const int QKV_N = (nq + 2 * nkv) * HD, G = nq / nkv;
+        const int G = nq / nkv;
         if (x_ext) launch_pdl(ext_embed_kernel, dim3(B), dim3(256), 0, s, x_ext, x.p, y.p, H);
         else launch_pdl(embed_kernel, dim3(B), dim3(256), 0, s, tokens.p, embed.p, x.p, y.p, H, cfg.vocab_size);
         const size_t kv_layer = (size_t)cfg.max_batch * nkv * cfg.max_context * HD;
         for (int l = 0; l < cfg.num_hidden_layers; ++l) {
             LayerW& L = layers[l];
             launch_pdl(add_rmsnorm_kernel, dim3(B), dim3(RN_THREADS), 0, s, x.p, l == 0 ? (float*)nullptr : y.p, L.ln1.p, xn.p, H,
-                       cfg.rms_norm_eps, trace_on ? trace.p + (size_t)(2 * l) * 8 * H : (float*)nullptr, (float*)nullptr, 0, LO_ROW,
+                       cfg.rms_norm_eps, trace_on ? trace.p + (size_t)(2 * l) * 8 * H : (float*)nullptr, LO_ROW,
                        (float*)nullptr, (float*)nullptr, 0);
             gemm(OP_QKV, l, B, s);
             AttnArgs aa{qkv.p, pos.p, freqs.p, kcache.p + l * kv_layer, vcache.p + l * kv_layer, attn.p, nq, nkv, cfg.max_context,
-                        1.0f / sqrtf((float)HD), spec.qk_norm ? L.qnorm.p : nullptr, spec.qk_norm ? L.knorm.p : nullptr, cfg.rms_norm_eps, 0};
+                        1.0f / sqrtf((float)HD), spec.qk_norm ? L.qnorm.p : nullptr, spec.qk_norm ? L.knorm.p : nullptr, cfg.rms_norm_eps};
             attn_launch(aa, B, s);
             gemm(OP_O, l, B, s);
-            // also zeroes this row of q|k|v so the next layer's stream-K QKV GEMM can accumulate into it
             launch_pdl(add_rmsnorm_kernel, dim3(B), dim3(RN_THREADS), 0, s, x.p, y.p, L.ln2.p, xn.p, H, cfg.rms_norm_eps,
-                       trace_on ? trace.p + (size_t)(2 * l + 1) * 8 * H : (float*)nullptr, qkv.p, QKV_N, LO_ROW, (float*)nullptr, (float*)nullptr, 0);
+                       trace_on ? trace.p + (size_t)(2 * l + 1) * 8 * H : (float*)nullptr, LO_ROW, (float*)nullptr, (float*)nullptr, 0);
             gemm(OP_GU, l, B, s);
             gemm(OP_DOWN, l, B, s);
         }
@@ -1369,7 +1385,7 @@ struct b2a_tts {
             return;
         }
         launch_pdl(add_rmsnorm_kernel, dim3(B), dim3(RN_THREADS), 0, s, x.p, y.p, final_ln.p, xn.p, cfg.hidden_size, cfg.rms_norm_eps,
-                   trace_on ? trace.p + (size_t)(2 * cfg.num_hidden_layers) * 8 * cfg.hidden_size : (float*)nullptr, (float*)nullptr, 0, LO_ROW,
+                   trace_on ? trace.p + (size_t)(2 * cfg.num_hidden_layers) * 8 * cfg.hidden_size : (float*)nullptr, LO_ROW,
                    normed_out, (float*)nullptr, 0);
     }
     void run_lm_head(int B, cudaStream_t s) {
@@ -1380,7 +1396,7 @@ struct b2a_tts {
     // after prefill_batched's gather_last (x, y hold the last position un-added): always the stand-alone norm + plain GEMM
     void run_lm_head_after_prefill(int B, cudaStream_t s) {
         launch_pdl(add_rmsnorm_kernel, dim3(B), dim3(RN_THREADS), 0, s, x.p, y.p, final_ln.p, xn.p, cfg.hidden_size, cfg.rms_norm_eps,
-                   (float*)nullptr, (float*)nullptr, 0, LO_ROW, (float*)nullptr, (float*)nullptr, 0);
+                   (float*)nullptr, LO_ROW, (float*)nullptr, (float*)nullptr, 0);
         gemm(OP_LM, -1, B, s);
     }
     // a head the caller owns (row N1: the code predictor's 15 lm heads): logits_out[b, :M] = W[M, H] * normed hidden
@@ -1445,7 +1461,7 @@ struct b2a_tts {
         for (int l = 0; l < cfg.num_hidden_layers; ++l) {
             LayerW& Lw = layers[l];
             launch_pdl(add_rmsnorm_kernel, dim3(T), dim3(RN_THREADS), 0, s, xp.p, l == 0 ? (float*)nullptr : yp.p, Lw.ln1.p, xnp.p, H,
-                       cfg.rms_norm_eps, (float*)nullptr, (float*)nullptr, 0, PF_HALF, (float*)nullptr, (float*)nullptr, 0);
+                       cfg.rms_norm_eps, (float*)nullptr, PF_HALF, (float*)nullptr, (float*)nullptr, 0);
             pf_gemm(tm_qkv[l], tmp_xn, tc::EPI_STORE, qkvp.p, nullptr, T, QKV_N, H, s);
             PrefillAttnArgs pa{qkvp.p, rope_tab.p, kcache.p + l * kv_layer, vcache.p + l * kv_layer, attnp.p, nq, nkv,
                                cfg.max_context, L, 1.0f / sqrtf((float)HD)};
@@ -1462,7 +1478,7 @@ struct b2a_tts {
             count_launch();
             pf_gemm(tm_o[l], tmp_attn, tc::EPI_STORE, yp.p, nullptr, T, H, NQ, s);
             launch_pdl(add_rmsnorm_kernel, dim3(T), dim3(RN_THREADS), 0, s, xp.p, yp.p, Lw.ln2.p, xnp.p, H, cfg.rms_norm_eps,
-                       (float*)nullptr, (float*)nullptr, 0, PF_HALF, (float*)nullptr, (float*)nullptr, 0);
+                       (float*)nullptr, PF_HALF, (float*)nullptr, (float*)nullptr, 0);
             pf_gemm(tm_gu[l], tmp_xn, tc::EPI_SWIGLU, nullptr, actp.p, T, 2 * I, H, s);
             pf_gemm(tm_down[l], tmp_act, tc::EPI_STORE, yp.p, nullptr, T, H, I, s);
         }
@@ -1933,6 +1949,21 @@ int32_t b2a_debug_step_smem(int32_t gqa, int32_t* out) {
         out[0] = (int32_t)tc::Smem<16>::bytes(b2a_tts::gemm_stages);
         out[1] = (int32_t)tc::SmemSplit::bytes(b2a_tts::splitk_stages, b2a_tts::fused_cluster);
         out[2] = (int32_t)attn_smem_bytes(gqa);
+    });
+}
+
+int32_t b2a_debug_qkv_split(int32_t m_tiles, int32_t k_blocks, int32_t* out) {
+    return guarded([&] {
+        B2A_CHECK(out && m_tiles >= 1 && k_blocks >= 1, B2A_ERR_INVALID_INPUT, "b2a_debug_qkv_split: bad argument");
+        require_device(0);
+        tc::set_attributes();
+        int sms = 0, sk_ctas = 0;
+        B2A_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0));
+        out[0] = b2a_tts::pick_qkv_cluster(m_tiles, k_blocks, sms, &sk_ctas);
+        out[1] = out[0] ? (int32_t)tc::SmemSplit::bytes(b2a_tts::splitk_stages, out[0]) : 0;
+        out[2] = out[0] ? tc::splitk_active_clusters(out[0], (size_t)out[1]) : 0;
+        out[3] = sk_ctas;
+        out[4] = tc::stream_k_slots(m_tiles, k_blocks, sk_ctas);
     });
 }
 

@@ -83,6 +83,8 @@ template void launch<128>(const CUtensorMap&, const CUtensorMap&, const Args&, i
 
 void launch_splitk(const CUtensorMap& tmA, const CUtensorMap& tmB, const SplitArgs& a, int m_tiles, int cluster, cudaStream_t s) {
     B2A_CHECK(SmemSplit::bytes(a.stages, cluster) <= 227 * 1024, B2A_ERR_INVALID_INPUT, "tc_gemm: split-K ring does not fit in shared memory");
+    B2A_CHECK(a.sk_ctas <= 0 || (!a.h && cluster >= stream_k_slots(m_tiles, a.k_blocks, a.sk_ctas)), B2A_ERR_INVALID_INPUT,
+              "tc_gemm: the stream-K cut is a store-mode option and needs a CTA per piece of a tile");
     cudaLaunchConfig_t cfg{};
     cfg.gridDim = dim3((unsigned)(m_tiles * cluster)); cfg.blockDim = dim3(THREADS);
     cfg.dynamicSmemBytes = SmemSplit::bytes(a.stages, cluster); cfg.stream = s;
@@ -94,6 +96,20 @@ void launch_splitk(const CUtensorMap& tmA, const CUtensorMap& tmB, const SplitAr
     cfg.attrs = at; cfg.numAttrs = 2;
     B2A_CUDA(cudaLaunchKernelEx(&cfg, tc_gemm_splitk_kernel, tmA, tmB, a));
     count_launch();
+}
+
+int splitk_active_clusters(int cluster, size_t smem_bytes) {
+    B2A_CHECK(cluster >= 1 && cluster <= SPLIT_MAX_CLUSTER, B2A_ERR_INVALID_INPUT, "tc_gemm: split-K cluster size must be in [1, 8]");
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = dim3((unsigned)cluster); cfg.blockDim = dim3(THREADS);
+    cfg.dynamicSmemBytes = smem_bytes;
+    cudaLaunchAttribute at[1];
+    at[0].id = cudaLaunchAttributeClusterDimension;
+    at[0].val.clusterDim.x = (unsigned)cluster; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
+    cfg.attrs = at; cfg.numAttrs = 1;
+    int n = 0;
+    B2A_CUDA(cudaOccupancyMaxActiveClusters(&n, tc_gemm_splitk_kernel, &cfg));
+    return n;
 }
 
 void set_attributes() {
@@ -114,7 +130,7 @@ void set_attributes() {
 // with the epilogue options the engines' call sites use.
 
 // out[N, M] = X[N, K] * W[M, K]^T through tc_gemm_kernel<bn>.  hilo: X holds cdiv(N, bn / 2) tiles of bn rows (hi rows, then lo rows).
-// split != 0 lets CTAs own partial K ranges (stream-K): epi must then be a store into the zeroed or an add into the caller's fp32 out.
+// split != 0 lets CTAs own partial K ranges (stream-K): epi must then be a store into or an add into the caller's fp32 out.
 extern "C" int32_t b2a_tc_gemm_epilogue_test(const void* W, const void* X, void* out, int32_t M, int32_t N, int32_t K, int32_t bn,
                                              int32_t epi, int32_t split, int32_t hilo, int32_t ctas, const float* bias, int32_t act,
                                              int32_t tile_rows, int32_t lo_rows, const float* rstd_ss, int32_t rstd_parts,
@@ -197,6 +213,32 @@ extern "C" int32_t b2a_tc_gemm_splitk_test(const void* W, const void* X, float* 
         SplitArgs a{};
         a.M = M; a.N = N; a.K = K; a.k_blocks = K / BK; a.stages = stages;
         a.h = h; a.gain = gain; a.xn = (__nv_bfloat16*)xn; a.ss = ss;
+        launch_splitk(ta, tb, a, cdiv(M, BM), cluster, (cudaStream_t)stream);
+        B2A_CUDA(cudaGetLastError());
+        B2A_CUDA(cudaStreamSynchronize((cudaStream_t)stream));
+    });
+}
+
+// The decode step's q|k|v GEMM: the same cluster split-K launch in store mode, out[t] = rstd[t] * W (x_hi[t] + x_lo[t]) for t < N,
+// rstd[t] = rsqrt(sum_p rstd_ss[p, t] / K + rstd_eps) (rstd_ss nullable: rstd = 1); sk_ctas > 0: k-blocks cut as stream-K over sk_ctas CTAs.
+extern "C" int32_t b2a_tc_gemm_splitk_store_test(const void* W, const void* X, float* out, const float* rstd_ss, int32_t rstd_parts,
+                                                 float rstd_eps, int32_t M, int32_t N, int32_t K, int32_t cluster, int32_t sk_ctas,
+                                                 int32_t stages, void* stream) {
+    using namespace b2a;
+    using namespace b2a::tc;
+    return guarded([&] {
+        B2A_CHECK(W && X && out && M > 0 && M % 8 == 0 && K > 0 && K % BK == 0 && N >= 1 && N <= 8 && stages >= 1 &&
+                      (!rstd_ss || rstd_parts >= 1),
+                  B2A_ERR_INVALID_INPUT, "b2a_tc_gemm_splitk_store_test: bad argument");
+        B2A_CHECK(cluster >= 1 && cluster <= SPLIT_MAX_CLUSTER && cluster <= K / BK, B2A_ERR_INVALID_INPUT,
+                  "b2a_tc_gemm_splitk_store_test: cluster must be in [1, min(8, K / 64)]");
+        require_device(0);
+        set_attributes();
+        CUtensorMap ta = make_tmap_bf16(W, M, K, BM), tb = make_tmap_bf16(X, 16, K, 16);
+        SplitArgs a{};
+        a.M = M; a.N = N; a.K = K; a.k_blocks = K / BK; a.stages = stages; a.sk_ctas = sk_ctas;
+        a.out = out;
+        a.rstd_ss = rstd_ss; a.rstd_parts = rstd_parts; a.rstd_inv_h = 1.0f / (float)K; a.rstd_eps = rstd_eps;
         launch_splitk(ta, tb, a, cdiv(M, BM), cluster, (cudaStream_t)stream);
         B2A_CUDA(cudaGetLastError());
         B2A_CUDA(cudaStreamSynchronize((cudaStream_t)stream));

@@ -8,8 +8,8 @@
 // of the producer warp issues TMA into a deep shared-memory ring (~100-200 KB in flight per SM), the consumer
 // warpgroups issue wgmma and run the epilogue.  Work is split stream-K style: the (m_tile, k_block) units are dealt
 // evenly and contiguously to the CTAs; a CTA that owns only part of a tile's K range writes its partial tile to a
-// workspace slot, and the last of the tile's CTAs to finish adds the slots in slot order into the fp32 output, so the
-// result is the same on every run.
+// workspace slot, and the last of the tile's CTAs to finish adds the slots in slot order and stores the sum into the fp32
+// output (EPI_STORE) or adds it there (EPI_ADD), so the result is the same on every run.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -32,8 +32,8 @@ struct Args {
     int m_tiles, k_blocks;   // ceil(M/128), K/64
     int stages;              // smem ring depth
     int epi_full;            // epilogue when a CTA owns a tile's whole K range
-    int epi_partial;         // epilogue for partial K ranges (EPI_PARTIAL: the tile's partials are summed and added into
-                             // out_f32); < 0 => CTAs own whole tiles only
+    int epi_partial;         // epilogue for partial K ranges (EPI_PARTIAL: the tile's partials are summed and stored into
+                             // out_f32, or added there when epi_full is EPI_ADD); < 0 => CTAs own whole tiles only
     int hilo;                // X rows [0, BN/2) = hi(x), rows [BN/2, BN) = lo(x) = bf16(x - hi): columns j and
                              // j + BN/2 of the accumulator are summed, giving fp32-activation accuracy for free
     const float* bias;       // nullable [M]: added to every output column before the activation
@@ -506,7 +506,10 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                         for (int e = 0; e < PER; ++e) {
                             const int i = i0 + threadIdx.x + e * NT;
                             const int tcol = i / BM, r = i - tcol * BM, mm = mt * BM + r, tok = ntok0 + tcol;
-                            if (i < n_el && tok < a.N && mm < a.M) a.out_f32[(long long)tok * a.ldo + mm] += sum[e];
+                            if (i < n_el && tok < a.N && mm < a.M) {
+                                float* o = a.out_f32 + (long long)tok * a.ldo + mm;
+                                *o = a.epi_full == EPI_ADD ? *o + sum[e] : sum[e];
+                            }
                         }
                     }
                     if (threadIdx.x == 0) a.part_cnt[tile_id] = 0;
@@ -527,13 +530,19 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 //     xn[t, m] = hi / lo of  h[t, m] * gain[m]        (UN-normalised: the consumer GEMM scales its accumulator by rstd[t])
 //     ss[mt, t] = sum over the tile's rows of h[t, m]^2   (the consumer reduces the m-tiles: rstd = rsqrt(sum / H + eps))
 // RMSNorm is linear in its per-token scale, so moving rstd behind the consumer GEMM is exact up to fp32 rounding.
+// Store mode (h == nullptr, the q|k|v projection): the leader instead stores out[t, m] = 0 + rstd[t] * P_0 + rstd[t] * P_1 + ...,
+// P_r the partial of CTA r and rstd of the norm the input went through (rstd_ss; 1 without).  With sk_ctas > 0 CTA r streams the
+// r-th piece of the tile as tc_gemm_kernel's stream-K over sk_ctas CTAs cuts it (split_range), so out is bit-identical to that
+// launch: the same wgmma accumulation per piece, each piece scaled before the pieces are summed in slot order from 0.
 struct SplitArgs {
     int M, N, K;                 // N = tokens (<= 8)
     int k_blocks, stages;
-    float* h;                    // [8, M] residual stream (read-modify-write by the leader)
+    int sk_ctas;                 // > 0: k-blocks cut as stream-K over this many CTAs (cluster >= stream_k_slots); 0: evenly
+    float* h;                    // [8, M] residual stream (read-modify-write by the leader); nullptr: store mode
     const float* gain;           // [M] the next norm's weight
     __nv_bfloat16* xn;           // [16, M] hi rows 0..7 / lo rows 8..15
     float* ss;                   // [m_tiles, 8] partial sums of squares
+    float* out;                  // store mode: [8, M] fp32, rows t < N written
     const float* rstd_ss;        // nullable: partial sums [rstd_parts, 8] of the norm this GEMM's INPUT went through
     int rstd_parts;
     float rstd_inv_h, rstd_eps;
@@ -552,6 +561,21 @@ __device__ __forceinline__ uint32_t map_to_rank(uint32_t saddr, uint32_t rank) {
 }
 __device__ __forceinline__ void st_cluster_f4(uint32_t addr, float a, float b, float c, float d) {
     asm volatile("st.shared::cluster.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
+}
+
+// k-blocks [kb0, kb1) of m-tile mt that CTA r of its cluster of C streams (empty when kb0 == kb1)
+__host__ __device__ __forceinline__ void split_range(const SplitArgs& a, int mt, int m_tiles, int r, int C, int& kb0, int& kb1) {
+    if (a.sk_ctas > 0) {   // the piece of stream-K CTA first_owner + r (stream_k_owner) that lies in this tile
+        const long long units = (long long)m_tiles * a.k_blocks, t0 = (long long)mt * a.k_blocks, t1 = t0 + a.k_blocks;
+        const long long c = stream_k_owner(t0, units, a.sk_ctas) + r;
+        const long long u0 = units * c / a.sk_ctas, u1 = units * (c + 1) / a.sk_ctas;
+        kb0 = (int)(u0 > t0 ? u0 - t0 : 0);
+        kb1 = (int)(u1 < t1 ? u1 - t0 : a.k_blocks);
+        if (kb1 < kb0) kb1 = kb0;
+    } else {
+        kb0 = (int)((long long)a.k_blocks * r / C);
+        kb1 = (int)((long long)a.k_blocks * (r + 1) / C);
+    }
 }
 
 constexpr int SPLIT_MAX_CLUSTER = 8;
@@ -578,11 +602,12 @@ tc_gemm_splitk_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
     float* sacc = reinterpret_cast<float*>(smem);                                                // [128][LD], over ring stage 0
     uint64_t* full = reinterpret_cast<uint64_t*>(part + (size_t)(C - 1) * BM * 8);
     uint64_t* empty = full + a.stages;
-    float* s_red = reinterpret_cast<float*>(empty + a.stages);                                   // [4][8] + [8]
+    float* s_red = reinterpret_cast<float*>(empty + a.stages);                                   // [4][8]
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int mt = blockIdx.x / C;
-    const int kb0 = (int)((long long)a.k_blocks * rank / C), kb1 = (int)((long long)a.k_blocks * (rank + 1) / C);
+    const int mt = blockIdx.x / C, m_tiles = gridDim.x / C;
+    int kb0, kb1;
+    split_range(a, mt, m_tiles, rank, C, kb0, kb1);
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
 
     check_smem_base(smem);
@@ -617,18 +642,35 @@ tc_gemm_splitk_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
         }
     }
     // ---- epilogue part 1 (warps 0..3): this CTA's partial = hi + lo columns; non-leaders hand it to the leader
-    float acc[8], hold[8];
+    float acc[8], hold[8], rstd[8];
     float g = 0.f;
     const int q = warp & 3, row = q * 32 + lane;
     const int m = mt * BM + row;
     const bool m_ok = m < a.M;
     if (warp < 4) {
         if (rank == 0) {
-            // the residual rows and the gain do not depend on this GEMM: fetch them while the weights stream
+            // the residual rows, the gain and the input norm's sums of squares do not depend on this GEMM: fetch them while the
+            // weights stream
             asm volatile("griddepcontrol.wait;" ::: "memory");
-            g = m_ok ? a.gain[m] : 0.f;
+            if (a.h) {
+                g = m_ok ? a.gain[m] : 0.f;
 #pragma unroll
-            for (int j = 0; j < 8; ++j) hold[j] = (j < a.N && m_ok) ? a.h[(long long)j * a.M + m] : 0.f;
+                for (int j = 0; j < 8; ++j) hold[j] = (j < a.N && m_ok) ? a.h[(long long)j * a.M + m] : 0.f;
+            }
+            if (a.rstd_ss) {
+                // rstd of the norm this GEMM's input went through (its producer wrote un-normalised hi/lo rows), reduced as
+                // tc_gemm_kernel does: one independent load per lane and step (lane = part * 8 + token)
+                float t = 0.f;
+                for (int p0 = 0; p0 < a.rstd_parts; p0 += 4) {
+                    const int p = p0 + (lane >> 3);
+                    if (p < a.rstd_parts) t += a.rstd_ss[p * 8 + (lane & 7)];
+                }
+                t += __shfl_xor_sync(0xffffffffu, t, 8);
+                t += __shfl_xor_sync(0xffffffffu, t, 16);
+                const float rs = rsqrtf(t * a.rstd_inv_h + a.rstd_eps);
+#pragma unroll
+                for (int j = 0; j < 8; ++j) rstd[j] = __shfl_sync(0xffffffffu, rs, j);
+            }
         }
         float d[2][8];
 #pragma unroll
@@ -673,24 +715,36 @@ tc_gemm_splitk_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
     __syncwarp();
     cluster_sync_all();                                          // partials are in the leader's shared memory
     if (rank == 0 && warp < 4) {
+        if (!a.h) {
+            // store mode: each CTA's piece scaled by rstd, the pieces added to 0 in rank order, with no fused multiply-add -- the
+            // arithmetic of tc_gemm_kernel's stream-K epilogue and slot reduction (a CTA with an empty piece has no slot there)
+            float sum[8];
+#pragma unroll
+            for (int j = 0; j < 8; ++j) sum[j] = __fadd_rn(0.f, a.rstd_ss ? __fmul_rn(acc[j], rstd[j]) : acc[j]);
+            for (uint32_t r = 1; r < C; ++r) {
+                int r0, r1;
+                split_range(a, mt, m_tiles, (int)r, (int)C, r0, r1);
+                if (r0 == r1) continue;
+                const float* p = part + ((size_t)(r - 1) * BM + row) * 8;
+#pragma unroll
+                for (int j = 0; j < 8; ++j) sum[j] = __fadd_rn(sum[j], a.rstd_ss ? __fmul_rn(p[j], rstd[j]) : p[j]);
+            }
+#pragma unroll
+            for (int j = 0; j < 8; ++j)
+                if (j < a.N && m_ok) a.out[(long long)j * a.M + m] = sum[j];
+            return;
+        }
         for (uint32_t r = 1; r < C; ++r) {                       // fixed order: deterministic sums
             const float4 p0 = *reinterpret_cast<const float4*>(part + ((size_t)(r - 1) * BM + row) * 8);
             const float4 p1 = *reinterpret_cast<const float4*>(part + ((size_t)(r - 1) * BM + row) * 8 + 4);
             acc[0] += p0.x; acc[1] += p0.y; acc[2] += p0.z; acc[3] += p0.w;
             acc[4] += p1.x; acc[5] += p1.y; acc[6] += p1.z; acc[7] += p1.w;
         }
-        const int w4 = warp;                                     // 0..3 (s_red rows)
-        // rstd of the norm this GEMM's input went through (its producer wrote un-normalised hi/lo rows)
         if (a.rstd_ss) {
-            if (w4 == 0 && lane < 8) {
-                float t = 0.f;
-                for (int p = 0; p < a.rstd_parts; ++p) t += a.rstd_ss[p * 8 + lane];
-                s_red[32 + lane] = rsqrtf(t * a.rstd_inv_h + a.rstd_eps);
-            }
-            asm volatile("bar.sync 1, 128;" ::: "memory");
 #pragma unroll
-            for (int j = 0; j < 8; ++j) acc[j] *= s_red[32 + j];
+            for (int j = 0; j < 8; ++j) acc[j] *= rstd[j];
         }
+        const int w4 = warp;                                     // 0..3 (s_red rows)
         float sq[8];
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
@@ -731,6 +785,9 @@ template <int BN>
 void launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const Args& a, int ctas, int n_tiles, cudaStream_t s);
 
 void launch_splitk(const CUtensorMap& tmA, const CUtensorMap& tmB, const SplitArgs& a, int m_tiles, int cluster, cudaStream_t s);
+// clusters of `cluster` tc_gemm_splitk_kernel CTAs of smem_bytes dynamic shared memory the current device can hold at once
+// (cudaOccupancyMaxActiveClusters: the clusters' GPC placement is part of the answer).  Needs set_attributes().
+int splitk_active_clusters(int cluster, size_t smem_bytes);
 
 void set_attributes();   // cudaFuncSetAttribute for every instantiation (call once, outside graph capture)
 
