@@ -340,12 +340,13 @@ int32_t b2a_vocos_decode_dev(b2a_vocos* h, const float* d_features, int32_t batc
 int32_t b2a_vocos_decode_cond(b2a_vocos* h, const float* features, const float* cond, int32_t batch, int32_t frames, float* wave);
 void b2a_vocos_destroy(b2a_vocos* h);
 
-/* ------------------------------------------------------------------ Encodec decode
- * Replaces class Encodec's decode side (Sources/MLXAudioCodecs/Encodec/Encodec.swift:170-402) behind AudioCodecModel /
+/* ------------------------------------------------------------------ Encodec decode and encode
+ * Replaces class Encodec (Sources/MLXAudioCodecs/Encodec/Encodec.swift:170-402) behind AudioCodecModel /
  * AudioDecoderModel (Sources/MLXAudioCodecs/AudioCodecModel.swift:4-27, conformance at Encodec.swift:447-461):
  *   Encodec(config:) + fromModelDirectory weights (:405-431; keys quantizer.layers.N.codebook.embed,
  *     decoder.layers.N.{conv,lstm.L.{Wx,Wh,bias},block.{1,3}.conv,shortcut.conv}.*, MLX layouts:
- *     Conv1d / ConvTranspose1d [out, k, in], LSTM [4H, in])                    -> b2a_encodec_create
+ *     Conv1d / ConvTranspose1d [out, k, in], LSTM [4H, in]; encoder.layers.N.* in the same layouts, loaded
+ *     only when present)                                                       -> b2a_encodec_create
  *   decode(_ audioCodes:_ audioScales:paddingMask:) / decodeAudio (:366-402,458-460) -> b2a_encodec_decode
  * audio_codes are [n_chunks, B, n_q, T] int32 (n_q <= the codebooks the checkpoint holds: the bandwidth chosen at encode
  * time), audio_scales [n_chunks, B] float32 or NULL (nil scales); the waveform is [B, samples, audio_channels] with
@@ -376,6 +377,7 @@ typedef struct b2a_encodec_config {
     float trim_right_ratio;
     float chunk_length_s;           /* <= 0: nil (one frame) */
     float overlap;                  /* < 0: nil */
+    int32_t normalize;              /* encode divides each chunk by its RMS scale (Encodec.swift:224-231); decode ignores it */
 } b2a_encodec_config;
 
 typedef struct b2a_encodec b2a_encodec;
@@ -388,6 +390,26 @@ int32_t b2a_encodec_decode(b2a_encodec* h, const int32_t* audio_codes, int32_t n
                            int32_t frames, const float* audio_scales, float* wave);
 int32_t b2a_encodec_decode_dev(b2a_encodec* h, const int32_t* d_audio_codes, int32_t n_chunks, int32_t batch, int32_t n_q,
                                int32_t frames, const float* d_audio_scales, float* d_wave, void* stream);
+/* Encode side (AudioCodecModel.encodeAudio, Encodec.swift:457-460):
+ *   EncodecEncoder (:17-88) + the residual quantizer's encode (EncodecQuantization.swift:22-38, 90-115)
+ *   encodeFrame / encode (:212-291)                                             -> b2a_encodec_encode
+ * audio is [B, samples, audio_channels] float32; codes are [n_chunks, B, n_q, frames] int32 with n_chunks and frames from
+ * b2a_encodec_encoded_shape.  n_q is getNumQuantizersForBandwidth(bandwidth) of the caller's bandwidth (the Python wrapper
+ * maps target_bandwidths); it must be in [1, the codebooks the checkpoint holds].  Chunking follows encode's loop: chunk c
+ * covers samples [c*stride, c*stride + chunk_length); every chunk must have the same length (the reference's MLX.stacked
+ * cannot stack a short last chunk).  With normalize, scales [n_chunks, B] receives each chunk's sqrt(mean_t(mono^2)) + 1e-8
+ * (NULL allowed); without it scales is not touched (nil scales).  The padding mask only multiplies the audio ahead of the
+ * normalisation, so callers apply it on the host.  Needs the checkpoint's encoder.* tensors: a decoder-only handle returns
+ * B2A_ERR_MODEL_NOT_INITIALIZED.  The reference's fatalErrors, a bad n_q, empty input, ragged chunks and sizes whose index
+ * arithmetic would overflow are B2A_ERR_INVALID_INPUT.  The code search is ordered fp32 (dot, |x|^2, |e|^2 each summed over
+ * d in order without FMA contraction; lowest index on ties), so the codes are reproducible bit for bit, and a batch gives
+ * the codes of its clips encoded one by one. */
+int32_t b2a_encodec_encoded_shape(const b2a_encodec* h, int64_t samples, int32_t* n_chunks, int32_t* frames);
+int32_t b2a_encodec_encode(b2a_encodec* h, const float* audio, int32_t batch, int64_t samples, int32_t n_q, int32_t* codes,
+                           float* scales);
+/* the same on DEVICE pointers, enqueued on `stream` (NULL: the handle's stream), no host synchronisation */
+int32_t b2a_encodec_encode_dev(b2a_encodec* h, const float* d_audio, int32_t batch, int64_t samples, int32_t n_q, int32_t* d_codes,
+                               float* d_scales, void* stream);
 void b2a_encodec_destroy(b2a_encodec* h);
 
 /* ------------------------------------------------------------------ Whisper STT

@@ -142,6 +142,10 @@ int32_t b2a_snac_convt_test(const float* x, float* y, const float* alpha, const 
 /* tests/test_gpu_snac_encode.py: the SNAC encoder's latent before the code search (what b2a_snac_encode quantizes) on HOST data:
  * wave [B, n_samples] -> z [B, latent, t_latent] float32, t_latent as b2a_snac_encoded_length gives it.  Errors as b2a_snac_encode. */
 int32_t b2a_snac_encode_latent_test(b2a_snac* h, const float* wave, int32_t batch, int64_t n_samples, float* z);
+/* tests/test_gpu_encodec_encode.py: the Encodec encoder's latent before the code search (what b2a_encodec_encode quantizes) on HOST
+ * data: audio [B, samples, audio_channels] -> z [n_chunks, B, frames, hidden_size] float32, shapes as b2a_encodec_encoded_shape
+ * gives them.  Errors as b2a_encodec_encode. */
+int32_t b2a_encodec_encode_latent_test(b2a_encodec* h, const float* audio, int32_t batch, int64_t samples, float* z);
 
 #ifdef __cplusplus
 }

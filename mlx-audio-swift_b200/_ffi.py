@@ -71,7 +71,8 @@ class EncodecConfig(C.Structure):
                                            "num_lstm_layers", "residual_kernel_size", "use_causal_conv", "pad_mode_reflect",
                                            "norm_type", "last_kernel_size", "compress", "n_upsampling_ratios")]
                 + [("upsampling_ratios", C.c_int32 * 8), ("sampling_rate", C.c_int32), ("use_conv_shortcut", C.c_int32),
-                   ("trim_right_ratio", C.c_float), ("chunk_length_s", C.c_float), ("overlap", C.c_float)])
+                   ("trim_right_ratio", C.c_float), ("chunk_length_s", C.c_float), ("overlap", C.c_float),
+                   ("normalize", C.c_int32)])
 
 
 class SpeechTokenizerConfig(C.Structure):
@@ -231,6 +232,10 @@ SIGNATURES = {
     "b2a_encodec_stream": (C.c_void_p, [_P]),
     "b2a_encodec_decode": (C.c_int32, [_P, _P, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _P, _P]),
     "b2a_encodec_decode_dev": (C.c_int32, [_P, _P, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _P, _P, _P]),
+    "b2a_encodec_encoded_shape": (C.c_int32, [_P, C.c_int64, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
+    "b2a_encodec_encode": (C.c_int32, [_P, _P, C.c_int32, C.c_int64, C.c_int32, _P, _P]),
+    "b2a_encodec_encode_dev": (C.c_int32, [_P, _P, C.c_int32, C.c_int64, C.c_int32, _P, _P, _P]),
+    "b2a_encodec_encode_latent_test": (C.c_int32, [_P, _P, C.c_int32, C.c_int64, _P]),
     "b2a_encodec_destroy": (None, [_P]),
     "b2a_weights_load": (C.c_int32, [C.c_char_p, C.POINTER(_P)]),
     "b2a_weights_count": (C.c_int32, [_P]),

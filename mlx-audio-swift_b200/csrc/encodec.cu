@@ -1,4 +1,4 @@
-// Encodec decode for sm_90a (SURVEY.md row a18).  Replaces (reference paths):
+// Encodec decode and encode for sm_90a (SURVEY.md rows a18, a18b).  Replaces (reference paths):
 //   Sources/MLXAudioCodecs/Encodec/EncodecQuantization.swift:117-133  EncodecResidualVectorQuantizer.decode
 //   Sources/MLXAudioCodecs/Encodec/Encodec.swift:94-167               EncodecDecoder
 //   Sources/MLXAudioCodecs/Encodec/EncodecLayers.swift:15-88          EncodecLSTM / EncodecLSTMBlock (T sequential tiny matmuls)
@@ -6,6 +6,9 @@
 //   Sources/MLXAudioCodecs/Encodec/EncodecLayers.swift:216-273,371-450 transposed conv (a 5-deep scalar host loop in the reference)
 //   Sources/MLXAudioCodecs/Encodec/EncodecLayers.swift:278-337        EncodecResnetBlock
 //   Sources/MLXAudioCodecs/Encodec/Encodec.swift:294-402              decodeFrame / linearOverlapAdd / decode
+//   Sources/MLXAudioCodecs/Encodec/Encodec.swift:17-88                EncodecEncoder
+//   Sources/MLXAudioCodecs/Encodec/Encodec.swift:212-291              encodeFrame (normalize) / encode (chunk loop)
+//   Sources/MLXAudioCodecs/Encodec/EncodecQuantization.swift:22-38,90-115  codebook quantize / residual encode
 // fp32, channels-last [N, T, C] (the reference's own layout), N = chunks x batch.
 //   * every dense conv is ONE kernel, ec_conv_kernel: an implicit-GEMM over (token tile x output tile) whose K axis gathers
 //     the taps straight from the activation (no im2col buffer), with the ELU of the *input*, the bias and the residual /
@@ -16,6 +19,10 @@
 //   * the LSTM stack is ONE persistent cooperative kernel: each CTA owns 4 hidden units of every layer, keeps its slices of
 //     Wh (and Wx of the upper layers) in shared memory for the whole sequence, layers run as a wavefront (layer l works on
 //     time s - l in step s), so the whole block costs T + L - 1 grid barriers instead of L*T dependent launches.
+//   * the encoder reuses all of it: its downsampling convs (k = 2s, stride s) are ec_conv_kernel launches whose K axis gathers
+//     the 2s contiguous input rows of an output (src = q*s + tap - padL), the right padding through the same edge rule.  New
+//     kernels sit only at the edges: the stem from 1-2 audio channels (reading each chunk of the waveform in place), the
+//     per-chunk RMS scale, and the residual code search in ordered fp32 (DESIGN.md §3.6b).
 #include "common.cuh"
 
 #include <algorithm>
@@ -51,7 +58,8 @@ __global__ void scale_kernel(float* __restrict__ x, long long n, float f) {
 // ------------------------------------------------------------------ implicit-GEMM conv / transposed conv
 struct ConvArgs {
     // source A: taps over xa [N, La, Ca]
-    const float* xa; int La, Ca, taps, padL, reflect, elu_a, backward;   // forward: src = q + tap - padL; backward: src = q - tap
+    const float* xa; int La, Ca, taps, padL, reflect, elu_a, backward;   // forward: src = q*stride + tap - padL; backward: src = q - tap
+    int stride = 1;          // forward only: an encoder downsampling conv (k = 2s) gathers its 2s contiguous rows per output
     // source B (optional): one tap at src = q over xb [N, Lq, Cb]
     const float* xb; int Cb, elu_b;
     const float* A;          // [M, K] row-major, K = taps*Ca + Cb
@@ -70,7 +78,7 @@ __device__ __forceinline__ int src_index(int q, int tap, const ConvArgs& a) {
         const int s = q - tap;
         return (s >= 0 && s < a.La) ? s : -1;
     }
-    int s = q + tap - a.padL;
+    int s = q * a.stride + tap - a.padL;
     if (s < 0) return a.reflect ? min(-s, a.La - 1) : -1;
     if (s >= a.La) return a.reflect ? max(a.La - 2 - (s - a.La), 0) : -1;
     return s;
@@ -393,6 +401,171 @@ __global__ void __launch_bounds__(256) lstm_kernel(LstmArgs a) {
     }
 }
 
+// ================================================================== encode side
+// Chunk c of batch row b is the frame n = c*B + b: samples [c*stride, c*stride + Lc) of wave [B, samples, C], read in place.
+
+// encodeFrame's normalisation (Encodec.swift:224-231): scale[n] = sqrt(mean_t(mono^2)) + 1e-8, mono = sum_ch x / C.  One CTA per
+// frame; each thread sums a fixed strided subset in double, then a fixed tree: the result does not depend on scheduling.
+__global__ void __launch_bounds__(256) chunk_scale_kernel(const float* __restrict__ wave, float* __restrict__ scale, int B,
+                                                          long long samples, int C, int Lc, int stride_c) {
+    __shared__ double red[256];
+    const int n = blockIdx.x, c = n / B, b = n - c * B;
+    const float* src = wave + ((long long)b * samples + (long long)c * stride_c) * C;
+    double acc = 0.0;
+    for (int t = threadIdx.x; t < Lc; t += 256) {
+        float m = 0.f;
+        for (int ch = 0; ch < C; ++ch) m += src[(long long)t * C + ch];
+        m = m / (float)C;
+        acc += (double)m * (double)m;
+    }
+    red[threadIdx.x] = acc;
+    __syncthreads();
+    for (int o = 128; o; o >>= 1) {
+        if (threadIdx.x < o) red[threadIdx.x] += red[threadIdx.x + o];
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) scale[n] = (float)sqrt(red[0] / (double)Lc) + 1e-8f;
+}
+
+// Encoder stem (Encodec.swift:24-29): k-tap conv from audio_channels (1 or 2, too few for ec_conv_kernel's float4 K axis) to
+// F filters, with the config's padding, on chunk n of the waveform divided by scale[n] (when normalize).  STEM_T outputs per CTA;
+// the padded input tile and the weights [F, k, C] sit in shared memory.
+constexpr int STEM_T = 128;
+__global__ void __launch_bounds__(256) stem_conv_kernel(const float* __restrict__ wave, const float* __restrict__ w,
+                                                        const float* __restrict__ bias, const float* __restrict__ scale,
+                                                        float* __restrict__ out, int B, long long samples, int C, int Lc,
+                                                        int stride_c, int F, int k, int padL, int reflect) {
+    extern __shared__ float sm[];
+    float* ws = sm;                        // [F][k][C]
+    float* xs = sm + F * k * C;            // [STEM_T + k - 1][C]
+    const int n = blockIdx.y, c = n / B, b = n - c * B, t0 = blockIdx.x * STEM_T;
+    const float* src = wave + ((long long)b * samples + (long long)c * stride_c) * C;
+    const float sc = scale ? scale[n] : 1.f;
+    for (int e = threadIdx.x; e < F * k * C; e += 256) ws[e] = w[e];
+    for (int e = threadIdx.x; e < (STEM_T + k - 1) * C; e += 256) {
+        const int r = e / C, ch = e - r * C;
+        int s = t0 + r - padL;
+        if (s < 0) s = reflect ? min(-s, Lc - 1) : -1;
+        else if (s >= Lc) s = reflect ? max(Lc - 2 - (s - Lc), 0) : -1;
+        const float v = s >= 0 ? src[(long long)s * C + ch] : 0.f;
+        xs[e] = scale ? __fdiv_rn(v, sc) : v;
+    }
+    __syncthreads();
+    for (int e = threadIdx.x; e < STEM_T * F; e += 256) {
+        const int t = e / F, f = e - t * F;
+        if (t0 + t >= Lc) break;
+        float acc = 0.f;
+        for (int kk = 0; kk < k; ++kk)
+            for (int ch = 0; ch < C; ++ch) acc = fmaf(ws[(f * k + kk) * C + ch], xs[(t + kk) * C + ch], acc);
+        out[((long long)n * Lc + t0 + t) * F + f] = acc + bias[f];
+    }
+}
+
+// |e|^2 of every codebook row, summed over d in order without contraction (the code search's `ee`).
+__global__ void sqnorm_rows_kernel(const float* __restrict__ e, float* __restrict__ out, long long rows, int D) {
+    const long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= rows) return;
+    float acc = 0.f;
+    for (int d = 0; d < D; ++d) acc = __fadd_rn(acc, __fmul_rn(e[r * D + d], e[r * D + d]));
+    out[r] = acc;
+}
+
+// Residual VQ encode (EncodecQuantization.swift:22-38, 100-115): z [rows = N*T, D] -> codes [N, n_q, T], levels in sequence with
+// residual -= embed[idx].  Ordered fp32: for each (frame, code) dot, |x|^2 and |e|^2 are summed over d = 0..D-1 as
+// acc = fl(acc + fl(a*b)), dist = fl(fl(xx - 2 dot) + ee), and the lowest index wins ties (== the reference's argMax(-dist)).
+// A CTA keeps VQ_FT frames' residuals in shared memory for all levels and streams VQ_KT-code tiles of each codebook through;
+// thread (tx = tid % 16, ty = tid / 16) scores frames ty, ty + 16 against codes tx + 16 j, j < 4, of a tile.
+constexpr int VQ_FT = 32, VQ_KT = 64;
+__global__ void __launch_bounds__(256) rvq_encode_kernel(const float* __restrict__ z, const float* __restrict__ books,
+                                                         const float* __restrict__ ee, int* __restrict__ codes, int rows, int T,
+                                                         int nq, int K, int D) {
+    extern __shared__ float sm[];
+    const int ld = D + 1;
+    float* rs = sm;                        // [VQ_FT][ld] residuals
+    float* es = rs + VQ_FT * ld;           // [VQ_KT][ld] codebook tile
+    float* ees = es + VQ_KT * ld;          // [VQ_KT]
+    float* xxs = ees + VQ_KT;              // [VQ_FT]
+    int* bidx = reinterpret_cast<int*>(xxs + VQ_FT);   // [VQ_FT]
+    const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
+    const int f0 = blockIdx.x * VQ_FT;
+    for (int e = tid; e < VQ_FT * D; e += 256) {
+        const int f = e / D, d = e - f * D;
+        rs[f * ld + d] = f0 + f < rows ? z[(long long)(f0 + f) * D + d] : 0.f;
+    }
+    __syncthreads();
+    for (int q = 0; q < nq; ++q) {
+        const float* book = books + (long long)q * K * D;
+        if (tid < VQ_FT) {
+            float xx = 0.f;
+            for (int d = 0; d < D; ++d) xx = __fadd_rn(xx, __fmul_rn(rs[tid * ld + d], rs[tid * ld + d]));
+            xxs[tid] = xx;
+        }
+        float best[2] = {INFINITY, INFINITY};
+        int bi[2] = {0, 0};
+        for (int k0 = 0; k0 < K; k0 += VQ_KT) {
+            __syncthreads();
+            for (int e = tid; e < VQ_KT * D; e += 256) {
+                const int c = e / D, d = e - c * D;
+                es[c * ld + d] = k0 + c < K ? book[(long long)(k0 + c) * D + d] : 0.f;
+            }
+            if (tid < VQ_KT) ees[tid] = k0 + tid < K ? ee[(long long)q * K + k0 + tid] : 0.f;
+            __syncthreads();
+            float dot[2][4];
+#pragma unroll
+            for (int i = 0; i < 2; ++i)
+#pragma unroll
+                for (int j = 0; j < 4; ++j) dot[i][j] = 0.f;
+            const float* r0 = rs + ty * ld;
+            const float* r1 = rs + (ty + 16) * ld;
+            const float* e0 = es + tx * ld;
+#pragma unroll 4
+            for (int d = 0; d < D; ++d) {
+                const float a0 = r0[d], a1 = r1[d];
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                    const float ev = e0[16 * j * ld + d];
+                    dot[0][j] = __fadd_rn(dot[0][j], __fmul_rn(a0, ev));
+                    dot[1][j] = __fadd_rn(dot[1][j], __fmul_rn(a1, ev));
+                }
+            }
+#pragma unroll
+            for (int i = 0; i < 2; ++i)
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                    const int c = tx + 16 * j;
+                    if (k0 + c >= K) continue;
+                    const float dist = __fadd_rn(__fsub_rn(xxs[ty + 16 * i], __fmul_rn(2.0f, dot[i][j])), ees[c]);
+                    if (dist < best[i]) { best[i] = dist; bi[i] = k0 + c; }
+                }
+        }
+        // lowest index among the 16 lanes' minima (each lane's is already its lowest)
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+#pragma unroll
+            for (int o = 8; o; o >>= 1) {
+                const float ob = __shfl_xor_sync(0xffffffffu, best[i], o);
+                const int oi = __shfl_xor_sync(0xffffffffu, bi[i], o);
+                if (ob < best[i] || (ob == best[i] && oi < bi[i])) { best[i] = ob; bi[i] = oi; }
+            }
+            const int f = ty + 16 * i;
+            if (tx == 0) {
+                bidx[f] = bi[i];
+                if (f0 + f < rows) {
+                    const int n = (f0 + f) / T, t = (f0 + f) - n * T;
+                    codes[((long long)n * nq + q) * T + t] = bi[i];
+                }
+            }
+        }
+        __syncthreads();
+        if (q + 1 < nq)
+            for (int e = tid; e < VQ_FT * D; e += 256) {
+                const int f = e / D, d = e - f * D;
+                rs[f * ld + d] = __fsub_rn(rs[f * ld + d], book[(long long)bidx[f] * D + d]);
+            }
+        __syncthreads();
+    }
+}
+
 }  // namespace ec
 }  // namespace b2a
 
@@ -403,24 +576,86 @@ struct EcConv {
     int M = 0, K = 0;
 };
 
+// an EncodecLSTMBlock's stack: layer 0's input projection runs as one GEMM (xproj), the rest inside lstm_kernel
+struct EcLstm {
+    EcConv xproj;
+    DBuf<float> Wh[ec::LSTM_MAX_LAYERS], Wx[ec::LSTM_MAX_LAYERS], b[ec::LSTM_MAX_LAYERS];
+};
+
+// an EncodecResnetBlock: r1 = k-tap conv dim -> hid (ELU of its input), r2 = [shortcut | block.3] over K = dim + hid, or
+// block.3 plus the identity residual without a conv shortcut
+struct EcRes {
+    EcConv r1, r2;
+};
+
 struct b2a_encodec {
     int device = 0, num_sms = 132;
     b2a_encodec_config cfg{};
     cudaStream_t stream = nullptr;
     int n_q = 0;
     DBuf<float> books;                       // [n_q][size][dim]
-    EcConv conv0, xproj;
-    DBuf<float> lWh[ec::LSTM_MAX_LAYERS], lWx[ec::LSTM_MAX_LAYERS], lb[ec::LSTM_MAX_LAYERS];
-    struct Stage { int ratio, cin, cout, taps; EcConv up, r1, r2; };
+    EcConv conv0;
+    EcLstm lstm;
+    struct Stage { int ratio, cin, cout, taps; EcConv up; EcRes res; };
     std::vector<Stage> stages;
     DBuf<float> wlast, blast;
+    // encoder (only when the checkpoint has encoder.* tensors)
+    bool has_enc = false;
+    std::string enc_error = "encodec encode: the checkpoint has no encoder weights";
+    DBuf<float> wstem, bstem;                // [num_filters, kernel_size, audio_channels]
+    struct EStage { int ratio, cin, cout; EcRes res; EcConv down; };
+    std::vector<EStage> estages;
+    EcLstm elstm;
+    EcConv elast;
+    DBuf<float> book_sq;                     // [n_q][size] |e|^2 in search order
     // workspaces
-    DBuf<float> bufA, bufB, bufC, xp, hseq[ec::LSTM_MAX_LAYERS], chunks, scales, wave;
+    DBuf<float> bufA, bufB, bufC, xp, hseq[ec::LSTM_MAX_LAYERS], chunks, scales, wave, zbuf, audio;
     DBuf<int> codes;
     DBuf<unsigned> bar;
     int dim0 = 0;
 
     static void up(DBuf<float>& d, const std::vector<float>& v) { d.upload(v.data(), v.size()); }
+    static void chan_ok(int ch) { B2A_CHECK(ch >= 4 && ch % 4 == 0, B2A_ERR_INVALID_INPUT, "encodec: channel counts must be multiples of 4"); }
+
+    // ---- weight loading shared by the decoder and the encoder (prefix p ends in '.')
+    static void plain(const TensorTable& tt, EcConv& cv, const std::string& p, int cout, int k, int cin) {
+        chan_ok(cin);
+        cv.M = cout; cv.K = k * cin;
+        up(cv.A, tt.f32(p + "conv.weight", (int64_t)cout * k * cin));      // [out, k, in] == [M, tap*Cin + ci]
+        up(cv.bias, tt.f32(p + "conv.bias", cout));
+    }
+    void load_resnet(const TensorTable& tt, EcRes& r, const std::string& p, int dim) const {
+        const int hid = dim / cfg.compress;
+        chan_ok(hid);
+        plain(tt, r.r1, p + "block.1.", hid, cfg.residual_kernel_size, dim);
+        // second launch: [shortcut | block.3] over K = dim + hid (x raw, hidden through ELU)
+        std::vector<float> w1 = tt.f32(p + "block.3.conv.weight", (int64_t)dim * hid), b1 = tt.f32(p + "block.3.conv.bias", dim);
+        if (cfg.use_conv_shortcut) {
+            std::vector<float> ws = tt.f32(p + "shortcut.conv.weight", (int64_t)dim * dim), bs = tt.f32(p + "shortcut.conv.bias", dim);
+            std::vector<float> A((size_t)dim * (dim + hid));
+            for (int m = 0; m < dim; ++m) {
+                memcpy(&A[(size_t)m * (dim + hid)], &ws[(size_t)m * dim], dim * sizeof(float));
+                memcpy(&A[(size_t)m * (dim + hid) + dim], &w1[(size_t)m * hid], hid * sizeof(float));
+                b1[m] += bs[m];
+            }
+            r.r2.M = dim; r.r2.K = dim + hid; up(r.r2.A, A);
+        } else {
+            r.r2.M = dim; r.r2.K = hid; up(r.r2.A, w1);
+        }
+        up(r.r2.bias, b1);
+    }
+    void load_lstm(const TensorTable& tt, EcLstm& m, const std::string& p, int H) const {
+        if (cfg.num_lstm_layers == 0) return;
+        B2A_CHECK(H % ec::LSTM_UNITS == 0, B2A_ERR_INVALID_INPUT, "encodec: LSTM width must be a multiple of 4");
+        for (int l = 0; l < cfg.num_lstm_layers; ++l) {
+            const std::string q = p + "lstm." + std::to_string(l) + ".";
+            std::vector<float> wx = tt.f32(q + "Wx", (int64_t)4 * H * H), wh = tt.f32(q + "Wh", (int64_t)4 * H * H);
+            std::vector<float> b = tt.find(q + "bias") ? tt.f32(q + "bias", 4 * H) : std::vector<float>(4 * H, 0.f);
+            up(m.Wh[l], wh);
+            if (l == 0) { m.xproj.M = 4 * H; m.xproj.K = H; up(m.xproj.A, wx); up(m.xproj.bias, b); }
+            else { up(m.Wx[l], wx); up(m.b[l], b); }
+        }
+    }
 
     b2a_encodec(int dev, const b2a_encodec_config& c, const TensorTable& tt) : device(dev), cfg(c) {
         require_device(dev);
@@ -451,26 +686,9 @@ struct b2a_encodec {
         int scaling = 1 << c.n_upsampling_ratios;
         int idx = 0;
         auto key = [&](int i, const char* rest) { return "decoder.layers." + std::to_string(i) + "." + rest; };
-        auto chan_ok = [&](int ch) { B2A_CHECK(ch >= 4 && ch % 4 == 0, B2A_ERR_INVALID_INPUT, "encodec: channel counts must be multiples of 4"); };
-        auto plain = [&](EcConv& cv, const std::string& p, int cout, int k, int cin) {
-            chan_ok(cin);
-            cv.M = cout; cv.K = k * cin;
-            up(cv.A, tt.f32(p + "conv.weight", (int64_t)cout * k * cin));      // [out, k, in] == [M, tap*Cin + ci]
-            up(cv.bias, tt.f32(p + "conv.bias", cout));
-        };
         dim0 = scaling * c.num_filters;
-        plain(conv0, key(idx, ""), dim0, c.kernel_size, c.hidden_size); ++idx;
-        if (c.num_lstm_layers > 0) {
-            B2A_CHECK(dim0 % ec::LSTM_UNITS == 0, B2A_ERR_INVALID_INPUT, "encodec: LSTM width must be a multiple of 4");
-            for (int l = 0; l < c.num_lstm_layers; ++l) {
-                const std::string p = key(idx, "lstm.") + std::to_string(l) + ".";
-                std::vector<float> wx = tt.f32(p + "Wx", (int64_t)4 * dim0 * dim0), wh = tt.f32(p + "Wh", (int64_t)4 * dim0 * dim0);
-                std::vector<float> b = tt.find(p + "bias") ? tt.f32(p + "bias", 4 * dim0) : std::vector<float>(4 * dim0, 0.f);
-                up(lWh[l], wh);
-                if (l == 0) { xproj.M = 4 * dim0; xproj.K = dim0; up(xproj.A, wx); up(xproj.bias, b); }
-                else { up(lWx[l], wx); up(lb[l], b); }
-            }
-        }
+        plain(tt, conv0, key(idx, ""), dim0, c.kernel_size, c.hidden_size); ++idx;
+        load_lstm(tt, lstm, key(idx, ""), dim0);
         ++idx;   // the LSTM block occupies a slot even when it has no layers
         for (int i = 0; i < c.n_upsampling_ratios; ++i) {
             Stage st{};
@@ -499,24 +717,7 @@ struct b2a_encodec {
             }
             for (int j = 0; j < c.num_residual_layers; ++j) {
                 B2A_CHECK(j == 0, B2A_ERR_INVALID_INPUT, "encodec: one residual layer per stage is implemented");
-                const int dim = st.cout, hid = dim / c.compress;
-                chan_ok(hid);
-                plain(st.r1, key(idx, "block.1."), hid, c.residual_kernel_size, dim);
-                // second launch: [shortcut | block.3] over K = dim + hid (x raw, hidden through ELU)
-                std::vector<float> w1 = tt.f32(key(idx, "block.3.conv.weight"), (int64_t)dim * hid), b1 = tt.f32(key(idx, "block.3.conv.bias"), dim);
-                if (c.use_conv_shortcut) {
-                    std::vector<float> ws = tt.f32(key(idx, "shortcut.conv.weight"), (int64_t)dim * dim), bs = tt.f32(key(idx, "shortcut.conv.bias"), dim);
-                    std::vector<float> A((size_t)dim * (dim + hid));
-                    for (int m = 0; m < dim; ++m) {
-                        memcpy(&A[(size_t)m * (dim + hid)], &ws[(size_t)m * dim], dim * sizeof(float));
-                        memcpy(&A[(size_t)m * (dim + hid) + dim], &w1[(size_t)m * hid], hid * sizeof(float));
-                        b1[m] += bs[m];
-                    }
-                    st.r2.M = dim; st.r2.K = dim + hid; up(st.r2.A, A);
-                } else {
-                    st.r2.M = dim; st.r2.K = hid; up(st.r2.A, w1);
-                }
-                up(st.r2.bias, b1);
+                load_resnet(tt, st.res, key(idx, ""), st.cout);
                 ++idx;
             }
             stages.push_back(std::move(st));
@@ -527,7 +728,43 @@ struct b2a_encodec {
         up(wlast, tt.f32(key(idx, "conv.weight"), (int64_t)c.audio_channels * c.last_kernel_size * c.num_filters));
         up(blast, tt.f32(key(idx, "conv.bias"), c.audio_channels));
         bar.alloc(1);
+        if (tt.find("encoder.layers.0.conv.weight")) {
+            // a malformed encoder leaves a working decoder: encode then reports why (B2A_ERR_MODEL_NOT_INITIALIZED)
+            try { load_encoder(tt); has_enc = true; }
+            catch (const Error& e) { estages.clear(); enc_error = std::string("encodec encode: encoder weights unusable: ") + e.what(); }
+        }
         B2A_CUDA(cudaDeviceSynchronize());
+    }
+
+    // EncodecEncoder (Encodec.swift:17-71): 0 stem, then per reversed ratio resnet(s), ELU, conv k = 2r stride r, then the LSTM
+    // block, ELU, last conv -> hidden_size.  Keys encoder.layers.{i}.* in the decoder's layouts, ELU modules counted.
+    void load_encoder(const TensorTable& tt) {
+        const int F = cfg.num_filters, CH = cfg.audio_channels, k = cfg.kernel_size;
+        auto key = [&](int i) { return "encoder.layers." + std::to_string(i) + "."; };
+        chan_ok(F);
+        int idx = 0;
+        up(wstem, tt.f32(key(idx) + "conv.weight", (int64_t)F * k * CH));
+        up(bstem, tt.f32(key(idx) + "conv.bias", F));
+        ++idx;
+        int scaling = 1;
+        for (int i = cfg.n_upsampling_ratios - 1; i >= 0; --i) {
+            EStage st{};
+            st.ratio = cfg.upsampling_ratios[i];
+            st.cin = scaling * F; st.cout = 2 * st.cin;
+            for (int j = 0; j < cfg.num_residual_layers; ++j) { load_resnet(tt, st.res, key(idx), st.cin); ++idx; }
+            ++idx;                                    // ELU slot
+            plain(tt, st.down, key(idx), st.cout, 2 * st.ratio, st.cin); ++idx;
+            estages.push_back(std::move(st));
+            scaling *= 2;
+        }
+        load_lstm(tt, elstm, key(idx), scaling * F); ++idx;
+        ++idx;                                        // ELU slot
+        plain(tt, elast, key(idx), cfg.hidden_size, cfg.last_kernel_size, scaling * F);
+        // |e|^2 of every codebook row, in the search's summation order
+        const long long rows = (long long)n_q * cfg.codebook_size;
+        book_sq.alloc((size_t)rows);
+        ec::sqnorm_rows_kernel<<<cdiv(rows, 256), 256>>>(books.p, book_sq.p, rows, cfg.codebook_dim);
+        B2A_CUDA(cudaGetLastError());
     }
     ~b2a_encodec() {
         if (stream) cudaStreamDestroy(stream);
@@ -570,6 +807,61 @@ struct b2a_encodec {
         count_launch();
     }
 
+    // EncodecResnetBlock (EncodecLayers.swift:278-337) on x [N, L, dim] as two launches (z: the hidden [N, L, hid]); result in x
+    void run_resnet(const EcRes& r, float*& x, float*& y, float* z, int N, long long L, int dim, cudaStream_t s) {
+        const int hid = r.r1.M;
+        ec::ConvArgs a{};
+        a.xa = x; a.La = (int)L; a.Ca = dim; a.taps = cfg.residual_kernel_size; pads(cfg.residual_kernel_size, a.padL); a.reflect = cfg.pad_mode_reflect; a.elu_a = 1;
+        a.A = r.r1.A.p; a.bias = r.r1.bias.p; a.M = hid; a.K = r.r1.K; a.Lq = (int)L; a.N = N; a.out = z; a.out_per_n = L * hid;
+        run_conv(a, s);
+        ec::ConvArgs b{};
+        b.N = N; b.Lq = (int)L; b.M = dim; b.K = r.r2.K; b.A = r.r2.A.p; b.bias = r.r2.bias.p; b.out = y; b.out_per_n = L * dim;
+        if (cfg.use_conv_shortcut) {
+            b.xa = x; b.La = (int)L; b.Ca = dim; b.taps = 1; b.xb = z; b.Cb = hid; b.elu_b = 1;
+        } else {
+            b.xa = z; b.La = (int)L; b.Ca = hid; b.taps = 1; b.elu_a = 1; b.res = x;
+        }
+        run_conv(b, s);
+        std::swap(x, y);
+    }
+
+    // EncodecLSTMBlock (EncodecLayers.swift:72-88) on x [N, T, H]: the stack plus its skip; result in x
+    void run_lstm_block(const EcLstm& m, float*& x, float*& y, int N, int T, int H, cudaStream_t s) {
+        const int NL = cfg.num_lstm_layers;
+        if (NL == 0) {
+            // an EncodecLSTMBlock without layers still adds its skip: h + hiddenStates = 2x (EncodecLayers.swift:82-88)
+            const long long cnt = (long long)N * T * H;
+            ec::scale_kernel<<<cdiv(cnt, 256), 256, 0, s>>>(x, cnt, 2.f);
+            count_launch();
+            return;
+        }
+        xp.alloc((size_t)N * T * 4 * H);
+        for (int l = 0; l < NL; ++l) hseq[l].alloc((size_t)N * T * H);
+        {
+            ec::ConvArgs a{};
+            a.xa = x; a.La = T; a.Ca = H; a.taps = 1; a.A = m.xproj.A.p; a.bias = m.xproj.bias.p; a.M = 4 * H; a.K = H; a.Lq = T; a.N = N;
+            a.out = xp.p; a.out_per_n = (long long)T * 4 * H;
+            run_conv(a, s);
+        }
+        const size_t smem = ((size_t)(2 * NL - 1) * 16 * H + (size_t)NL * ec::LSTM_BC * H + NL * 16 * ec::LSTM_BC + NL * ec::LSTM_UNITS * ec::LSTM_BC) * sizeof(float);
+        B2A_CHECK(smem <= 220 * 1024, B2A_ERR_INVALID_INPUT, "encodec: LSTM slice does not fit shared memory");
+        B2A_CUDA(cudaFuncSetAttribute(ec::lstm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        const int grid = H / ec::LSTM_UNITS;
+        int per_sm = 0;
+        B2A_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, ec::lstm_kernel, 256, smem));
+        B2A_CHECK((long long)per_sm * num_sms >= grid, B2A_ERR_INVALID_INPUT, "encodec: LSTM too wide for a co-resident grid");
+        for (int n0 = 0; n0 < N; n0 += ec::LSTM_BC) {
+            ec::LstmArgs la{};
+            la.xproj = xp.p; la.skip = x; la.out = y; la.bar = bar.p; la.n0 = n0; la.nb = std::min(ec::LSTM_BC, N - n0); la.T = T; la.H = H; la.NL = NL;
+            for (int l = 0; l < NL; ++l) { la.Wh[l] = m.Wh[l].p; la.Wx[l] = m.Wx[l].p; la.bias[l] = m.b[l].p; la.hseq[l] = hseq[l].p; }
+            B2A_CUDA(cudaMemsetAsync(bar.p, 0, sizeof(unsigned), s));
+            void* params[] = {&la};
+            B2A_CUDA(cudaLaunchCooperativeKernel((void*)ec::lstm_kernel, dim3(grid), dim3(256), params, smem, s));
+            count_launch();
+        }
+        std::swap(x, y);
+    }
+
     // d_codes [n_chunks, B, n_q_used, T] int32 (device), d_scales [n_chunks, B] or null -> d_wave [B, out_len, channels]
     void decode_dev(const int* d_codes, int n_chunks, int B, int nq, int T, const float* d_scales, float* d_wave, cudaStream_t s) {
         B2A_CHECK(n_chunks >= 1 && B >= 1 && T >= 1, B2A_ERR_INVALID_INPUT, "encodec decode: empty input");
@@ -599,39 +891,7 @@ struct b2a_encodec {
             std::swap(x, y);
         }
         // 3. LSTM block
-        if (cfg.num_lstm_layers > 0) {
-            const int H = dim0, NL = cfg.num_lstm_layers;
-            xp.alloc((size_t)N * T * 4 * H);
-            for (int l = 0; l < NL; ++l) hseq[l].alloc((size_t)N * T * H);
-            {
-                ec::ConvArgs a{};
-                a.xa = x; a.La = T; a.Ca = H; a.taps = 1; a.A = xproj.A.p; a.bias = xproj.bias.p; a.M = 4 * H; a.K = H; a.Lq = T; a.N = N;
-                a.out = xp.p; a.out_per_n = (long long)T * 4 * H;
-                run_conv(a, s);
-            }
-            const size_t smem = ((size_t)(2 * NL - 1) * 16 * H + (size_t)NL * ec::LSTM_BC * H + NL * 16 * ec::LSTM_BC + NL * ec::LSTM_UNITS * ec::LSTM_BC) * sizeof(float);
-            B2A_CHECK(smem <= 220 * 1024, B2A_ERR_INVALID_INPUT, "encodec: LSTM slice does not fit shared memory");
-            B2A_CUDA(cudaFuncSetAttribute(ec::lstm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            const int grid = H / ec::LSTM_UNITS;
-            int per_sm = 0;
-            B2A_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, ec::lstm_kernel, 256, smem));
-            B2A_CHECK((long long)per_sm * num_sms >= grid, B2A_ERR_INVALID_INPUT, "encodec: LSTM too wide for a co-resident grid");
-            for (int n0 = 0; n0 < N; n0 += ec::LSTM_BC) {
-                ec::LstmArgs la{};
-                la.xproj = xp.p; la.skip = x; la.out = y; la.bar = bar.p; la.n0 = n0; la.nb = std::min(ec::LSTM_BC, N - n0); la.T = T; la.H = H; la.NL = NL;
-                for (int l = 0; l < NL; ++l) { la.Wh[l] = lWh[l].p; la.Wx[l] = lWx[l].p; la.bias[l] = lb[l].p; la.hseq[l] = hseq[l].p; }
-                B2A_CUDA(cudaMemsetAsync(bar.p, 0, sizeof(unsigned), s));
-                void* params[] = {&la};
-                B2A_CUDA(cudaLaunchCooperativeKernel((void*)ec::lstm_kernel, dim3(grid), dim3(256), params, smem, s));
-                count_launch();
-            }
-            std::swap(x, y);
-        } else {
-            // an EncodecLSTMBlock without layers still adds its skip: h + hiddenStates = 2x (EncodecLayers.swift:82-88)
-            const long long cnt = (long long)N * T * dim0;
-            ec::scale_kernel<<<cdiv(cnt, 256), 256, 0, s>>>(x, cnt, 2.f);
-            count_launch();
-        }
+        run_lstm_block(lstm, x, y, N, T, dim0, s);
         // 4. upsampling stages
         long long L = T;
         for (auto& st : stages) {
@@ -649,22 +909,7 @@ struct b2a_encodec {
                 std::swap(x, y);
             }
             L = Lo;
-            {
-                const int hid = st.r1.M;
-                ec::ConvArgs a{};
-                a.xa = x; a.La = (int)L; a.Ca = st.cout; a.taps = cfg.residual_kernel_size; pads(cfg.residual_kernel_size, a.padL); a.reflect = cfg.pad_mode_reflect; a.elu_a = 1;
-                a.A = st.r1.A.p; a.bias = st.r1.bias.p; a.M = hid; a.K = st.r1.K; a.Lq = (int)L; a.N = N; a.out = z; a.out_per_n = L * hid;
-                run_conv(a, s);
-                ec::ConvArgs b{};
-                b.N = N; b.Lq = (int)L; b.M = st.cout; b.K = st.r2.K; b.A = st.r2.A.p; b.bias = st.r2.bias.p; b.out = y; b.out_per_n = L * st.cout;
-                if (cfg.use_conv_shortcut) {
-                    b.xa = x; b.La = (int)L; b.Ca = st.cout; b.taps = 1; b.xb = z; b.Cb = hid; b.elu_b = 1;
-                } else {
-                    b.xa = z; b.La = (int)L; b.Ca = hid; b.taps = 1; b.elu_a = 1; b.res = x;
-                }
-                run_conv(b, s);
-                std::swap(x, y);
-            }
+            run_resnet(st.res, x, y, z, N, L, st.cout, s);
         }
         // 5. ELU -> last conv (+ per-chunk scale), 6. overlap-add when chunked
         const bool chunked = chunk_length() != 0;
@@ -683,6 +928,110 @@ struct b2a_encodec {
             const long long total = out_len(n_chunks, T);
             const int hopc = chunk_stride() > 0 ? chunk_stride() : 1;
             ec::overlap_add_kernel<<<dim3(cdiv(total, 256), B), 256, 0, s>>>(chunks.p, d_wave, n_chunks, B, (int)L, CH, hopc, total);
+            count_launch();
+        }
+        B2A_CUDA(cudaGetLastError());
+    }
+
+    // ---- encode (Encodec.swift:212-291)
+    // EncodecConv1d's output length (EncodecLayers.swift:139-145, 191-205): padding_total = k - stride plus the extra right
+    // padding that completes the last window, in the reference's Float arithmetic
+    static long long conv_out_len(long long L, int k, int stride) {
+        const int pt = k - stride;
+        const float n_frames = (float)(L - k + pt) / (float)stride + 1.f;
+        const long long ideal = ((long long)std::ceil(n_frames) - 1) * stride + k - pt;
+        const long long extra = std::max(0ll, ideal - L);
+        return (L + pt + extra - k) / stride + 1;
+    }
+    struct EncShape { int n_chunks, chunk_len, chunk_stride, frames; };
+    // encode's chunk loop (:267-287): offsets 0, stride, ... below samples - (chunk_len - stride), every chunk the same length
+    // (what MLX.stacked needs); frames = the encoder's output length for one chunk
+    EncShape encoded_shape(long long samples) const {
+        B2A_CHECK(has_enc, B2A_ERR_MODEL_NOT_INITIALIZED, enc_error);
+        B2A_CHECK(samples >= 1, B2A_ERR_INVALID_INPUT, "encodec encode: empty input");
+        B2A_CHECK(samples < (1ll << 30), B2A_ERR_INVALID_INPUT, "encodec encode: too long");
+        const long long clen = chunk_length() > 0 ? chunk_length() : samples;
+        const long long stride = chunk_stride() > 0 ? chunk_stride() : samples;
+        const long long step = clen - stride;
+        B2A_CHECK(samples - step > 0, B2A_ERR_INVALID_INPUT, "encodec encode: input shorter than one chunk step");
+        const long long n = (samples - step + stride - 1) / stride;
+        const long long first = std::min(clen, samples), last = std::min(clen, samples - (n - 1) * stride);
+        B2A_CHECK(first == last && last >= 1, B2A_ERR_INVALID_INPUT,
+                  "encodec encode: the last chunk would be shorter than the others (chunks of unequal length cannot be stacked)");
+        long long L = first;
+        for (auto& st : estages) L = conv_out_len(L, 2 * st.ratio, st.ratio);
+        return EncShape{(int)n, (int)first, (int)(n > 1 ? stride : 0), (int)L};
+    }
+
+    // d_audio [B, samples, audio_channels] -> d_codes [n_chunks, B, nq, frames] (+ d_scales [n_chunks, B] when normalize, if
+    // given); the latent z stays in zbuf [n_chunks*B, frames, hidden]
+    void encode_dev(const float* d_audio, int B, long long samples, int nq, int* d_codes, float* d_scales, cudaStream_t s) {
+        B2A_CHECK(B >= 1, B2A_ERR_INVALID_INPUT, "encodec encode: empty input");
+        const EncShape sh = encoded_shape(samples);
+        B2A_CHECK(nq >= 1 && nq <= n_q, B2A_ERR_INVALID_INPUT, "encodec encode: n_q must be in [1, the codebooks the checkpoint holds]");
+        B2A_CUDA(cudaSetDevice(device));
+        const int N = sh.n_chunks * B, CH = cfg.audio_channels, F = cfg.num_filters, D = cfg.codebook_dim;
+        long long L = sh.chunk_len;
+        B2A_CHECK((long long)N * L * 64 < (1ll << 40) && (long long)B * samples * CH < (1ll << 40), B2A_ERR_INVALID_INPUT, "encodec encode: too long");
+        // the widest activation: max over stages of N * L * C (the LSTM and z have buffers of their own)
+        size_t big = (size_t)N * L * F;
+        {
+            long long l = L;
+            for (auto& st : estages) { l = conv_out_len(l, 2 * st.ratio, st.ratio); big = std::max(big, (size_t)((long long)N * l * st.cout)); }
+        }
+        bufA.alloc(big); bufB.alloc(big); bufC.alloc(big);
+        float* x = bufA.p; float* y = bufB.p; float* z = bufC.p;
+        // 1. per-chunk scale (normalize), 2. stem on the waveform in place
+        const float* sc = nullptr;
+        if (cfg.normalize) {
+            float* dst = d_scales;
+            if (!dst) { scales.alloc((size_t)N); dst = scales.p; }
+            ec::chunk_scale_kernel<<<N, 256, 0, s>>>(d_audio, dst, B, samples, CH, sh.chunk_len, sh.chunk_stride);
+            count_launch();
+            sc = dst;
+        }
+        {
+            int padL; pads(cfg.kernel_size, padL);
+            const int k = cfg.kernel_size;
+            const size_t smem = ((size_t)F * k * CH + (size_t)(ec::STEM_T + k - 1) * CH) * sizeof(float);
+            B2A_CHECK(smem <= 200 * 1024, B2A_ERR_INVALID_INPUT, "encodec: stem too wide");
+            B2A_CUDA(cudaFuncSetAttribute(ec::stem_conv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            ec::stem_conv_kernel<<<dim3(cdiv(L, ec::STEM_T), N), 256, smem, s>>>(d_audio, wstem.p, bstem.p, sc, x, B, samples, CH, sh.chunk_len,
+                                                                                sh.chunk_stride, F, k, padL, cfg.pad_mode_reflect);
+            count_launch();
+        }
+        // 3. downsampling stages: resnet, ELU + conv k = 2r stride r (one implicit-GEMM launch; ELU fused on its input)
+        for (auto& st : estages) {
+            if (cfg.num_residual_layers > 0) run_resnet(st.res, x, y, z, N, L, st.cin, s);
+            const int r = st.ratio, k = 2 * r;
+            const long long Lo = conv_out_len(L, k, r);
+            ec::ConvArgs a{};
+            a.xa = x; a.La = (int)L; a.Ca = st.cin; a.taps = k; a.stride = r; a.elu_a = 1; a.reflect = cfg.pad_mode_reflect;
+            a.padL = cfg.use_causal_conv ? k - r : (k - r) - (k - r) / 2;     // the right pad and the extra pad: src_index's edge rule
+            a.A = st.down.A.p; a.bias = st.down.bias.p; a.M = st.down.M; a.K = st.down.K; a.Lq = (int)Lo; a.N = N;
+            a.out = y; a.out_per_n = Lo * st.cout;
+            run_conv(a, s);
+            std::swap(x, y);
+            L = Lo;
+        }
+        const int T = (int)L, H = F << estages.size();
+        // 4. LSTM block, 5. ELU -> last conv -> z
+        run_lstm_block(elstm, x, y, N, T, H, s);
+        zbuf.alloc((size_t)N * T * D);
+        {
+            ec::ConvArgs a{};
+            a.xa = x; a.La = T; a.Ca = H; a.taps = cfg.last_kernel_size; pads(cfg.last_kernel_size, a.padL); a.reflect = cfg.pad_mode_reflect; a.elu_a = 1;
+            a.A = elast.A.p; a.bias = elast.bias.p; a.M = elast.M; a.K = elast.K; a.Lq = T; a.N = N; a.out = zbuf.p; a.out_per_n = (long long)T * D;
+            run_conv(a, s);
+        }
+        // 6. residual VQ encode
+        {
+            const int ld = D + 1;
+            const size_t smem = ((size_t)(ec::VQ_FT + ec::VQ_KT) * ld + ec::VQ_KT + 2 * ec::VQ_FT) * sizeof(float);
+            B2A_CHECK(smem <= 220 * 1024, B2A_ERR_INVALID_INPUT, "encodec: codebook_dim too large for the code search");
+            B2A_CUDA(cudaFuncSetAttribute(ec::rvq_encode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            const int rows = N * T;
+            ec::rvq_encode_kernel<<<cdiv(rows, ec::VQ_FT), 256, smem, s>>>(zbuf.p, books.p, book_sq.p, d_codes, rows, T, nq, cfg.codebook_size, D);
             count_launch();
         }
         B2A_CUDA(cudaGetLastError());
@@ -734,6 +1083,60 @@ int32_t b2a_encodec_decode(b2a_encodec* h, const int32_t* codes, int32_t n_chunk
         h->decode_dev(h->codes.p, n_chunks, B, nq, T, dsc, h->wave.p, s);
         B2A_CUDA(cudaMemcpyAsync(wave, h->wave.p, nout * sizeof(float), cudaMemcpyDeviceToHost, s));
         B2A_CUDA(cudaStreamSynchronize(s));
+    });
+}
+
+int32_t b2a_encodec_encoded_shape(const b2a_encodec* h, int64_t samples, int32_t* n_chunks, int32_t* frames) {
+    return guarded([&] {
+        B2A_CHECK(h && n_chunks && frames, B2A_ERR_INVALID_INPUT, "b2a_encodec_encoded_shape: null argument");
+        const auto sh = h->encoded_shape(samples);
+        *n_chunks = sh.n_chunks;
+        *frames = sh.frames;
+    });
+}
+
+int32_t b2a_encodec_encode_dev(b2a_encodec* h, const float* d_audio, int32_t batch, int64_t samples, int32_t n_q, int32_t* d_codes,
+                               float* d_scales, void* stream) {
+    return guarded([&] {
+        B2A_CHECK(h && d_audio && d_codes, B2A_ERR_INVALID_INPUT, "b2a_encodec_encode_dev: null argument");
+        h->encode_dev(d_audio, batch, samples, n_q, d_codes, d_scales, stream ? (cudaStream_t)stream : h->stream);
+    });
+}
+
+// host entry: stage the waveform, encode on the handle's stream, copy codes (and scales) back; z_out (test hook) gets the latent
+static void encodec_encode_host(b2a_encodec* h, const float* audio, int32_t batch, int64_t samples, int32_t n_q, int32_t* codes,
+                                float* scales, float* z_out) {
+    B2A_CHECK(h && audio && (codes || z_out), B2A_ERR_INVALID_INPUT, "b2a_encodec_encode: null argument");
+    B2A_CHECK(batch >= 1, B2A_ERR_INVALID_INPUT, "encodec encode: empty input");
+    const auto sh = h->encoded_shape(samples);
+    B2A_CHECK(n_q >= 1 && n_q <= h->n_q, B2A_ERR_INVALID_INPUT, "encodec encode: n_q must be in [1, the codebooks the checkpoint holds]");
+    B2A_CUDA(cudaSetDevice(h->device));
+    cudaStream_t s = h->stream;
+    const size_t nin = (size_t)batch * samples * h->cfg.audio_channels, N = (size_t)sh.n_chunks * batch;
+    const size_t ncodes = N * n_q * sh.frames;
+    h->audio.alloc(nin); h->codes.alloc(ncodes);
+    const bool want_scales = h->cfg.normalize && scales;
+    if (want_scales) h->scales.alloc(N);
+    B2A_CUDA(cudaMemcpyAsync(h->audio.p, audio, nin * sizeof(float), cudaMemcpyHostToDevice, s));
+    h->encode_dev(h->audio.p, batch, samples, n_q, h->codes.p, want_scales ? h->scales.p : nullptr, s);
+    if (codes) B2A_CUDA(cudaMemcpyAsync(codes, h->codes.p, ncodes * sizeof(int), cudaMemcpyDeviceToHost, s));
+    if (want_scales) B2A_CUDA(cudaMemcpyAsync(scales, h->scales.p, N * sizeof(float), cudaMemcpyDeviceToHost, s));
+    if (z_out) B2A_CUDA(cudaMemcpyAsync(z_out, h->zbuf.p, N * sh.frames * h->cfg.codebook_dim * sizeof(float), cudaMemcpyDeviceToHost, s));
+    B2A_CUDA(cudaStreamSynchronize(s));
+}
+
+int32_t b2a_encodec_encode(b2a_encodec* h, const float* audio, int32_t batch, int64_t samples, int32_t n_q, int32_t* codes,
+                           float* scales) {
+    return guarded([&] {
+        B2A_CHECK(codes, B2A_ERR_INVALID_INPUT, "b2a_encodec_encode: null argument");
+        encodec_encode_host(h, audio, batch, samples, n_q, codes, scales, nullptr);
+    });
+}
+
+int32_t b2a_encodec_encode_latent_test(b2a_encodec* h, const float* audio, int32_t batch, int64_t samples, float* z) {
+    return guarded([&] {
+        B2A_CHECK(z, B2A_ERR_INVALID_INPUT, "b2a_encodec_encode_latent_test: null argument");
+        encodec_encode_host(h, audio, batch, samples, 1, nullptr, nullptr, z);
     });
 }
 

@@ -1,8 +1,9 @@
-"""Host-side mirror of `Encodec`'s decode side (Sources/MLXAudioCodecs/Encodec/Encodec.swift:170-461) behind
-AudioCodecModel / AudioDecoderModel (Sources/MLXAudioCodecs/AudioCodecModel.swift:4-27), over the C ABI."""
+"""Host-side mirror of `Encodec` (Sources/MLXAudioCodecs/Encodec/Encodec.swift:170-461) behind AudioCodecModel (encode and
+decode) (Sources/MLXAudioCodecs/AudioCodecModel.swift:4-27), over the C ABI."""
 from __future__ import annotations
 
 import ctypes as C
+import math
 from dataclasses import dataclass, field
 from typing import Dict, List, Optional, Sequence
 
@@ -67,6 +68,7 @@ class Encodec:
         c.trim_right_ratio = float(config.trim_right_ratio)
         c.chunk_length_s = float(config.chunk_length_s) if config.chunk_length_s is not None else 0.0
         c.overlap = float(config.overlap) if config.overlap is not None else -1.0
+        c.normalize = int(config.normalize)
         table, keep = _ffi.make_tensor_table(weights)
         self._h = C.c_void_p()
         _ffi.check(_ffi.lib().b2a_encodec_create(device, C.byref(c), table, len(weights), C.byref(self._h)))
@@ -119,8 +121,9 @@ class Encodec:
         return int(_ffi.lib().b2a_encodec_stream(self._h) or 0)
 
     @staticmethod
-    def random_init_weights(config: EncodecConfig, seed: int = 1234, n_codebooks: int = 8) -> Dict[str, np.ndarray]:
-        """Random-init weights with the checkpoint's keys / MLX layouts (benchmarks): U(+-1/sqrt(fan_in)), N(0,1) codebooks."""
+    def random_init_weights(config: EncodecConfig, seed: int = 1234, n_codebooks: int = 8, encoder: bool = False) -> Dict[str, np.ndarray]:
+        """Random-init weights with the checkpoint's keys / MLX layouts (benchmarks): U(+-1/sqrt(fan_in)), N(0,1) codebooks.
+        encoder=True appends the encoder's weights (drawn after everything else, so the decoder / codebooks do not change)."""
         rng = np.random.default_rng(seed)
         w: Dict[str, np.ndarray] = {}
 
@@ -156,6 +159,25 @@ class Encodec:
             scaling //= 2
         i += 1
         conv(f"decoder.layers.{i}.", config.audio_channels, config.last_kernel_size, config.num_filters)
+        if encoder:                     # EncodecEncoder's module array (Encodec.swift:20-70), ELU slots counted
+            i, cur = 0, config.num_filters
+            conv(f"encoder.layers.{i}.", cur, config.kernel_size, config.audio_channels); i += 1
+            for ratio in reversed(config.upsampling_ratios):
+                for _ in range(config.num_residual_layers):
+                    hid = cur // config.compress
+                    conv(f"encoder.layers.{i}.block.1.", hid, config.residual_kernel_size, cur)
+                    conv(f"encoder.layers.{i}.block.3.", cur, 1, hid)
+                    if config.use_conv_shortcut:
+                        conv(f"encoder.layers.{i}.shortcut.", cur, 1, cur)
+                    i += 1
+                i += 1
+                conv(f"encoder.layers.{i}.", 2 * cur, 2 * ratio, cur); i += 1
+                cur *= 2
+            for l in range(config.num_lstm_layers):
+                for n, shape in (("Wx", (4 * cur, cur)), ("Wh", (4 * cur, cur)), ("bias", (4 * cur,))):
+                    w[f"encoder.layers.{i}.lstm.{l}.{n}"] = u(shape, cur)
+            i += 2
+            conv(f"encoder.layers.{i}.", config.hidden_size, config.last_kernel_size, cur)
         return w
 
     def output_length(self, n_chunks: int, frames: int) -> int:
@@ -188,6 +210,86 @@ class Encodec:
         nc, B, nq, T = d_codes.shape
         _ffi.check(_ffi.lib().b2a_encodec_decode_dev(self._h, _ffi.ptr(d_codes), nc, B, nq, T, _ffi.ptr(d_scales), _ffi.ptr(d_wave),
                                                      C.c_void_p(stream)))
+
+    # ---- encode side (Encodec.swift:212-291, 457-460)
+    def num_quantizers_for_bandwidth(self, bandwidth: Optional[float]) -> int:
+        """getNumQuantizersForBandwidth (EncodecQuantization.swift:90-97), in the reference's Float arithmetic."""
+        c = self.config
+        frame_rate = math.ceil(c.sampling_rate / int(np.prod(c.upsampling_ratios)))
+        n = int(1000 * max(c.target_bandwidths) / (frame_rate * 10))
+        bw_per_q = np.float32(math.log2(c.codebook_size)) * np.float32(frame_rate)
+        if bandwidth is not None and bandwidth > 0.0:
+            n = max(1, int(math.floor(np.float32(bandwidth) * np.float32(1000) / bw_per_q)))
+        return n
+
+    def encoded_shape(self, samples: int):
+        """(n_chunks, frames) of the codes of a `samples`-long input (encode's chunk loop, Encodec.swift:267-287)."""
+        nc, fr = C.c_int32(0), C.c_int32(0)
+        _ffi.check(_ffi.lib().b2a_encodec_encoded_shape(self._h, int(samples), C.byref(nc), C.byref(fr)))
+        return nc.value, fr.value
+
+    def _bandwidth_codebooks(self, bandwidth: Optional[float]) -> int:
+        bw = self.config.target_bandwidths[0] if bandwidth is None else bandwidth
+        if bw not in self.config.target_bandwidths:       # the reference's fatalError (Encodec.swift:253-255)
+            raise _ffi.AudioGenerationError(_ffi.ERR_INVALID_INPUT,
+                                            f"This model doesn't support bandwidth {bw}. Select one of {self.config.target_bandwidths}")
+        return self.num_quantizers_for_bandwidth(bw)
+
+    def _check_audio_shape(self, shape) -> None:
+        if len(shape) != 3 or shape[2] != self.config.audio_channels:
+            raise _ffi.AudioGenerationError(_ffi.ERR_INVALID_INPUT,
+                                            f"expected audio [B, samples, {self.config.audio_channels}], got {tuple(shape)}")
+
+    def encode(self, input_values, padding_mask=None, bandwidth: Optional[float] = None):
+        """encode(_:paddingMask:bandwidth:) (Encodec.swift:245-291): [B, samples, channels] -> (codes [n_chunks, B, n_q, frames]
+        int32, scales: per chunk a [B] float32 array with normalize, else None)."""
+        x = np.ascontiguousarray(input_values, dtype=np.float32)
+        self._check_audio_shape(x.shape)
+        nq = self._bandwidth_codebooks(bandwidth)
+        if padding_mask is not None and self.config.normalize:    # only ever `values * mask` ahead of the normalisation (:224-226)
+            x = np.ascontiguousarray(x * np.asarray(padding_mask, dtype=np.float32).reshape(x.shape[0], x.shape[1], 1))
+        B, n, _ = x.shape
+        nc, T = self.encoded_shape(n)
+        codes = np.empty((nc, B, nq, T), dtype=np.int32)
+        scales = np.empty((nc, B), dtype=np.float32) if self.config.normalize else None
+        _ffi.check(_ffi.lib().b2a_encodec_encode(self._h, _ffi.ptr(x), B, n, nq, _ffi.ptr(codes), _ffi.ptr(scales)))
+        return codes, ([scales[i] for i in range(nc)] if scales is not None else [None] * nc)
+
+    def encode_audio(self, waveform) -> EncodecEncodedAudio:
+        """AudioCodecModel.encodeAudio (Encodec.swift:457-460): default bandwidth, no padding mask."""
+        codes, scales = self.encode(waveform)
+        return EncodecEncodedAudio(codes, scales)
+
+    def reconstruct(self, waveform) -> np.ndarray:
+        """AudioCodecModel.reconstruct: decodeAudio(encodeAudio(x))."""
+        return self.decode_audio(self.encode_audio(waveform))
+
+    def encode_dev(self, d_audio, d_codes, d_scales=None, stream: int = 0, bandwidth: Optional[float] = None) -> None:
+        """Device-resident encode: torch CUDA float32 d_audio [B, samples, channels] -> int32 d_codes [n_chunks, B, n_q, frames]
+        (+ float32 d_scales [n_chunks, B] with normalize), enqueued on `stream`.  n_q follows `bandwidth` as in encode."""
+        import torch
+        if not isinstance(d_audio, torch.Tensor):
+            raise _ffi.AudioGenerationError(_ffi.ERR_INVALID_INPUT, "d_audio must be a CUDA tensor")
+        self._check_audio_shape(tuple(d_audio.shape))
+        B, n, ch = d_audio.shape
+        self._check_dev(d_audio, "float32", (B, n, ch), "d_audio")
+        nq = self._bandwidth_codebooks(bandwidth)
+        nc, T = self.encoded_shape(n)
+        self._check_dev(d_codes, "int32", (nc, B, nq, T), "d_codes")
+        if d_scales is not None:
+            self._check_dev(d_scales, "float32", (nc, B), "d_scales")
+        _ffi.check(_ffi.lib().b2a_encodec_encode_dev(self._h, _ffi.ptr(d_audio), B, n, nq, _ffi.ptr(d_codes), _ffi.ptr(d_scales),
+                                                     C.c_void_p(stream)))
+
+    @staticmethod
+    def _check_dev(t, dtype: str, shape, what: str) -> None:
+        # the library reads / writes exactly these extents through raw device pointers: anything else is an input error, not a fault
+        import torch
+        ok = (isinstance(t, torch.Tensor) and t.is_cuda and t.dtype == getattr(torch, dtype) and t.is_contiguous()
+              and tuple(t.shape) == tuple(shape))
+        if not ok:
+            got = tuple(t.shape) if hasattr(t, "shape") else type(t).__name__
+            raise _ffi.AudioGenerationError(_ffi.ERR_INVALID_INPUT, f"{what}: expected a contiguous CUDA {dtype} tensor {tuple(shape)}, got {got}")
 
     def __del__(self):
         try:
