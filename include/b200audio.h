@@ -655,6 +655,11 @@ void* b2a_qwen3_talker_stream(b2a_qwen3_talker* h);
 /* out [n, hidden] float32 (host): text_projection(text_embedding(ids)) resp. codec_embedding(ids) */
 int32_t b2a_qwen3_talker_embed_text(b2a_qwen3_talker* h, const int32_t* ids, int32_t n, float* out);
 int32_t b2a_qwen3_talker_embed_codec(b2a_qwen3_talker* h, const int32_t* ids, int32_t n, float* out);
+/* codecEmbedIcl's frame rows (Qwen3TTS.swift:249-265), the reference-code part of a voice-cloning (ICL) prompt: codes [n, groups]
+ * int32 (row r = frame r's first `groups` code groups, 1 <= groups <= num_code_groups; fewer groups than num_code_groups is the
+ * reference's `break`) -> out [n, hidden] = codec_embedding(c0) + sum over g = 1 .. groups-1 of code_predictor.codec_embedding[g-1](c_g),
+ * the same sum the frame loop feeds back.  The leading codec_bos row is the caller's (b2a_qwen3_talker_embed_codec).          */
+int32_t b2a_qwen3_talker_embed_code_frames(b2a_qwen3_talker* h, const int32_t* codes, int32_t n, int32_t groups, float* out);
 /* Parity hook: the talker over input_embeds [B, L, hidden] from an empty cache -> codec logits of the LAST position
  * [B, vocab] and its final-norm hidden state [B, hidden] (Qwen3TTSTalker.swift:340-350).                                   */
 int32_t b2a_qwen3_talker_forward(b2a_qwen3_talker* h, const float* input_embeds, int32_t batch, int32_t len, float* logits_out,
@@ -679,6 +684,67 @@ int32_t b2a_qwen3_talker_create_from_directory(const char* model_dir, int32_t de
                                                b2a_qwen3_talker** out);
 int32_t b2a_qwen3_talker_cancel(b2a_qwen3_talker* h);
 void b2a_qwen3_talker_destroy(b2a_qwen3_talker* h);
+
+/* ------------------------------------------------------------------ Qwen3-TTS speech-tokenizer ENCODER (24 kHz audio -> 12.5 Hz codes)
+ * Replaces Qwen3TTSSpeechTokenizerEncoder.encode (Sources/MLXAudioTTS/Models/Qwen3TTS/Qwen3TTSSpeechTokenizer.swift:790-884), the
+ * speechTokenizer.encode(refAudio) step of the in-context-learning (voice-cloning) prompt (Qwen3TTS.swift:267-302): the Mimi
+ * SEANet encoder (causal, zero padding), the 8-layer transformer (interleaved RoPE, full causal attention over the clip), the
+ * edge-padded stride-2 downsample and the split residual quantizer's code search, cut to valid_num_quantizers code groups.
+ * audio is [B, 1, n] float32 (mono 24 kHz), codes are [B, valid_num_quantizers, encoded_length(n)] int32.
+ * A separate handle from the decoder's b2a_speech_tokenizer, so b2a_speech_tokenizer_config keeps its layout.  Config defaults:
+ * Qwen3TTSConfig.swift:391-494 and encoder_valid_num_quantizers (:518-527).  Errors: a checkpoint without encoder tensors ->
+ * B2A_ERR_MODEL_NOT_INITIALIZED (the reference's hasEncoder == false); empty audio -> B2A_ERR_AUDIO_ENCODING_FAILED; audio_channels
+ * != 1, num_residual_layers != 1, a geometry the device path does not run, sizes whose indices would overflow ->
+ * B2A_ERR_INVALID_INPUT.  Deterministic: the same input gives the same codes, batched or one row at a time.                  */
+typedef struct b2a_speech_tokenizer_encoder_config {
+    int32_t sampling_rate;
+    float frame_rate;
+    int32_t audio_channels;
+    int32_t num_filters;
+    int32_t num_residual_layers;
+    int32_t num_upsampling_ratios;
+    int32_t upsampling_ratios[8]; /* the decoder order; the encoder runs them reversed */
+    int32_t kernel_size;
+    int32_t residual_kernel_size;
+    int32_t last_kernel_size;
+    int32_t compress;
+    int32_t use_causal_conv;
+    int32_t use_conv_shortcut;
+    int32_t hidden_size;
+    int32_t intermediate_size;
+    int32_t num_hidden_layers;
+    int32_t num_attention_heads;
+    int32_t num_key_value_heads;
+    int32_t head_dim;
+    float rope_theta;
+    int32_t codebook_size;
+    int32_t codebook_dim;
+    int32_t num_quantizers;
+    int32_t valid_num_quantizers; /* encoder_valid_num_quantizers: the code groups encode returns */
+} b2a_speech_tokenizer_encoder_config;
+
+typedef struct b2a_speech_tokenizer_encoder b2a_speech_tokenizer_encoder;
+/* tensors: b2a_weights_sanitize_speech_tokenizer_encoder's keys (encoder.*, encoder_transformer.*, downsample.*, quantizer.*) */
+int32_t b2a_speech_tokenizer_encoder_create(int32_t device, const b2a_speech_tokenizer_encoder_config* cfg, const b2a_tensor* tensors,
+                                            int32_t n_tensors, b2a_speech_tokenizer_encoder** out);
+/* code frames for n samples: ceil(ceil(n / 960) / 2) at the shipped geometry (0 for n < 1 or a null handle) */
+int64_t b2a_speech_tokenizer_encoder_encoded_length(const b2a_speech_tokenizer_encoder* h, int64_t n_samples);
+int32_t b2a_speech_tokenizer_encoder_num_code_groups(const b2a_speech_tokenizer_encoder* h);
+int32_t b2a_speech_tokenizer_encoder_encode(b2a_speech_tokenizer_encoder* h, const float* audio, int32_t batch, int64_t n_samples,
+                                            int32_t* codes);
+/* device buffers, enqueued on `stream` (NULL: the handle's stream) without a host synchronisation */
+int32_t b2a_speech_tokenizer_encoder_encode_dev(b2a_speech_tokenizer_encoder* h, const float* d_audio, int32_t batch, int64_t n_samples,
+                                                int32_t* d_codes, void* stream);
+void* b2a_speech_tokenizer_encoder_stream(b2a_speech_tokenizer_encoder* h);
+void b2a_speech_tokenizer_encoder_destroy(b2a_speech_tokenizer_encoder* h);
+/* Loading: the encoder half of Qwen3TTSSpeechTokenizer.sanitize (:1093-1440) on an open checkpoint (encoder.encoder.layers.N ->
+ * SEANet paths, separate or fused q|k|v -> in_proj, norms, layer scales, downsample, semantic_/acoustic_residual_vector_quantizer
+ * or rvq_first/rvq_rest -> rvq_first/rvq_rest with their codebook statistics; every other key dropped); config.json's
+ * "encoder_config" and "encoder_valid_num_quantizers" (a missing file or block -> B2A_ERR_MODEL_NOT_INITIALIZED); both from a
+ * directory.                                                                                                                  */
+int32_t b2a_weights_sanitize_speech_tokenizer_encoder(b2a_weights* w);
+int32_t b2a_speech_tokenizer_encoder_config_from_json(const char* config_path, b2a_speech_tokenizer_encoder_config* cfg);
+int32_t b2a_speech_tokenizer_encoder_create_from_directory(const char* dir, int32_t device, b2a_speech_tokenizer_encoder** out);
 
 #ifdef __cplusplus
 }

@@ -52,6 +52,10 @@ int32_t b2a_speech_tokenizer_debug_layout(const float* w, int32_t out, int32_t k
  * output before the final norm, 1 + i = upsample layer i, 10 + 4 b = decoder block b after its transposed conv, 11 + 4 b + j = after
  * its residual unit j); out != null first copies the last kept tensor to the host (capacity in floats, length in *n).            */
 int32_t b2a_speech_tokenizer_debug_stage(b2a_speech_tokenizer* h, int32_t stage, float* out, int64_t capacity, int64_t* n);
+/* tests/test_gpu_qwen3_tts_encode.py: the speech-tokenizer encoder's code-search input z [B, encoded_length, hidden_size] float32
+ * (the downsample's output) for audio [B, 1, n]; codes (nullable) receives the codes of the same run.                        */
+int32_t b2a_speech_tokenizer_encoder_latent_test(b2a_speech_tokenizer_encoder* h, const float* audio, int32_t batch, int64_t n_samples,
+                                                 float* z, int32_t* codes);
 /* tests/test_gpu_qwen3_sampler.py: the Qwen3-TTS in-graph sampler kernel (csrc/qwen3_sampler.cu = sampleToken,
  * Qwen3TTS.swift:1003-1118) on HOST logits [B, V <= 4096]; suppress [lo, hi) except eos; seen = bitmap of the tokens generated
  * so far [B, ceil(V/32)] (nullable; updated when track != 0); tokens_out [B]; filtered_out [B, V] (nullable) = the logits handed

@@ -85,6 +85,17 @@ class SpeechTokenizerConfig(C.Structure):
                    ("max_batch", C.c_int32), ("max_cache_frames", C.c_int32)])
 
 
+class SpeechTokenizerEncoderConfig(C.Structure):
+    _fields_ = ([("sampling_rate", C.c_int32), ("frame_rate", C.c_float)]
+                + [(n, C.c_int32) for n in ("audio_channels", "num_filters", "num_residual_layers", "num_upsampling_ratios")]
+                + [("upsampling_ratios", C.c_int32 * 8)]
+                + [(n, C.c_int32) for n in ("kernel_size", "residual_kernel_size", "last_kernel_size", "compress", "use_causal_conv",
+                                           "use_conv_shortcut", "hidden_size", "intermediate_size", "num_hidden_layers",
+                                           "num_attention_heads", "num_key_value_heads", "head_dim")]
+                + [("rope_theta", C.c_float)]
+                + [(n, C.c_int32) for n in ("codebook_size", "codebook_dim", "num_quantizers", "valid_num_quantizers")])
+
+
 class Qwen3TalkerConfig(C.Structure):
     _fields_ = ([(n, C.c_int32) for n in ("vocab_size", "hidden_size", "intermediate_size", "num_hidden_layers", "num_attention_heads",
                                            "num_key_value_heads", "head_dim")]
@@ -236,6 +247,17 @@ SIGNATURES = {
     "b2a_encodec_encode": (C.c_int32, [_P, _P, C.c_int32, C.c_int64, C.c_int32, _P, _P]),
     "b2a_encodec_encode_dev": (C.c_int32, [_P, _P, C.c_int32, C.c_int64, C.c_int32, _P, _P, _P]),
     "b2a_encodec_encode_latent_test": (C.c_int32, [_P, _P, C.c_int32, C.c_int64, _P]),
+    "b2a_speech_tokenizer_encoder_create": (C.c_int32, [C.c_int32, C.POINTER(SpeechTokenizerEncoderConfig), C.POINTER(Tensor), C.c_int32, C.POINTER(_P)]),
+    "b2a_speech_tokenizer_encoder_encoded_length": (C.c_int64, [_P, C.c_int64]),
+    "b2a_speech_tokenizer_encoder_num_code_groups": (C.c_int32, [_P]),
+    "b2a_speech_tokenizer_encoder_encode": (C.c_int32, [_P, _P, C.c_int32, C.c_int64, _P]),
+    "b2a_speech_tokenizer_encoder_encode_dev": (C.c_int32, [_P, _P, C.c_int32, C.c_int64, _P, _P]),
+    "b2a_speech_tokenizer_encoder_stream": (C.c_void_p, [_P]),
+    "b2a_speech_tokenizer_encoder_destroy": (None, [_P]),
+    "b2a_speech_tokenizer_encoder_latent_test": (C.c_int32, [_P, _P, C.c_int32, C.c_int64, _P, _P]),
+    "b2a_weights_sanitize_speech_tokenizer_encoder": (C.c_int32, [_P]),
+    "b2a_speech_tokenizer_encoder_config_from_json": (C.c_int32, [C.c_char_p, C.POINTER(SpeechTokenizerEncoderConfig)]),
+    "b2a_speech_tokenizer_encoder_create_from_directory": (C.c_int32, [C.c_char_p, C.c_int32, C.POINTER(_P)]),
     "b2a_encodec_destroy": (None, [_P]),
     "b2a_weights_load": (C.c_int32, [C.c_char_p, C.POINTER(_P)]),
     "b2a_weights_count": (C.c_int32, [_P]),
@@ -261,6 +283,7 @@ SIGNATURES = {
     "b2a_qwen3_talker_stream": (C.c_void_p, [_P]),
     "b2a_qwen3_talker_embed_text": (C.c_int32, [_P, _P, C.c_int32, _P]),
     "b2a_qwen3_talker_embed_codec": (C.c_int32, [_P, _P, C.c_int32, _P]),
+    "b2a_qwen3_talker_embed_code_frames": (C.c_int32, [_P, _P, C.c_int32, C.c_int32, _P]),
     "b2a_qwen3_talker_forward": (C.c_int32, [_P, _P, C.c_int32, C.c_int32, _P, _P]),
     "b2a_qwen3_talker_generate": (C.c_int32, [_P, _P, C.c_int32, C.c_int32, _P, _P, C.c_int32, _P, C.POINTER(Qwen3GenParams), _P, _P,
                                               C.POINTER(GenInfo), _P, _P]),

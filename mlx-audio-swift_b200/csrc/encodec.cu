@@ -24,14 +24,13 @@
 //     kernels sit only at the edges: the stem from 1-2 audio channels (reading each chunk of the waveform in place), the
 //     per-chunk RMS scale, and the residual code search in ordered fp32 (DESIGN.md §3.6b).
 #include "common.cuh"
+#include "seanet.cuh"
 
 #include <algorithm>
 #include <cmath>
 
 namespace b2a {
 namespace ec {
-
-__device__ __forceinline__ float elu1(float v) { return v > 0.f ? v : expm1f(v); }
 
 // ------------------------------------------------------------------ RVQ decode: sum of codebook gathers
 // codes [N, n_q, T] int32, books [n_q][size, dim] contiguous -> out [N, T, dim]
@@ -53,145 +52,6 @@ __global__ void rvq_sum_kernel(const int* __restrict__ codes, const float* __res
 __global__ void scale_kernel(float* __restrict__ x, long long n, float f) {
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) x[i] *= f;
-}
-
-// ------------------------------------------------------------------ implicit-GEMM conv / transposed conv
-struct ConvArgs {
-    // source A: taps over xa [N, La, Ca]
-    const float* xa; int La, Ca, taps, padL, reflect, elu_a, backward;   // forward: src = q*stride + tap - padL; backward: src = q - tap
-    int stride = 1;          // forward only: an encoder downsampling conv (k = 2s) gathers its 2s contiguous rows per output
-    // source B (optional): one tap at src = q over xb [N, Lq, Cb]
-    const float* xb; int Cb, elu_b;
-    const float* A;          // [M, K] row-major, K = taps*Ca + Cb
-    const float* bias;       // [M] or null
-    const float* res;        // optional residual, same addressing as out
-    float* out;              // [N, Tout, Cout]; element (q, m) lives at q*M + m - shift, valid inside [0, Tout*Cout)
-    int M, K, Lq, N;
-    long long out_per_n;     // Tout * Cout
-    long long shift;         // pl * Cout (left trim of a transposed conv)
-};
-
-constexpr int BK = 16;
-
-__device__ __forceinline__ int src_index(int q, int tap, const ConvArgs& a) {
-    if (a.backward) {
-        const int s = q - tap;
-        return (s >= 0 && s < a.La) ? s : -1;
-    }
-    int s = q * a.stride + tap - a.padL;
-    if (s < 0) return a.reflect ? min(-s, a.La - 1) : -1;
-    if (s >= a.La) return a.reflect ? max(a.La - 2 - (s - a.La), 0) : -1;
-    return s;
-}
-
-// BM outputs x BT tokens per CTA, 256 threads, thread (tx = tid % 16 -> m, ty = tid / 16 -> token).
-template <int BM, int BT>
-__global__ void __launch_bounds__(256) ec_conv_kernel(ConvArgs a) {
-    constexpr int RM = BM / 16, RT = BT / 16;
-    __shared__ __align__(16) float As[BK][BM + 4];
-    __shared__ __align__(16) float Xs[BK][BT + 4];
-    const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
-    const int n = blockIdx.z;
-    const int q0 = blockIdx.x * BT, m0 = blockIdx.y * BM;
-    const int Ka = a.taps * a.Ca;
-    float acc[RM][RT];
-#pragma unroll
-    for (int i = 0; i < RM; ++i)
-#pragma unroll
-        for (int j = 0; j < RT; ++j) acc[i][j] = 0.f;
-
-    // register double buffering: the global loads of k-tile i+1 are in flight while tile i is multiplied out of shared memory
-    constexpr int NA = (BM * 4 + 255) / 256, NX = (BT * 4 + 255) / 256;
-    float4 ra[NA], rx[NX];
-    auto load_tiles = [&](int k0) {
-#pragma unroll
-        for (int i = 0; i < NA; ++i) {
-            const int e = tid + i * 256;
-            const int m = e >> 2, k4 = (e & 3) * 4;
-            ra[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (e < BM * 4 && m0 + m < a.M && k0 + k4 < a.K) ra[i] = *reinterpret_cast<const float4*>(a.A + (long long)(m0 + m) * a.K + k0 + k4);
-        }
-#pragma unroll
-        for (int i = 0; i < NX; ++i) {
-            const int e = tid + i * 256;
-            const int t = e >> 2, k4 = (e & 3) * 4;
-            const int q = q0 + t, kk = k0 + k4;
-            float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (e < BT * 4 && q < a.Lq && kk < a.K) {
-                if (kk < Ka) {
-                    const int tap = kk / a.Ca, ci = kk - tap * a.Ca;
-                    const int s = src_index(q, tap, a);
-                    if (s >= 0) {
-                        v = *reinterpret_cast<const float4*>(a.xa + ((long long)n * a.La + s) * a.Ca + ci);
-                        if (a.elu_a) { v.x = elu1(v.x); v.y = elu1(v.y); v.z = elu1(v.z); v.w = elu1(v.w); }
-                    }
-                } else {
-                    v = *reinterpret_cast<const float4*>(a.xb + ((long long)n * a.Lq + q) * a.Cb + (kk - Ka));
-                    if (a.elu_b) { v.x = elu1(v.x); v.y = elu1(v.y); v.z = elu1(v.z); v.w = elu1(v.w); }
-                }
-            }
-            rx[i] = v;
-        }
-    };
-    auto store_tiles = [&]() {
-#pragma unroll
-        for (int i = 0; i < NA; ++i) {
-            const int e = tid + i * 256;
-            if (e < BM * 4) {
-                const int m = e >> 2, k4 = (e & 3) * 4;
-                As[k4 + 0][m] = ra[i].x; As[k4 + 1][m] = ra[i].y; As[k4 + 2][m] = ra[i].z; As[k4 + 3][m] = ra[i].w;
-            }
-        }
-#pragma unroll
-        for (int i = 0; i < NX; ++i) {
-            const int e = tid + i * 256;
-            if (e < BT * 4) {
-                const int t = e >> 2, k4 = (e & 3) * 4;
-                Xs[k4 + 0][t] = rx[i].x; Xs[k4 + 1][t] = rx[i].y; Xs[k4 + 2][t] = rx[i].z; Xs[k4 + 3][t] = rx[i].w;
-            }
-        }
-    };
-    load_tiles(0);
-    store_tiles();
-    __syncthreads();
-    for (int k0 = 0; k0 < a.K; k0 += BK) {
-        const bool more = k0 + BK < a.K;
-        if (more) load_tiles(k0 + BK);
-#pragma unroll
-        for (int k = 0; k < BK; ++k) {
-            float av[RM], xv[RT];
-#pragma unroll
-            for (int i = 0; i < RM; ++i) av[i] = As[k][tx + 16 * i];
-#pragma unroll
-            for (int j = 0; j < RT; ++j) xv[j] = Xs[k][ty + 16 * j];
-#pragma unroll
-            for (int i = 0; i < RM; ++i)
-#pragma unroll
-                for (int j = 0; j < RT; ++j) acc[i][j] = fmaf(av[i], xv[j], acc[i][j]);
-        }
-        __syncthreads();
-        if (more) {
-            store_tiles();
-            __syncthreads();
-        }
-    }
-    float* outn = a.out + (long long)n * a.out_per_n;
-    const float* resn = a.res ? a.res + (long long)n * a.out_per_n : nullptr;
-#pragma unroll
-    for (int j = 0; j < RT; ++j) {
-        const int q = q0 + ty + 16 * j;
-        if (q >= a.Lq) continue;
-#pragma unroll
-        for (int i = 0; i < RM; ++i) {
-            const int m = m0 + tx + 16 * i;
-            if (m >= a.M) continue;
-            const long long o = (long long)q * a.M + m - a.shift;
-            if (o < 0 || o >= a.out_per_n) continue;
-            float v = acc[i][j] + (a.bias ? a.bias[m] : 0.f);
-            if (resn) v += resn[o];
-            outn[o] = v;
-        }
-    }
 }
 
 // ------------------------------------------------------------------ last conv: ELU -> k-tap conv C -> audio channels (1 or 2)
@@ -427,165 +287,21 @@ __global__ void __launch_bounds__(256) chunk_scale_kernel(const float* __restric
     if (threadIdx.x == 0) scale[n] = (float)sqrt(red[0] / (double)Lc) + 1e-8f;
 }
 
-// Encoder stem (Encodec.swift:24-29): k-tap conv from audio_channels (1 or 2, too few for ec_conv_kernel's float4 K axis) to
-// F filters, with the config's padding, on chunk n of the waveform divided by scale[n] (when normalize).  STEM_T outputs per CTA;
-// the padded input tile and the weights [F, k, C] sit in shared memory.
-constexpr int STEM_T = 128;
-__global__ void __launch_bounds__(256) stem_conv_kernel(const float* __restrict__ wave, const float* __restrict__ w,
-                                                        const float* __restrict__ bias, const float* __restrict__ scale,
-                                                        float* __restrict__ out, int B, long long samples, int C, int Lc,
-                                                        int stride_c, int F, int k, int padL, int reflect) {
-    extern __shared__ float sm[];
-    float* ws = sm;                        // [F][k][C]
-    float* xs = sm + F * k * C;            // [STEM_T + k - 1][C]
-    const int n = blockIdx.y, c = n / B, b = n - c * B, t0 = blockIdx.x * STEM_T;
-    const float* src = wave + ((long long)b * samples + (long long)c * stride_c) * C;
-    const float sc = scale ? scale[n] : 1.f;
-    for (int e = threadIdx.x; e < F * k * C; e += 256) ws[e] = w[e];
-    for (int e = threadIdx.x; e < (STEM_T + k - 1) * C; e += 256) {
-        const int r = e / C, ch = e - r * C;
-        int s = t0 + r - padL;
-        if (s < 0) s = reflect ? min(-s, Lc - 1) : -1;
-        else if (s >= Lc) s = reflect ? max(Lc - 2 - (s - Lc), 0) : -1;
-        const float v = s >= 0 ? src[(long long)s * C + ch] : 0.f;
-        xs[e] = scale ? __fdiv_rn(v, sc) : v;
-    }
-    __syncthreads();
-    for (int e = threadIdx.x; e < STEM_T * F; e += 256) {
-        const int t = e / F, f = e - t * F;
-        if (t0 + t >= Lc) break;
-        float acc = 0.f;
-        for (int kk = 0; kk < k; ++kk)
-            for (int ch = 0; ch < C; ++ch) acc = fmaf(ws[(f * k + kk) * C + ch], xs[(t + kk) * C + ch], acc);
-        out[((long long)n * Lc + t0 + t) * F + f] = acc + bias[f];
-    }
-}
-
-// |e|^2 of every codebook row, summed over d in order without contraction (the code search's `ee`).
-__global__ void sqnorm_rows_kernel(const float* __restrict__ e, float* __restrict__ out, long long rows, int D) {
-    const long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (r >= rows) return;
-    float acc = 0.f;
-    for (int d = 0; d < D; ++d) acc = __fadd_rn(acc, __fmul_rn(e[r * D + d], e[r * D + d]));
-    out[r] = acc;
-}
-
-// Residual VQ encode (EncodecQuantization.swift:22-38, 100-115): z [rows = N*T, D] -> codes [N, n_q, T], levels in sequence with
-// residual -= embed[idx].  Ordered fp32: for each (frame, code) dot, |x|^2 and |e|^2 are summed over d = 0..D-1 as
-// acc = fl(acc + fl(a*b)), dist = fl(fl(xx - 2 dot) + ee), and the lowest index wins ties (== the reference's argMax(-dist)).
-// A CTA keeps VQ_FT frames' residuals in shared memory for all levels and streams VQ_KT-code tiles of each codebook through;
-// thread (tx = tid % 16, ty = tid / 16) scores frames ty, ty + 16 against codes tx + 16 j, j < 4, of a tile.
-constexpr int VQ_FT = 32, VQ_KT = 64;
-__global__ void __launch_bounds__(256) rvq_encode_kernel(const float* __restrict__ z, const float* __restrict__ books,
-                                                         const float* __restrict__ ee, int* __restrict__ codes, int rows, int T,
-                                                         int nq, int K, int D) {
-    extern __shared__ float sm[];
-    const int ld = D + 1;
-    float* rs = sm;                        // [VQ_FT][ld] residuals
-    float* es = rs + VQ_FT * ld;           // [VQ_KT][ld] codebook tile
-    float* ees = es + VQ_KT * ld;          // [VQ_KT]
-    float* xxs = ees + VQ_KT;              // [VQ_FT]
-    int* bidx = reinterpret_cast<int*>(xxs + VQ_FT);   // [VQ_FT]
-    const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
-    const int f0 = blockIdx.x * VQ_FT;
-    for (int e = tid; e < VQ_FT * D; e += 256) {
-        const int f = e / D, d = e - f * D;
-        rs[f * ld + d] = f0 + f < rows ? z[(long long)(f0 + f) * D + d] : 0.f;
-    }
-    __syncthreads();
-    for (int q = 0; q < nq; ++q) {
-        const float* book = books + (long long)q * K * D;
-        if (tid < VQ_FT) {
-            float xx = 0.f;
-            for (int d = 0; d < D; ++d) xx = __fadd_rn(xx, __fmul_rn(rs[tid * ld + d], rs[tid * ld + d]));
-            xxs[tid] = xx;
-        }
-        float best[2] = {INFINITY, INFINITY};
-        int bi[2] = {0, 0};
-        for (int k0 = 0; k0 < K; k0 += VQ_KT) {
-            __syncthreads();
-            for (int e = tid; e < VQ_KT * D; e += 256) {
-                const int c = e / D, d = e - c * D;
-                es[c * ld + d] = k0 + c < K ? book[(long long)(k0 + c) * D + d] : 0.f;
-            }
-            if (tid < VQ_KT) ees[tid] = k0 + tid < K ? ee[(long long)q * K + k0 + tid] : 0.f;
-            __syncthreads();
-            float dot[2][4];
-#pragma unroll
-            for (int i = 0; i < 2; ++i)
-#pragma unroll
-                for (int j = 0; j < 4; ++j) dot[i][j] = 0.f;
-            const float* r0 = rs + ty * ld;
-            const float* r1 = rs + (ty + 16) * ld;
-            const float* e0 = es + tx * ld;
-#pragma unroll 4
-            for (int d = 0; d < D; ++d) {
-                const float a0 = r0[d], a1 = r1[d];
-#pragma unroll
-                for (int j = 0; j < 4; ++j) {
-                    const float ev = e0[16 * j * ld + d];
-                    dot[0][j] = __fadd_rn(dot[0][j], __fmul_rn(a0, ev));
-                    dot[1][j] = __fadd_rn(dot[1][j], __fmul_rn(a1, ev));
-                }
-            }
-#pragma unroll
-            for (int i = 0; i < 2; ++i)
-#pragma unroll
-                for (int j = 0; j < 4; ++j) {
-                    const int c = tx + 16 * j;
-                    if (k0 + c >= K) continue;
-                    const float dist = __fadd_rn(__fsub_rn(xxs[ty + 16 * i], __fmul_rn(2.0f, dot[i][j])), ees[c]);
-                    if (dist < best[i]) { best[i] = dist; bi[i] = k0 + c; }
-                }
-        }
-        // lowest index among the 16 lanes' minima (each lane's is already its lowest)
-#pragma unroll
-        for (int i = 0; i < 2; ++i) {
-#pragma unroll
-            for (int o = 8; o; o >>= 1) {
-                const float ob = __shfl_xor_sync(0xffffffffu, best[i], o);
-                const int oi = __shfl_xor_sync(0xffffffffu, bi[i], o);
-                if (ob < best[i] || (ob == best[i] && oi < bi[i])) { best[i] = ob; bi[i] = oi; }
-            }
-            const int f = ty + 16 * i;
-            if (tx == 0) {
-                bidx[f] = bi[i];
-                if (f0 + f < rows) {
-                    const int n = (f0 + f) / T, t = (f0 + f) - n * T;
-                    codes[((long long)n * nq + q) * T + t] = bi[i];
-                }
-            }
-        }
-        __syncthreads();
-        if (q + 1 < nq)
-            for (int e = tid; e < VQ_FT * D; e += 256) {
-                const int f = e / D, d = e - f * D;
-                rs[f * ld + d] = __fsub_rn(rs[f * ld + d], book[(long long)bidx[f] * D + d]);
-            }
-        __syncthreads();
-    }
-}
-
 }  // namespace ec
 }  // namespace b2a
 
 using namespace b2a;
 
-struct EcConv {
-    DBuf<float> A, bias;
-    int M = 0, K = 0;
-};
-
 // an EncodecLSTMBlock's stack: layer 0's input projection runs as one GEMM (xproj), the rest inside lstm_kernel
 struct EcLstm {
-    EcConv xproj;
+    ec::Conv xproj;
     DBuf<float> Wh[ec::LSTM_MAX_LAYERS], Wx[ec::LSTM_MAX_LAYERS], b[ec::LSTM_MAX_LAYERS];
 };
 
 // an EncodecResnetBlock: r1 = k-tap conv dim -> hid (ELU of its input), r2 = [shortcut | block.3] over K = dim + hid, or
 // block.3 plus the identity residual without a conv shortcut
 struct EcRes {
-    EcConv r1, r2;
+    ec::Conv r1, r2;
 };
 
 struct b2a_encodec {
@@ -594,19 +310,19 @@ struct b2a_encodec {
     cudaStream_t stream = nullptr;
     int n_q = 0;
     DBuf<float> books;                       // [n_q][size][dim]
-    EcConv conv0;
+    ec::Conv conv0;
     EcLstm lstm;
-    struct Stage { int ratio, cin, cout, taps; EcConv up; EcRes res; };
+    struct Stage { int ratio, cin, cout, taps; ec::Conv up; EcRes res; };
     std::vector<Stage> stages;
     DBuf<float> wlast, blast;
     // encoder (only when the checkpoint has encoder.* tensors)
     bool has_enc = false;
     std::string enc_error = "encodec encode: the checkpoint has no encoder weights";
     DBuf<float> wstem, bstem;                // [num_filters, kernel_size, audio_channels]
-    struct EStage { int ratio, cin, cout; EcRes res; EcConv down; };
+    struct EStage { int ratio, cin, cout; EcRes res; ec::Conv down; };
     std::vector<EStage> estages;
     EcLstm elstm;
-    EcConv elast;
+    ec::Conv elast;
     DBuf<float> book_sq;                     // [n_q][size] |e|^2 in search order
     // workspaces
     DBuf<float> bufA, bufB, bufC, xp, hseq[ec::LSTM_MAX_LAYERS], chunks, scales, wave, zbuf, audio;
@@ -618,7 +334,7 @@ struct b2a_encodec {
     static void chan_ok(int ch) { B2A_CHECK(ch >= 4 && ch % 4 == 0, B2A_ERR_INVALID_INPUT, "encodec: channel counts must be multiples of 4"); }
 
     // ---- weight loading shared by the decoder and the encoder (prefix p ends in '.')
-    static void plain(const TensorTable& tt, EcConv& cv, const std::string& p, int cout, int k, int cin) {
+    static void plain(const TensorTable& tt, ec::Conv& cv, const std::string& p, int cout, int k, int cin) {
         chan_ok(cin);
         cv.M = cout; cv.K = k * cin;
         up(cv.A, tt.f32(p + "conv.weight", (int64_t)cout * k * cin));      // [out, k, in] == [M, tap*Cin + ci]
@@ -763,7 +479,7 @@ struct b2a_encodec {
         // |e|^2 of every codebook row, in the search's summation order
         const long long rows = (long long)n_q * cfg.codebook_size;
         book_sq.alloc((size_t)rows);
-        ec::sqnorm_rows_kernel<<<cdiv(rows, 256), 256>>>(books.p, book_sq.p, rows, cfg.codebook_dim);
+        ec::sqnorm_rows_kernel<<<cdiv(rows, 256), 256>>>(books.p, book_sq.p, rows, cfg.codebook_dim, 1.0f);
         B2A_CUDA(cudaGetLastError());
     }
     ~b2a_encodec() {
@@ -792,37 +508,10 @@ struct b2a_encodec {
         padL = cfg.use_causal_conv ? total : total - total / 2;
     }
 
-    void run_conv(ec::ConvArgs a, cudaStream_t s) {
-        const int M = a.M;
-        if (M >= 64) {
-            dim3 g(cdiv(a.Lq, 64), cdiv(M, 64), a.N);
-            ec::ec_conv_kernel<64, 64><<<g, 256, 0, s>>>(a);
-        } else if (M >= 32) {
-            dim3 g(cdiv(a.Lq, 128), cdiv(M, 32), a.N);
-            ec::ec_conv_kernel<32, 128><<<g, 256, 0, s>>>(a);
-        } else {
-            dim3 g(cdiv(a.Lq, 256), cdiv(M, 16), a.N);
-            ec::ec_conv_kernel<16, 256><<<g, 256, 0, s>>>(a);
-        }
-        count_launch();
-    }
-
     // EncodecResnetBlock (EncodecLayers.swift:278-337) on x [N, L, dim] as two launches (z: the hidden [N, L, hid]); result in x
     void run_resnet(const EcRes& r, float*& x, float*& y, float* z, int N, long long L, int dim, cudaStream_t s) {
-        const int hid = r.r1.M;
-        ec::ConvArgs a{};
-        a.xa = x; a.La = (int)L; a.Ca = dim; a.taps = cfg.residual_kernel_size; pads(cfg.residual_kernel_size, a.padL); a.reflect = cfg.pad_mode_reflect; a.elu_a = 1;
-        a.A = r.r1.A.p; a.bias = r.r1.bias.p; a.M = hid; a.K = r.r1.K; a.Lq = (int)L; a.N = N; a.out = z; a.out_per_n = L * hid;
-        run_conv(a, s);
-        ec::ConvArgs b{};
-        b.N = N; b.Lq = (int)L; b.M = dim; b.K = r.r2.K; b.A = r.r2.A.p; b.bias = r.r2.bias.p; b.out = y; b.out_per_n = L * dim;
-        if (cfg.use_conv_shortcut) {
-            b.xa = x; b.La = (int)L; b.Ca = dim; b.taps = 1; b.xb = z; b.Cb = hid; b.elu_b = 1;
-        } else {
-            b.xa = z; b.La = (int)L; b.Ca = hid; b.taps = 1; b.elu_a = 1; b.res = x;
-        }
-        run_conv(b, s);
-        std::swap(x, y);
+        int padL; pads(cfg.residual_kernel_size, padL);
+        ec::resnet_block(r.r1, r.r2, cfg.use_conv_shortcut != 0, cfg.residual_kernel_size, padL, cfg.pad_mode_reflect, x, y, z, N, L, dim, s);
     }
 
     // EncodecLSTMBlock (EncodecLayers.swift:72-88) on x [N, T, H]: the stack plus its skip; result in x
@@ -841,7 +530,7 @@ struct b2a_encodec {
             ec::ConvArgs a{};
             a.xa = x; a.La = T; a.Ca = H; a.taps = 1; a.A = m.xproj.A.p; a.bias = m.xproj.bias.p; a.M = 4 * H; a.K = H; a.Lq = T; a.N = N;
             a.out = xp.p; a.out_per_n = (long long)T * 4 * H;
-            run_conv(a, s);
+            ec::launch_conv(a, s);
         }
         const size_t smem = ((size_t)(2 * NL - 1) * 16 * H + (size_t)NL * ec::LSTM_BC * H + NL * 16 * ec::LSTM_BC + NL * ec::LSTM_UNITS * ec::LSTM_BC) * sizeof(float);
         B2A_CHECK(smem <= 220 * 1024, B2A_ERR_INVALID_INPUT, "encodec: LSTM slice does not fit shared memory");
@@ -887,7 +576,7 @@ struct b2a_encodec {
             ec::ConvArgs a{};
             a.xa = x; a.La = T; a.Ca = cfg.hidden_size; a.taps = cfg.kernel_size; pads(cfg.kernel_size, a.padL); a.reflect = cfg.pad_mode_reflect;
             a.A = conv0.A.p; a.bias = conv0.bias.p; a.M = conv0.M; a.K = conv0.K; a.Lq = T; a.N = N; a.out = y; a.out_per_n = (long long)T * dim0;
-            run_conv(a, s);
+            ec::launch_conv(a, s);
             std::swap(x, y);
         }
         // 3. LSTM block
@@ -905,7 +594,7 @@ struct b2a_encodec {
                 a.xa = x; a.La = (int)L; a.Ca = st.cin; a.taps = st.taps; a.backward = 1; a.elu_a = 1;
                 a.A = st.up.A.p; a.bias = st.up.bias.p; a.M = st.up.M; a.K = st.up.K; a.Lq = (int)L + st.taps - 1; a.N = N;
                 a.out = y; a.out_per_n = Lo * st.cout; a.shift = (long long)pl * st.cout;
-                run_conv(a, s);
+                ec::launch_conv(a, s);
                 std::swap(x, y);
             }
             L = Lo;
@@ -1010,7 +699,7 @@ struct b2a_encodec {
             a.padL = cfg.use_causal_conv ? k - r : (k - r) - (k - r) / 2;     // the right pad and the extra pad: src_index's edge rule
             a.A = st.down.A.p; a.bias = st.down.bias.p; a.M = st.down.M; a.K = st.down.K; a.Lq = (int)Lo; a.N = N;
             a.out = y; a.out_per_n = Lo * st.cout;
-            run_conv(a, s);
+            ec::launch_conv(a, s);
             std::swap(x, y);
             L = Lo;
         }
@@ -1022,16 +711,16 @@ struct b2a_encodec {
             ec::ConvArgs a{};
             a.xa = x; a.La = T; a.Ca = H; a.taps = cfg.last_kernel_size; pads(cfg.last_kernel_size, a.padL); a.reflect = cfg.pad_mode_reflect; a.elu_a = 1;
             a.A = elast.A.p; a.bias = elast.bias.p; a.M = elast.M; a.K = elast.K; a.Lq = T; a.N = N; a.out = zbuf.p; a.out_per_n = (long long)T * D;
-            run_conv(a, s);
+            ec::launch_conv(a, s);
         }
         // 6. residual VQ encode
         {
-            const int ld = D + 1;
-            const size_t smem = ((size_t)(ec::VQ_FT + ec::VQ_KT) * ld + ec::VQ_KT + 2 * ec::VQ_FT) * sizeof(float);
+            const size_t smem = ec::rvq_encode_smem(D);
             B2A_CHECK(smem <= 220 * 1024, B2A_ERR_INVALID_INPUT, "encodec: codebook_dim too large for the code search");
-            B2A_CUDA(cudaFuncSetAttribute(ec::rvq_encode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            B2A_CUDA(cudaFuncSetAttribute(ec::rvq_encode_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
             const int rows = N * T;
-            ec::rvq_encode_kernel<<<cdiv(rows, ec::VQ_FT), 256, smem, s>>>(zbuf.p, books.p, book_sq.p, d_codes, rows, T, nq, cfg.codebook_size, D);
+            ec::rvq_encode_kernel<false><<<cdiv(rows, ec::VQ_FT), 256, smem, s>>>(zbuf.p, D, books.p, book_sq.p, d_codes, rows, T, nq, 0, nq,
+                                                                                  cfg.codebook_size, D);
             count_launch();
         }
         B2A_CUDA(cudaGetLastError());

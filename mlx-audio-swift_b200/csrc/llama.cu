@@ -2156,17 +2156,22 @@ struct Q3Feedback {
     int G, H, max_tokens, eos, mask_eos;
 };
 // x_next = text + codec_embed(c0) + sum_i predictor_embed_i(c_{i+1})  (Qwen3TTS.swift:470-487) + per-row bookkeeping (:424-428)
+// channel i of one code frame's embedding: codec_embedding(c0) + sum over g >= 1 of the predictor's codec_embedding[g-1](c_g), in
+// that order (the talker's feedback, Qwen3TTS.swift:470-480, and codecEmbedIcl's rows, :249-265)
+__device__ __forceinline__ float q3_frame_sum(const bf16* codec_emb, int codec_rows, const bf16* const* cp_emb, int cp_rows, const int* c, int G,
+                                              int H, int i) {
+    float e = __bfloat162float(codec_emb[(long long)min(max(c[0], 0), codec_rows - 1) * H + i]);
+    for (int g = 1; g < G; ++g) e += __bfloat162float(cp_emb[g - 1][(long long)min(max(c[g], 0), cp_rows - 1) * H + i]);
+    return e;
+}
 __global__ void q3_feedback_kernel(Q3Feedback a) {
     const int b = blockIdx.x;
     pdl_wait();                  // NO pdl_trigger(): writes the talker's pos[]
     const int f = a.row_frame[b];
     const float* text = f < a.n_trailing[b] ? a.trailing + ((long long)b * a.n_max + f) * a.H : a.pad;
     const int* c = a.codes + b * a.G;
-    for (int i = threadIdx.x; i < a.H; i += blockDim.x) {
-        float e = __bfloat162float(a.codec_emb[(long long)min(max(c[0], 0), a.codec_rows - 1) * a.H + i]);
-        for (int g = 1; g < a.G; ++g) e += __bfloat162float(a.cp_emb[g - 1][(long long)min(max(c[g], 0), a.cp_rows - 1) * a.H + i]);
-        a.x_in[(long long)b * a.H + i] = text[i] + e;
-    }
+    for (int i = threadIdx.x; i < a.H; i += blockDim.x)
+        a.x_in[(long long)b * a.H + i] = text[i] + q3_frame_sum(a.codec_emb, a.codec_rows, a.cp_emb, a.cp_rows, c, a.G, a.H, i);
     __syncthreads();
     if (threadIdx.x == 0) {
         a.row_frame[b] = f + 1;
@@ -2181,6 +2186,12 @@ __global__ void q3_feedback_kernel(Q3Feedback a) {
             }
         }
     }
+}
+// codes [n, G] -> out [n, H]: one frame's summed embedding per row (codecEmbedIcl without its leading codec_bos row)
+__global__ void q3_code_frames_kernel(const bf16* codec_emb, int codec_rows, const bf16* const* cp_emb, int cp_rows, const int* codes, int G,
+                                      int H, float* out) {
+    const long long r = blockIdx.x;
+    for (int i = threadIdx.x; i < H; i += blockDim.x) out[r * H + i] = q3_frame_sum(codec_emb, codec_rows, cp_emb, cp_rows, codes + r * G, G, H, i);
 }
 __global__ void q3_init_rows_kernel(int B, int L, int* talker_pos, int* row_frame, int* n_frames, int* done, int* n_active, unsigned* seen, int words) {
     const int b = threadIdx.x;
@@ -2464,6 +2475,28 @@ int32_t b2a_qwen3_talker_embed_codec(b2a_qwen3_talker* h, const int32_t* ids, in
         h->embeds.alloc((size_t)n * h->H());
         q3_gather_kernel<<<n, 256, 0, s>>>(h->codec_emb.p, h->cfg.vocab_size, h->ids.p, 1, 0, h->embeds.p, h->H(), nullptr, 0);
         count_launch();
+        B2A_CUDA(cudaMemcpyAsync(out, h->embeds.p, (size_t)n * h->H() * sizeof(float), cudaMemcpyDeviceToHost, s));
+        B2A_CUDA(cudaStreamSynchronize(s));
+    });
+}
+
+// codecEmbedIcl's frame rows (Qwen3TTS.swift:249-265): codes [n, groups] (a frame's first `groups` code groups; groups below
+// num_code_groups is the reference's `break`) -> out [n, hidden]
+int32_t b2a_qwen3_talker_embed_code_frames(b2a_qwen3_talker* h, const int32_t* codes, int32_t n, int32_t groups, float* out) {
+    return guarded([&] {
+        B2A_CHECK(h && codes && out && n >= 1 && groups >= 1 && groups <= h->G(), B2A_ERR_INVALID_INPUT, "b2a_qwen3_talker_embed_code_frames: bad argument");
+        B2A_CHECK((long long)n * groups < (1ll << 31) && (long long)n * h->H() < (1ll << 40), B2A_ERR_INVALID_INPUT, "b2a_qwen3_talker_embed_code_frames: too many frames");
+        for (long long i = 0; i < (long long)n * groups; ++i) {
+            const int lim = i % groups == 0 ? h->cfg.vocab_size : h->cfg.cp_vocab_size;
+            B2A_CHECK(codes[i] >= 0 && codes[i] < lim, B2A_ERR_INVALID_INPUT, "b2a_qwen3_talker_embed_code_frames: code out of range");
+        }
+        B2A_CUDA(cudaSetDevice(h->device));
+        cudaStream_t s = h->stream;
+        h->ids.upload(codes, (size_t)n * groups, s);
+        h->embeds.alloc((size_t)n * h->H());
+        q3_code_frames_kernel<<<n, 256, 0, s>>>(h->codec_emb.p, h->cfg.vocab_size, h->cp_emb_ptrs.p, h->cfg.cp_vocab_size, h->ids.p, groups, h->H(), h->embeds.p);
+        count_launch();
+        B2A_CUDA(cudaGetLastError());
         B2A_CUDA(cudaMemcpyAsync(out, h->embeds.p, (size_t)n * h->H() * sizeof(float), cudaMemcpyDeviceToHost, s));
         B2A_CUDA(cudaStreamSynchronize(s));
     });

@@ -1,4 +1,5 @@
 // Qwen3-TTS speech-tokenizer DECODER for sm_90a (SURVEY.md section 8f row N1: 12.5 Hz codes -> 24 kHz waveform).
+// The ENCODER (24 kHz audio -> 12.5 Hz codes, voice cloning) is b2a_speech_tokenizer_encoder below, on the same kernels.
 // Replaces (reference paths, file = Sources/MLXAudioTTS/Models/Qwen3TTS/Qwen3TTSSpeechTokenizer.swift):
 //   :9-121      split residual vector quantizer decode (usage-normalised Euclidean codebooks, k1 output projections)
 //   :135-232    CausalConv1d (+ streaming step), :257-297 ConvNeXtBlock, :301-491 DecoderTransformer (KV cache)
@@ -19,6 +20,7 @@
 // reproduced (Args::bias_twice_t0).
 #include "common.cuh"
 #include "implicit_conv.cuh"
+#include "seanet.cuh"
 
 #include <algorithm>
 #include <cmath>
@@ -82,7 +84,10 @@ rmsnorm_planes_kernel(const float* __restrict__ x, const float* __restrict__ w, 
     for (int c = threadIdx.x; c < C; c += RN_THREADS) put_planes(out, N * C, n * C + c, w[c] * (x[n * C + c] * r), f16);
 }
 
-// rotate-half RoPE on q (in place) and k (into the cache), v copied into the cache.  qkv [N, (nh + 2 nkv) * hd] fp32.
+// RoPE on q (in place) and k (into the cache), v copied into the cache.  qkv [N, (nh + 2 nkv) * hd] fp32.  Frequency i rotates the
+// pair (i, i + hd/2) (rotate-half: the decoder, DecoderTransformer) or (2i, 2i + 1) (INTERLEAVED: the encoder, MLX RoPE traditional:
+// true, Mimi/Transformer.swift:130).
+template <bool INTERLEAVED>
 __global__ void rope_cache_kernel(float* __restrict__ qkv, float* __restrict__ Kc, float* __restrict__ Vc, const float* __restrict__ inv_freq,
                                   int T, int pos0, int nh, int nkv, int hd, int cap) {
     const long long n = blockIdx.x;
@@ -93,15 +98,16 @@ __global__ void rope_cache_kernel(float* __restrict__ qkv, float* __restrict__ K
         const int head = idx / half, i = idx - head * half;
         float sn, cs;
         sincosf((float)pos * inv_freq[i], &sn, &cs);
-        const float x1 = row[head * hd + i], x2 = row[head * hd + i + half];
+        const int i1 = INTERLEAVED ? 2 * i : i, i2 = INTERLEAVED ? 2 * i + 1 : i + half;
+        const float x1 = row[head * hd + i1], x2 = row[head * hd + i2];
         const float o1 = x1 * cs - x2 * sn, o2 = x2 * cs + x1 * sn;
         if (head < nh) {
-            row[head * hd + i] = o1;
-            row[head * hd + i + half] = o2;
+            row[head * hd + i1] = o1;
+            row[head * hd + i2] = o2;
         } else {
             float* dst = Kc + (((long long)b * nkv + (head - nh)) * cap + pos) * hd;
-            dst[i] = o1;
-            dst[i + half] = o2;
+            dst[i1] = o1;
+            dst[i2] = o2;
         }
     }
     for (int idx = threadIdx.x; idx < nkv * hd; idx += blockDim.x) {
@@ -165,6 +171,48 @@ attn_kernel(const float* __restrict__ qkv, const float* __restrict__ Kc, const f
     const long long N = (long long)B * T;
 #pragma unroll
     for (int d = 0; d < DPL; ++d) put_planes(out, N * nh * HD, n * nh * HD + h * HD + lane * DPL + d, acc[d] * inv, f16);
+}
+
+// LayerNorm with bias over channels -> planes [2][N][C]   (MLXNN LayerNorm: (x - mean) * rsqrt(var + eps) * w + b)
+__global__ void __launch_bounds__(RN_THREADS)
+layernorm_planes_kernel(const float* __restrict__ x, const float* __restrict__ w, const float* __restrict__ bias, bf16* __restrict__ out,
+                        long long N, int C, float eps, int f16) {
+    __shared__ float red[RN_THREADS / 32];
+    const long long n = blockIdx.x;
+    float s = 0.f;
+    for (int c = threadIdx.x; c < C; c += RN_THREADS) s += x[n * C + c];
+    const float mean = block_sum<RN_THREADS>(s, red) / (float)C;
+    float q = 0.f;
+    for (int c = threadIdx.x; c < C; c += RN_THREADS) { const float d = x[n * C + c] - mean; q += d * d; }
+    const float r = rsqrtf(block_sum<RN_THREADS>(q, red) / (float)C + eps);
+    for (int c = threadIdx.x; c < C; c += RN_THREADS) put_planes(out, N * C, n * C + c, (x[n * C + c] - mean) * r * w[c] + bias[c], f16);
+}
+
+// The split quantizer's k1 input projections in ordered fp32, so that the code search is a function of z alone:
+// out[r][o] = sum over d = 0..K-1 of fl(wt[d][o] * x[r][d]), accumulated in order without contraction.  x [rows, K], wt [K, M]
+// (transposed: a warp reads 32 consecutive outputs' weights), out [rows, M].  PJ_R rows per CTA share their x tile in shared memory.
+constexpr int PJ_R = 8, PJ_THREADS = 256;
+__global__ void __launch_bounds__(PJ_THREADS)
+ordered_proj_kernel(const float* __restrict__ x, const float* __restrict__ wt, float* __restrict__ out, int rows, int K, int M) {
+    extern __shared__ float xs[];          // [PJ_R][K]
+    const int r0 = blockIdx.x * PJ_R, o = blockIdx.y * PJ_THREADS + threadIdx.x;
+    for (int e = threadIdx.x; e < PJ_R * K; e += PJ_THREADS) {
+        const int r = e / K;
+        xs[e] = r0 + r < rows ? x[(long long)(r0 + r) * K + (e - r * K)] : 0.f;
+    }
+    __syncthreads();
+    if (o >= M) return;
+    float acc[PJ_R];
+#pragma unroll
+    for (int r = 0; r < PJ_R; ++r) acc[r] = 0.f;
+    for (int d = 0; d < K; ++d) {
+        const float wv = wt[(long long)d * M + o];
+#pragma unroll
+        for (int r = 0; r < PJ_R; ++r) acc[r] = __fadd_rn(acc[r], __fmul_rn(wv, xs[r * K + d]));
+    }
+#pragma unroll
+    for (int r = 0; r < PJ_R; ++r)
+        if (r0 + r < rows) out[(long long)(r0 + r) * M + o] = acc[r];
 }
 
 // gu [N, 2I] (gate | up) -> silu(gate) * up as planes [2][N][I]     (DecoderMLP :412-414)
@@ -335,6 +383,24 @@ struct IW {                       // implicit-conv weight: [M][taps][cblocks * 6
     }
     void set_bias(const std::vector<float>& b) { bias.upload(b.data(), b.size()); has_bias = true; B2A_CUDA(cudaDeviceSynchronize()); }
 };
+
+// one implicit_conv_kernel launch of weight W over planes `in` [2][B][in_frames][W.Cin]
+static void ic_conv(const IW& W, const bf16* in, long long in_frames, ic::Args a, int f16, int num_sms, cudaStream_t s) {
+    a.M = W.M; a.m_tiles = cdiv(W.M, tc::BM);
+    a.taps = W.taps; a.cblocks = W.cblocks;
+    if (a.dil == 0) a.dil = 1;
+    if (a.up == 0) a.up = 1;
+    a.Cout = W.M / a.up;
+    a.t_tiles = cdiv(a.T, ic::HALF);
+    a.bias = W.has_bias ? W.bias.p : nullptr;
+    a.f16 = f16;
+    a.seg_kb = SEG_KB;
+    a.wscale = f16 ? W.rscale.p : nullptr;
+    const CUtensorMap tb = tc::make_tmap_planes(in, W.Cin, in_frames, a.B, ic::HALF, f16);
+    const long long tiles = (long long)a.B * a.t_tiles * a.m_tiles;
+    launch_pdl(a.f16 ? ic::implicit_conv_kernel<1> : ic::implicit_conv_kernel<0>, dim3((unsigned)std::min<long long>(num_sms, tiles)), dim3(ic::IC_THREADS), ic::SMEM_BYTES, s,
+               W.th, W.tl, tb, a);
+}
 
 struct Snake { DBuf<float> a, ib; };                 // a = exp(alpha), ib = 1 / (exp(beta) + 1e-9)
 struct PlaneState { DBuf<bf16> s[2]; int H = 0, C = 0; };      // [2][B][H][C]
@@ -598,22 +664,7 @@ struct b2a_speech_tokenizer {
         B2A_CHECK(need <= buf.n, B2A_ERR_GENERATION_FAILED, "speech tokenizer: internal workspace too small");
         return buf.p;
     }
-    void conv(const IW& W, const bf16* in, long long in_frames, ic::Args a, cudaStream_t s) {
-        a.M = W.M; a.m_tiles = cdiv(W.M, tc::BM);
-        a.taps = W.taps; a.cblocks = W.cblocks;
-        if (a.dil == 0) a.dil = 1;
-        if (a.up == 0) a.up = 1;
-        a.Cout = W.M / a.up;
-        a.t_tiles = cdiv(a.T, ic::HALF);
-        a.bias = W.has_bias ? W.bias.p : nullptr;
-        a.f16 = use_f16;
-        a.seg_kb = SEG_KB;
-        a.wscale = use_f16 ? W.rscale.p : nullptr;
-        const CUtensorMap tb = tc::make_tmap_planes(in, W.Cin, in_frames, a.B, ic::HALF, use_f16);
-        const long long tiles = (long long)a.B * a.t_tiles * a.m_tiles;
-        launch_pdl(a.f16 ? ic::implicit_conv_kernel<1> : ic::implicit_conv_kernel<0>, dim3((unsigned)std::min<long long>(num_sms, tiles)), dim3(ic::IC_THREADS), ic::SMEM_BYTES, s,
-                   W.th, W.tl, tb, a);
-    }
+    void conv(const IW& W, const bf16* in, long long in_frames, ic::Args a, cudaStream_t s) { ic_conv(W, in, in_frames, a, use_f16, num_sms, s); }
     void carry(bf16* X, PlaneState& st, int B, long long T, cudaStream_t s) {
         if (st.H == 0) return;
         const long long n = (long long)2 * B * st.H * (st.C / 8);
@@ -678,7 +729,7 @@ struct b2a_speech_tokenizer {
             rmsnorm_planes_kernel<<<(unsigned)N, RN_THREADS, 0, s>>>(Xh.p, Ly.ln1.p, planes(P0, B, T, Hd), N, Hd, c.rms_norm_eps, use_f16);
             count_launch();
             { ic::Args a{}; a.B = B; a.T = T; a.xo = Q.p; conv(Ly.qkv, P0.p, T, a, s); }
-            rope_cache_kernel<<<(unsigned)N, 256, 0, s>>>(Q.p, Ly.K.p, Ly.V.p, inv_freq.p, T, cache_len, nh, c.num_key_value_heads, hd, c.max_cache_frames);
+            rope_cache_kernel<false><<<(unsigned)N, 256, 0, s>>>(Q.p, Ly.K.p, Ly.V.p, inv_freq.p, T, cache_len, nh, c.num_key_value_heads, hd, c.max_cache_frames);
             count_launch();
             attention(Ly, B, T, planes(P1, B, T, nh * hd), s);
             { ic::Args a{}; a.B = B; a.T = T; a.xo = Xh.p; a.add = 1; a.gamma = Ly.sc_attn.p; conv(Ly.o, P1.p, T, a, s); }
@@ -762,6 +813,272 @@ struct b2a_speech_tokenizer {
         step_dev(d_codes.p, B, nq, T, wave.p, s);
         B2A_CUDA(cudaMemcpy2DAsync(out, (size_t)out_stride * sizeof(float), wave.p + drop, (size_t)nout * sizeof(float), (size_t)(nout - drop) * sizeof(float),
                                    (size_t)B, cudaMemcpyDeviceToHost, s));
+        B2A_CUDA(cudaStreamSynchronize(s));
+    }
+};
+
+// ================================================================================================ encoder
+// Qwen3TTSSpeechTokenizerEncoder.encode (Qwen3TTSSpeechTokenizer.swift:790-884): audio [B, 1, n] -> codes [B, G, T].
+//   1. SEANet encoder (Mimi/Seanet.swift:157-257) in fp32 channels-last on the shared SEANet kernels (seanet.cuh): the stem from the
+//      waveform, per reversed ratio a resnet block (identity skip) and ELU + conv k = 2r stride r, then ELU + the last conv.  Causal
+//      zero padding kEff - stride on the left plus getExtraPaddingForConv1d on the right (Mimi/Conv.swift:150-156, 205-221).
+//   2. The transformer (Mimi/Transformer.swift:110-369) on the decoder's machinery: LayerNorm into hi/lo planes, implicit-GEMM
+//      linears with the layer scale + residual (and exact GELU) fused, interleaved RoPE, causal attention over the whole clip (the
+//      encode trims its caches to empty and passes the clip at once, so the 250-frame context never drops a key).
+//   3. ConvDownsample1d (Conv.swift:333-347): k = 2 s, stride s, no bias, EDGE padding -> z [B, T, hidden].
+//   4. SplitResidualVectorQuantizer.encode (Mimi/Quantization.swift:7-211): both k1 input projections as one ordered-fp32 product
+//      z -> [first | rest], then the code search (dist = |e|^2/2 - x.e, ordered fp32) -- rvq_first's one level, rvq_rest's first
+//      G - 1 levels, the only ones the cut to valid_num_quantizers keeps.
+struct b2a_speech_tokenizer_encoder {
+    int device = 0, num_sms = 132;
+    b2a_speech_tokenizer_encoder_config cfg{};
+    cudaStream_t stream = nullptr;
+    int G = 0, ds = 1;                 // code groups returned, downsample stride
+    struct Stage { int ratio, cin; ec::Conv r1, r2, down; };
+    DBuf<float> wstem, bstem;          // [F, k, 1]
+    std::vector<Stage> stages;
+    ec::Conv last, down;
+    struct Layer { IW qkv, o, fc1, fc2; DBuf<float> ln1w, ln1b, ln2w, ln2b, ls1, ls2; };
+    std::vector<Layer> layers;
+    DBuf<float> inv_freq, proj_t, books, c2;     // proj_t [hidden, 2 D] (first | rest, transposed); books [G][size][D]; c2 [G][size]
+    // workspaces
+    DBuf<float> bufA, bufB, bufC, Q, Kc, Vc, zbuf, xproj, audio;
+    DBuf<bf16> P0, P1;
+    DBuf<int> codes;
+
+    static void up(DBuf<float>& d, const std::vector<float>& v) { d.upload(v.data(), v.size()); }
+    static void load(const TensorTable& tt, ec::Conv& cv, const std::string& p, int cout, int k, int cin, bool bias) {
+        cv.M = cout; cv.K = k * cin;
+        up(cv.A, tt.f32(p + ".weight", (int64_t)cout * k * cin));       // MLX [out, k, in] == [M, tap * Cin + ci]
+        if (bias) up(cv.bias, tt.f32(p + ".bias", cout));
+    }
+    void load_linear(IW& w, const TensorTable& tt, const std::string& p, int out, int in) {
+        w.build(tt.f32(p + ".weight", (int64_t)out * in), out, 1, in, 1);
+    }
+
+    b2a_speech_tokenizer_encoder(int dev, const b2a_speech_tokenizer_encoder_config& c, const TensorTable& tt) : device(dev), cfg(c) {
+        B2A_CHECK(c.audio_channels == 1, B2A_ERR_INVALID_INPUT, "speech tokenizer encoder: audio_channels must be 1");
+        B2A_CHECK(c.num_residual_layers == 1, B2A_ERR_INVALID_INPUT,
+                  "speech tokenizer encoder: num_residual_layers must be 1 (dilated residual layers are not implemented)");
+        B2A_CHECK(c.use_causal_conv && !c.use_conv_shortcut, B2A_ERR_INVALID_INPUT,
+                  "speech tokenizer encoder: only the causal, identity-skip SEANet (use_causal_conv, !use_conv_shortcut) is implemented");
+        B2A_CHECK(c.num_upsampling_ratios >= 1 && c.num_upsampling_ratios <= 8 && c.kernel_size >= 1 && c.kernel_size <= 16 &&
+                      c.residual_kernel_size >= 1 && c.last_kernel_size >= 1 && c.compress >= 1 && c.num_filters >= 4 && c.num_filters % 4 == 0,
+                  B2A_ERR_INVALID_INPUT, "speech tokenizer encoder: bad SEANet config");
+        B2A_CHECK(c.head_dim == 32 || c.head_dim == 64 || c.head_dim == 128, B2A_ERR_INVALID_INPUT, "speech tokenizer encoder: head_dim must be 32, 64 or 128");
+        B2A_CHECK(c.num_attention_heads >= 1 && c.num_key_value_heads == c.num_attention_heads && c.num_attention_heads * c.head_dim == c.hidden_size,
+                  B2A_ERR_INVALID_INPUT, "speech tokenizer encoder: heads * head_dim must equal hidden_size, without grouped keys (Transformer.swift:121)");
+        B2A_CHECK(c.hidden_size % 64 == 0 && c.intermediate_size % 8 == 0 && c.num_hidden_layers >= 0, B2A_ERR_INVALID_INPUT,
+                  "speech tokenizer encoder: hidden_size must be a multiple of 64, intermediate_size of 8");
+        B2A_CHECK(c.codebook_size >= 1 && c.codebook_dim >= 1 && ec::rvq_encode_smem(c.codebook_dim) <= 220 * 1024, B2A_ERR_INVALID_INPUT,
+                  "speech tokenizer encoder: bad codebook geometry");
+        B2A_CHECK(c.num_quantizers >= 1 && c.valid_num_quantizers >= 1, B2A_ERR_INVALID_INPUT, "speech tokenizer encoder: bad quantizer counts");
+        B2A_CHECK(tt.find("encoder.init_conv1d.conv.conv.weight"), B2A_ERR_MODEL_NOT_INITIALIZED,
+                  "speech tokenizer encoder: the checkpoint has no encoder weights");
+        B2A_CHECK((size_t)PJ_R * c.hidden_size * sizeof(float) <= 200 * 1024, B2A_ERR_INVALID_INPUT,
+                  "speech tokenizer encoder: hidden_size too large for the input projection's shared-memory tile");
+        require_device(dev);
+        B2A_CUDA(cudaSetDevice(dev));
+        B2A_CUDA(cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, device));
+        B2A_CUDA(cudaFuncSetAttribute(ic::implicit_conv_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ic::SMEM_BYTES));
+        B2A_CUDA(cudaFuncSetAttribute(ordered_proj_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(PJ_R * c.hidden_size * sizeof(float))));
+        G = std::min(c.valid_num_quantizers, c.num_quantizers);
+        {   // Qwen3TTSSpeechTokenizerEncoder.init (:810-812): stride = max(1, Int(sampling_rate / prod(ratios) / frame_rate))
+            long long hop = 1;
+            for (int i = 0; i < c.num_upsampling_ratios; ++i) {
+                B2A_CHECK(c.upsampling_ratios[i] >= 1 && c.upsampling_ratios[i] <= 64, B2A_ERR_INVALID_INPUT, "speech tokenizer encoder: bad ratio");
+                hop *= c.upsampling_ratios[i];
+            }
+            ds = std::max(1, (int)((double)c.sampling_rate / (double)hop / (double)c.frame_rate));
+        }
+        const int F = c.num_filters, H = c.hidden_size, D = c.codebook_dim;
+        up(wstem, tt.f32("encoder.init_conv1d.conv.conv.weight", (int64_t)F * c.kernel_size));
+        up(bstem, tt.f32("encoder.init_conv1d.conv.conv.bias", F));
+        int ch = F;
+        for (int i = 0; i < c.num_upsampling_ratios; ++i) {
+            Stage st{};
+            st.ratio = c.upsampling_ratios[c.num_upsampling_ratios - 1 - i];
+            st.cin = ch;
+            const int hid = ch / c.compress;
+            B2A_CHECK(hid >= 4 && hid % 4 == 0, B2A_ERR_INVALID_INPUT, "speech tokenizer encoder: channel counts must be multiples of 4");
+            const std::string p = "encoder.layers." + std::to_string(i) + ".";
+            load(tt, st.r1, p + "residuals.0.block.0.conv.conv", hid, c.residual_kernel_size, ch, true);
+            load(tt, st.r2, p + "residuals.0.block.1.conv.conv", ch, 1, hid, true);
+            load(tt, st.down, p + "downsample.conv.conv", 2 * ch, 2 * st.ratio, ch, true);
+            stages.push_back(std::move(st));
+            ch *= 2;
+        }
+        load(tt, last, "encoder.final_conv1d.conv.conv", H, c.last_kernel_size, ch, true);
+        layers.resize(c.num_hidden_layers);
+        for (int l = 0; l < c.num_hidden_layers; ++l) {
+            const std::string p = "encoder_transformer.transformer.layers." + std::to_string(l) + ".";
+            Layer& L = layers[l];
+            load_linear(L.qkv, tt, p + "self_attn.in_proj", 3 * H, H);
+            load_linear(L.o, tt, p + "self_attn.out_proj", H, H);
+            load_linear(L.fc1, tt, p + "gating.linear1", c.intermediate_size, H);
+            load_linear(L.fc2, tt, p + "gating.linear2", H, c.intermediate_size);
+            up(L.ln1w, tt.f32(p + "norm1.weight", H)); up(L.ln1b, tt.f32(p + "norm1.bias", H));
+            up(L.ln2w, tt.f32(p + "norm2.weight", H)); up(L.ln2b, tt.f32(p + "norm2.bias", H));
+            up(L.ls1, tt.f32(p + "layer_scale_1.scale", H)); up(L.ls2, tt.f32(p + "layer_scale_2.scale", H));
+        }
+        {   // RoPE(dimensions: head_dim, traditional: true, base: Float(maxPeriod)), maxPeriod = Int(ropeTheta) (:844)
+            const float base = (float)(int)c.rope_theta;
+            std::vector<float> f(c.head_dim / 2);
+            for (int i = 0; i < c.head_dim / 2; ++i) f[i] = 1.0f / powf(base, (float)(2 * i) / (float)c.head_dim);
+            up(inv_freq, f);
+        }
+        load(tt, down, "downsample.conv.conv.conv", H, 2 * ds, H, false);
+        {   // input projections [D, 1, H] each -> proj_t [H][2 D]; codebooks: embedding = embedding_sum / max(cluster_usage, 1e-5)
+            std::vector<float> w1 = tt.f32("quantizer.rvq_first.input_proj.weight", (int64_t)D * H), w2((size_t)D * H, 0.f);
+            if (G > 1) w2 = tt.f32("quantizer.rvq_rest.input_proj.weight", (int64_t)D * H);
+            std::vector<float> pt((size_t)H * 2 * D);
+            for (int o = 0; o < D; ++o)
+                for (int h = 0; h < H; ++h) { pt[(size_t)h * 2 * D + o] = w1[(size_t)o * H + h]; pt[(size_t)h * 2 * D + D + o] = w2[(size_t)o * H + h]; }
+            up(proj_t, pt);
+            const int bins = c.codebook_size;
+            std::vector<float> e((size_t)G * bins * D);
+            for (int q = 0; q < G; ++q) {
+                const std::string p = q == 0 ? std::string("quantizer.rvq_first.vq.layers.0") : "quantizer.rvq_rest.vq.layers." + std::to_string(q - 1);
+                const std::vector<float> sum = tt.f32(p + ".codebook.embedding_sum", (int64_t)bins * D), use = tt.f32(p + ".codebook.cluster_usage", bins);
+                for (int r = 0; r < bins; ++r) {
+                    const float u = std::max(use[r], 1e-5f);
+                    for (int d = 0; d < D; ++d) e[((size_t)q * bins + r) * D + d] = sum[(size_t)r * D + d] / u;
+                }
+            }
+            up(books, e);
+            c2.alloc((size_t)G * bins);
+            ec::sqnorm_rows_kernel<<<cdiv((long long)G * bins, 256), 256>>>(books.p, c2.p, (long long)G * bins, D, 0.5f);
+            B2A_CUDA(cudaGetLastError());
+        }
+        B2A_CUDA(cudaDeviceSynchronize());
+        // last: a check that throws above leaves no stream behind (the destructor does not run for a half-built object)
+        B2A_CUDA(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
+    }
+    ~b2a_speech_tokenizer_encoder() { if (stream) cudaStreamDestroy(stream); }
+
+    // StreamableConv1d's output length (Mimi/Conv.swift:150-156, 205-221): (L + kEff - stride + extra - kEff) / stride + 1
+    static long long conv_len(long long L, int k, int stride) {
+        const long long pt = k - stride, nframes = std::max(L + pt - k, 0ll);
+        const double nf = (double)nframes / (double)stride + 1.0;
+        const long long ideal = ((long long)std::ceil(nf) - 1) * stride + k - pt;
+        return (L + pt + std::max(0ll, ideal - L) - k) / stride + 1;
+    }
+    long long seanet_len(long long n) const {
+        long long L = n;
+        for (auto& st : stages) L = conv_len(L, 2 * st.ratio, st.ratio);
+        return L;
+    }
+    long long encoded_length(long long n) const { return n >= 1 ? conv_len(seanet_len(n), 2 * ds, ds) : 0; }
+
+    // d_audio [B, n] -> d_codes [B, G, T]; z stays in zbuf [B, T, hidden]
+    void encode_dev(const float* d_audio, int B, long long n, int* d_codes, cudaStream_t s) {
+        B2A_CHECK(n >= 1, B2A_ERR_AUDIO_ENCODING_FAILED, "speech tokenizer encoder: empty audio");
+        B2A_CHECK(B >= 1, B2A_ERR_INVALID_INPUT, "speech tokenizer encoder: batch must be >= 1");
+        const int F = cfg.num_filters, H = cfg.hidden_size, D = cfg.codebook_dim, I = cfg.intermediate_size, nh = cfg.num_attention_heads, hd = cfg.head_dim;
+        // 32-bit frame indices and grid sizes, 64-bit element offsets below 2^40
+        B2A_CHECK(n < (1ll << 30) && (long long)B * n * std::max(F, 64) < (1ll << 40) && (long long)B * n < (1ll << 31), B2A_ERR_INVALID_INPUT,
+                  "speech tokenizer encoder: input too long");
+        B2A_CUDA(cudaSetDevice(device));
+        const long long T25 = seanet_len(n), T = encoded_length(n), N25 = (long long)B * T25, N = (long long)B * T;
+        size_t big = (size_t)B * n * F;
+        {
+            long long L = n;
+            for (auto& st : stages) { L = conv_len(L, 2 * st.ratio, st.ratio); big = std::max(big, (size_t)((long long)B * L * 2 * st.cin)); }
+            big = std::max(big, (size_t)(N25 * H));
+        }
+        bufA.alloc(big); bufB.alloc(big); bufC.alloc(big);
+        float* x = bufA.p; float* y = bufB.p; float* z = bufC.p;
+        // 1. SEANet
+        {
+            const int k = cfg.kernel_size;
+            const size_t smem = ((size_t)F * k + (size_t)(ec::STEM_T + k - 1)) * sizeof(float);
+            B2A_CHECK(smem <= 200 * 1024, B2A_ERR_INVALID_INPUT, "speech tokenizer encoder: stem too wide");
+            B2A_CUDA(cudaFuncSetAttribute(ec::stem_conv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            ec::stem_conv_kernel<<<dim3(cdiv(n, ec::STEM_T), B), 256, smem, s>>>(d_audio, wstem.p, bstem.p, nullptr, x, B, n, 1, (int)n, 0, F, k, k - 1, 0);
+            count_launch();
+        }
+        long long L = n;
+        for (auto& st : stages) {
+            ec::resnet_block(st.r1, st.r2, false, cfg.residual_kernel_size, cfg.residual_kernel_size - 1, 0, x, y, z, B, L, st.cin, s);
+            const int r = st.ratio, k = 2 * r;
+            const long long Lo = conv_len(L, k, r);
+            ec::ConvArgs a{};
+            a.xa = x; a.La = (int)L; a.Ca = st.cin; a.taps = k; a.stride = r; a.padL = k - r; a.elu_a = 1;       // right pad: zero rows
+            a.A = st.down.A.p; a.bias = st.down.bias.p; a.M = st.down.M; a.K = st.down.K; a.Lq = (int)Lo; a.N = B; a.out = y; a.out_per_n = Lo * st.down.M;
+            ec::launch_conv(a, s);
+            std::swap(x, y);
+            L = Lo;
+        }
+        {
+            ec::ConvArgs a{};
+            a.xa = x; a.La = (int)L; a.Ca = last.K / cfg.last_kernel_size; a.taps = cfg.last_kernel_size; a.padL = cfg.last_kernel_size - 1; a.elu_a = 1;
+            a.A = last.A.p; a.bias = last.bias.p; a.M = H; a.K = last.K; a.Lq = (int)L; a.N = B; a.out = y; a.out_per_n = L * H;
+            ec::launch_conv(a, s);
+            std::swap(x, y);
+        }
+        // 2. transformer on x [B, T25, H] (fp32 residual stream), one-shot: cache capacity = T25, positions from 0
+        P0.alloc((size_t)2 * N25 * H); P1.alloc((size_t)2 * N25 * std::max(H, I));
+        Q.alloc((size_t)N25 * 3 * H); Kc.alloc((size_t)N25 * H); Vc.alloc((size_t)N25 * H);
+        const int cap = (int)T25;
+        const float scale = 1.0f / sqrtf((float)hd);
+        for (auto& Ly : layers) {
+            layernorm_planes_kernel<<<(unsigned)N25, RN_THREADS, 0, s>>>(x, Ly.ln1w.p, Ly.ln1b.p, P0.p, N25, H, 1e-5f, 1);
+            count_launch();
+            { ic::Args a{}; a.B = B; a.T = cap; a.xo = Q.p; ic_conv(Ly.qkv, P0.p, cap, a, 1, num_sms, s); }
+            rope_cache_kernel<true><<<(unsigned)N25, 256, 0, s>>>(Q.p, Kc.p, Vc.p, inv_freq.p, cap, 0, nh, nh, hd, cap);
+            count_launch();
+            {
+                const dim3 grid(cdiv(cap, AT_WARPS), nh, B), block(AT_WARPS * 32);
+                if (hd == 32) attn_kernel<1><<<grid, block, 0, s>>>(Q.p, Kc.p, Vc.p, P1.p, B, cap, 0, nh, nh, cap, scale, 1);
+                else if (hd == 64) attn_kernel<2><<<grid, block, 0, s>>>(Q.p, Kc.p, Vc.p, P1.p, B, cap, 0, nh, nh, cap, scale, 1);
+                else attn_kernel<4><<<grid, block, 0, s>>>(Q.p, Kc.p, Vc.p, P1.p, B, cap, 0, nh, nh, cap, scale, 1);
+                count_launch();
+            }
+            { ic::Args a{}; a.B = B; a.T = cap; a.xo = x; a.add = 1; a.gamma = Ly.ls1.p; ic_conv(Ly.o, P1.p, cap, a, 1, num_sms, s); }
+            layernorm_planes_kernel<<<(unsigned)N25, RN_THREADS, 0, s>>>(x, Ly.ln2w.p, Ly.ln2b.p, P0.p, N25, H, 1e-5f, 1);
+            count_launch();
+            { ic::Args a{}; a.B = B; a.T = cap; a.gelu = 1; a.hl = P1.p; ic_conv(Ly.fc1, P0.p, cap, a, 1, num_sms, s); }
+            { ic::Args a{}; a.B = B; a.T = cap; a.xo = x; a.add = 1; a.gamma = Ly.ls2.p; ic_conv(Ly.fc2, P1.p, cap, a, 1, num_sms, s); }
+        }
+        // 3. downsample: k = 2 ds, stride ds, edge padding on both sides, no bias -> z
+        zbuf.alloc((size_t)N * H);
+        {
+            ec::ConvArgs a{};
+            a.xa = x; a.La = cap; a.Ca = H; a.taps = 2 * ds; a.stride = ds; a.padL = ds; a.edge = 1;
+            a.A = down.A.p; a.M = H; a.K = down.K; a.Lq = (int)T; a.N = B; a.out = zbuf.p; a.out_per_n = T * H;
+            ec::launch_conv(a, s);
+        }
+        // 4. input projections, then the code search: level 0 on the first block, levels 1 .. G-1 on the rest block
+        xproj.alloc((size_t)N * 2 * D);
+        ordered_proj_kernel<<<dim3(cdiv(N, PJ_R), cdiv(2 * D, PJ_THREADS)), PJ_THREADS, (size_t)PJ_R * H * sizeof(float), s>>>(zbuf.p, proj_t.p, xproj.p, (int)N, H, 2 * D);
+        count_launch();
+        {
+            const size_t smem = ec::rvq_encode_smem(D);
+            B2A_CUDA(cudaFuncSetAttribute(ec::rvq_encode_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            const int bins = cfg.codebook_size;
+            ec::rvq_encode_kernel<true><<<cdiv(N, ec::VQ_FT), 256, smem, s>>>(xproj.p, 2 * D, books.p, c2.p, d_codes, (int)N, (int)T, 1, 0, G, bins, D);
+            count_launch();
+            if (G > 1) {
+                ec::rvq_encode_kernel<true><<<cdiv(N, ec::VQ_FT), 256, smem, s>>>(xproj.p + D, 2 * D, books.p + (size_t)bins * D, c2.p + bins, d_codes,
+                                                                                 (int)N, (int)T, G - 1, 1, G, bins, D);
+                count_launch();
+            }
+        }
+        B2A_CUDA(cudaGetLastError());
+    }
+
+    // host audio [B, n] -> host codes [B, G, T] (and z [B, T, hidden] when asked)
+    void encode_host(const float* a, int B, long long n, int* out_codes, float* z_out) {
+        B2A_CHECK(n >= 1, B2A_ERR_AUDIO_ENCODING_FAILED, "speech tokenizer encoder: empty audio");
+        B2A_CHECK(B >= 1 && (long long)B * n < (1ll << 31), B2A_ERR_INVALID_INPUT, "speech tokenizer encoder: bad batch or input too long");
+        B2A_CUDA(cudaSetDevice(device));
+        cudaStream_t s = stream;
+        const long long T = encoded_length(n);
+        audio.alloc((size_t)B * n); codes.alloc((size_t)B * G * T);
+        B2A_CUDA(cudaMemcpyAsync(audio.p, a, (size_t)B * n * sizeof(float), cudaMemcpyHostToDevice, s));
+        encode_dev(audio.p, B, n, codes.p, s);
+        if (out_codes) B2A_CUDA(cudaMemcpyAsync(out_codes, codes.p, (size_t)B * G * T * sizeof(int), cudaMemcpyDeviceToHost, s));
+        if (z_out) B2A_CUDA(cudaMemcpyAsync(z_out, zbuf.p, (size_t)B * T * cfg.hidden_size * sizeof(float), cudaMemcpyDeviceToHost, s));
         B2A_CUDA(cudaStreamSynchronize(s));
     }
 };
@@ -932,5 +1249,47 @@ int32_t b2a_implicit_conv_test(const float* w, int32_t M, int32_t taps, int32_t 
         }
     });
 }
+
+int32_t b2a_speech_tokenizer_encoder_create(int32_t device, const b2a_speech_tokenizer_encoder_config* cfg, const b2a_tensor* tensors, int32_t n,
+                                            b2a_speech_tokenizer_encoder** out) {
+    return guarded([&] {
+        B2A_CHECK(out, B2A_ERR_INVALID_INPUT, "b2a_speech_tokenizer_encoder_create: null out");
+        *out = nullptr;
+        B2A_CHECK(cfg && tensors && n > 0, B2A_ERR_MODEL_NOT_INITIALIZED, "b2a_speech_tokenizer_encoder_create: missing config or weights");
+        TensorTable tt(tensors, n);
+        *out = new b2a_speech_tokenizer_encoder(device, *cfg, tt);
+    });
+}
+
+int64_t b2a_speech_tokenizer_encoder_encoded_length(const b2a_speech_tokenizer_encoder* h, int64_t n_samples) {
+    return h ? h->encoded_length(n_samples) : 0;
+}
+int32_t b2a_speech_tokenizer_encoder_num_code_groups(const b2a_speech_tokenizer_encoder* h) { return h ? h->G : 0; }
+void* b2a_speech_tokenizer_encoder_stream(b2a_speech_tokenizer_encoder* h) { return h ? (void*)h->stream : nullptr; }
+
+int32_t b2a_speech_tokenizer_encoder_encode(b2a_speech_tokenizer_encoder* h, const float* audio, int32_t batch, int64_t n_samples, int32_t* codes) {
+    return guarded([&] {
+        B2A_CHECK(h && audio && codes, B2A_ERR_INVALID_INPUT, "b2a_speech_tokenizer_encoder_encode: null argument");
+        h->encode_host(audio, batch, n_samples, codes, nullptr);
+    });
+}
+
+int32_t b2a_speech_tokenizer_encoder_encode_dev(b2a_speech_tokenizer_encoder* h, const float* d_audio, int32_t batch, int64_t n_samples,
+                                                int32_t* d_codes, void* stream) {
+    return guarded([&] {
+        B2A_CHECK(h && d_audio && d_codes, B2A_ERR_INVALID_INPUT, "b2a_speech_tokenizer_encoder_encode_dev: null argument");
+        h->encode_dev(d_audio, batch, n_samples, d_codes, stream ? (cudaStream_t)stream : h->stream);
+    });
+}
+
+int32_t b2a_speech_tokenizer_encoder_latent_test(b2a_speech_tokenizer_encoder* h, const float* audio, int32_t batch, int64_t n_samples,
+                                                 float* z, int32_t* codes) {
+    return guarded([&] {
+        B2A_CHECK(h && audio && z, B2A_ERR_INVALID_INPUT, "b2a_speech_tokenizer_encoder_latent_test: null argument");
+        h->encode_host(audio, batch, n_samples, codes, z);
+    });
+}
+
+void b2a_speech_tokenizer_encoder_destroy(b2a_speech_tokenizer_encoder* h) { delete h; }
 
 }  // extern "C"

@@ -578,6 +578,177 @@ struct b2a_weights {
         items = std::move(out);
     }
 
+    // ---- Qwen3-TTS speech tokenizer, encoder half of Qwen3TTSSpeechTokenizer.sanitize (Qwen3TTSSpeechTokenizer.swift:1093-1440).
+    // Output: the keys b2a_speech_tokenizer_encoder_create takes -- the reference's "encoder_model." paths without that prefix -- in
+    // MLX layouts.  Every non-encoder key is dropped; the codebooks' "initialized" flags are not emitted (nothing reads them).
+    static WItem f32_item(const std::string& name, std::vector<float>&& v, int64_t rows, int64_t cols) {
+        WItem t;
+        auto o = std::make_shared<std::vector<uint8_t>>(v.size() * 4);
+        memcpy(o->data(), v.data(), v.size() * 4);
+        t.name = name; t.owned = o; t.data = o->data(); t.dtype = B2A_DTYPE_F32; t.ndim = 2; t.shape[0] = rows; t.shape[1] = cols;
+        return t;
+    }
+    void sanitize_speech_tokenizer_encoder() {
+        static const std::map<int, std::string> conv_map = {{0, "encoder.init_conv1d"}, {3, "encoder.layers.0.downsample"},
+                                                            {6, "encoder.layers.1.downsample"}, {9, "encoder.layers.2.downsample"},
+                                                            {12, "encoder.layers.3.downsample"}, {14, "encoder.final_conv1d"}};
+        static const std::map<int, int> res_layer = {{1, 0}, {4, 1}, {7, 2}, {10, 3}}, res_block = {{1, 0}, {3, 1}};
+        auto split = [](const std::string& k) {
+            std::vector<std::string> p;
+            size_t a = 0;
+            for (size_t b; (b = k.find('.', a)) != std::string::npos; a = b + 1) p.push_back(k.substr(a, b - a));
+            p.push_back(k.substr(a));
+            return p;
+        };
+        auto join_from = [](const std::vector<std::string>& p, size_t i) {
+            std::string s;
+            for (; i < p.size(); ++i) s += (s.empty() ? "" : ".") + p[i];
+            return s;
+        };
+        auto to_int = [](const std::string& s, int& v) {
+            if (s.empty() || s.size() > 9) return false;
+            for (char c : s) if (!isdigit((unsigned char)c)) return false;
+            v = atoi(s.c_str());
+            return true;
+        };
+        auto ends_with = [](const std::string& s, const std::string& e) { return s.size() >= e.size() && s.compare(s.size() - e.size(), e.size(), e) == 0; };
+        auto has = [](const std::string& s, const char* x) { return s.find(x) != std::string::npos; };
+        auto quant_prefix = [&](const std::string& r, bool contains) {      // mapEncoderQuantizerPrefix / encoderCodebookPrefix
+            auto test = [&](const char* x) { return contains ? has(r, x) : r.rfind(x, 0) == 0; };
+            if (test("semantic_residual_vector_quantizer") || test("rvq_first.")) return std::string("quantizer.rvq_first");
+            return std::string("quantizer.rvq_rest");
+        };
+        std::vector<WItem> out;
+        std::map<int, std::map<char, WItem>> qkv;
+        std::map<std::string, std::map<std::string, WItem>> books;
+        for (auto& it : items) {
+            std::string k = it.name;
+            for (bool stripped = true; stripped;) {
+                stripped = false;
+                for (const char* pre : {"speech_tokenizer.", "encoder_model.", "decoder_model."}) {
+                    std::string rest;
+                    if (strip(k, pre, rest)) { k = rest; stripped = true; break; }
+                }
+            }
+            if (k.empty() || k == "encoder_model" || k == "decoder_model" || k == "speech_tokenizer") continue;
+            if (has_component_with_suffix(k, "speaker_encoder")) continue;
+            if (has(k, "_codebook.cluster_usage") || has(k, "_codebook.embedding_sum")) continue;        // the decoder's codebooks
+            if (has(k, "_codebook.initialized") || has(k, ".codebook.initialized")) continue;
+            if (k.rfind("encoder.", 0) != 0) continue;
+            WItem t = it;
+            const std::vector<std::string> parts = split(k);
+            if (k.rfind("encoder.encoder.layers.", 0) == 0) {                                           // :1241-1269
+                int n = 0;
+                if (parts.size() < 4 || !to_int(parts[3], n)) continue;
+                std::string key;
+                if (has(k, ".block.")) {
+                    int blk = 0;
+                    if (!res_layer.count(n) || parts.size() <= 5 || !to_int(parts[5], blk) || !res_block.count(blk)) continue;
+                    key = "encoder.layers." + std::to_string(res_layer.at(n)) + ".residuals.0.block." + std::to_string(res_block.at(blk)) + ".conv." + join_from(parts, 6);
+                } else if (conv_map.count(n)) {
+                    key = conv_map.at(n) + ".conv." + join_from(parts, 4);
+                } else {
+                    continue;
+                }
+                if (ends_with(key, "weight") && t.ndim == 3) permute3(t, 0, 2, 1);
+                t.name = key;
+                out.push_back(std::move(t));
+                continue;
+            }
+            if (k.rfind("encoder.encoder_transformer.layers.", 0) == 0 || k.rfind("encoder.encoder_transformer.transformer.layers.", 0) == 0) {   // :1271-1322
+                const bool nested = parts.size() >= 5 && parts[2] == "transformer" && parts[3] == "layers";
+                const size_t off = nested ? 4 : 3;
+                int l = 0;
+                if (parts.size() <= off || !to_int(parts[off], l)) continue;
+                const std::string sfx = join_from(parts, off + 1), p = "encoder_transformer.transformer.layers." + std::to_string(l) + ".";
+                std::string key;
+                if (has(sfx, "self_attn.q_proj.weight")) { qkv[l]['q'] = t; continue; }
+                else if (has(sfx, "self_attn.k_proj.weight")) { qkv[l]['k'] = t; continue; }
+                else if (has(sfx, "self_attn.v_proj.weight")) { qkv[l]['v'] = t; continue; }
+                else if (has(sfx, "self_attn.qkv.weight") && t.ndim == 2) {
+                    const int64_t rows = t.shape[0], cols = t.shape[1], third = rows / 3;
+                    if (rows % 3 != 0 || third <= 0) continue;
+                    const std::vector<float> v = as_f32(t);
+                    const char names[3] = {'q', 'k', 'v'};
+                    for (int i = 0; i < 3; ++i)
+                        qkv[l][names[i]] = f32_item("", std::vector<float>(v.begin() + i * third * cols, v.begin() + (i + 1) * third * cols), third, cols);
+                    continue;
+                }
+                else if (has(sfx, "self_attn.out_proj.weight") || has(sfx, "self_attn.o_proj.weight")) key = p + "self_attn.out_proj.weight";
+                else if (has(sfx, "mlp.fc1.weight")) key = p + "gating.linear1.weight";
+                else if (has(sfx, "mlp.fc2.weight")) key = p + "gating.linear2.weight";
+                else if (has(sfx, "input_layernorm.weight")) key = p + "norm1.weight";
+                else if (has(sfx, "input_layernorm.bias")) key = p + "norm1.bias";
+                else if (has(sfx, "post_attention_layernorm.weight")) key = p + "norm2.weight";
+                else if (has(sfx, "post_attention_layernorm.bias")) key = p + "norm2.bias";
+                else if (has(sfx, "self_attn_layer_scale.scale")) key = p + "layer_scale_1.scale";
+                else if (has(sfx, "mlp_layer_scale.scale")) key = p + "layer_scale_2.scale";
+                else continue;
+                t.name = key;
+                out.push_back(std::move(t));
+                continue;
+            }
+            if (k.rfind("encoder.downsample.", 0) == 0) {                                                 // :1324-1332
+                const std::string sfx = k.substr(19);
+                if (ends_with(sfx, "weight") && t.ndim == 3) permute3(t, 0, 2, 1);
+                t.name = "downsample.conv.conv." + sfx;
+                out.push_back(std::move(t));
+                continue;
+            }
+            if (k.rfind("encoder.quantizer.", 0) == 0) {                                                  // :1334-1376
+                const std::string rest = k.substr(18);
+                if (has(rest, ".codebook.embed.weight") || ends_with(rest, "codebook.embed")) continue;
+                if (has(rest, "codebook.cluster_usage") || has(rest, "codebook.embed_sum") || has(rest, "codebook.embedding_sum")) {
+                    const std::string base = rest.substr(0, rest.rfind(".codebook.") == std::string::npos ? rest.size() : rest.rfind(".codebook."));
+                    books[base][has(rest, "cluster_usage") ? "cluster_usage" : "embedding_sum"] = t;
+                    continue;
+                }
+                if (has(rest, "codebook.initialized")) continue;
+                if (has(rest, "input_proj.weight") || has(rest, "output_proj.weight")) {
+                    if (ends_with(rest, "weight") && t.ndim == 3) permute3(t, 0, 2, 1);
+                    WItem c = t;
+                    c.name = quant_prefix(rest, false) + (has(rest, "input_proj") ? ".input_proj.weight" : ".output_proj.weight");
+                    out.push_back(std::move(c));
+                }
+                if (!has(rest, "codebook.") && (rest.rfind("layers.", 0) == 0 || has(rest, ".layers."))) {   // mapEncoderQuantizerLayers
+                    std::string key;
+                    for (const char* pre : {"rvq_first.", "rvq_rest.", "semantic_residual_vector_quantizer.", "acoustic_residual_vector_quantizer."})
+                        if (key.empty() && rest.rfind(pre, 0) == 0)
+                            key = std::string(pre[0] == 's' || pre[4] == 'f' ? "quantizer.rvq_first.vq." : "quantizer.rvq_rest.vq.") + rest.substr(strlen(pre));
+                    if (key.empty() && rest.rfind("layers.", 0) == 0) key = "quantizer.rvq_rest.vq." + rest;
+                    if (!key.empty()) { t.name = key; out.push_back(std::move(t)); }
+                }
+                continue;
+            }
+        }
+        for (auto& e : qkv) {                                                                               // :1397-1401
+            auto& m = e.second;
+            if (!m.count('q') || !m.count('k') || !m.count('v')) continue;
+            std::vector<float> w = as_f32(m['q']), kk = as_f32(m['k']), vv = as_f32(m['v']);
+            const int64_t cols = m['q'].ndim == 2 ? m['q'].shape[1] : 0;
+            B2A_CHECK(cols > 0 && m['k'].ndim == 2 && m['v'].ndim == 2 && m['k'].shape[1] == cols && m['v'].shape[1] == cols, B2A_ERR_MODEL_NOT_INITIALIZED,
+                      "bad shape for tensor: speech tokenizer encoder q / k / v projection");
+            const int64_t rows = m['q'].shape[0] + m['k'].shape[0] + m['v'].shape[0];
+            w.insert(w.end(), kk.begin(), kk.end());
+            w.insert(w.end(), vv.begin(), vv.end());
+            out.push_back(f32_item("encoder_transformer.transformer.layers." + std::to_string(e.first) + ".self_attn.in_proj.weight", std::move(w), rows, cols));
+        }
+        for (auto& e : books) {                                                                             // :1403-1419
+            if (!e.second.count("cluster_usage") || !e.second.count("embedding_sum")) continue;
+            const std::vector<std::string> parts = split(e.first);
+            int idx = -1;
+            for (size_t i = 0; i + 1 < parts.size(); ++i)
+                if (parts[i] == "layers") { if (!to_int(parts[i + 1], idx)) idx = -1; break; }
+            if (idx < 0) continue;
+            const std::string p = quant_prefix(e.first, true) + ".vq.layers." + std::to_string(idx) + ".codebook.";
+            WItem a = e.second["cluster_usage"], b = e.second["embedding_sum"];
+            a.name = p + "cluster_usage"; b.name = p + "embedding_sum";
+            out.push_back(std::move(a));
+            out.push_back(std::move(b));
+        }
+        items = std::move(out);
+    }
+
     std::vector<b2a_tensor> table() const {
         std::vector<b2a_tensor> t(items.size());
         for (size_t i = 0; i < items.size(); ++i) {
@@ -830,6 +1001,68 @@ int32_t b2a_speech_tokenizer_create_from_directory(const char* dir, int32_t devi
         w->sanitize_speech_tokenizer();
         const std::vector<b2a_tensor> tab = w->table();
         st = b2a_speech_tokenizer_create(device, &cfg, tab.data(), (int32_t)tab.size(), out);
+        if (st != B2A_OK) throw Error(st, b2a_last_error());
+    });
+}
+
+int32_t b2a_weights_sanitize_speech_tokenizer_encoder(b2a_weights* w) {
+    return guarded([&] {
+        B2A_CHECK(w, B2A_ERR_INVALID_INPUT, "b2a_weights_sanitize_speech_tokenizer_encoder: null handle");
+        w->sanitize_speech_tokenizer_encoder();
+    });
+}
+
+// speech_tokenizer/config.json's "encoder_config" (Qwen3TTSTokenizerEncoderConfig, Qwen3TTSConfig.swift:391-494, the same defaults) and
+// "encoder_valid_num_quantizers" (:518-527, default 16).  No file or no block is the reference's encoderConfig == nil: no encoder.
+int32_t b2a_speech_tokenizer_encoder_config_from_json(const char* config_path, b2a_speech_tokenizer_encoder_config* cfg) {
+    return guarded([&] {
+        B2A_CHECK(config_path && cfg, B2A_ERR_INVALID_INPUT, "b2a_speech_tokenizer_encoder_config_from_json: null argument");
+        struct stat st{};
+        B2A_CHECK(stat(config_path, &st) == 0, B2A_ERR_MODEL_NOT_INITIALIZED, "speech tokenizer: no config.json, so no encoder_config");
+        const Json j = read_json_file(config_path);
+        B2A_CHECK(j.kind == Json::Obj, B2A_ERR_MODEL_NOT_INITIALIZED, "speech tokenizer config.json is not an object");
+        const Json* ej = j.find("encoder_config");
+        B2A_CHECK(ej && ej->kind == Json::Obj, B2A_ERR_MODEL_NOT_INITIALIZED, "speech tokenizer config.json has no encoder_config");
+        const Json& e = *ej;
+        b2a_speech_tokenizer_encoder_config c{};
+        c.sampling_rate = (int)e.number("sampling_rate", 24000); c.frame_rate = (float)e.number("frame_rate", 12.5);
+        c.audio_channels = (int)e.number("audio_channels", 1); c.num_filters = (int)e.number("num_filters", 64);
+        c.num_residual_layers = (int)e.number("num_residual_layers", 1);
+        std::vector<int> ratios = {8, 6, 5, 4};
+        if (const Json* a = e.find("upsampling_ratios"); a && a->kind == Json::Arr) { ratios.clear(); for (auto& x : a->arr) ratios.push_back((int)x.num); }
+        B2A_CHECK(ratios.size() <= 8, B2A_ERR_MODEL_NOT_INITIALIZED, "speech tokenizer encoder config: more than 8 upsampling_ratios");
+        c.num_upsampling_ratios = (int32_t)ratios.size();
+        for (size_t i = 0; i < ratios.size(); ++i) c.upsampling_ratios[i] = ratios[i];
+        c.kernel_size = (int)e.number("kernel_size", 7); c.residual_kernel_size = (int)e.number("residual_kernel_size", 3);
+        c.last_kernel_size = (int)e.number("last_kernel_size", 3); c.compress = (int)e.number("compress", 2);
+        c.use_causal_conv = (int)e.number("use_causal_conv", 1); c.use_conv_shortcut = (int)e.number("use_conv_shortcut", 0);
+        c.hidden_size = (int)e.number("hidden_size", 512); c.intermediate_size = (int)e.number("intermediate_size", 2048);
+        c.num_hidden_layers = (int)e.number("num_hidden_layers", 8); c.num_attention_heads = (int)e.number("num_attention_heads", 8);
+        c.num_key_value_heads = (int)e.number("num_key_value_heads", 8);
+        c.head_dim = c.num_attention_heads > 0 ? c.hidden_size / c.num_attention_heads : 0;     // the transformer's dModel / numHeads
+        c.rope_theta = (float)e.number("rope_theta", 10000.0);
+        c.codebook_size = (int)e.number("codebook_size", 2048); c.codebook_dim = (int)e.number("codebook_dim", 256);
+        c.num_quantizers = (int)e.number("num_quantizers", 32);
+        c.valid_num_quantizers = (int)j.number("encoder_valid_num_quantizers", 16);
+        *cfg = c;
+    });
+}
+
+// the encoder half of loadSpeechTokenizer (Qwen3TTS.swift:1244-1275): <dir>/config.json + every *.safetensors -> sanitize -> create
+int32_t b2a_speech_tokenizer_encoder_create_from_directory(const char* dir, int32_t device, b2a_speech_tokenizer_encoder** out) {
+    return guarded([&] {
+        B2A_CHECK(dir && out, B2A_ERR_INVALID_INPUT, "b2a_speech_tokenizer_encoder_create_from_directory: null argument");
+        *out = nullptr;
+        b2a_speech_tokenizer_encoder_config cfg{};
+        const std::string d = dir;
+        int32_t st = b2a_speech_tokenizer_encoder_config_from_json((d + "/config.json").c_str(), &cfg);
+        if (st != B2A_OK) throw Error(st, b2a_last_error());
+        std::unique_ptr<b2a_weights> w(new b2a_weights());
+        w->load(d);
+        w->sanitize_speech_tokenizer_encoder();
+        B2A_CHECK(!w->items.empty(), B2A_ERR_MODEL_NOT_INITIALIZED, "speech tokenizer: the checkpoint has no encoder weights");
+        const std::vector<b2a_tensor> tab = w->table();
+        st = b2a_speech_tokenizer_encoder_create(device, &cfg, tab.data(), (int32_t)tab.size(), out);
         if (st != B2A_OK) throw Error(st, b2a_last_error());
     });
 }

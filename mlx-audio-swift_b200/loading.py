@@ -46,6 +46,11 @@ class Weights:
         """Decoder half of Qwen3TTSSpeechTokenizer.sanitize (Qwen3TTSSpeechTokenizer.swift:1094-1440); keys end up relative to the decoder."""
         _ffi.check(_ffi.lib().b2a_weights_sanitize_speech_tokenizer(self._h))
 
+    def sanitize_speech_tokenizer_encoder(self) -> None:
+        """Encoder half of Qwen3TTSSpeechTokenizer.sanitize (:1093-1440); keys are the encoder's (encoder.*, encoder_transformer.*,
+        downsample.*, quantizer.*) in MLX layouts, every other key dropped."""
+        _ffi.check(_ffi.lib().b2a_weights_sanitize_speech_tokenizer_encoder(self._h))
+
     def tensors(self) -> Dict[str, object]:
         """name -> numpy array (float32 / int32) or torch.bfloat16 tensor.  COPIES (the handle owns the mapped bytes)."""
         import torch

@@ -2,7 +2,8 @@
 `Qwen3TTSTalkerForConditionalGeneration` + `Qwen3TTSCodePredictor` + the frame loop / `sampleToken` of `Qwen3TTSModel.generate`
 (Sources/MLXAudioTTS/Models/Qwen3TTS/{Qwen3TTSTalker,Qwen3TTSCodePredictor,Qwen3TTS}.swift).  Every number comes from the library
 (`b2a_qwen3_talker_*`); this file only composes the prompt rows the way `prepareGenerationInputs` does (Qwen3TTS.swift:883-999) and
-chains the speech-tokenizer decoder for audio.  Tokenisation stays with the host tokenizer: the entry points take token ids."""
+chains the speech-tokenizer decoder for audio; `prepare_icl_generation_inputs` composes the voice-cloning (ICL) prompt from
+reference codes (Qwen3TTS.swift:694-837).  Tokenisation stays with the host tokenizer: the entry points take token ids."""
 from __future__ import annotations
 
 import ctypes as C
@@ -54,6 +55,8 @@ class Qwen3TalkerConfig:
     codec_think_eos_id: int = 2157
     codec_pad_id: int = 2148
     codec_bos_id: int = 2149
+    # config.json's top-level "tts_model_type" ("base" checkpoints clone voices from an x-vector, Qwen3TTS.swift:709-750)
+    tts_model_type: str = ""
 
     def _c(self, max_batch: int, max_context: int) -> _ffi.Qwen3TalkerConfig:
         cp = self.code_predictor
@@ -122,6 +125,10 @@ class Qwen3TTSTalker:
                                         num_key_value_heads=c.num_key_value_heads, head_dim=c.head_dim, rms_norm_eps=c.rms_norm_eps,
                                         rope_theta=c.rope_theta, num_code_groups=c.num_code_groups, text_hidden_size=c.text_hidden_size,
                                         text_vocab_size=c.text_vocab_size, codec_eos_token_id=c.codec_eos_token_id, code_predictor=cp)
+        import json
+        from pathlib import Path
+        cj = Path(model_dir) / "config.json"
+        self.config.tts_model_type = str(json.loads(cj.read_text()).get("tts_model_type", "")) if cj.exists() else ""
         self._h = C.c_void_p()
         _ffi.check(_ffi.lib().b2a_qwen3_talker_create_from_directory(str(model_dir).encode(), device, max_batch, max_context, C.byref(self._h)))
         return self
@@ -143,6 +150,57 @@ class Qwen3TTSTalker:
         out = np.empty((len(a), self.config.hidden_size), dtype=np.float32)
         _ffi.check(_ffi.lib().b2a_qwen3_talker_embed_codec(self._h, _ffi.ptr(a), len(a), _ffi.ptr(out)))
         return out
+
+    def embed_code_frames(self, codes) -> np.ndarray:
+        """codecEmbedIcl's frame rows (Qwen3TTS.swift:249-265): codes [n, groups] -> [n, hidden], codec_embedding(c0) plus the code
+        predictor's embeddings of c1 .. c_{groups-1} (groups < num_code_groups is the reference's `break`)."""
+        a = np.ascontiguousarray(codes, dtype=np.int32)
+        if a.ndim != 2 or a.shape[0] < 1:
+            raise _ffi.AudioGenerationError(_ffi.ERR_INVALID_INPUT, "codes must be [frames, groups]")
+        out = np.empty((a.shape[0], self.config.hidden_size), dtype=np.float32)
+        _ffi.check(_ffi.lib().b2a_qwen3_talker_embed_code_frames(self._h, _ffi.ptr(a), a.shape[0], a.shape[1], _ffi.ptr(out)))
+        return out
+
+    def prepare_icl_generation_inputs(self, ref_codes, ref_chat_ids: Sequence[int], target_chat_ids: Sequence[int], tts_bos: int,
+                                      tts_eos: int, tts_pad: int, language_id: Optional[int] = None,
+                                      speaker_embedding=None) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+        """prepareReferenceConditioning's id slicing + prepareICLGenerationInputs (Qwen3TTS.swift:709-837) from token ids, the
+        voice-cloning prompt.  ref_codes [groups, T] or [1, groups, T] (the speech tokenizer's encode of the reference clip);
+        ref_chat_ids = tokens of "<|im_start|>assistant\n{ref_text}<|im_end|>\n"; target_chat_ids = tokens of
+        "<|im_start|>assistant\n{text}<|im_end|>\n<|im_start|>assistant\n"; speaker_embedding [hidden] (the caller's x-vector; the
+        speaker encoder is not built here).  Returns (input_embeds [L, H], trailing_text_hidden [1, H] = tts_pad, tts_pad_embed [H])."""
+        c = self.config
+        if speaker_embedding is None and c.tts_model_type == "base":
+            raise _ffi.AudioGenerationError(_ffi.ERR_INVALID_INPUT, "a Base checkpoint clones from a speaker embedding (x-vector), and the "
+                                            "speaker encoder (Qwen3TTSSpeakerEncoder) is not built: pass speaker_embedding")
+        rc = np.asarray(ref_codes)
+        rc = rc[0] if rc.ndim == 3 else rc
+        if rc.ndim != 2 or rc.shape[1] < 1:
+            raise _ffi.AudioGenerationError(_ffi.ERR_INVALID_INPUT, "ref_codes must be [groups, frames]")
+        rid, tid = list(ref_chat_ids), list(target_chat_ids)
+        r0 = min(3, len(rid)); ref_text = rid[r0:max(r0, len(rid) - 2)]                   # :731-735
+        t0 = min(3, len(tid)); target_text = tid[t0:max(t0, len(tid) - 5)]                # :762-766
+        tts = self.embed_text([tts_bos, tts_eos, tts_pad])
+        bos_e, eos_e, pad_e = tts[0:1], tts[1:2], tts[2:3]
+        text_ids = ref_text + target_text
+        text = np.concatenate(([self.embed_text(text_ids)] if text_ids else []) + [eos_e], axis=0)            # :775-778
+        codec_pad = self.embed_codec([c.codec_pad_id])
+        icl_codec = np.concatenate([self.embed_codec([c.codec_bos_id]), self.embed_code_frames(rc.T[:, :min(rc.shape[0], c.num_code_groups)])], axis=0)
+        icl = np.concatenate([text + codec_pad, icl_codec + pad_e], axis=0)                                   # :786-797
+        prefill = ([c.codec_think_id, c.codec_think_bos_id, language_id, c.codec_think_eos_id] if language_id is not None
+                   else [c.codec_nothink_id, c.codec_think_bos_id, c.codec_think_eos_id])                    # :800-812
+        pieces = [self.embed_codec(prefill)]
+        if speaker_embedding is not None:
+            se = np.asarray(speaker_embedding, dtype=np.float32).reshape(-1)
+            if se.shape[0] != c.hidden_size:
+                raise _ffi.AudioGenerationError(_ffi.ERR_INVALID_INPUT, "speaker_embedding must have hidden_size values")
+            pieces.append(se[None])
+        codec_prefix = np.concatenate(pieces + [self.embed_codec([c.codec_pad_id, c.codec_bos_id])], axis=0)   # :814-823
+        role = self.embed_text(tid[0:3])                                                                       # :825
+        pad_count = codec_prefix.shape[0] - 2
+        combined = np.concatenate([np.repeat(pad_e, pad_count, axis=0), bos_e], axis=0) + codec_prefix[:-1]   # :827-830
+        inputs = np.concatenate([role, combined, icl], axis=0)                                                 # :832
+        return inputs.astype(np.float32), pad_e.astype(np.float32), pad_e[0].astype(np.float32)
 
     def prepare_generation_inputs(self, chat_ids: Sequence[int], tts_bos: int, tts_eos: int, tts_pad: int,
                                   language_id: Optional[int] = None, speaker_id: Optional[int] = None,
@@ -233,21 +291,37 @@ class Qwen3TTSModel:
     def __init__(self, talker: Qwen3TTSTalker, speech_tokenizer=None):
         self.talker, self.speech_tokenizer = talker, speech_tokenizer
 
-    def generate(self, input_embeds, trailing_text_hidden, tts_pad_embed, parameters: Optional[Qwen3GenerateParameters] = None) -> np.ndarray:
-        """generate (:412-510) after prepare_generation_inputs: one utterance -> 1-D waveform (chunked decode, :1059-1068)."""
+    def generate(self, input_embeds, trailing_text_hidden, tts_pad_embed, parameters: Optional[Qwen3GenerateParameters] = None,
+                 ref_codes=None) -> np.ndarray:
+        """generate (:412-510) after prepare_generation_inputs / prepare_icl_generation_inputs: one utterance -> 1-D waveform (chunked
+        decode, :1059-1068).  With ref_codes [groups, T] (or [1, groups, T]; a voice-cloning prompt), the reference codes are decoded in
+        front of the generated ones and the first int(T / total_frames * samples) samples are cut off (:550-565)."""
         if self.speech_tokenizer is None:
             raise _ffi.AudioGenerationError(_ffi.ERR_MODEL_NOT_INITIALIZED, "speech tokenizer not loaded")
         codes, _ = self.talker.generate_codes(np.asarray(input_embeds)[None], [trailing_text_hidden], tts_pad_embed, parameters)
         if codes[0].shape[0] == 0:
             raise _ffi.AudioGenerationError(_ffi.ERR_GENERATION_FAILED, "No audio codes generated")
-        wav, lengths = self.speech_tokenizer.decode(codes[0][None])
-        return wav[0, :int(lengths[0])]
+        frames = codes[0]
+        if ref_codes is not None:
+            rc = np.asarray(ref_codes, dtype=np.int32)
+            rc = rc[0] if rc.ndim == 3 else rc
+            if rc.ndim != 2 or rc.shape[0] != frames.shape[1]:
+                raise _ffi.AudioGenerationError(_ffi.ERR_INVALID_INPUT, "ref_codes must be [num_code_groups, frames]")
+            frames = np.concatenate([rc.T, frames], axis=0)
+        wav, lengths = self.speech_tokenizer.decode(frames[None])
+        audio = wav[0, :int(lengths[0])] if 0 < int(lengths[0]) < wav.shape[1] else wav[0]
+        if ref_codes is not None:
+            cut = int(rc.shape[1] / max(frames.shape[0], 1) * audio.shape[0])
+            if 0 < cut < audio.shape[0]:
+                audio = audio[cut:]
+        return audio
 
     def generate_stream(self, input_embeds, trailing_text_hidden, tts_pad_embed, parameters: Optional[Qwen3GenerateParameters] = None,
-                        streaming_interval: float = 2.0) -> Iterator:
+                        streaming_interval: float = 2.0, ref_codes=None) -> Iterator:
         """generateStream (:512-569): audio chunks DURING generation -- every int(streaming_interval * 12.5) frames the new codes go
         through the speech tokenizer's streaming step (decodeChunk -> streamingDecode, Qwen3TTS.swift:214-231) and are yielded as
-        ('audio', samples); ('token', c0) per frame, ('info', ...) at the end."""
+        ('audio', samples); ('token', c0) per frame, ('info', ...) at the end.  A voice-cloning prompt streams only the generated
+        codes: like the reference's streaming path (:532-545), ref_codes are not decoded in front, so there is nothing to cut."""
         if self.speech_tokenizer is None:
             raise _ffi.AudioGenerationError(_ffi.ERR_MODEL_NOT_INITIALIZED, "speech tokenizer not loaded")
         chunk = max(1, int(streaming_interval * 12.5))

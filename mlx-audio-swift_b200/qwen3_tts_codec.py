@@ -1,10 +1,11 @@
-"""Host-side mirror of the Qwen3-TTS speech tokenizer's DECODE side
-(Sources/MLXAudioTTS/Models/Qwen3TTS/Qwen3TTSSpeechTokenizer.swift:888-1092) over the C ABI (SURVEY.md section 8f row N1;
-parity tests: tests/test_gpu_qwen3_tts_codec.py)."""
+"""Host-side mirror of the Qwen3-TTS speech tokenizer (Sources/MLXAudioTTS/Models/Qwen3TTS/Qwen3TTSSpeechTokenizer.swift:790-1092)
+over the C ABI (SURVEY.md section 8f row N1): the decoder (parity tests: tests/test_gpu_qwen3_tts_codec.py) and the encoder that
+turns reference audio into codes for voice cloning (tests/test_gpu_qwen3_tts_encode.py)."""
 from __future__ import annotations
 
 import ctypes as C
 import re
+from pathlib import Path
 from dataclasses import dataclass, field
 from typing import Dict, List, Optional, Tuple
 
@@ -40,9 +41,133 @@ class Qwen3TTSTokenizerDecoderConfig:
         return cls(**{k: v for k, v in d.items() if k in known})
 
 
-def random_init_weights(cfg: "Qwen3TTSTokenizerDecoderConfig", seed: int = 1234, layer_scale: float = 0.01, out_gain: float = 0.02) -> Dict[str, np.ndarray]:
+@dataclass
+class Qwen3TTSTokenizerEncoderConfig:
+    """Qwen3TTSTokenizerEncoderConfig (Qwen3TTSConfig.swift:391-494: same keys, same defaults) plus the tokenizer config's
+    encoder_valid_num_quantizers (:518-527)."""
+    frame_rate: float = 12.5
+    audio_channels: int = 1
+    codebook_dim: int = 256
+    codebook_size: int = 2048
+    compress: int = 2
+    hidden_size: int = 512
+    intermediate_size: int = 2048
+    kernel_size: int = 7
+    last_kernel_size: int = 3
+    layer_scale_initial_scale: float = 0.01
+    num_attention_heads: int = 8
+    num_filters: int = 64
+    num_hidden_layers: int = 8
+    num_key_value_heads: int = 8
+    num_quantizers: int = 32
+    num_residual_layers: int = 1
+    residual_kernel_size: int = 3
+    rope_theta: float = 10000.0
+    sampling_rate: int = 24000
+    sliding_window: int = 250
+    upsampling_ratios: List[int] = field(default_factory=lambda: [8, 6, 5, 4])
+    use_causal_conv: bool = True
+    use_conv_shortcut: bool = False
+    valid_num_quantizers: int = 16
+
+    @classmethod
+    def from_dict(cls, d: dict, valid_num_quantizers: int = 16) -> "Qwen3TTSTokenizerEncoderConfig":
+        known = {f for f in cls.__dataclass_fields__}
+        return cls(**{k: v for k, v in d.items() if k in known and k != "valid_num_quantizers"}, valid_num_quantizers=valid_num_quantizers)
+
+    @property
+    def head_dim(self) -> int:
+        return self.hidden_size // self.num_attention_heads
+
+    @property
+    def downsample_stride(self) -> int:                 # :810-812
+        return max(1, int(self.sampling_rate / int(np.prod(self.upsampling_ratios)) / self.frame_rate))
+
+    @property
+    def num_code_groups(self) -> int:
+        return min(self.valid_num_quantizers, self.num_quantizers)
+
+    @classmethod
+    def from_ffi(cls, c: "_ffi.SpeechTokenizerEncoderConfig") -> "Qwen3TTSTokenizerEncoderConfig":
+        d = {name: getattr(c, name) for name, _ in c._fields_ if name in cls.__dataclass_fields__ and name != "upsampling_ratios"}
+        d["upsampling_ratios"] = list(c.upsampling_ratios)[: c.num_upsampling_ratios]
+        d["use_causal_conv"], d["use_conv_shortcut"] = bool(c.use_causal_conv), bool(c.use_conv_shortcut)
+        return cls(**d)
+
+    def to_ffi(self) -> "_ffi.SpeechTokenizerEncoderConfig":
+        if len(self.upsampling_ratios) > 8:
+            raise _ffi.AudioGenerationError(_ffi.ERR_INVALID_INPUT, "at most 8 upsampling ratios")
+        c = _ffi.SpeechTokenizerEncoderConfig()
+        for name in ("sampling_rate", "audio_channels", "num_filters", "num_residual_layers", "kernel_size", "residual_kernel_size",
+                     "last_kernel_size", "compress", "hidden_size", "intermediate_size", "num_hidden_layers", "num_attention_heads",
+                     "num_key_value_heads", "head_dim", "codebook_size", "codebook_dim", "num_quantizers", "valid_num_quantizers"):
+            setattr(c, name, int(getattr(self, name)))
+        c.frame_rate, c.rope_theta = float(self.frame_rate), float(self.rope_theta)
+        c.use_causal_conv, c.use_conv_shortcut = int(bool(self.use_causal_conv)), int(bool(self.use_conv_shortcut))
+        c.num_upsampling_ratios = len(self.upsampling_ratios)
+        for i, r in enumerate(self.upsampling_ratios):
+            c.upsampling_ratios[i] = int(r)
+        return c
+
+
+def random_init_encoder_weights(cfg: Qwen3TTSTokenizerEncoderConfig, seed: int = 4321, layer_scale: float = 0.01) -> Dict[str, np.ndarray]:
+    """Random-init encoder weights with the sanitized key set (Qwen3TTSSpeechTokenizer.sanitize's encoder paths without
+    "encoder_model.") in MLX layouts: conv / linear weights N(0, 1 / fan_in), biases N(0, 0.05^2), LayerNorm gains 1 + N(0, 0.1^2)
+    and biases N(0, 0.05^2), layer scales `layer_scale`, codebooks N(0, 1) sums over usages in [0.5, 2]."""
+    rng = np.random.default_rng(seed)
+    W: Dict[str, np.ndarray] = {}
+
+    def rn(shape, s):
+        return (rng.standard_normal(shape) * s).astype(np.float32)
+
+    def conv(prefix, cout, k, cin, bias=True):
+        W[prefix + ".weight"] = rn((cout, k, cin), 1.0 / np.sqrt(k * cin))
+        if bias:
+            W[prefix + ".bias"] = rn((cout,), 0.05)
+
+    F, H = cfg.num_filters, cfg.hidden_size
+    conv("encoder.init_conv1d.conv.conv", F, cfg.kernel_size, cfg.audio_channels)
+    ch = F
+    for i, r in enumerate(reversed(cfg.upsampling_ratios)):
+        conv(f"encoder.layers.{i}.residuals.0.block.0.conv.conv", ch // cfg.compress, cfg.residual_kernel_size, ch)
+        conv(f"encoder.layers.{i}.residuals.0.block.1.conv.conv", ch, 1, ch // cfg.compress)
+        conv(f"encoder.layers.{i}.downsample.conv.conv", 2 * ch, 2 * r, ch)
+        ch *= 2
+    conv("encoder.final_conv1d.conv.conv", H, cfg.last_kernel_size, ch)
+    for l in range(cfg.num_hidden_layers):
+        p = f"encoder_transformer.transformer.layers.{l}."
+        W[p + "self_attn.in_proj.weight"] = rn((3 * H, H), 1.0 / np.sqrt(H))
+        W[p + "self_attn.out_proj.weight"] = rn((H, H), 1.0 / np.sqrt(H))
+        W[p + "gating.linear1.weight"] = rn((cfg.intermediate_size, H), 1.0 / np.sqrt(H))
+        W[p + "gating.linear2.weight"] = rn((H, cfg.intermediate_size), 1.0 / np.sqrt(cfg.intermediate_size))
+        for n in ("norm1", "norm2"):
+            W[p + n + ".weight"] = (1.0 + rn((H,), 0.1)).astype(np.float32)
+            W[p + n + ".bias"] = rn((H,), 0.05)
+        W[p + "layer_scale_1.scale"] = np.full(H, layer_scale, np.float32)
+        W[p + "layer_scale_2.scale"] = np.full(H, layer_scale, np.float32)
+    conv("downsample.conv.conv.conv", H, 2 * cfg.downsample_stride, H, bias=False)
+    D = cfg.codebook_dim
+    for name, n in (("rvq_first", 1), ("rvq_rest", cfg.num_quantizers - 1)):
+        conv(f"quantizer.{name}.input_proj", D, 1, H, bias=False)
+        conv(f"quantizer.{name}.output_proj", H, 1, D, bias=False)
+        for i in range(n):
+            p = f"quantizer.{name}.vq.layers.{i}.codebook"
+            use = rng.uniform(0.5, 2.0, cfg.codebook_size).astype(np.float32)
+            W[p + ".cluster_usage"] = use
+            W[p + ".embedding_sum"] = (rn((cfg.codebook_size, D), 1.0) * use[:, None]).astype(np.float32)
+    return W
+
+
+def random_init_weights(cfg: "Qwen3TTSTokenizerDecoderConfig", seed: int = 1234, layer_scale: float = 0.01, out_gain: float = 0.02,
+                        encoder: bool = False, encoder_config: Optional[Qwen3TTSTokenizerEncoderConfig] = None) -> Dict[str, np.ndarray]:
     """Random-init weights with the reference's key set and MLX layouts (benchmarks; there are no checkpoints here): conv / linear
-    weights N(0, 1 / fan_in), biases N(0, 0.05^2), norm gains 1, SnakeBeta alpha = beta = 0."""
+    weights N(0, 1 / fan_in), biases N(0, 0.05^2), norm gains 1, SnakeBeta alpha = beta = 0.  encoder=True appends the encoder's
+    weights (random_init_encoder_weights; keys prefixed "encoder_model.") after the decoder's, which stay the same draws."""
+    if encoder:
+        W = random_init_weights(cfg, seed, layer_scale, out_gain)
+        for k, v in random_init_encoder_weights(encoder_config or Qwen3TTSTokenizerEncoderConfig(), seed + 1).items():
+            W["encoder_model." + k] = v
+        return W
     rng = np.random.default_rng(seed)
     W: Dict[str, np.ndarray] = {}
 
@@ -129,8 +254,9 @@ def check_array_shape(shape: Tuple[int, ...]) -> bool:
 
 
 def sanitize(weights: Dict[str, np.ndarray]) -> Dict[str, np.ndarray]:
-    """Qwen3TTSSpeechTokenizer.sanitize (:1094-1440), decoder keys only (encoder.* / speaker-encoder keys are dropped: the
-    encoder serves voice cloning, outside this row).  PyTorch-layout checkpoint -> keys below ``decoder.`` in MLX layouts."""
+    """Qwen3TTSSpeechTokenizer.sanitize (:1094-1440), decoder keys only (encoder.* keys are the library's encoder sanitize's,
+    loading.Weights.sanitize_speech_tokenizer_encoder; speaker-encoder keys are dropped).  PyTorch-layout checkpoint -> keys below
+    ``decoder.`` in MLX layouts."""
     out: Dict[str, np.ndarray] = {}
     books: Dict[str, Dict[str, np.ndarray]] = {}
     for raw, v in weights.items():
@@ -269,18 +395,115 @@ class Qwen3TTSSpeechTokenizerDecoder:
             pass
 
 
+class Qwen3TTSSpeechTokenizerEncoder:
+    """Qwen3TTSSpeechTokenizerEncoder (:790-884) on the device: audio [B, 1, n] at 24 kHz -> codes [B, num_code_groups, T] int32,
+    T = encoded_length(n).  ``weights``: the sanitized encoder keys (random_init_encoder_weights' key set); a leading
+    "encoder_model." is dropped.  No encoder weights -> AudioGenerationError modelNotInitialized."""
+
+    def __init__(self, config: Optional[Qwen3TTSTokenizerEncoderConfig] = None, *, weights: Dict[str, np.ndarray], device: int = 0):
+        self.config = config or Qwen3TTSTokenizerEncoderConfig()
+        c = self.config.to_ffi()
+        w = {(k[len("encoder_model."):] if k.startswith("encoder_model.") else k): v for k, v in weights.items() if not k.endswith(".initialized")}
+        self._h = C.c_void_p()
+        if not w:
+            raise _ffi.AudioGenerationError(_ffi.ERR_MODEL_NOT_INITIALIZED, "speech tokenizer encoder: no weights")
+        table, keep = _ffi.make_tensor_table(w)
+        _ffi.check(_ffi.lib().b2a_speech_tokenizer_encoder_create(device, C.byref(c), table, len(w), C.byref(self._h)))
+        del keep
+        self.num_code_groups = int(_ffi.lib().b2a_speech_tokenizer_encoder_num_code_groups(self._h))
+
+    @classmethod
+    def from_model_directory(cls, path, device: int = 0) -> "Qwen3TTSSpeechTokenizerEncoder":
+        """The encoder half of loadSpeechTokenizer (Qwen3TTS.swift:1244-1275): <path>/config.json's encoder_config + every
+        *.safetensors -> sanitize -> weights on the device, all inside the library."""
+        self = cls.__new__(cls)
+        self._h = C.c_void_p()
+        c = _ffi.SpeechTokenizerEncoderConfig()
+        _ffi.check(_ffi.lib().b2a_speech_tokenizer_encoder_config_from_json(str(Path(path) / "config.json").encode(), C.byref(c)))
+        self.config = Qwen3TTSTokenizerEncoderConfig.from_ffi(c)
+        _ffi.check(_ffi.lib().b2a_speech_tokenizer_encoder_create_from_directory(str(path).encode(), device, C.byref(self._h)))
+        self.num_code_groups = int(_ffi.lib().b2a_speech_tokenizer_encoder_num_code_groups(self._h))
+        return self
+
+    @property
+    def stream(self) -> int:
+        return int(_ffi.lib().b2a_speech_tokenizer_encoder_stream(self._h) or 0)
+
+    def encoded_length(self, n_samples: int) -> int:
+        return int(_ffi.lib().b2a_speech_tokenizer_encoder_encoded_length(self._h, int(n_samples)))
+
+    @staticmethod
+    def _audio(audio) -> np.ndarray:
+        a = np.ascontiguousarray(audio, dtype=np.float32)
+        if a.ndim != 3 or a.shape[1] != 1:
+            raise _ffi.AudioGenerationError(_ffi.ERR_INVALID_INPUT, "audio must be [batch, 1, samples]")
+        return a
+
+    def encode(self, audio) -> np.ndarray:
+        """encode (:872-883): audio [B, 1, n] -> codes [B, num_code_groups, T]."""
+        a = self._audio(audio)
+        B, _, n = a.shape
+        out = np.empty((B, self.num_code_groups, max(self.encoded_length(n), 0)), dtype=np.int32)
+        _ffi.check(_ffi.lib().b2a_speech_tokenizer_encoder_encode(self._h, _ffi.ptr(a), B, n, _ffi.ptr(out)))
+        return out
+
+    def encode_dev(self, audio, codes, stream: int = 0) -> None:
+        """Device tensors (torch, contiguous): audio float32 [B, 1, n] -> codes int32 [B, num_code_groups, T], enqueued on `stream`
+        (0: the handle's) without a host synchronisation."""
+        import torch
+        if not (isinstance(audio, torch.Tensor) and isinstance(codes, torch.Tensor) and audio.is_cuda and codes.is_cuda):
+            raise _ffi.AudioGenerationError(_ffi.ERR_INVALID_INPUT, "encode_dev takes CUDA tensors")
+        if audio.dtype != torch.float32 or codes.dtype != torch.int32 or not audio.is_contiguous() or not codes.is_contiguous() or audio.dim() != 3 \
+                or audio.shape[1] != 1 or tuple(codes.shape) != (audio.shape[0], self.num_code_groups, self.encoded_length(audio.shape[2])):
+            raise _ffi.AudioGenerationError(_ffi.ERR_INVALID_INPUT, "encode_dev: audio must be float32 [B, 1, n] and codes int32 [B, groups, T]")
+        _ffi.check(_ffi.lib().b2a_speech_tokenizer_encoder_encode_dev(self._h, _ffi.ptr(audio), int(audio.shape[0]), int(audio.shape[2]),
+                                                                       _ffi.ptr(codes), C.c_void_p(stream or None)))
+
+    def encode_latent(self, audio) -> Tuple[np.ndarray, np.ndarray]:
+        """Parity hook: (z [B, T, hidden_size], codes [B, num_code_groups, T]) of one run."""
+        a = self._audio(audio)
+        B, _, n = a.shape
+        T = self.encoded_length(n)
+        z = np.empty((B, T, self.config.hidden_size), dtype=np.float32)
+        codes = np.empty((B, self.num_code_groups, T), dtype=np.int32)
+        _ffi.check(_ffi.lib().b2a_speech_tokenizer_encoder_latent_test(self._h, _ffi.ptr(a), B, n, _ffi.ptr(z), _ffi.ptr(codes)))
+        return z, codes
+
+    def __del__(self):
+        try:
+            if getattr(self, "_h", None) and self._h.value:
+                _ffi.lib().b2a_speech_tokenizer_encoder_destroy(self._h)
+                self._h = C.c_void_p()
+        except Exception:
+            pass
+
+
 class Qwen3TTSSpeechTokenizer:
-    """Decode side of Qwen3TTSSpeechTokenizer (:1027-1092).  ``audio_codes`` are ``[batch, time, num_quantizers]``."""
+    """Qwen3TTSSpeechTokenizer (:1027-1092).  ``audio_codes`` are ``[batch, time, num_quantizers]``.  ``encoder`` (optional, borrowed)
+    is a Qwen3TTSSpeechTokenizerEncoder; without it the tokenizer only decodes, as the reference does without encoder_config."""
 
     def __init__(self, decoder_config: Optional[Qwen3TTSTokenizerDecoderConfig] = None, *, weights: Dict[str, np.ndarray], decode_upsample_rate: int = 1920,
-                 device: int = 0, max_batch: int = 1, max_cache_frames: int = 4096):
+                 device: int = 0, max_batch: int = 1, max_cache_frames: int = 4096, encoder: Optional[Qwen3TTSSpeechTokenizerEncoder] = None):
         self.decode_upsample_rate = int(decode_upsample_rate)
         self.decoder = Qwen3TTSSpeechTokenizerDecoder(decoder_config or Qwen3TTSTokenizerDecoderConfig(), weights=weights, device=device,
                                                       max_batch=max_batch, max_cache_frames=max_cache_frames)
+        self.encoder = encoder
 
     @property
-    def has_encoder(self) -> bool:        # the encoder (voice cloning) is outside this row
-        return False
+    def has_encoder(self) -> bool:
+        return self.encoder is not None
+
+    def encode(self, audio) -> np.ndarray:
+        """encode (:1049-1057) with referenceAudioForEncoder's shapes (Qwen3TTS.swift:239-247): [n] -> [1, 1, n], [B, n] -> [B, 1, n],
+        [B, 1, n] as is.  Returns codes [B, num_code_groups, T]."""
+        if self.encoder is None:
+            raise _ffi.AudioGenerationError(_ffi.ERR_MODEL_NOT_INITIALIZED, "Speech tokenizer encoder not available")
+        a = np.asarray(audio, dtype=np.float32)
+        if a.ndim == 1:
+            a = a[None, None, :]
+        elif a.ndim == 2:
+            a = a[:, None, :]
+        return self.encoder.encode(a)
 
     def decode(self, audio_codes) -> Tuple[np.ndarray, np.ndarray]:
         """decode (:1059-1068) -> (wav [B, samples], valid lengths [B])."""
