@@ -97,7 +97,9 @@ void b2a_mel_destroy(b2a_mel* h);
  * kind 1: WhisperAudio.encoderFeatures (Sources/MLXAudioSTT/Models/Whisper/WhisperAudio.swift:
  *         7-13,38-87): pad/trim each clip to 480000, periodic Hann, Slaney scale, last frame
  *         dropped, per-clip max-8 clamp, out [B, 3000, n_mels].
- * pcm is [B, n_samples] (every clip the same length); b2a_logmel_frames gives frames per clip. */
+ * pcm is [B, n_samples] (every clip the same length); b2a_logmel_frames gives frames per clip.
+ * n_fft is 400 or 1024 (the Qwen3-TTS speaker encoder's front-end), here and in b2a_mel_create;
+ * any other size -> B2A_ERR_INVALID_INPUT. */
 typedef struct b2a_logmel b2a_logmel;
 int32_t b2a_logmel_create(int32_t device, int32_t kind, int32_t sample_rate, int32_t n_fft,
                           int32_t hop_length, int32_t n_mels, b2a_logmel** out);
@@ -745,6 +747,51 @@ void b2a_speech_tokenizer_encoder_destroy(b2a_speech_tokenizer_encoder* h);
 int32_t b2a_weights_sanitize_speech_tokenizer_encoder(b2a_weights* w);
 int32_t b2a_speech_tokenizer_encoder_config_from_json(const char* config_path, b2a_speech_tokenizer_encoder_config* cfg);
 int32_t b2a_speech_tokenizer_encoder_create_from_directory(const char* dir, int32_t device, b2a_speech_tokenizer_encoder** out);
+
+/* ---- Qwen3-TTS speaker encoder (Qwen3TTSSpeakerEncoder.swift, an ECAPA-TDNN): the x-vector a Base checkpoint's voice-cloning
+ * prompt carries in its codec prefix (Qwen3TTS.swift:820-823).  audio [B, n] float32 at sample_rate -> log-mel
+ * (computeMelSpectrogram with n_fft 1024, hop 256, 128 mels; b2a_logmel kind 0) [B, T = 1 + n / 256, 128] -> TDNN block ->
+ * SE-Res2Net blocks -> multi-layer feature aggregation -> attentive statistics pooling -> fc -> [B, enc_dim].  fp32 throughout;
+ * every reduction over time has a fixed order and no atomics, so a clip's embedding does not depend on the batch it runs in.
+ * Config defaults: Qwen3TTSConfig.swift:92-103.  Errors: mel_dim != 128, lists of unequal length (config_from_json), a channel count
+ * not divisible by enc_res2net_scale (or whose chunks are not a multiple of 4 channels), sum(enc_channels[1:-1]) !=
+ * enc_channels[-1], an SE-Res2Net block whose input and output widths differ, (k - 1) * d odd, empty audio, n <= 512 samples,
+ * T <= max((k - 1) * d / 2) frames -> B2A_ERR_INVALID_INPUT; no or partial weights -> B2A_ERR_MODEL_NOT_INITIALIZED.          */
+typedef struct b2a_qwen3_speaker_encoder_config {
+    int32_t mel_dim;
+    int32_t enc_dim;
+    int32_t num_enc_layers;        /* entries used in each of the three lists below (3..8) */
+    int32_t enc_channels[8];
+    int32_t enc_kernel_sizes[8];
+    int32_t enc_dilations[8];
+    int32_t enc_attention_channels;
+    int32_t enc_res2net_scale;
+    int32_t enc_se_channels;
+    int32_t sample_rate;
+} b2a_qwen3_speaker_encoder_config;
+
+typedef struct b2a_qwen3_speaker_encoder b2a_qwen3_speaker_encoder;
+/* tensors: b2a_weights_sanitize_qwen3_speaker_encoder's keys (blocks.*, mfa.*, asp.*, fc.*) in MLX layout ([out, k, in]) */
+int32_t b2a_qwen3_speaker_encoder_create(int32_t device, const b2a_qwen3_speaker_encoder_config* cfg, const b2a_tensor* tensors,
+                                         int32_t n_tensors, b2a_qwen3_speaker_encoder** out);
+/* mel frames T for n samples: 1 + n / 256 (0 for a null handle) */
+int64_t b2a_qwen3_speaker_encoder_frames(const b2a_qwen3_speaker_encoder* h, int64_t n_samples);
+/* host audio [B, n] -> host embeddings [B, enc_dim] */
+int32_t b2a_qwen3_speaker_encoder_embed(b2a_qwen3_speaker_encoder* h, const float* audio, int32_t batch, int64_t n_samples, float* out);
+/* device buffers, enqueued on `stream` (NULL: the handle's stream) without a host synchronisation */
+int32_t b2a_qwen3_speaker_encoder_embed_dev(b2a_qwen3_speaker_encoder* h, const float* d_audio, int32_t batch, int64_t n_samples,
+                                            float* d_out, void* stream);
+/* the module's own input: host log-mel [B, T, mel_dim] -> host embeddings [B, enc_dim] */
+int32_t b2a_qwen3_speaker_encoder_embed_mel(b2a_qwen3_speaker_encoder* h, const float* mel, int32_t batch, int64_t frames, float* out);
+void* b2a_qwen3_speaker_encoder_stream(b2a_qwen3_speaker_encoder* h);
+void b2a_qwen3_speaker_encoder_destroy(b2a_qwen3_speaker_encoder* h);
+/* Loading: Qwen3TTSSpeakerEncoder.sanitize (:324-354) on an open checkpoint -- the keys after the "speaker_encoder" component, 3-D
+ * ".weight" tensors that fail checkArrayShapeQwen3 transposed [out, in, k] -> [out, k, in], every other key dropped; the top-level
+ * config.json's "speaker_encoder_config" (defaults for missing keys); both from a model directory, where a config whose
+ * tts_model_type is not "base" or a checkpoint without speaker-encoder keys -> B2A_ERR_MODEL_NOT_INITIALIZED.                 */
+int32_t b2a_weights_sanitize_qwen3_speaker_encoder(b2a_weights* w);
+int32_t b2a_qwen3_speaker_encoder_config_from_json(const char* config_path, b2a_qwen3_speaker_encoder_config* cfg);
+int32_t b2a_qwen3_speaker_encoder_create_from_directory(const char* model_dir, int32_t device, b2a_qwen3_speaker_encoder** out);
 
 #ifdef __cplusplus
 }

@@ -12,13 +12,15 @@ from .vocos import Vocos
 from .encodec import Encodec, EncodecConfig, EncodecEncodedAudio
 from .loading import Weights, llama_config_from_json
 from .whisper import STTGenerateParameters, STTOutput, StreamingConfig, StreamingInferenceSession, StreamingUpdate, WhisperModel
-from .qwen3_tts import Qwen3CodePredictorConfig, Qwen3GenerateParameters, Qwen3TalkerConfig, Qwen3TTSModel, Qwen3TTSTalker
+from .qwen3_tts import (Qwen3CodePredictorConfig, Qwen3GenerateParameters, Qwen3SpeakerEncoderConfig, Qwen3TalkerConfig, Qwen3TTSModel,
+                        Qwen3TTSSpeakerEncoder, Qwen3TTSTalker)
 
 __all__ = ["AudioGenerationError", "IncrementalMelSpectrogram", "LogMel", "compute_mel_spectrogram", "hanning_window", "hamming_window", "power_to_db",
            "mel_filters", "whisper_encoder_features", "SNAC", "LlamaTTSModel", "GenerateParameters",
            "AudioGenerationInfo", "Vocos", "Weights", "llama_config_from_json", "Encodec", "EncodecConfig", "EncodecEncodedAudio", "WhisperModel", "STTGenerateParameters", "STTOutput",
            "StreamingInferenceSession", "StreamingConfig", "StreamingUpdate",
-           "Qwen3TTSTalker", "Qwen3TTSModel", "Qwen3TalkerConfig", "Qwen3CodePredictorConfig", "Qwen3GenerateParameters"]
+           "Qwen3TTSTalker", "Qwen3TTSModel", "Qwen3TalkerConfig", "Qwen3CodePredictorConfig", "Qwen3GenerateParameters",
+           "Qwen3TTSSpeakerEncoder", "Qwen3SpeakerEncoderConfig"]
 
 
 def device_count() -> int:

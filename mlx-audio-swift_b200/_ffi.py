@@ -96,6 +96,12 @@ class SpeechTokenizerEncoderConfig(C.Structure):
                 + [(n, C.c_int32) for n in ("codebook_size", "codebook_dim", "num_quantizers", "valid_num_quantizers")])
 
 
+class Qwen3SpeakerEncoderConfig(C.Structure):
+    _fields_ = ([(n, C.c_int32) for n in ("mel_dim", "enc_dim", "num_enc_layers")]
+                + [(n, C.c_int32 * 8) for n in ("enc_channels", "enc_kernel_sizes", "enc_dilations")]
+                + [(n, C.c_int32) for n in ("enc_attention_channels", "enc_res2net_scale", "enc_se_channels", "sample_rate")])
+
+
 class Qwen3TalkerConfig(C.Structure):
     _fields_ = ([(n, C.c_int32) for n in ("vocab_size", "hidden_size", "intermediate_size", "num_hidden_layers", "num_attention_heads",
                                            "num_key_value_heads", "head_dim")]
@@ -258,6 +264,16 @@ SIGNATURES = {
     "b2a_weights_sanitize_speech_tokenizer_encoder": (C.c_int32, [_P]),
     "b2a_speech_tokenizer_encoder_config_from_json": (C.c_int32, [C.c_char_p, C.POINTER(SpeechTokenizerEncoderConfig)]),
     "b2a_speech_tokenizer_encoder_create_from_directory": (C.c_int32, [C.c_char_p, C.c_int32, C.POINTER(_P)]),
+    "b2a_qwen3_speaker_encoder_create": (C.c_int32, [C.c_int32, C.POINTER(Qwen3SpeakerEncoderConfig), C.POINTER(Tensor), C.c_int32, C.POINTER(_P)]),
+    "b2a_qwen3_speaker_encoder_frames": (C.c_int64, [_P, C.c_int64]),
+    "b2a_qwen3_speaker_encoder_embed": (C.c_int32, [_P, _P, C.c_int32, C.c_int64, _P]),
+    "b2a_qwen3_speaker_encoder_embed_dev": (C.c_int32, [_P, _P, C.c_int32, C.c_int64, _P, _P]),
+    "b2a_qwen3_speaker_encoder_embed_mel": (C.c_int32, [_P, _P, C.c_int32, C.c_int64, _P]),
+    "b2a_qwen3_speaker_encoder_stream": (C.c_void_p, [_P]),
+    "b2a_qwen3_speaker_encoder_destroy": (None, [_P]),
+    "b2a_weights_sanitize_qwen3_speaker_encoder": (C.c_int32, [_P]),
+    "b2a_qwen3_speaker_encoder_config_from_json": (C.c_int32, [C.c_char_p, C.POINTER(Qwen3SpeakerEncoderConfig)]),
+    "b2a_qwen3_speaker_encoder_create_from_directory": (C.c_int32, [C.c_char_p, C.c_int32, C.POINTER(_P)]),
     "b2a_encodec_destroy": (None, [_P]),
     "b2a_weights_load": (C.c_int32, [C.c_char_p, C.POINTER(_P)]),
     "b2a_weights_count": (C.c_int32, [_P]),

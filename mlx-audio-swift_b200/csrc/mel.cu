@@ -1,4 +1,4 @@
-// Log-mel front-end for sm_90a: STFT(400) -> power -> mel filterbank -> log10 in ONE kernel,
+// Log-mel front-end for sm_90a: STFT(400 or 1024) -> power -> mel filterbank -> log10 in ONE kernel,
 // plus the elementwise max-8 clamp pass.  Replaces (reference paths):
 //   Sources/MLXAudioCore/DSP.swift:15-22,76-168,181-273
 //   Sources/MLXAudioSTT/Streaming/IncrementalMelSpectrogram.swift:18-208
@@ -8,8 +8,9 @@
 // log-mel float32 [B, F, n_mels] (written once by kernel 1, clamped in place by kernel 2).
 // The 400-point real DFT is done as a 20x20 Cooley-Tukey split in shared memory (two passes of
 // 20-point DFTs with a twiddle in between, exploiting conjugate symmetry of the real input; every
-// 20-point transform is a folded real-input DFT, real_dft20: 10 FMAs per output);
-// the filterbank is applied in its sparse (contiguous-support) form.
+// 20-point transform is a folded real-input DFT, real_dft20: 10 FMAs per output); the 1024-point DFT (the Qwen3-TTS speaker
+// encoder's front-end) is the same kernel split 32x32 with real_dft32.  The filterbank is applied in its sparse (contiguous-support)
+// form.
 #include "common.cuh"
 
 #include <math.h>
@@ -64,8 +65,11 @@ static void mel_filters_host(int sr, int n_fft, int n_mels, float f_min, float f
 // ------------------------------------------------------------------------------------------------
 // Device side
 // ------------------------------------------------------------------------------------------------
-constexpr int NFFT = 400, NBINS = 201, R = 20, K1N = 11;  // 400 = 20*20, k1 = 0..10 by symmetry
-constexpr int FR = 10;                                       // frames per CTA (20 threads per frame in the DFT passes)
+// The kernel is a template on the radix R of the R x R split: R = 20 (n_fft 400) or 32 (n_fft 1024).  FR frames per CTA; R
+// threads per frame in the DFT passes.  FR = 4 at R = 32 keeps the static shared memory below 48 KB.
+template <int R> struct MelGeom {
+    static constexpr int NFFT = R * R, NBINS = NFFT / 2 + 1, K1N = R / 2 + 1, FR = R == 20 ? 10 : 4;
+};
 constexpr int MEL_THREADS = 256;
 
 // exp(-2*pi*i*j/20) = (C20[j], S20[j]): with both DFT loops fully unrolled every twiddle index is a compile-time constant, so the
@@ -82,7 +86,8 @@ __device__ constexpr float S20[20] = {-0.f, -0.309017003f, -0.587785244f, -0.809
 // cosine / sine differ by the sign (-1)^k): 10 FMAs per output instead of 40.  Fully unrolled: every twiddle is an immediate.
 //   re[k] = x0 + (-1)^k x10 + a5 cos(pi k / 2) + sum_{n=1..4} (a[n] + (-1)^k a[10-n]) cos(2 pi n k / 20),    a[n] = x[n] + x[20-n]
 //   im[k] =                   d5 S20[5k]       + sum_{n=1..4} (d[n] - (-1)^k d[10-n]) S20[n k],              d[n] = x[n] - x[20-n]
-__device__ __forceinline__ void real_dft20(const float (&x)[R], float (&re)[K1N], float (&im)[K1N]) {
+__device__ __forceinline__ void real_dft20(const float (&x)[20], float (&re)[11], float (&im)[11]) {
+    constexpr int R = 20, K1N = 11;
     float a[10], d[10];
 #pragma unroll
     for (int n = 1; n < 10; ++n) { a[n] = x[n] + x[R - n]; d[n] = x[n] - x[R - n]; }
@@ -104,10 +109,51 @@ __device__ __forceinline__ void real_dft20(const float (&x)[R], float (&re)[K1N]
     }
 }
 
+// exp(-2*pi*i*j/32) = (C32[j], S32[j])
+__device__ constexpr float C32[32] = {1.f, 0.980785251f, 0.923879504f, 0.831469595f, 0.707106769f, 0.555570245f, 0.382683426f, 0.195090324f,
+                                      6.12323426e-17f, -0.195090324f, -0.382683426f, -0.555570245f, -0.707106769f, -0.831469595f, -0.923879504f,
+                                      -0.980785251f, -1.f, -0.980785251f, -0.923879504f, -0.831469595f, -0.707106769f, -0.555570245f,
+                                      -0.382683426f, -0.195090324f, -1.83697015e-16f, 0.195090324f, 0.382683426f, 0.555570245f, 0.707106769f,
+                                      0.831469595f, 0.923879504f, 0.980785251f};
+__device__ constexpr float S32[32] = {-0.f, -0.195090324f, -0.382683426f, -0.555570245f, -0.707106769f, -0.831469595f, -0.923879504f,
+                                      -0.980785251f, -1.f, -0.980785251f, -0.923879504f, -0.831469595f, -0.707106769f, -0.555570245f,
+                                      -0.382683426f, -0.195090324f, -1.22464685e-16f, 0.195090324f, 0.382683426f, 0.555570245f, 0.707106769f,
+                                      0.831469595f, 0.923879504f, 0.980785251f, 1.f, 0.980785251f, 0.923879504f, 0.831469595f, 0.707106769f,
+                                      0.555570245f, 0.382683426f, 0.195090324f};
+
+// Forward 32-point DFT of a REAL sequence, outputs k = 0..16, folded as real_dft20 is (x[n] +- x[32-n], then n <-> 16-n):
+//   re[k] = x0 + (-1)^k x16 + a8 cos(pi k / 2) + sum_{n=1..7} (a[n] + (-1)^k a[16-n]) cos(2 pi n k / 32)
+//   im[k] =                   d8 S32[8k]       + sum_{n=1..7} (d[n] - (-1)^k d[16-n]) S32[n k]
+__device__ __forceinline__ void real_dft32(const float (&x)[32], float (&re)[17], float (&im)[17]) {
+    constexpr int R = 32, K1N = 17;
+    float a[16], d[16];
+#pragma unroll
+    for (int n = 1; n < 16; ++n) { a[n] = x[n] + x[R - n]; d[n] = x[n] - x[R - n]; }
+    float ee[8], eo[8], de[8], dd[8];
+#pragma unroll
+    for (int n = 1; n < 8; ++n) { ee[n] = a[n] + a[16 - n]; eo[n] = a[n] - a[16 - n]; de[n] = d[n] - d[16 - n]; dd[n] = d[n] + d[16 - n]; }
+    const float b_even = x[0] + x[16], b_odd = x[0] - x[16];
+#pragma unroll
+    for (int k = 0; k < K1N; ++k) {
+        const bool ev = (k & 1) == 0;
+        float r = fmaf(a[8], C32[(8 * k) % R], ev ? b_even : b_odd);
+        float i = d[8] * S32[(8 * k) % R];
+#pragma unroll
+        for (int n = 1; n < 8; ++n) {
+            r = fmaf(ev ? ee[n] : eo[n], C32[(n * k) % R], r);
+            i = fmaf(ev ? de[n] : dd[n], S32[(n * k) % R], i);
+        }
+        re[k] = r; im[k] = i;
+    }
+}
+
+__device__ __forceinline__ void real_dft(const float (&x)[20], float (&re)[11], float (&im)[11]) { real_dft20(x, re, im); }
+__device__ __forceinline__ void real_dft(const float (&x)[32], float (&re)[17], float (&im)[17]) { real_dft32(x, re, im); }
+
 struct MelTables {          // device pointers, owned by MelCore
-    const float* window;    // [400]
-    const float2* tw20;     // [20]  exp(-2*pi*i*j/20)
-    const float2* tw400;    // [400] exp(-2*pi*i*j/400)
+    const float* window;    // [n_fft]
+    const float2* tw20;     // [R]     exp(-2*pi*i*j/R)
+    const float2* tw400;    // [n_fft] exp(-2*pi*i*j/n_fft)
     const int* fb_start;    // [n_mels] first bin of the filter's support
     const int* fb_count;    // [n_mels]
     const int* fb_off;      // [n_mels] offset into fb_w
@@ -123,13 +169,15 @@ __device__ __forceinline__ void atomic_max_float(float* addr, float v) {
 // pad_mode 0: frames index the signal directly.  pad_mode 1: centred STFT -- the signal is
 // virtually reflect-padded by NFFT/2 on both sides and zero-extended from n_valid to n_total
 // (WhisperAudio.padOrTrimToWindow + reflectPad; DSP.stft reflect branch).
+template <int R>
 __global__ void __launch_bounds__(MEL_THREADS)
 mel_log_kernel(const float* __restrict__ pcm, long long pcm_stride, long long n_valid, long long n_total,
                int pad_mode, int hop, int n_frames, MelTables tb, float* __restrict__ out,
                float* __restrict__ max_buf) {
+    constexpr int NFFT = MelGeom<R>::NFFT, NBINS = MelGeom<R>::NBINS, K1N = MelGeom<R>::K1N, FR = MelGeom<R>::FR;
     __shared__ float s_x[(FR - 1) * 160 + NFFT + 8 + (FR - 1) * 96];  // sized for hop <= 256
     __shared__ float s_win[NFFT];
-    __shared__ float2 s_tw[K1N][R];                 // tw400[n2 * k1] as [k1][n2]: the 20 threads of a frame read consecutive entries
+    __shared__ float2 s_tw[K1N][R];                 // tw400[n2 * k1] as [k1][n2]: the R threads of a frame read consecutive entries
     __shared__ float2 s_y[FR][K1N][R + 1];          // + 1: the rows k1 of pass 2's readers fall into different banks
     __shared__ float s_p[FR][NBINS + 3];
     __shared__ float s_red[MEL_THREADS / 32];
@@ -159,8 +207,8 @@ mel_log_kernel(const float* __restrict__ pcm, long long pcm_stride, long long n_
     }
     __syncthreads();
 
-    // pass 1: Y[k1][n2] = tw400[n2*k1] * sum_n1 xw[20*n1+n2] * tw20[(n1*k1)%20], k1 = 0..10.  One thread per (frame, n2): its 20
-    // windowed samples live in registers and feed all 11 k1 sums.
+    // pass 1: Y[k1][n2] = tw400[n2*k1] * sum_n1 xw[R*n1+n2] * tw20[(n1*k1)%R], k1 = 0..R/2.  One thread per (frame, n2): its R
+    // windowed samples live in registers and feed all R/2+1 k1 sums.
     for (int o = tid; o < nf * R; o += MEL_THREADS) {
         const int f = o / R, n2 = o - f * R;
         const float* x = s_x + f * hop + n2;
@@ -168,7 +216,7 @@ mel_log_kernel(const float* __restrict__ pcm, long long pcm_stride, long long n_
 #pragma unroll
         for (int n1 = 0; n1 < R; ++n1) xr[n1] = x[R * n1] * s_win[R * n1 + n2];
         float re[K1N], im[K1N];
-        real_dft20(xr, re, im);
+        real_dft(xr, re, im);
 #pragma unroll
         for (int k1 = 0; k1 < K1N; ++k1) {
             const float2 w = s_tw[k1][n2];
@@ -177,9 +225,9 @@ mel_log_kernel(const float* __restrict__ pcm, long long pcm_stride, long long n_
     }
     __syncthreads();
 
-    // pass 2: X[k1+20*k2] = sum_n2 Y[k1][n2] tw20[(n2*k2)%20]; for k1 > 10, Y[k1][n2] = conj(Y[20-k1][n2]) * tw20[n2] (real input),
-    // i.e. X[k1+20*k2] = T[k2+1] with T[kk] = sum_n2 conj(Y[20-k1][n2]) tw20[(n2*kk)%20].  One thread per (frame, k1): it loads its
-    // row of Y once and evaluates T[0..10] against compile-time twiddles.
+    // pass 2: X[k1+R*k2] = sum_n2 Y[k1][n2] tw20[(n2*k2)%R]; for k1 > R/2, Y[k1][n2] = conj(Y[R-k1][n2]) * tw20[n2] (real input),
+    // i.e. X[k1+R*k2] = T[k2+1] with T[kk] = sum_n2 conj(Y[R-k1][n2]) tw20[(n2*kk)%R].  One thread per (frame, k1): it loads its
+    // row of Y once and evaluates T[0..R/2] against compile-time twiddles.
     for (int o = tid; o < nf * R; o += MEL_THREADS) {
         const int f = o / R, k1 = o - f * R;
         const bool mirror = k1 > R / 2;
@@ -190,8 +238,8 @@ mel_log_kernel(const float* __restrict__ pcm, long long pcm_stride, long long n_
         for (int n2 = 0; n2 < R; ++n2) { const float2 v = y[n2]; yr[n2] = v.x; yi[n2] = sgn * v.y; }
         // DFT(yr + i yi) = DFT(yr) + i DFT(yi): two real-input transforms
         float ra[K1N], ia[K1N], rb[K1N], ib[K1N];
-        real_dft20(yr, ra, ia);
-        real_dft20(yi, rb, ib);
+        real_dft(yr, ra, ia);
+        real_dft(yi, rb, ib);
 #pragma unroll
         for (int kk = 0; kk < K1N; ++kk) {
             const float re = ra[kk] - ib[kk], im = ia[kk] + rb[kk];
@@ -251,12 +299,13 @@ struct MelCore {
 
     MelCore(int device_, int sr_, int n_fft_, int hop_, int n_mels_, bool periodic, int mel_scale)
         : device(device_), sr(sr_), n_fft(n_fft_), hop(hop_), n_mels(n_mels_) {
-        B2A_CHECK(n_fft == NFFT, B2A_ERR_INVALID_INPUT, "only n_fft == 400 is implemented on the device path");
+        B2A_CHECK(n_fft == 400 || n_fft == 1024, B2A_ERR_INVALID_INPUT, "only n_fft == 400 or 1024 is implemented on the device path");
         B2A_CHECK(hop > 0 && hop <= 256, B2A_ERR_INVALID_INPUT, "hop_length must be in 1..256");
         B2A_CHECK(n_mels > 0 && n_mels <= 512, B2A_ERR_INVALID_INPUT, "n_mels must be in 1..512");
         require_device(device);
-        std::vector<float> win(NFFT), fb((size_t)NBINS * n_mels);
-        hanning_window_host(NFFT, periodic, win.data());
+        const int R = n_fft == 400 ? 20 : 32, NBINS = n_fft / 2 + 1;
+        std::vector<float> win(n_fft), fb((size_t)NBINS * n_mels);
+        hanning_window_host(n_fft, periodic, win.data());
         mel_filters_host(sr, n_fft, n_mels, 0.f, -1.f, true, mel_scale, fb.data());
         std::vector<int> start(n_mels), count(n_mels), off(n_mels);
         std::vector<float> w;
@@ -270,13 +319,13 @@ struct MelCore {
             for (int k = 0; k < count[m]; ++k) w.push_back(fb[(size_t)(start[m] + k) * n_mels + m]);
         }
         if (w.empty()) w.push_back(0.f);
-        std::vector<float2> t20(R), t400(NFFT);
+        std::vector<float2> t20(R), t400(n_fft);
         for (int j = 0; j < R; ++j) t20[j] = make_float2((float)cos(2.0 * M_PI * j / R), (float)-sin(2.0 * M_PI * j / R));
-        for (int j = 0; j < NFFT; ++j) t400[j] = make_float2((float)cos(2.0 * M_PI * j / NFFT), (float)-sin(2.0 * M_PI * j / NFFT));
-        d_window.upload(win.data(), NFFT);
+        for (int j = 0; j < n_fft; ++j) t400[j] = make_float2((float)cos(2.0 * M_PI * j / n_fft), (float)-sin(2.0 * M_PI * j / n_fft));
+        d_window.upload(win.data(), n_fft);
         d_fbw.upload(w.data(), w.size());
         d_tw20.upload(t20.data(), R);
-        d_tw400.upload(t400.data(), NFFT);
+        d_tw400.upload(t400.data(), n_fft);
         d_start.upload(start.data(), n_mels);
         d_count.upload(count.data(), n_mels);
         d_off.upload(off.data(), n_mels);
@@ -288,9 +337,15 @@ struct MelCore {
     void launch(const float* d_pcm, long long stride, long long n_valid, long long n_total, int pad_mode,
                 int batch, int n_frames, float* d_out, float* d_max, cudaStream_t s) const {
         if (n_frames <= 0 || batch <= 0) return;
-        dim3 grid(cdiv(n_frames, FR), batch);
-        mel_log_kernel<<<grid, MEL_THREADS, 0, s>>>(d_pcm, stride, n_valid, n_total, pad_mode, hop, n_frames,
-                                                    tb, d_out, d_max);
+        if (n_fft == 400) {
+            dim3 grid(cdiv(n_frames, MelGeom<20>::FR), batch);
+            mel_log_kernel<20><<<grid, MEL_THREADS, 0, s>>>(d_pcm, stride, n_valid, n_total, pad_mode, hop, n_frames,
+                                                            tb, d_out, d_max);
+        } else {
+            dim3 grid(cdiv(n_frames, MelGeom<32>::FR), batch);
+            mel_log_kernel<32><<<grid, MEL_THREADS, 0, s>>>(d_pcm, stride, n_valid, n_total, pad_mode, hop, n_frames,
+                                                            tb, d_out, d_max);
+        }
         const long long per_clip = (long long)n_frames * n_mels;
         dim3 g2((unsigned)std::min<long long>(cdiv(per_clip, 256), 1024), batch);
         mel_clamp_kernel<<<g2, 256, 0, s>>>(d_out, per_clip, d_max);

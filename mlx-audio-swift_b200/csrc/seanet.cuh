@@ -3,6 +3,8 @@
 // search in ordered fp32 (DESIGN.md §3.6b).  Both encoders pad their convs causally by kernel - stride at dilation 1:
 // Encodec's paddingTotal = kernelSize - stride (EncodecLayers.swift:118, extra right padding :137-139) equals Mimi's
 // kEff - stride (Mimi/Conv.swift:207-211), and one residual layer per stage keeps every encoder conv at dilation 1.
+// The Qwen3-TTS speaker encoder (speaker_encoder.cu) runs its convs on the same conv kernel, with the dilation, channel-slice
+// strides, input addend and ReLU / tanh epilogue that only it sets (DESIGN.md §3.8c).
 #pragma once
 #include "common.cuh"
 
@@ -19,8 +21,12 @@ struct ConvArgs {
     const float* xa; int La, Ca, taps, padL, reflect, elu_a, backward;   // forward: src = q*stride + tap - padL; backward: src = q - tap
     int edge = 0;            // forward only: out-of-range rows replicate the nearest edge row (Mimi's ConvDownsample1d pads with .edge)
     int stride = 1;          // forward only: an encoder downsampling conv (k = 2s) gathers its 2s contiguous rows per output
+    int dil = 1;             // forward only: tap spacing (src = q*stride + tap*dil - padL)
+    int lda = 0;             // row stride of xa in floats (0: Ca), so a conv can read a channel slice of a wider tensor
+    const float* xa_add = nullptr;   // optional second addend of xa, same addressing: the conv reads xa + xa_add
     // source B (optional): one tap at src = q over xb [N, Lq, Cb]
     const float* xb; int Cb, elu_b;
+    int ldb = 0;             // row stride of xb in floats (0: Cb)
     const float* A;          // [M, K] row-major, K = taps*Ca + Cb
     const float* bias;       // [M] or null
     const float* res;        // optional residual, same addressing as out
@@ -28,6 +34,9 @@ struct ConvArgs {
     int M, K, Lq, N;
     long long out_per_n;     // Tout * Cout
     long long shift;         // pl * Cout (left trim of a transposed conv)
+    int ldo = 0;             // output row stride in floats (0: M), so a conv can write a channel slice of a wider tensor
+    int act = 0;             // epilogue after bias and residual: 1 ReLU, 2 tanh(ReLU)
+    long long bias_n = 0;    // bias stride per batch row n (0: one bias for all rows)
 };
 
 constexpr int BK = 16;
@@ -37,7 +46,7 @@ __device__ __forceinline__ int src_index(int q, int tap, const ConvArgs& a) {
         const int s = q - tap;
         return (s >= 0 && s < a.La) ? s : -1;
     }
-    int s = q * a.stride + tap - a.padL;
+    int s = q * a.stride + tap * a.dil - a.padL;
     if (s < 0) return a.edge ? 0 : a.reflect ? min(-s, a.La - 1) : -1;
     if (s >= a.La) return a.edge ? a.La - 1 : a.reflect ? max(a.La - 2 - (s - a.La), 0) : -1;
     return s;
@@ -81,11 +90,16 @@ __global__ void __launch_bounds__(256) ec_conv_kernel(ConvArgs a) {
                     const int tap = kk / a.Ca, ci = kk - tap * a.Ca;
                     const int s = src_index(q, tap, a);
                     if (s >= 0) {
-                        v = *reinterpret_cast<const float4*>(a.xa + ((long long)n * a.La + s) * a.Ca + ci);
+                        const long long off = ((long long)n * a.La + s) * (a.lda ? a.lda : a.Ca) + ci;
+                        v = *reinterpret_cast<const float4*>(a.xa + off);
+                        if (a.xa_add) {
+                            const float4 u = *reinterpret_cast<const float4*>(a.xa_add + off);
+                            v.x += u.x; v.y += u.y; v.z += u.z; v.w += u.w;
+                        }
                         if (a.elu_a) { v.x = elu1(v.x); v.y = elu1(v.y); v.z = elu1(v.z); v.w = elu1(v.w); }
                     }
                 } else {
-                    v = *reinterpret_cast<const float4*>(a.xb + ((long long)n * a.Lq + q) * a.Cb + (kk - Ka));
+                    v = *reinterpret_cast<const float4*>(a.xb + ((long long)n * a.Lq + q) * (a.ldb ? a.ldb : a.Cb) + (kk - Ka));
                     if (a.elu_b) { v.x = elu1(v.x); v.y = elu1(v.y); v.z = elu1(v.z); v.w = elu1(v.w); }
                 }
             }
@@ -136,6 +150,8 @@ __global__ void __launch_bounds__(256) ec_conv_kernel(ConvArgs a) {
     }
     float* outn = a.out + (long long)n * a.out_per_n;
     const float* resn = a.res ? a.res + (long long)n * a.out_per_n : nullptr;
+    const float* biasn = a.bias ? a.bias + (long long)n * a.bias_n : nullptr;
+    const int ldo = a.ldo ? a.ldo : a.M;
 #pragma unroll
     for (int j = 0; j < RT; ++j) {
         const int q = q0 + ty + 16 * j;
@@ -144,10 +160,11 @@ __global__ void __launch_bounds__(256) ec_conv_kernel(ConvArgs a) {
         for (int i = 0; i < RM; ++i) {
             const int m = m0 + tx + 16 * i;
             if (m >= a.M) continue;
-            const long long o = (long long)q * a.M + m - a.shift;
+            const long long o = (long long)q * ldo + m - a.shift;
             if (o < 0 || o >= a.out_per_n) continue;
-            float v = acc[i][j] + (a.bias ? a.bias[m] : 0.f);
+            float v = acc[i][j] + (biasn ? biasn[m] : 0.f);
             if (resn) v += resn[o];
+            if (a.act) { v = fmaxf(v, 0.f); if (a.act == 2) v = tanhf(v); }
             outn[o] = v;
         }
     }

@@ -749,6 +749,34 @@ struct b2a_weights {
         items = std::move(out);
     }
 
+    // ---- Qwen3TTSSpeakerEncoder.sanitize (Qwen3TTSSpeakerEncoder.swift:324-354): the keys after the "speaker_encoder" component
+    // (stripSpeakerEncoderPrefix); a 3-D ".weight" that fails checkArrayShapeQwen3 is taken for torch [out, in, k] and transposed to
+    // [out, k, in].  Every other key is dropped.
+    void sanitize_qwen3_speaker_encoder() {
+        std::vector<WItem> out;
+        for (auto& it : items) {
+            std::vector<std::string> parts;                           // key.split(separator: "."): empty pieces dropped
+            for (size_t a = 0; a <= it.name.size();) {
+                const size_t b = std::min(it.name.find('.', a), it.name.size());
+                if (b > a) parts.push_back(it.name.substr(a, b - a));
+                a = b + 1;
+            }
+            std::string rest;
+            for (size_t i = 0; i < parts.size(); ++i)
+                if (parts[i] == "speaker_encoder") {
+                    for (size_t j = i + 1; j < parts.size(); ++j) rest += (j > i + 1 ? "." : "") + parts[j];
+                    break;
+                }
+            if (rest.empty()) continue;
+            WItem t = it;
+            t.name = rest;
+            const bool weight = rest.size() >= 7 && rest.compare(rest.size() - 7, 7, ".weight") == 0;
+            if (weight && t.ndim == 3 && !check_array_shape(t)) permute3(t, 0, 2, 1);
+            out.push_back(std::move(t));
+        }
+        items = std::move(out);
+    }
+
     std::vector<b2a_tensor> table() const {
         std::vector<b2a_tensor> t(items.size());
         for (size_t i = 0; i < items.size(); ++i) {
@@ -1063,6 +1091,71 @@ int32_t b2a_speech_tokenizer_encoder_create_from_directory(const char* dir, int3
         B2A_CHECK(!w->items.empty(), B2A_ERR_MODEL_NOT_INITIALIZED, "speech tokenizer: the checkpoint has no encoder weights");
         const std::vector<b2a_tensor> tab = w->table();
         st = b2a_speech_tokenizer_encoder_create(device, &cfg, tab.data(), (int32_t)tab.size(), out);
+        if (st != B2A_OK) throw Error(st, b2a_last_error());
+    });
+}
+
+int32_t b2a_weights_sanitize_qwen3_speaker_encoder(b2a_weights* w) {
+    return guarded([&] {
+        B2A_CHECK(w, B2A_ERR_INVALID_INPUT, "b2a_weights_sanitize_qwen3_speaker_encoder: null handle");
+        w->sanitize_qwen3_speaker_encoder();
+    });
+}
+
+// config.json's "speaker_encoder_config" (Qwen3TTSSpeakerEncoderConfig, Qwen3TTSConfig.swift:92-103: the same keys and defaults; a
+// missing block is all defaults, as decodeIfPresent gives).  The three lists must have the same length, at most 8.
+static b2a_qwen3_speaker_encoder_config qwen3_speaker_config_of(const Json& root) {
+    Json empty;
+    empty.kind = Json::Obj;
+    const Json* sj = root.find("speaker_encoder_config");
+    const Json& e = (sj && sj->kind == Json::Obj) ? *sj : empty;
+    b2a_qwen3_speaker_encoder_config c{};
+    c.mel_dim = (int)e.number("mel_dim", 128); c.enc_dim = (int)e.number("enc_dim", 1024);
+    c.enc_attention_channels = (int)e.number("enc_attention_channels", 128); c.enc_res2net_scale = (int)e.number("enc_res2net_scale", 8);
+    c.enc_se_channels = (int)e.number("enc_se_channels", 128); c.sample_rate = (int)e.number("sample_rate", 24000);
+    auto list = [&](const char* key, std::initializer_list<int> dflt, int32_t* dst) {
+        std::vector<int> v(dflt);
+        if (const Json* a = e.find(key); a && a->kind == Json::Arr) { v.clear(); for (auto& x : a->arr) v.push_back((int)x.num); }
+        B2A_CHECK(v.size() <= 8, B2A_ERR_INVALID_INPUT, std::string("speaker encoder config: more than 8 entries in ") + key);
+        for (size_t i = 0; i < v.size(); ++i) dst[i] = v[i];
+        return (int)v.size();
+    };
+    const int n0 = list("enc_channels", {512, 512, 512, 512, 1536}, c.enc_channels);
+    const int n1 = list("enc_kernel_sizes", {5, 3, 3, 3, 1}, c.enc_kernel_sizes);
+    const int n2 = list("enc_dilations", {1, 2, 3, 4, 1}, c.enc_dilations);
+    B2A_CHECK(n0 == n1 && n0 == n2, B2A_ERR_INVALID_INPUT, "speaker encoder config: enc_channels, enc_kernel_sizes and enc_dilations must have the same length");
+    c.num_enc_layers = n0;
+    return c;
+}
+
+int32_t b2a_qwen3_speaker_encoder_config_from_json(const char* config_path, b2a_qwen3_speaker_encoder_config* cfg) {
+    return guarded([&] {
+        B2A_CHECK(config_path && cfg, B2A_ERR_INVALID_INPUT, "b2a_qwen3_speaker_encoder_config_from_json: null argument");
+        const Json j = read_json_file(config_path);
+        B2A_CHECK(j.kind == Json::Obj, B2A_ERR_MODEL_NOT_INITIALIZED, "config.json is not an object");
+        *cfg = qwen3_speaker_config_of(j);
+    });
+}
+
+// The speaker-encoder half of Qwen3TTSModel.fromModelDirectory (Qwen3TTS.swift:46-48, 1224-1237): only a "base" checkpoint builds
+// the encoder; config.json + every *.safetensors -> sanitize -> create.
+int32_t b2a_qwen3_speaker_encoder_create_from_directory(const char* model_dir, int32_t device, b2a_qwen3_speaker_encoder** out) {
+    return guarded([&] {
+        B2A_CHECK(model_dir && out, B2A_ERR_INVALID_INPUT, "b2a_qwen3_speaker_encoder_create_from_directory: null argument");
+        *out = nullptr;
+        const std::string dir = model_dir;
+        const Json j = read_json_file(dir + "/config.json");
+        B2A_CHECK(j.kind == Json::Obj, B2A_ERR_MODEL_NOT_INITIALIZED, "config.json is not an object");
+        const Json* mt = j.find("tts_model_type");
+        B2A_CHECK(mt && mt->kind == Json::Str && mt->str == "base", B2A_ERR_MODEL_NOT_INITIALIZED,
+                  "speaker encoder: only a Base checkpoint (tts_model_type \"base\") has one");
+        const b2a_qwen3_speaker_encoder_config cfg = qwen3_speaker_config_of(j);
+        std::unique_ptr<b2a_weights> w(new b2a_weights());
+        w->load(dir);
+        w->sanitize_qwen3_speaker_encoder();
+        B2A_CHECK(!w->items.empty(), B2A_ERR_MODEL_NOT_INITIALIZED, "speaker encoder: the checkpoint has no speaker_encoder weights");
+        const std::vector<b2a_tensor> tab = w->table();
+        const int32_t st = b2a_qwen3_speaker_encoder_create(device, &cfg, tab.data(), (int32_t)tab.size(), out);
         if (st != B2A_OK) throw Error(st, b2a_last_error());
     });
 }

@@ -3,7 +3,9 @@
 (Sources/MLXAudioTTS/Models/Qwen3TTS/{Qwen3TTSTalker,Qwen3TTSCodePredictor,Qwen3TTS}.swift).  Every number comes from the library
 (`b2a_qwen3_talker_*`); this file only composes the prompt rows the way `prepareGenerationInputs` does (Qwen3TTS.swift:883-999) and
 chains the speech-tokenizer decoder for audio; `prepare_icl_generation_inputs` composes the voice-cloning (ICL) prompt from
-reference codes (Qwen3TTS.swift:694-837).  Tokenisation stays with the host tokenizer: the entry points take token ids."""
+reference codes (Qwen3TTS.swift:694-837), and `Qwen3TTSModel.prepare_reference_conditioning` builds it from reference audio with the
+speech tokenizer's encoder and the speaker encoder (`Qwen3TTSSpeakerEncoder`, the x-vector of a Base checkpoint).  Tokenisation
+stays with the host tokenizer: the entry points take token ids."""
 from __future__ import annotations
 
 import ctypes as C
@@ -81,6 +83,176 @@ class Qwen3GenerateParameters:
 
     def _c(self) -> _ffi.Qwen3GenParams:
         return _ffi.Qwen3GenParams(self.max_tokens, self.temperature, self.top_p, self.top_k, self.min_p, self.repetition_penalty, self.seed)
+
+
+@dataclass
+class Qwen3SpeakerEncoderConfig:
+    """Qwen3TTSSpeakerEncoderConfig (Qwen3TTSConfig.swift:92-103: same keys, same defaults)."""
+    mel_dim: int = 128
+    enc_dim: int = 1024
+    enc_channels: List[int] = field(default_factory=lambda: [512, 512, 512, 512, 1536])
+    enc_kernel_sizes: List[int] = field(default_factory=lambda: [5, 3, 3, 3, 1])
+    enc_dilations: List[int] = field(default_factory=lambda: [1, 2, 3, 4, 1])
+    enc_attention_channels: int = 128
+    enc_res2net_scale: int = 8
+    enc_se_channels: int = 128
+    sample_rate: int = 24000
+
+    def to_ffi(self) -> _ffi.Qwen3SpeakerEncoderConfig:
+        n = len(self.enc_channels)
+        if len(self.enc_kernel_sizes) != n or len(self.enc_dilations) != n:
+            raise _ffi.AudioGenerationError(_ffi.ERR_INVALID_INPUT, "enc_channels, enc_kernel_sizes and enc_dilations must have the same length")
+        if n > 8:
+            raise _ffi.AudioGenerationError(_ffi.ERR_INVALID_INPUT, "at most 8 speaker-encoder layers")
+        c = _ffi.Qwen3SpeakerEncoderConfig()
+        for name in ("mel_dim", "enc_dim", "enc_attention_channels", "enc_res2net_scale", "enc_se_channels", "sample_rate"):
+            setattr(c, name, int(getattr(self, name)))
+        c.num_enc_layers = n
+        for name in ("enc_channels", "enc_kernel_sizes", "enc_dilations"):
+            for i, v in enumerate(getattr(self, name)):
+                getattr(c, name)[i] = int(v)
+        return c
+
+    @classmethod
+    def from_ffi(cls, c: _ffi.Qwen3SpeakerEncoderConfig) -> "Qwen3SpeakerEncoderConfig":
+        n = c.num_enc_layers
+        return cls(mel_dim=c.mel_dim, enc_dim=c.enc_dim, enc_channels=list(c.enc_channels)[:n], enc_kernel_sizes=list(c.enc_kernel_sizes)[:n],
+                   enc_dilations=list(c.enc_dilations)[:n], enc_attention_channels=c.enc_attention_channels,
+                   enc_res2net_scale=c.enc_res2net_scale, enc_se_channels=c.enc_se_channels, sample_rate=c.sample_rate)
+
+
+def random_init_speaker_encoder_weights(cfg: Qwen3SpeakerEncoderConfig, seed: int = 2468) -> Dict[str, np.ndarray]:
+    """Random-init speaker-encoder weights with the reference's module keys (blocks.*, mfa.*, asp.*, fc.*; a checkpoint prefixes
+    them with "speaker_encoder.") in torch layout [out, in, k]: weights N(0, 1 / fan_in), biases N(0, 0.05^2)."""
+    rng = np.random.default_rng(seed)
+    W: Dict[str, np.ndarray] = {}
+
+    def conv(prefix, cout, cin, k):
+        W[prefix + ".weight"] = (rng.standard_normal((cout, cin, k)) / np.sqrt(cin * k)).astype(np.float32)
+        W[prefix + ".bias"] = (rng.standard_normal(cout) * 0.05).astype(np.float32)
+
+    ch, ks, ds = cfg.enc_channels, cfg.enc_kernel_sizes, cfg.enc_dilations
+    conv("blocks.0.conv", ch[0], cfg.mel_dim, ks[0])
+    for i in range(1, len(ch) - 1):
+        p, w = f"blocks.{i}.", ch[i] // cfg.enc_res2net_scale
+        conv(p + "tdnn1.conv", ch[i], ch[i - 1], 1)
+        for j in range(cfg.enc_res2net_scale - 1):
+            conv(p + f"res2net_block.blocks.{j}.conv", w, w, ks[i])
+        conv(p + "tdnn2.conv", ch[i], ch[i], 1)
+        conv(p + "se_block.conv1", cfg.enc_se_channels, ch[i], 1)
+        conv(p + "se_block.conv2", ch[i], cfg.enc_se_channels, 1)
+    conv("mfa.conv", ch[-1], ch[-1], ks[-1])
+    conv("asp.tdnn.conv", cfg.enc_attention_channels, 3 * ch[-1], 1)
+    conv("asp.conv", ch[-1], cfg.enc_attention_channels, 1)
+    conv("fc", cfg.enc_dim, 2 * ch[-1], 1)
+    return W
+
+
+def check_array_shape(shape) -> bool:
+    """checkArrayShapeQwen3 (Qwen3TTSSpeechTokenizer.swift:1445-1455): True when a 3-D conv weight already looks like MLX [out, k, in]."""
+    if len(shape) != 3:
+        return False
+    _, d2, d3 = shape
+    if d2 == 1:
+        return d3 > 64
+    if d3 == 1:
+        return d2 <= 64
+    return d2 < d3
+
+
+class Qwen3TTSSpeakerEncoder:
+    """Qwen3TTSSpeakerEncoder (Qwen3TTSSpeakerEncoder.swift) on the device: audio at sample_rate -> the x-vector [enc_dim].
+    ``weights``: the module's keys (blocks.*, mfa.*, asp.*, fc.*; anything up to a "speaker_encoder." component is stripped) in
+    torch or MLX layout -- 3-D weights go through the reference's layout rule (check_array_shape), as sanitize does."""
+
+    def __init__(self, config: Optional[Qwen3SpeakerEncoderConfig] = None, weights: Optional[Dict] = None, device: int = 0):
+        self.config = config or Qwen3SpeakerEncoderConfig()
+        c = self.config.to_ffi()
+        w = {}
+        for k, v in (weights or {}).items():
+            parts = [p for p in k.split(".") if p]
+            if "speaker_encoder" in parts:
+                parts = parts[parts.index("speaker_encoder") + 1:]
+            v = np.asarray(v, dtype=np.float32)
+            if k.endswith(".weight") and v.ndim == 3 and not check_array_shape(v.shape):
+                v = v.transpose(0, 2, 1)
+            if parts:
+                w[".".join(parts)] = np.ascontiguousarray(v)
+        self._h = C.c_void_p()
+        if not w:
+            raise _ffi.AudioGenerationError(_ffi.ERR_MODEL_NOT_INITIALIZED, "speaker encoder: no weights")
+        table, keep = _ffi.make_tensor_table(w)
+        _ffi.check(_ffi.lib().b2a_qwen3_speaker_encoder_create(device, C.byref(c), table, len(w), C.byref(self._h)))
+        del keep
+
+    @classmethod
+    def from_model_directory(cls, model_dir, device: int = 0) -> "Qwen3TTSSpeakerEncoder":
+        """The speaker-encoder half of Qwen3TTSModel.fromModelDirectory (Qwen3TTS.swift:46-48, 1224-1237): config.json's
+        speaker_encoder_config + every *.safetensors -> sanitize -> weights on the device.  Only a Base checkpoint has one."""
+        self = cls.__new__(cls)
+        self._h = C.c_void_p()
+        c = _ffi.Qwen3SpeakerEncoderConfig()
+        _ffi.check(_ffi.lib().b2a_qwen3_speaker_encoder_config_from_json(str(model_dir).encode() + b"/config.json", C.byref(c)))
+        self.config = Qwen3SpeakerEncoderConfig.from_ffi(c)
+        _ffi.check(_ffi.lib().b2a_qwen3_speaker_encoder_create_from_directory(str(model_dir).encode(), device, C.byref(self._h)))
+        return self
+
+    @property
+    def stream(self) -> int:
+        return int(_ffi.lib().b2a_qwen3_speaker_encoder_stream(self._h) or 0)
+
+    def frames(self, n_samples: int) -> int:
+        return int(_ffi.lib().b2a_qwen3_speaker_encoder_frames(self._h, int(n_samples)))
+
+    def embed(self, audio) -> np.ndarray:
+        """audio [B, n] (or [n]) -> x-vectors [B, enc_dim]: the 1024-point log-mel and the network, both on the device."""
+        a = np.ascontiguousarray(audio, dtype=np.float32)
+        a = a[None] if a.ndim == 1 else a
+        if a.ndim != 2:
+            raise _ffi.AudioGenerationError(_ffi.ERR_INVALID_INPUT, "audio must be [batch, samples]")
+        out = np.empty((a.shape[0], self.config.enc_dim), dtype=np.float32)
+        _ffi.check(_ffi.lib().b2a_qwen3_speaker_encoder_embed(self._h, _ffi.ptr(a), a.shape[0], a.shape[1], _ffi.ptr(out)))
+        return out
+
+    def embed_dev(self, audio, out, stream: int = 0) -> None:
+        """Device tensors (torch, contiguous float32): audio [B, n] -> out [B, enc_dim], enqueued on `stream` (0: the handle's)
+        without a host synchronisation."""
+        import torch
+        if not (isinstance(audio, torch.Tensor) and isinstance(out, torch.Tensor) and audio.is_cuda and out.is_cuda and audio.dim() == 2
+                and audio.dtype == torch.float32 and out.dtype == torch.float32 and audio.is_contiguous() and out.is_contiguous()
+                and tuple(out.shape) == (audio.shape[0], self.config.enc_dim)):
+            raise _ffi.AudioGenerationError(_ffi.ERR_INVALID_INPUT, "embed_dev: audio must be float32 [B, n] and out float32 [B, enc_dim] on the device")
+        _ffi.check(_ffi.lib().b2a_qwen3_speaker_encoder_embed_dev(self._h, _ffi.ptr(audio), int(audio.shape[0]), int(audio.shape[1]),
+                                                                  _ffi.ptr(out), C.c_void_p(stream or None)))
+
+    def embed_mel(self, mels) -> np.ndarray:
+        """The module's own input (callAsFunction, :299-322): log-mel [B, T, mel_dim] -> [B, enc_dim]."""
+        m = np.ascontiguousarray(mels, dtype=np.float32)
+        m = m[None] if m.ndim == 2 else m
+        if m.ndim != 3 or m.shape[2] != self.config.mel_dim:
+            raise _ffi.AudioGenerationError(_ffi.ERR_INVALID_INPUT, "mels must be [batch, frames, mel_dim]")
+        out = np.empty((m.shape[0], self.config.enc_dim), dtype=np.float32)
+        _ffi.check(_ffi.lib().b2a_qwen3_speaker_encoder_embed_mel(self._h, _ffi.ptr(m), m.shape[0], m.shape[1], _ffi.ptr(out)))
+        return out
+
+    def __call__(self, ref_audio) -> np.ndarray:
+        """extractSpeakerEmbedding (Qwen3TTS.swift:839-881): [n], [1, n], [B, n] (row 0) or [B, 1, n] (row 0) -> [enc_dim]."""
+        a = np.asarray(ref_audio, dtype=np.float32)
+        if a.ndim == 3 and a.shape[1] == 1:
+            a = a[:, 0]
+        if a.ndim == 1:
+            a = a[None]
+        elif a.ndim != 2:
+            raise _ffi.AudioGenerationError(_ffi.ERR_INVALID_INPUT, "reference audio must be [n], [B, n] or [B, 1, n]")
+        return self.embed(a[:1])[0]
+
+    def __del__(self):
+        try:
+            if getattr(self, "_h", None) and self._h.value:
+                _ffi.lib().b2a_qwen3_speaker_encoder_destroy(self._h)
+                self._h = C.c_void_p()
+        except Exception:   # interpreter shutdown
+            pass
 
 
 FRAME_CB = C.CFUNCTYPE(None, C.c_void_p, C.c_int32, C.c_int32, C.POINTER(C.c_int32))
@@ -167,12 +339,14 @@ class Qwen3TTSTalker:
         """prepareReferenceConditioning's id slicing + prepareICLGenerationInputs (Qwen3TTS.swift:709-837) from token ids, the
         voice-cloning prompt.  ref_codes [groups, T] or [1, groups, T] (the speech tokenizer's encode of the reference clip);
         ref_chat_ids = tokens of "<|im_start|>assistant\n{ref_text}<|im_end|>\n"; target_chat_ids = tokens of
-        "<|im_start|>assistant\n{text}<|im_end|>\n<|im_start|>assistant\n"; speaker_embedding [hidden] (the caller's x-vector; the
-        speaker encoder is not built here).  Returns (input_embeds [L, H], trailing_text_hidden [1, H] = tts_pad, tts_pad_embed [H])."""
+        "<|im_start|>assistant\n{text}<|im_end|>\n<|im_start|>assistant\n"; speaker_embedding [hidden] (the x-vector;
+        Qwen3TTSModel.prepare_reference_conditioning computes it from the reference audio).  Returns (input_embeds [L, H],
+        trailing_text_hidden [1, H] = tts_pad, tts_pad_embed [H])."""
         c = self.config
         if speaker_embedding is None and c.tts_model_type == "base":
-            raise _ffi.AudioGenerationError(_ffi.ERR_INVALID_INPUT, "a Base checkpoint clones from a speaker embedding (x-vector), and the "
-                                            "speaker encoder (Qwen3TTSSpeakerEncoder) is not built: pass speaker_embedding")
+            raise _ffi.AudioGenerationError(_ffi.ERR_INVALID_INPUT, "a Base checkpoint clones from a speaker embedding (x-vector): pass "
+                                            "speaker_embedding, or build the prompt from audio with Qwen3TTSModel.prepare_reference_conditioning "
+                                            "and a Qwen3TTSSpeakerEncoder")
         rc = np.asarray(ref_codes)
         rc = rc[0] if rc.ndim == 3 else rc
         if rc.ndim != 2 or rc.shape[1] < 1:
@@ -285,11 +459,29 @@ class Qwen3TTSTalker:
 
 class Qwen3TTSModel:
     """SpeechGenerationModel face of Qwen3-TTS (Qwen3TTS.swift:306-569): talker + code predictor -> codes -> speech-tokenizer
-    decoder.  `speech_tokenizer` is a qwen3_tts_codec.Qwen3TTSSpeechTokenizer (the decode side; borrowed)."""
+    decoder.  `speech_tokenizer` is a qwen3_tts_codec.Qwen3TTSSpeechTokenizer (borrowed; its encoder, when present, turns reference
+    audio into codes); `speaker_encoder` a Qwen3TTSSpeakerEncoder (borrowed; a Base checkpoint's x-vector)."""
     sample_rate = 24000
 
-    def __init__(self, talker: Qwen3TTSTalker, speech_tokenizer=None):
-        self.talker, self.speech_tokenizer = talker, speech_tokenizer
+    def __init__(self, talker: Qwen3TTSTalker, speech_tokenizer=None, speaker_encoder: Optional[Qwen3TTSSpeakerEncoder] = None):
+        self.talker, self.speech_tokenizer, self.speaker_encoder = talker, speech_tokenizer, speaker_encoder
+
+    def prepare_reference_conditioning(self, ref_audio, ref_chat_ids: Sequence[int], target_chat_ids: Sequence[int], tts_bos: int,
+                                       tts_eos: int, tts_pad: int, language_id: Optional[int] = None):
+        """The voice-cloning prompt from reference audio: referenceAudioContext + prepareReferenceConditioning +
+        prepareICLGenerationInputs (Qwen3TTS.swift:267-300, 709-837).  ref_audio [n], [B, n] or [B, 1, n] at 24 kHz is encoded to
+        codes by the speech tokenizer's encoder and, with a speaker encoder, to the x-vector (extractSpeakerEmbedding: row 0).
+        The token ids are prepare_icl_generation_inputs'.  Returns (input_embeds, trailing_text_hidden, tts_pad_embed, ref_codes),
+        ready for generate(..., ref_codes=ref_codes)."""
+        if self.speech_tokenizer is None or not self.speech_tokenizer.has_encoder:
+            raise _ffi.AudioGenerationError(_ffi.ERR_INVALID_INPUT, "Qwen3TTS reference conditioning requires a speech tokenizer encoder")
+        a = np.asarray(ref_audio, dtype=np.float32)
+        codes = self.speech_tokenizer.encode(a)                               # referenceAudioForEncoder's shapes (:239-247)
+        xvec = self.speaker_encoder(a) if self.speaker_encoder is not None else None
+        ref_codes = codes[0]
+        inputs, trailing, pad = self.talker.prepare_icl_generation_inputs(ref_codes, ref_chat_ids, target_chat_ids, tts_bos, tts_eos, tts_pad,
+                                                                          language_id=language_id, speaker_embedding=xvec)
+        return inputs, trailing, pad, ref_codes
 
     def generate(self, input_embeds, trailing_text_hidden, tts_pad_embed, parameters: Optional[Qwen3GenerateParameters] = None,
                  ref_codes=None) -> np.ndarray:
