@@ -32,13 +32,6 @@ struct Args {
     int T, Tp, nh, d_model, half;
 };
 
-__device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2) {
-    asm volatile(
-        "cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-        ::"r"(tc::smem_u32(dst)), "l"(map), "r"(tc::smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
-        : "memory");
-}
-
 __global__ void __launch_bounds__(FA_THREADS, 1)
 mha_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV, Args a) {
     extern __shared__ __align__(1024) uint8_t fa_raw[];
@@ -62,17 +55,17 @@ mha_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ C
     if (warp == 8) {
         if (lane == 0) {
             tc::mbar_arrive_expect_tx(qfull, Q_BYTES);
-            tma_load_3d(sQ, &tmQ, qfull, 0, qt * BQ, bh);
+            tc::tma_load_3d(sQ, &tmQ, qfull, 0, qt * BQ, bh);
             for (int i = 0; i < n_it; ++i) {
                 const int j = i % n_kv, pass = i / n_kv, st = i % FA_STAGES;
                 const uint32_t ph = (uint32_t)((i / FA_STAGES) & 1);
                 tc::mbar_wait(&empty[st], ph ^ 1);
                 uint8_t* sk = sKV + (size_t)st * STAGE_BYTES;
                 tc::mbar_arrive_expect_tx(&full[st], pass ? STAGE_BYTES : K_BYTES);
-                tma_load_3d(sk, &tmK, &full[st], 0, j * BKV, bh);
+                tc::tma_load_3d(sk, &tmK, &full[st], 0, j * BKV, bh);
                 if (pass) {
-                    tma_load_3d(sk + K_BYTES, &tmV, &full[st], j * BKV, 0, bh);                 // keys [0, 64) of the tile: [64 d][64 keys]
-                    tma_load_3d(sk + K_BYTES + V_BYTES / 2, &tmV, &full[st], j * BKV + 64, 0, bh);
+                    tc::tma_load_3d(sk + K_BYTES, &tmV, &full[st], j * BKV, 0, bh);                 // keys [0, 64) of the tile: [64 d][64 keys]
+                    tc::tma_load_3d(sk + K_BYTES + V_BYTES / 2, &tmV, &full[st], j * BKV + 64, 0, bh);
                 }
             }
         }

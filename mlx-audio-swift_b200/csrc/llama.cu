@@ -15,6 +15,7 @@
 #include "common.cuh"
 #include <cooperative_groups.h>
 #include "tc_gemm.cuh"
+#include "prompt_attn_tc.cuh"
 #include "qwen3_sampler.cuh"
 
 #include <algorithm>
@@ -477,7 +478,8 @@ attn_decode_cluster_kernel(const __grid_constant__ AttnArgs a) {
 // ------------------------------------------------------------------------------------------------
 // Batched prefill (LlamaTTS.swift:711 `self(inputIds, cache)` on the whole prompt): all B*L prompt tokens go
 // through each layer at once -- GEMMs on the wgmma kernel with 128-column tiles (64 tokens as hi/lo pairs),
-// causal attention over the prompt per (row, kv head, 32-query tile), K/V written to the fp32 cache.
+// causal attention over the prompt, K/V written to the fp32 cache.  Prompts whose K/V rows fit in shared memory take the SIMT
+// prefill_attn_kernel (per (row, kv head, 32-query tile)), longer ones pack + pfa::prompt_attn_kernel (prompt_attn_tc.cuh).
 // ------------------------------------------------------------------------------------------------
 constexpr int PF_HALF = 64;      // tokens per 128-row TMA tile
 constexpr int PA_QT = 32, PA_THREADS = 256, PA_MAXL = 128;
@@ -604,6 +606,32 @@ prefill_attn_kernel(PrefillAttnArgs a) {
         tc::store_hilo(a.out, ldo, tok, col + 3, o.w * inv, PF_HALF);
     }
 }
+
+// pfa::prompt_attn_kernel's operands for B rows of L positions (padded to Lp = a multiple of pfa::BQ) and their tensor maps;
+// grown, never shrunk.  run(): pack_prompt_kernel then prompt_attn_kernel, the attention of one layer.
+struct PromptAttnOps {
+    DBuf<__half> q, k, vt;
+    CUtensorMap tq{}, tk{}, tv{};
+    int B = 0, Lp = 0, nq = 0, nkv = 0;
+    void prepare(int B_, int L, int nq_, int nkv_) {
+        const int Lp_ = cdiv(L, pfa::BQ) * pfa::BQ;
+        if (B_ == B && Lp_ == Lp && nq_ == nq && nkv_ == nkv) return;
+        B = B_; Lp = Lp_; nq = nq_; nkv = nkv_;
+        q.alloc((size_t)B * nq * Lp * pfa::OPW); k.alloc((size_t)B * nkv * Lp * pfa::OPW); vt.alloc((size_t)B * nkv * Lp * pfa::OPW);
+        tq = tc::make_tmap_f16_3d(q.p, pfa::OPW, Lp, (long long)B * nq, 64, pfa::BQ);
+        tk = tc::make_tmap_f16_3d(k.p, pfa::OPW, Lp, (long long)B * nkv, 64, pfa::BKV);
+        tv = tc::make_tmap_f16_3d(vt.p, Lp, pfa::OPW, (long long)B * nkv, 64, pfa::HDIM);
+        B2A_CUDA(cudaFuncSetAttribute(pfa::prompt_attn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pfa::SMEM_BYTES));
+    }
+    // qkv [B * L, (nq + 2 nkv) * 128] fp32; rope [>= L][64]; caches [B][nkv][max_ctx][128]; out: 64-token hi/lo tiles [.., nq * 128]
+    void run(const float* qkv, const float2* rope, float* kcache, float* vcache, bf16* out, int L, int max_ctx, cudaStream_t s) {
+        pfa::pack_prompt_kernel<<<dim3(Lp / 64, B, nq + nkv), 256, 0, s>>>(qkv, rope, q.p, k.p, vt.p, kcache, vcache, L, Lp, nq, nkv,
+                                                                         max_ctx);
+        const pfa::Args a{out, L, Lp, nq, nkv, 1.0f / sqrtf((float)HD)};
+        pfa::prompt_attn_kernel<<<dim3(Lp / pfa::BQ, nq, B), pfa::THREADS, pfa::SMEM_BYTES, s>>>(tq, tk, tv, a);
+        count_launch(2);
+    }
+};
 
 // decode buffers <- last prompt position of every row:  x[b] = xp[b*L + L-1], y[b] = yp[...], pos[b] = L - 1
 __global__ void gather_last_kernel(const float* __restrict__ xp, const float* __restrict__ yp, float* __restrict__ x,
@@ -932,6 +960,7 @@ struct b2a_tts {
     DBuf<float> xp, yp, qkvp;
     DBuf<bf16> xnp, attnp, actp;
     DBuf<float2> rope_tab;
+    PromptAttnOps pfa_ops;
     CUtensorMap tmp_xn{}, tmp_attn{}, tmp_act{};
     int pf_tokens_cap = 0;
     bool use_batched_prefill = true;
@@ -1416,8 +1445,11 @@ struct b2a_tts {
         const int G = cfg.num_attention_heads / cfg.num_key_value_heads;
         return ((size_t)2 * L * HD + (size_t)G * PA_QT * HD) * sizeof(float);
     }
+    // the prompt attention for L positions: the SIMT kernel while its K/V rows fit in shared memory (the outputs of short prompts stay
+    // what they were), the wgmma kernel beyond
+    bool simt_prompt_attn(int L) const { return L <= PA_MAXL && pattn_smem(L) <= 220 * 1024; }
     bool can_batch_prefill(int L) const {
-        return use_tc && use_batched_prefill && spec.has_embed && !spec.qk_norm && L >= 2 && L <= PA_MAXL && pattn_smem(L) <= 220 * 1024;
+        return use_tc && use_batched_prefill && spec.has_embed && !spec.qk_norm && L >= 2 && L <= cfg.max_context;
     }
 
     // D[T, M] = X[T, K] W^T for all prompt tokens: 128-column tiles (64 tokens as hi/lo), CTAs own whole tiles
@@ -1449,11 +1481,18 @@ struct b2a_tts {
             tmp_act = tc::make_tmap_bf16(actp.p, 2 * Tp, I, 128);
             pattn_attr<1>(); pattn_attr<2>(); pattn_attr<3>(); pattn_attr<4>(); pattn_attr<6>(); pattn_attr<8>();
         }
-        rope_tab.alloc((size_t)PA_MAXL * (HD / 2));
-        // padding tokens of the last tile must read as zero
-        B2A_CUDA(cudaMemsetAsync(xnp.p, 0, (size_t)2 * pf_tokens_cap * H * sizeof(bf16), s));
-        B2A_CUDA(cudaMemsetAsync(attnp.p, 0, (size_t)2 * pf_tokens_cap * NQ * sizeof(bf16), s));
-        B2A_CUDA(cudaMemsetAsync(actp.p, 0, (size_t)2 * pf_tokens_cap * I * sizeof(bf16), s));
+        rope_tab.alloc((size_t)cfg.max_context * (HD / 2));
+        const bool simt_attn = simt_prompt_attn(L);
+        if (!simt_attn) pfa_ops.prepare(B, L, nq, nkv);
+        // padding tokens of the last tile must read as zero (no kernel writes them): its hi rows T % 64 .. 63 and the lo rows below
+        if (const int r0 = T % PF_HALF) {
+            const size_t row0 = (size_t)(n_tiles - 1) * 2 * PF_HALF + r0;
+            auto zero = [&](bf16* p, int cols) {
+                B2A_CUDA(cudaMemset2DAsync(p + row0 * cols, (size_t)PF_HALF * cols * sizeof(bf16), 0,
+                                           (size_t)(PF_HALF - r0) * cols * sizeof(bf16), 2, s));
+            };
+            zero(xnp.p, H); zero(attnp.p, NQ); zero(actp.p, I);
+        }
         embed_rows_kernel<<<T, 256, 0, s>>>(ids.p, embed.p, xp.p, H, cfg.vocab_size);
         rope_table_kernel<<<cdiv(L * (HD / 2), 256), 256, 0, s>>>(freqs.p, rope_tab.p, L);
         count_launch(2);
@@ -1463,19 +1502,23 @@ struct b2a_tts {
             launch_pdl(add_rmsnorm_kernel, dim3(T), dim3(RN_THREADS), 0, s, xp.p, l == 0 ? (float*)nullptr : yp.p, Lw.ln1.p, xnp.p, H,
                        cfg.rms_norm_eps, (float*)nullptr, PF_HALF, (float*)nullptr, (float*)nullptr, 0);
             pf_gemm(tm_qkv[l], tmp_xn, tc::EPI_STORE, qkvp.p, nullptr, T, QKV_N, H, s);
-            PrefillAttnArgs pa{qkvp.p, rope_tab.p, kcache.p + l * kv_layer, vcache.p + l * kv_layer, attnp.p, nq, nkv,
-                               cfg.max_context, L, 1.0f / sqrtf((float)HD)};
-            const dim3 grid(nkv, B, cdiv(L, PA_QT));
-            const size_t sm = pattn_smem(L);
-            switch (G) {
-                case 1: prefill_attn_kernel<1><<<grid, PA_THREADS, sm, s>>>(pa); break;
-                case 2: prefill_attn_kernel<2><<<grid, PA_THREADS, sm, s>>>(pa); break;
-                case 3: prefill_attn_kernel<3><<<grid, PA_THREADS, sm, s>>>(pa); break;
-                case 4: prefill_attn_kernel<4><<<grid, PA_THREADS, sm, s>>>(pa); break;
-                case 6: prefill_attn_kernel<6><<<grid, PA_THREADS, sm, s>>>(pa); break;
-                default: prefill_attn_kernel<8><<<grid, PA_THREADS, sm, s>>>(pa); break;
+            if (simt_attn) {
+                PrefillAttnArgs pa{qkvp.p, rope_tab.p, kcache.p + l * kv_layer, vcache.p + l * kv_layer, attnp.p, nq, nkv,
+                                   cfg.max_context, L, 1.0f / sqrtf((float)HD)};
+                const dim3 grid(nkv, B, cdiv(L, PA_QT));
+                const size_t sm = pattn_smem(L);
+                switch (G) {
+                    case 1: prefill_attn_kernel<1><<<grid, PA_THREADS, sm, s>>>(pa); break;
+                    case 2: prefill_attn_kernel<2><<<grid, PA_THREADS, sm, s>>>(pa); break;
+                    case 3: prefill_attn_kernel<3><<<grid, PA_THREADS, sm, s>>>(pa); break;
+                    case 4: prefill_attn_kernel<4><<<grid, PA_THREADS, sm, s>>>(pa); break;
+                    case 6: prefill_attn_kernel<6><<<grid, PA_THREADS, sm, s>>>(pa); break;
+                    default: prefill_attn_kernel<8><<<grid, PA_THREADS, sm, s>>>(pa); break;
+                }
+                count_launch();
+            } else {
+                pfa_ops.run(qkvp.p, rope_tab.p, kcache.p + l * kv_layer, vcache.p + l * kv_layer, attnp.p, L, cfg.max_context, s);
             }
-            count_launch();
             pf_gemm(tm_o[l], tmp_attn, tc::EPI_STORE, yp.p, nullptr, T, H, NQ, s);
             launch_pdl(add_rmsnorm_kernel, dim3(T), dim3(RN_THREADS), 0, s, xp.p, yp.p, Lw.ln2.p, xnp.p, H, cfg.rms_norm_eps,
                        (float*)nullptr, PF_HALF, (float*)nullptr, (float*)nullptr, 0);
@@ -1607,7 +1650,7 @@ static void tts_generate_impl(b2a_tts* h, const int32_t* input_ids, bool ids_on_
                                       h->recent_n.p, h->n_gen.p, h->done.p, h->n_active.p, 0);
     count_launch();
     // prefill.  Batched: every prompt token through each layer at once (wgmma GEMMs, 64 tokens per tile), then
-    // lm head + sampler on the last position.  Fallback (B2A_PREFILL=step, L > 128, SIMT mode): replay the decode
+    // lm head + sampler on the last position.  Fallback (B2A_PREFILL=step, SIMT mode, q/k norm): replay the decode
     // step per position -- positions 0..L-2 need no logits, position L-1 runs the full step.
     int steps = 0;
     if (h->can_batch_prefill(L)) {
@@ -1964,6 +2007,27 @@ int32_t b2a_debug_qkv_split(int32_t m_tiles, int32_t k_blocks, int32_t* out) {
         out[2] = out[0] ? tc::splitk_active_clusters(out[0], (size_t)out[1]) : 0;
         out[3] = sk_ctas;
         out[4] = tc::stream_k_slots(m_tiles, k_blocks, sk_ctas);
+    });
+}
+
+// The long-prompt attention on its own (include/b200audio_internal.h): rope_table_kernel + pack_prompt_kernel + prompt_attn_kernel,
+// as prefill_batched runs them for one layer, on DEVICE buffers the caller owns.
+int32_t b2a_prompt_attn_test(const float* qkv, const float* freqs, float* kcache, float* vcache, void* out, int32_t B, int32_t L,
+                             int32_t nq, int32_t nkv, int32_t max_ctx, void* stream) {
+    return guarded([&] {
+        B2A_CHECK(qkv && freqs && kcache && vcache && out && B >= 1 && L >= 1 && L <= max_ctx && nkv >= 1 && nq >= nkv && nq % nkv == 0,
+                  B2A_ERR_INVALID_INPUT, "b2a_prompt_attn_test: bad argument");
+        require_device(0);
+        const cudaStream_t s = (cudaStream_t)stream;
+        DBuf<float2> rope;
+        rope.alloc((size_t)L * (HD / 2));
+        rope_table_kernel<<<cdiv(L * (HD / 2), 256), 256, 0, s>>>(freqs, rope.p, L);
+        count_launch();
+        PromptAttnOps ops;
+        ops.prepare(B, L, nq, nkv);
+        ops.run(qkv, rope.p, kcache, vcache, (bf16*)out, L, max_ctx, s);
+        B2A_CUDA(cudaGetLastError());
+        B2A_CUDA(cudaStreamSynchronize(s));
     });
 }
 

@@ -6,7 +6,7 @@ generated and TTFB is the latency of the first .audio event, as the CLI measures
 
 With --ref-seconds S every row carries a voice-cloning reference block (prepareInputIds with refAudio / refText, LlamaTTS.swift:446-553):
 a synthetic S-second clip encoded by SNAC on the device and a 16-token stand-in transcript.  The encode runs before the timed call;
-prompts longer than 128 tokens take the token-by-token prefill.
+prompts of any length take the batched prefill (longer than 128 tokens with the wgmma prompt attention, csrc/prompt_attn_tc.cuh).
 
     python tools/tts_benchmark.py [--batch 1] [--prompt 64] [--max-tokens 512] [--model-dir DIR] [--stream] [--interval 0.32]
                                   [--ref-seconds S]"""
