@@ -63,7 +63,7 @@ int32_t b2a_speech_tokenizer_encoder_latent_test(b2a_speech_tokenizer_encoder* h
 int32_t b2a_qwen3_sample_test(const float* logits, int32_t batch, int32_t vocab, float temperature, float top_p, int32_t top_k,
                               float min_p, float repetition_penalty, int32_t eos, int32_t suppress_lo, int32_t suppress_hi,
                               uint32_t* seen, int32_t track, uint64_t seed, int32_t step, int32_t* tokens_out, float* filtered_out);
-/* tests/test_gpu_implicit_conv.py: one launch of the implicit-GEMM causal convolution kernel (csrc/implicit_conv.cuh) on HOST
+/* tests/test_gpu_implicit_conv.py: one launch of the implicit-GEMM causal convolution kernel (csrc/conv_gemm.cu) on HOST
  * data: w [M][taps][Cin], x [B][Ttot][Cin]; out[b, t*up + rho, co] for m = rho * (M/up) + co is
  * sum_j sum_c w[m, j, c] * x[b, t + shift0 + j*dil, c] through the fused epilogue (bias, bias twice at t = 0, GELU, gamma, add,
  * SnakeBeta on the hi/lo copy).  xo [B][T*up][M/up] in/out or null; hl_out [B][Hout + T*up][M/up] or null.  fp16 != 0: operands

@@ -807,16 +807,16 @@ struct b2a_snac {
             fused_attrs<64>(); fused_attrs<128>();
             B2A_CUDA(cudaFuncSetAttribute(rf::convt_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rf::convt_smem_bytes()));
             B2A_CUDA(cudaFuncSetAttribute(final_nlc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (FN_TT + 6) * FN_MAXC * (int)sizeof(float)));
-            pw0_tc.build(host_pw0, C, latent);
+            pw0_tc.build(host_pw0, C, 1, latent);
             size_t ip = 0;
             for (size_t i = 0; i < blocks.size(); ++i) {
                 DecBlock& B = blocks[i];
-                B.ct_tc.build(host_ct[i], B.cout * B.stride, 2 * B.cin);
-                B.noise_tc.build(host_noise[i], B.cout, B.cout);
-                if (B.cout == 64) B.noise_bd.build(block_diag2(host_noise[i]), 128, 128);
+                B.ct_tc.build(host_ct[i], B.cout * B.stride, 1, 2 * B.cin);
+                B.noise_tc.build(host_noise[i], B.cout, 1, B.cout);
+                if (B.cout == 64) B.noise_bd.build(block_diag2(host_noise[i]), 128, 1, 128);
                 for (int u = 0; u < 3; ++u) {
-                    if (B.cout == 64) B.ru[u].pw_bd.build(block_diag2(host_pw[ip]), 128, 128);
-                    B.ru[u].pw_tc.build(host_pw[ip++], B.cout, B.cout);
+                    if (B.cout == 64) B.ru[u].pw_bd.build(block_diag2(host_pw[ip]), 128, 1, 128);
+                    B.ru[u].pw_tc.build(host_pw[ip++], B.cout, 1, B.cout);
                 }
             }
         }
@@ -866,8 +866,8 @@ struct b2a_snac {
                 std::vector<float> bd = pad2(tt.f32(r + "1.bias", c), 1, c, 1, E.cp);
                 R.dw.bias.upload(bd.data(), bd.size()); R.dw.has_bias = true;
                 std::vector<float> wp = pad2(fold_wn(tt, r + "3", c, 1, c, true), c, c, E.cp, E.cp);
-                R.pw_tc.build(wp, E.cp, E.cp);
-                if (E.cp == 64) R.pw_bd.build(block_diag2(wp), 128, 128);
+                R.pw_tc.build(wp, E.cp, 1, E.cp);
+                if (E.cp == 64) R.pw_bd.build(block_diag2(wp), 128, 1, 128);
                 std::vector<float> bp = pad2(tt.f32(r + "3.bias", c), 1, c, 1, E.cp);
                 R.pw.bias.upload(bp.data(), bp.size()); R.pw.has_bias = true;
             }
@@ -879,7 +879,7 @@ struct b2a_snac {
             for (int co = 0; co < E.cout; ++co)
                 for (int j = 0; j < k; ++j)
                     for (int ci = 0; ci < c; ++ci) A[(size_t)co * k * E.cp + (size_t)j * E.cp + ci] = wt[((size_t)co * k + j) * c + ci];
-            E.down.build(A, E.cp_out, k * E.cp);
+            E.down.build(A, E.cp_out, 1, k * E.cp);
             std::vector<float> bb = pad2(tt.f32(b + "4.bias", E.cout), 1, E.cout, 1, E.cp_out);
             E.down_b.bias.upload(bb.data(), bb.size()); E.down_b.has_bias = true;
         }
@@ -1447,7 +1447,7 @@ extern "C" int32_t b2a_conv_gemm_test(const float* w, int32_t M, int32_t K, cons
                   B2A_ERR_INVALID_INPUT, "b2a_conv_gemm_test: cg::E_CONVT needs M = stride * Cout, N = B * (Tin + 1) and T = Tin * stride");
         require_device(0);
         TcW W;
-        W.build(std::vector<float>(w, w + (size_t)M * K), M, K);
+        W.build(std::vector<float>(w, w + (size_t)M * K), M, 1, K);
         cg::Args a{};
         a.N = N; a.epi = epi; a.bias = bias; a.alpha = alpha; a.gamma = gamma; a.gelu = gelu; a.x = x; a.ldx = ldx;
         a.hl = (__nv_bfloat16*)hl; a.ldh = ldh; a.dual = dual; a.T = T; a.Cout = Cout; a.stride = stride; a.pad = pad; a.Tin = Tin;
@@ -1478,7 +1478,7 @@ extern "C" int32_t b2a_snac_unit_test(int32_t mode, int32_t C, int32_t dil, cons
         b2a_snac::fused_attrs<128>();
         std::vector<float> pw(pw_w, pw_w + (size_t)C * C);
         TcW W;                                              // the [128, 128] operand: W itself (C = 128) or [W 0; 0 W] (C = 64)
-        W.build(C == 64 ? block_diag2(pw) : pw, 128, 128);
+        W.build(C == 64 ? block_diag2(pw) : pw, 128, 1, 128);
         rf::Args a{};
         a.x = x; a.y = y; a.C = C; a.mode = mode; a.dil = dil; a.dw_w = dw_w; a.dw_b = dw_b; a.a_in = a_in; a.a_mid = a_mid;
         a.pw_bias = pw_bias; a.noise = noise; a.seed = seed; a.hl = (__nv_bfloat16*)hl; a.a_next = a_next;
@@ -1505,7 +1505,7 @@ extern "C" int32_t b2a_snac_convt_test(const float* x, float* y, const float* al
             for (int co = 0; co < cout; ++co)
                 for (int j = 0; j < k; ++j) wt[((size_t)ci * k + j) * cout + co] = w[((size_t)ci * cout + co) * k + j];
         TcW W;
-        W.build(convt_phase_major(convt_gemm_rows(wt, CIN, cout, stride), CIN, cout, stride), stride * cout, 2 * CIN);
+        W.build(convt_phase_major(convt_gemm_rows(wt, CIN, cout, stride), CIN, cout, stride), stride * cout, 1, 2 * CIN);
         rf::ConvtArgs a{};
         a.x = x; a.y = y; a.alpha = alpha; a.bias = bias;
         a.Tin = Tin; a.T = Tin * stride; a.B = B; a.stride = stride; a.cout = cout; a.pad = (stride + 1) / 2;    // DecBlock::pad

@@ -12,14 +12,14 @@
 // Design.  Every chunk of code frames is decoded by the streaming step with carried state; the one-shot call is the
 // same step after a reset (zero state == the reference's causal zero padding).  All dense layers -- RVQ projections,
 // k3 / k7 / dilated causal convolutions, transposed convolutions (as phase-major causal convolutions), transformer
-// and ConvNeXt linears -- run on the implicit-GEMM wgmma kernel of implicit_conv.cuh over planar bf16 hi/lo
+// and ConvNeXt linears -- run on the implicit-GEMM wgmma kernel of conv_gemm.cuh over planar bf16 hi/lo
 // activations; its epilogue fuses bias, layer scale / gamma, exact GELU, the residual add, the next layer's SnakeBeta
 // and the hi/lo split, and writes behind the H history frames the consumer's taps reach back over.  Small SIMT
 // kernels cover the gathers, norms, RoPE + attention over the cache, the depthwise conv + LayerNorm and the 1-channel
 // output conv.  The reference's double-counted transposed-conv bias at chunk boundaries (see the oracle's header) is
 // reproduced (Args::bias_twice_t0).
 #include "common.cuh"
-#include "implicit_conv.cuh"
+#include "conv_gemm.cuh"
 #include "seanet.cuh"
 
 #include <algorithm>
@@ -31,26 +31,9 @@ namespace st {
 
 typedef __nv_bfloat16 bf16;
 
-// host-side hi / lo split in the operand format, as raw 16-bit words
-static inline void split16(float v, int f16, uint16_t& hi, uint16_t& lo) {
-    if (f16) {
-        const __half h = __float2half_rn(v);
-        hi = __half_as_ushort(h);
-        lo = __half_as_ushort(__float2half_rn(v - __half2float(h)));
-    } else {
-        const bf16 h = __float2bfloat16_rn(v);
-        hi = __bfloat16_as_ushort(h);
-        lo = __bfloat16_as_ushort(__float2bfloat16_rn(v - __bfloat162float(h)));
-    }
-}
-static inline float join16(uint16_t hi, uint16_t lo, int f16) {
-    return f16 ? __half2float(__ushort_as_half(hi)) + __half2float(__ushort_as_half(lo))
-               : __bfloat162float(__ushort_as_bfloat16(hi)) + __bfloat162float(__ushort_as_bfloat16(lo));
-}
-
 // ----------------------------------------------------------------------------------------------- SIMT kernels
 __device__ __forceinline__ void put_planes(bf16* base, long long plane, long long idx, float v, int f16) {
-    ic::put_hilo16(reinterpret_cast<uint16_t*>(base), plane, idx, v, f16);
+    cg::put_hilo16(reinterpret_cast<uint16_t*>(base), plane, idx, v, f16);
 }
 
 // codes [B, nq, T] -> planes [2][B*T][2*D2]: channels [0, D2) = sum of the semantic codebooks, [D2, 2*D2) = sum of the rest
@@ -316,7 +299,7 @@ final_conv_kernel(const float* __restrict__ x, const float* __restrict__ st, con
         float v = 0.f;
         if (ti >= 0) { if (ti < T) v = x[((long long)b * T + ti) * C + c]; }
         else v = st[((long long)b * H + (H + ti)) * C + c];
-        tile[rr * ldc + c] = ic::snake_beta(v, sa[c], sb[c]);
+        tile[rr * ldc + c] = cg::snake_inv(v, sa[c], sb[c]);
     }
     __syncthreads();
     const int o = threadIdx.x & (FC_TILE - 1), part = threadIdx.x / FC_TILE;      // two threads per output, channels split in halves
@@ -333,83 +316,16 @@ final_conv_kernel(const float* __restrict__ x, const float* __restrict__ st, con
 }
 
 // ----------------------------------------------------------------------------------------------- weights
-// k-blocks per accumulation segment of the implicit convolution (ic::Args::seg_kb)
-constexpr int SEG_KB = 4;
-
-struct IW {                       // implicit-conv weight: [M][taps][cblocks * 64] as bf16 hi / lo, K-major
-    DBuf<bf16> hi, lo;
-    DBuf<float> bias, rscale;     // rscale[m] (fp16 operands only): 1 / the power of two row m is stored times
-    CUtensorMap th{}, tl{};
-    int M = 0, taps = 1, cblocks = 0, Cin = 0;
-    bool has_bias = false;
-    // [M][taps][Cin] -> [M][taps][cblocks * 64], every tap's channel run zero-padded to whole 64-channel k-blocks
-    static std::vector<float> pad_k(const std::vector<float>& W, int M, int taps, int Cin) {
-        const int cb = cdiv(Cin, tc::BK);
-        const size_t K = (size_t)taps * cb * tc::BK;
-        std::vector<float> g((size_t)M * K, 0.f);
-        for (int m = 0; m < M; ++m)
-            for (int j = 0; j < taps; ++j)
-                memcpy(&g[(size_t)m * K + (size_t)j * cb * tc::BK], &W[((size_t)m * taps + j) * Cin], (size_t)Cin * sizeof(float));
-        return g;
-    }
-    void build(const std::vector<float>& W /*[M][taps][Cin]*/, int M_, int taps_, int Cin_, int f16) {
-        M = M_; taps = taps_; Cin = Cin_; cblocks = cdiv(Cin, tc::BK);
-        const size_t K = (size_t)taps * cblocks * tc::BK;
-        std::vector<float> g = pad_k(W, M, taps, Cin);
-        if (f16) {
-            // fp16 pairs: a weight of magnitude 0.01 has a SUBNORMAL lo half (|lo| < 2^-11 |w| < 6.1e-5), i.e. ~18 bits instead of 22.
-            // Store row m times 2^e with max|w_m| * 2^e in [8192, 16384) and undo the (exact) scaling in the epilogue.
-            std::vector<float> rs((size_t)M, 1.f);
-            for (int m = 0; m < M; ++m) {
-                float mx = 0.f;
-                for (size_t k = 0; k < K; ++k) mx = std::max(mx, fabsf(g[(size_t)m * K + k]));
-                if (mx > 0.f && std::isfinite(mx)) {
-                    int e = 0;
-                    frexpf(mx, &e);                              // mx = f * 2^e, f in [0.5, 1)
-                    const float sc = ldexpf(1.0f, 14 - e);       // mx * sc in [8192, 16384)
-                    for (size_t k = 0; k < K; ++k) g[(size_t)m * K + k] *= sc;
-                    rs[m] = 1.0f / sc;
-                }
-            }
-            rscale.upload(rs.data(), rs.size());
-        }
-        std::vector<uint16_t> h(g.size()), l(g.size());
-        for (size_t i = 0; i < g.size(); ++i) split16(g[i], f16, h[i], l[i]);
-        hi.upload(reinterpret_cast<const bf16*>(h.data()), h.size());
-        lo.upload(reinterpret_cast<const bf16*>(l.data()), l.size());
-        B2A_CUDA(cudaDeviceSynchronize());
-        th = tc::make_tmap_bf16(hi.p, M, (long long)K, tc::BM, f16);
-        tl = tc::make_tmap_bf16(lo.p, M, (long long)K, tc::BM, f16);
-    }
-    void set_bias(const std::vector<float>& b) { bias.upload(b.data(), b.size()); has_bias = true; B2A_CUDA(cudaDeviceSynchronize()); }
-};
-
-// one implicit_conv_kernel launch of weight W over planes `in` [2][B][in_frames][W.Cin]
-static void ic_conv(const IW& W, const bf16* in, long long in_frames, ic::Args a, int f16, int num_sms, cudaStream_t s) {
-    a.M = W.M; a.m_tiles = cdiv(W.M, tc::BM);
-    a.taps = W.taps; a.cblocks = W.cblocks;
-    if (a.dil == 0) a.dil = 1;
-    if (a.up == 0) a.up = 1;
-    a.Cout = W.M / a.up;
-    a.t_tiles = cdiv(a.T, ic::HALF);
-    a.bias = W.has_bias ? W.bias.p : nullptr;
-    a.f16 = f16;
-    a.seg_kb = SEG_KB;
-    a.wscale = f16 ? W.rscale.p : nullptr;
-    const CUtensorMap tb = tc::make_tmap_planes(in, W.Cin, in_frames, a.B, ic::HALF, f16);
-    const long long tiles = (long long)a.B * a.t_tiles * a.m_tiles;
-    launch_pdl(a.f16 ? ic::implicit_conv_kernel<1> : ic::implicit_conv_kernel<0>, dim3((unsigned)std::min<long long>(num_sms, tiles)), dim3(ic::IC_THREADS), ic::SMEM_BYTES, s,
-               W.th, W.tl, tb, a);
-}
+using cg::TcW;
 
 struct Snake { DBuf<float> a, ib; };                 // a = exp(alpha), ib = 1 / (exp(beta) + 1e-9)
 struct PlaneState { DBuf<bf16> s[2]; int H = 0, C = 0; };      // [2][B][H][C]
 struct F32State { DBuf<float> s[2]; int H = 0, C = 0; };       // [B][H][C]
 
-struct TLayer { IW qkv, o, gu, down; DBuf<float> ln1, ln2, sc_attn, sc_mlp; DBuf<float> K, V; };
-struct UpLayer { IW ct, pw1, pw2; DBuf<float> dw_w, dw_b, ln_w, ln_b, gamma; F32State st; int factor = 1; };
-struct ResUnit { Snake a1, a2; IW c1, c2; PlaneState st; int dil = 1; };
-struct DecBlock { Snake sn; IW ct; PlaneState st; ResUnit ru[3]; int rate = 1, cin = 0, cout = 0; };
+struct TLayer { TcW qkv, o, gu, down; DBuf<float> ln1, ln2, sc_attn, sc_mlp; DBuf<float> K, V; };
+struct UpLayer { TcW ct, pw1, pw2; DBuf<float> dw_w, dw_b, ln_w, ln_b, gamma; F32State st; int factor = 1; };
+struct ResUnit { Snake a1, a2; TcW c1, c2; PlaneState st; int dil = 1; };
+struct DecBlock { Snake sn; TcW ct; PlaneState st; ResUnit ru[3]; int rate = 1, cin = 0, cout = 0; };
 
 }  // namespace st
 }  // namespace b2a
@@ -426,7 +342,7 @@ struct b2a_speech_tokenizer {
     int use_f16 = 1;              // fp16 hi/lo operand pairs (22 mantissa bits, saturating at 65504); B2A_ST_FP16=0: bf16 pairs (16 bits, fp32 range)
     // weights
     DBuf<float> emb;              // [nq][bins][D2] usage-normalised codebooks
-    IW rvq_proj, pre_conv, in_proj, out_proj, dec0;
+    TcW rvq_proj, pre_conv, in_proj, out_proj, dec0;
     PlaneState st_pre, st_dec0;
     DBuf<float> final_norm, inv_freq;
     std::vector<TLayer> layers;
@@ -475,11 +391,11 @@ struct b2a_speech_tokenizer {
         for (int c = 0; c < C; ++c) { a[c] = expf(al[c]); ib[c] = 1.0f / (expf(be[c]) + 1e-9f); }
         up(s.a, a); up(s.ib, ib);
     }
-    void load_conv(IW& w, const TensorTable& tt, const std::string& p, int out, int k, int in, bool bias = true) {
+    void load_conv(TcW& w, const TensorTable& tt, const std::string& p, int out, int k, int in, bool bias = true) {
         w.build(conv_w(tt, p + ".weight", out, k, in), out, k, in, use_f16);
         if (bias) w.set_bias(tt.f32(p + ".bias", out));
     }
-    void load_linear(IW& w, const TensorTable& tt, const std::string& p, int out, int in, bool bias) {
+    void load_linear(TcW& w, const TensorTable& tt, const std::string& p, int out, int in, bool bias) {
         w.build(tt.f32(p + ".weight", (int64_t)out * in), out, 1, in, use_f16);
         if (bias) w.set_bias(tt.f32(p + ".bias", out));
     }
@@ -503,8 +419,6 @@ struct b2a_speech_tokenizer {
         { const char* e = getenv("B2A_ST_FP16"); use_f16 = (e && e[0] == '0') ? 0 : 1; }
         B2A_CUDA(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
         B2A_CUDA(cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, device));
-        B2A_CUDA(cudaFuncSetAttribute(ic::implicit_conv_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ic::SMEM_BYTES));
-        B2A_CUDA(cudaFuncSetAttribute(ic::implicit_conv_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ic::SMEM_BYTES));
         const int nq = c.num_quantizers, ns = c.num_semantic_quantizers, bins = c.codebook_size, cbd = c.codebook_dim, L = c.latent_dim,
                   Hd = c.hidden_size, I = c.intermediate_size, nh = c.num_attention_heads, nkv = c.num_key_value_heads, hd = c.head_dim;
         D2 = cbd / 2;
@@ -664,7 +578,7 @@ struct b2a_speech_tokenizer {
         B2A_CHECK(need <= buf.n, B2A_ERR_GENERATION_FAILED, "speech tokenizer: internal workspace too small");
         return buf.p;
     }
-    void conv(const IW& W, const bf16* in, long long in_frames, ic::Args a, cudaStream_t s) { ic_conv(W, in, in_frames, a, use_f16, num_sms, s); }
+    void conv(const TcW& W, const bf16* in, long long in_frames, ic::Args a, cudaStream_t s) { ic::launch(W, in, in_frames, a, num_sms, s); }
     void carry(bf16* X, PlaneState& st, int B, long long T, cudaStream_t s) {
         if (st.H == 0) return;
         const long long n = (long long)2 * B * st.H * (st.C / 8);
@@ -838,7 +752,7 @@ struct b2a_speech_tokenizer_encoder {
     DBuf<float> wstem, bstem;          // [F, k, 1]
     std::vector<Stage> stages;
     ec::Conv last, down;
-    struct Layer { IW qkv, o, fc1, fc2; DBuf<float> ln1w, ln1b, ln2w, ln2b, ls1, ls2; };
+    struct Layer { TcW qkv, o, fc1, fc2; DBuf<float> ln1w, ln1b, ln2w, ln2b, ls1, ls2; };
     std::vector<Layer> layers;
     DBuf<float> inv_freq, proj_t, books, c2;     // proj_t [hidden, 2 D] (first | rest, transposed); books [G][size][D]; c2 [G][size]
     // workspaces
@@ -852,7 +766,7 @@ struct b2a_speech_tokenizer_encoder {
         up(cv.A, tt.f32(p + ".weight", (int64_t)cout * k * cin));       // MLX [out, k, in] == [M, tap * Cin + ci]
         if (bias) up(cv.bias, tt.f32(p + ".bias", cout));
     }
-    void load_linear(IW& w, const TensorTable& tt, const std::string& p, int out, int in) {
+    void load_linear(TcW& w, const TensorTable& tt, const std::string& p, int out, int in) {
         w.build(tt.f32(p + ".weight", (int64_t)out * in), out, 1, in, 1);
     }
 
@@ -880,7 +794,6 @@ struct b2a_speech_tokenizer_encoder {
         require_device(dev);
         B2A_CUDA(cudaSetDevice(dev));
         B2A_CUDA(cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, device));
-        B2A_CUDA(cudaFuncSetAttribute(ic::implicit_conv_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ic::SMEM_BYTES));
         B2A_CUDA(cudaFuncSetAttribute(ordered_proj_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(PJ_R * c.hidden_size * sizeof(float))));
         G = std::min(c.valid_num_quantizers, c.num_quantizers);
         {   // Qwen3TTSSpeechTokenizerEncoder.init (:810-812): stride = max(1, Int(sampling_rate / prod(ratios) / frame_rate))
@@ -1024,7 +937,7 @@ struct b2a_speech_tokenizer_encoder {
         for (auto& Ly : layers) {
             layernorm_planes_kernel<<<(unsigned)N25, RN_THREADS, 0, s>>>(x, Ly.ln1w.p, Ly.ln1b.p, P0.p, N25, H, 1e-5f, 1);
             count_launch();
-            { ic::Args a{}; a.B = B; a.T = cap; a.xo = Q.p; ic_conv(Ly.qkv, P0.p, cap, a, 1, num_sms, s); }
+            { ic::Args a{}; a.B = B; a.T = cap; a.xo = Q.p; ic::launch(Ly.qkv, P0.p, cap, a, num_sms, s); }
             rope_cache_kernel<true><<<(unsigned)N25, 256, 0, s>>>(Q.p, Kc.p, Vc.p, inv_freq.p, cap, 0, nh, nh, hd, cap);
             count_launch();
             {
@@ -1034,11 +947,11 @@ struct b2a_speech_tokenizer_encoder {
                 else attn_kernel<4><<<grid, block, 0, s>>>(Q.p, Kc.p, Vc.p, P1.p, B, cap, 0, nh, nh, cap, scale, 1);
                 count_launch();
             }
-            { ic::Args a{}; a.B = B; a.T = cap; a.xo = x; a.add = 1; a.gamma = Ly.ls1.p; ic_conv(Ly.o, P1.p, cap, a, 1, num_sms, s); }
+            { ic::Args a{}; a.B = B; a.T = cap; a.xo = x; a.add = 1; a.gamma = Ly.ls1.p; ic::launch(Ly.o, P1.p, cap, a, num_sms, s); }
             layernorm_planes_kernel<<<(unsigned)N25, RN_THREADS, 0, s>>>(x, Ly.ln2w.p, Ly.ln2b.p, P0.p, N25, H, 1e-5f, 1);
             count_launch();
-            { ic::Args a{}; a.B = B; a.T = cap; a.gelu = 1; a.hl = P1.p; ic_conv(Ly.fc1, P0.p, cap, a, 1, num_sms, s); }
-            { ic::Args a{}; a.B = B; a.T = cap; a.xo = x; a.add = 1; a.gamma = Ly.ls2.p; ic_conv(Ly.fc2, P1.p, cap, a, 1, num_sms, s); }
+            { ic::Args a{}; a.B = B; a.T = cap; a.gelu = 1; a.hl = P1.p; ic::launch(Ly.fc1, P0.p, cap, a, num_sms, s); }
+            { ic::Args a{}; a.B = B; a.T = cap; a.xo = x; a.add = 1; a.gamma = Ly.ls2.p; ic::launch(Ly.fc2, P1.p, cap, a, num_sms, s); }
         }
         // 3. downsample: k = 2 ds, stride ds, edge padding on both sides, no bias -> z
         zbuf.alloc((size_t)N * H);
@@ -1191,14 +1104,15 @@ int32_t b2a_speech_tokenizer_debug_layout(const float* w, int32_t out, int32_t k
         B2A_CHECK(stride == 0 || k % stride == 0, B2A_ERR_INVALID_INPUT, "b2a_speech_tokenizer_debug_layout: kernel must be a multiple of the stride");
         std::vector<float> src(w, w + (size_t)out * k * in);
         const int M = stride ? stride * out : out, T = stride ? k / stride : k;
-        const std::vector<float> g = IW::pad_k(stride ? b2a_speech_tokenizer::convt_w(src, out, k, in, stride) : src, M, T, in);
+        const std::vector<float> g = TcW::pad_k(stride ? b2a_speech_tokenizer::convt_w(src, out, k, in, stride) : src, M, T, in);
         B2A_CHECK((int64_t)g.size() <= capacity, B2A_ERR_INVALID_INPUT, "b2a_speech_tokenizer_debug_layout: output buffer too small");
         memcpy(layout_out, g.data(), g.size() * sizeof(float));
         *rows = M; *taps = T; *kpad = cdiv(in, tc::BK) * tc::BK;
     });
 }
 
-// Standalone entry for tests/test_gpu_implicit_conv.py: one launch of ic::implicit_conv_kernel on host data.
+// Standalone entry for tests/test_gpu_implicit_conv.py: one implicit convolution on host data, through the engines' weight
+// operand and launch (ic::launch).
 //   w [M][taps][Cin], x [B][Ttot][Cin] (split into hi/lo planes here), bias / gamma / sa / sb [M / up] or null,
 //   xo [B][T*up][M/up] in/out or null, hl_out [B][Hout + T*up][M/up] (hi + lo recombined; frames below Hout come back 0) or null.
 int32_t b2a_implicit_conv_test(const float* w, int32_t M, int32_t taps, int32_t Cin, const float* x, int32_t B, int32_t Ttot, int32_t T,
@@ -1210,42 +1124,34 @@ int32_t b2a_implicit_conv_test(const float* w, int32_t M, int32_t taps, int32_t 
                   B2A_ERR_INVALID_INPUT, "b2a_implicit_conv_test: bad argument");
         require_device(0);
         B2A_CUDA(cudaSetDevice(0));
-        B2A_CUDA(cudaFuncSetAttribute(ic::implicit_conv_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ic::SMEM_BYTES));
-        B2A_CUDA(cudaFuncSetAttribute(ic::implicit_conv_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ic::SMEM_BYTES));
         int num_sms = 132;
         B2A_CUDA(cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, 0));
         const int Cout = M / up;
         const long long To = (long long)T * up;
-        IW W;
+        TcW W;
         W.build(std::vector<float>(w, w + (size_t)M * taps * Cin), M, taps, Cin, fp16);
+        if (bias) W.set_bias(std::vector<float>(bias, bias + Cout));
         const size_t nx = (size_t)B * Ttot * Cin, no = (size_t)B * To * Cout, nh = (size_t)B * (Hout + To) * Cout;
         std::vector<uint16_t> xp(2 * nx);
-        for (size_t i = 0; i < nx; ++i) split16(x[i], fp16, xp[i], xp[nx + i]);
+        for (size_t i = 0; i < nx; ++i) cg::split16(x[i], fp16, xp[i], xp[nx + i]);
         DBuf<bf16> dx, dh;
-        DBuf<float> dxo, dbias, dgamma, dsa, dsb;
+        DBuf<float> dxo, dgamma, dsa, dsb;
         dx.upload(reinterpret_cast<const bf16*>(xp.data()), xp.size());
         ic::Args a{};
-        a.M = M; a.m_tiles = cdiv(M, tc::BM); a.taps = taps; a.cblocks = W.cblocks; a.dil = dil; a.shift0 = shift0;
-        a.B = B; a.T = T; a.t_tiles = cdiv(T, ic::HALF); a.Cout = Cout; a.up = up; a.gelu = gelu; a.add = add; a.bias_twice_t0 = bias_twice_t0; a.Hout = Hout; a.f16 = fp16;
-        a.seg_kb = SEG_KB;
-        a.wscale = fp16 ? W.rscale.p : nullptr;
-        if (bias) { dbias.upload(bias, Cout); a.bias = dbias.p; }
+        a.dil = dil; a.shift0 = shift0; a.B = B; a.T = T; a.up = up; a.gelu = gelu; a.add = add; a.bias_twice_t0 = bias_twice_t0; a.Hout = Hout;
         if (gamma) { dgamma.upload(gamma, Cout); a.gamma = dgamma.p; }
         if (sa) { dsa.upload(sa, Cout); dsb.upload(sb, Cout); a.sa = dsa.p; a.sb = dsb.p; }
         if (xo) { dxo.upload(xo, no); a.xo = dxo.p; }
         if (hl_out) { dh.alloc(2 * nh); B2A_CUDA(cudaMemset(dh.p, 0, 2 * nh * sizeof(bf16))); a.hl = dh.p; }
         B2A_CUDA(cudaDeviceSynchronize());
-        const CUtensorMap tb = tc::make_tmap_planes(dx.p, Cin, Ttot, B, ic::HALF, fp16);
-        const long long tiles = (long long)B * a.t_tiles * a.m_tiles;
-        launch_pdl(a.f16 ? ic::implicit_conv_kernel<1> : ic::implicit_conv_kernel<0>, dim3((unsigned)std::min<long long>(num_sms, tiles)), dim3(ic::IC_THREADS), ic::SMEM_BYTES, (cudaStream_t)0,
-                   W.th, W.tl, tb, a);
+        ic::launch(W, dx.p, Ttot, a, num_sms, (cudaStream_t)0);
         B2A_CUDA(cudaGetLastError());
         B2A_CUDA(cudaDeviceSynchronize());
         if (xo) B2A_CUDA(cudaMemcpy(xo, dxo.p, no * sizeof(float), cudaMemcpyDeviceToHost));
         if (hl_out) {
             std::vector<uint16_t> hp(2 * nh);
             B2A_CUDA(cudaMemcpy(hp.data(), dh.p, 2 * nh * sizeof(uint16_t), cudaMemcpyDeviceToHost));
-            for (size_t i = 0; i < nh; ++i) hl_out[i] = join16(hp[i], hp[nh + i], fp16);
+            for (size_t i = 0; i < nh; ++i) hl_out[i] = cg::join16(hp[i], hp[nh + i], fp16);
         }
     });
 }

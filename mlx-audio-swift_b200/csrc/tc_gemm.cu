@@ -54,7 +54,7 @@ CUtensorMap make_tmap_f16_3d(const void* base, long long d0, long long d1, long 
     return m;
 }
 
-// the operand of implicit_conv.cuh: one box is 64 channels of box_frames frames, hi plane then lo plane
+// the operand of the implicit convolution (conv_gemm.cuh): one box is 64 channels of box_frames frames, hi plane then lo plane
 CUtensorMap make_tmap_planes(const void* base, int C, long long Ttot, int B, int box_frames, int f16) {
     B2A_CHECK(C % 8 == 0 && ((uintptr_t)base & 15) == 0 && Ttot >= 1 && B >= 1, B2A_ERR_INVALID_INPUT,
               "TMA: activation planes must be 16-byte aligned with channels % 8 == 0");

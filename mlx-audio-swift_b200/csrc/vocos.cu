@@ -175,7 +175,7 @@ struct b2a_vocos {
         {
             std::vector<float> w = tt.f32("backbone.embed.weight", (int64_t)D * k * Cin), wp((size_t)D * kp_embed, 0.f);
             for (int o = 0; o < D; ++o) memcpy(&wp[(size_t)o * kp_embed], &w[(size_t)o * k * Cin], (size_t)k * Cin * sizeof(float));
-            embed.build(wp, D, kp_embed);
+            embed.build(wp, D, 1, kp_embed);
             up(embed_b, "backbone.embed.bias", D);
         }
         const int E = c.adanorm_num_embeddings, norms = 1 + c.num_layers;
@@ -200,12 +200,12 @@ struct b2a_vocos {
             up(B.dw_b, p + "dwconv.bias", D);
             if (E > 0) ada(1 + l, p + "norm.");
             else { up(B.ln_w, p + "norm.weight", D); up(B.ln_b, p + "norm.bias", D); }
-            B.pw1.build(tt.f32(p + "pwconv1.weight", (int64_t)I * D), I, D); up(B.pw1_b, p + "pwconv1.bias", I);
-            B.pw2.build(tt.f32(p + "pwconv2.weight", (int64_t)D * I), D, I); up(B.pw2_b, p + "pwconv2.bias", D);
+            B.pw1.build(tt.f32(p + "pwconv1.weight", (int64_t)I * D), I, 1, D); up(B.pw1_b, p + "pwconv1.bias", I);
+            B.pw2.build(tt.f32(p + "pwconv2.weight", (int64_t)D * I), D, 1, I); up(B.pw2_b, p + "pwconv2.bias", D);
             if (tt.find(p + "gamma")) up(B.gamma, p + "gamma", D);
         }
         if (E > 0) { ada_w.upload(aw.data(), aw.size()); ada_b.upload(ab.data(), ab.size()); B2A_CUDA(cudaDeviceSynchronize()); }
-        head.build(tt.f32("head.out.weight", (int64_t)(N + 2) * D), N + 2, D);
+        head.build(tt.f32("head.out.weight", (int64_t)(N + 2) * D), N + 2, 1, D);
         up(head_b, "head.out.bias", N + 2);
         // windowed inverse real DFT as a matrix: frame[j] = w[j]/N * (Re0 + (-1)^j Re_{N/2} + 2 sum_k (Re_k cos - Im_k sin))
         kp_spec = (int)pad64(2 * half);
@@ -219,7 +219,7 @@ struct b2a_vocos {
                     A[(size_t)j * kp_spec + kq] = (float)(wv[j] * ck * std::cos(ang) / N);
                     A[(size_t)j * kp_spec + half + kq] = (kq == 0 || kq == N / 2) ? 0.f : (float)(-wv[j] * 2.0 * std::sin(ang) / N);
                 }
-            idft.build(A, N, kp_spec);
+            idft.build(A, N, 1, kp_spec);
             win.upload(wv.data(), N);
         }
         B2A_CUDA(cudaDeviceSynchronize());

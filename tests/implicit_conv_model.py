@@ -1,4 +1,4 @@
-"""numpy statement of the Args contract of ic::implicit_conv_kernel (csrc/implicit_conv.cuh).  Shared by the CPU data-flow
+"""numpy statement of the Args contract of ic::implicit_conv_kernel (csrc/conv_gemm.cuh).  Shared by the CPU data-flow
 model (test_speech_tokenizer_design.py) and the gated GPU kernel test (test_gpu_implicit_conv.py).  Test infrastructure."""
 import math
 

@@ -1,5 +1,5 @@
-"""The implicit-GEMM causal convolution kernel (csrc/implicit_conv.cuh) alone, through b2a_implicit_conv_test, against its numpy
-contract (tests/implicit_conv_model.py).  (row N1)."""
+"""The implicit-GEMM causal convolution kernel (csrc/conv_gemm.cu) alone, through b2a_implicit_conv_test and the engines' launch
+(ic::launch), against its numpy contract (tests/implicit_conv_model.py).  (row N1)."""
 import os
 
 import numpy as np

@@ -86,7 +86,7 @@ def test_default_geometry_and_errors(b2a, codec):
     codes = np.random.default_rng(0).integers(0, 2048, (1, 16, 6))
     ref = oc.SpeechTokenizerDecoder(cfg, W)(codes).numpy()
     # A tensor core that truncates its fp32 accumulation biases each long convolution (tools/probe_n1_dec0.py measures it) and this
-    # stack amplifies the bias; the contraction is accumulated in segments of 256 that are added in registers (implicit_conv.cuh,
+    # stack amplifies the bias; the contraction is accumulated in segments of 256 that are added in registers (conv_gemm.cuh,
     # Args::seg_kb), and fp16 operand pairs (the default) carry more mantissa than bf16 ones.
     assert max_rel_to_peak(m(codes), ref) < TOL
     os.environ["B2A_ST_FP16"] = "0"                              # read when a handle is created

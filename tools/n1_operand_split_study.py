@@ -1,7 +1,7 @@
 """CPU study: the Qwen3-TTS speech-tokenizer decoder (float64 oracle) with the operands of every weight GEMM / dense convolution
 replaced by what a tensor-core split holds, products in float64 (so only the operand representation is modelled):
 
-    bf16x2   hi + lo bf16 (16 mantissa bits), the lo*lo product dropped          -- what implicit_conv.cuh runs
+    bf16x2   hi + lo bf16 (16 mantissa bits), the lo*lo product dropped          -- what the implicit convolution runs
     f16x2    hi + lo fp16 (subnormals kept: absolute floor 2^-24), lo*lo dropped
     bf16x3   hi + mid + lo bf16 (24 bits), products with weight >= 2^-16 kept (hh, hm, mh, mm, hl, lh)
 
