@@ -7,8 +7,8 @@
 //   mlx-swift-lm 3.31.4 (un-vendored): TopPSampler / RepetitionContext (call sites :691-692)
 //
 // HBM layout: weights bf16 [out, in] row-major (q|k|v fused into one matrix, gate/up row-
-// interleaved so SwiGLU is a GEMV epilogue); KV cache bf16 [layer][B][kv_head][ctx][128];
-// residual stream fp32 [B, H]; GEMV inputs bf16 [B, K] (staged in shared memory per CTA).
+// interleaved so SwiGLU is a GEMM epilogue); KV cache fp32 [layer][B][kv_head][ctx][128];
+// residual stream fp32 [B, H]; GEMM inputs bf16 hi/lo pairs [16, K] (LO_ROW).
 // The whole decode step (embed -> 28 layers -> lm head -> logits processors -> sampler ->
 // bookkeeping) is captured in one CUDA graph and replayed per token; nothing syncs with the
 // host inside the loop except a poll of the "all rows finished" flag every few steps.
@@ -34,15 +34,6 @@ constexpr int TOK_AUDIO_OFFSET = 128266;
 constexpr int TOK_AUDIO_START = 128261, TOK_AUDIO_END = 128262;        // LlamaTTS.swift:27-28
 
 __device__ __forceinline__ float bf16_round(float x) { return __bfloat162float(__float2bfloat16_rn(x)); }
-__device__ __forceinline__ float bf_lo(unsigned u) { return __uint_as_float(u << 16); }
-__device__ __forceinline__ float bf_hi(unsigned u) { return __uint_as_float(u & 0xffff0000u); }
-
-__device__ __forceinline__ uint4 ldg_stream(const uint4* p) {
-    uint4 r;
-    asm volatile("ld.global.nc.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%4];"
-                 : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "l"(p));
-    return r;
-}
 
 // ------------------------------------------------------------------------------------------------
 // embed + RMSNorm
@@ -92,8 +83,7 @@ constexpr int LO_ROW = 8;   // activation matrices are [16, K] bf16: row b = hi(
 constexpr int RN_THREADS = 1024, RN_MAXV = 8;
 __global__ void __launch_bounds__(RN_THREADS)
 add_rmsnorm_kernel(float* __restrict__ x, float* __restrict__ delta, const float* __restrict__ w,
-                   bf16* __restrict__ xn, int H, float eps, float* __restrict__ trace, int half,
-                   float* __restrict__ normed = nullptr, float* __restrict__ ss_out = nullptr, int ss_parts = 0) {
+                   bf16* __restrict__ xn, int H, float eps, int half, float* __restrict__ ss_out, int ss_parts) {
     __shared__ float red[RN_THREADS / 32];
     const int b = blockIdx.x, tid = threadIdx.x;
     pdl_trigger();
@@ -108,7 +98,6 @@ add_rmsnorm_kernel(float* __restrict__ x, float* __restrict__ delta, const float
         if (i < H) {
             val = xr[i];
             if (delta) { val += delta[(long long)b * H + i]; xr[i] = val; delta[(long long)b * H + i] = 0.f; }
-            if (trace) trace[(long long)b * H + i] = val;
         }
         v[j] = val;
         ss += val * val;
@@ -126,96 +115,7 @@ add_rmsnorm_kernel(float* __restrict__ x, float* __restrict__ delta, const float
 #pragma unroll
     for (int j = 0; j < RN_MAXV; ++j) {
         const int i = tid + j * RN_THREADS;
-        if (i < H) {
-            const float o = v[j] * r * w[i];
-            tc::store_hilo(xn, H, b, i, o, half);
-            if (normed) normed[(long long)b * H + i] = o;     // the fp32 normalised row (the talker's hidden state, row N1)
-        }
-    }
-}
-
-// ------------------------------------------------------------------------------------------------
-// Weight-streaming GEMV: y[b, n] = sum_k W[n,k] * x[b,k],  NB rows of x in shared memory (bf16),
-// each warp owns ROWS consecutive weight rows and streams them with 16-byte no-allocate loads.
-// ------------------------------------------------------------------------------------------------
-constexpr int GV_MAX_THREADS = 256;
-enum : int { GV_F32 = 0, GV_SWIGLU = 1, GV_F32_ATOMIC = 2 };
-
-// SIMT fallback (B2A_GEMM=simt, or K not a multiple of 64): same numerics as the tensor-core path -- the
-// activation matrix holds hi rows [0, NB) and lo rows [8, 8 + NB); both halves are accumulated and summed.
-// grid = (row tiles, K splits); with gridDim.y == 2 the two K halves are combined by atomicAdd into a zeroed y.
-template <int NB, int ROWS, int EPI>
-__global__ void __launch_bounds__(GV_MAX_THREADS)
-gemv_bf16_kernel(const bf16* __restrict__ W, const bf16* __restrict__ xin, float* __restrict__ y,
-                 bf16* __restrict__ act, int N, int K) {
-    extern __shared__ uint4 sx[];  // [2*NB][Kc/8]
-    pdl_trigger();
-    pdl_wait();
-    const int K8 = K >> 3;
-    const int Kc8 = K8 / gridDim.y, kbase = blockIdx.y * Kc8;
-    for (int i = threadIdx.x; i < 2 * NB * Kc8; i += blockDim.x) {
-        const int r = i / Kc8, k = i - r * Kc8;
-        const int grow = r < NB ? r : LO_ROW + (r - NB);
-        sx[i] = reinterpret_cast<const uint4*>(xin)[(long long)grow * K8 + kbase + k];
-    }
-    __syncthreads();
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int row0 = (blockIdx.x * (blockDim.x >> 5) + warp) * ROWS;
-    if (row0 >= N) return;
-    const uint4* Wr[ROWS];
-#pragma unroll
-    for (int r = 0; r < ROWS; ++r)
-        Wr[r] = reinterpret_cast<const uint4*>(W) + (long long)min(row0 + r, N - 1) * K8 + kbase;
-
-    float acc[ROWS][2 * NB];
-#pragma unroll
-    for (int r = 0; r < ROWS; ++r)
-#pragma unroll
-        for (int b = 0; b < 2 * NB; ++b) acc[r][b] = 0.f;
-
-    for (int k8 = lane; k8 < Kc8; k8 += 32) {
-        float wf[ROWS][8];
-#pragma unroll
-        for (int r = 0; r < ROWS; ++r) {
-            const uint4 wv = ldg_stream(Wr[r] + k8);
-            wf[r][0] = bf_lo(wv.x); wf[r][1] = bf_hi(wv.x); wf[r][2] = bf_lo(wv.y); wf[r][3] = bf_hi(wv.y);
-            wf[r][4] = bf_lo(wv.z); wf[r][5] = bf_hi(wv.z); wf[r][6] = bf_lo(wv.w); wf[r][7] = bf_hi(wv.w);
-        }
-#pragma unroll
-        for (int b = 0; b < 2 * NB; ++b) {
-            const uint4 xv = sx[b * Kc8 + k8];
-            const float xf[8] = {bf_lo(xv.x), bf_hi(xv.x), bf_lo(xv.y), bf_hi(xv.y),
-                                 bf_lo(xv.z), bf_hi(xv.z), bf_lo(xv.w), bf_hi(xv.w)};
-#pragma unroll
-            for (int r = 0; r < ROWS; ++r)
-#pragma unroll
-                for (int j = 0; j < 8; ++j) acc[r][b] = fmaf(wf[r][j], xf[j], acc[r][b]);
-        }
-    }
-#pragma unroll
-    for (int r = 0; r < ROWS; ++r)
-#pragma unroll
-        for (int b = 0; b < NB; ++b) acc[r][b] = warp_sum(acc[r][b] + acc[r][NB + b]);
-    if (lane == 0) {
-        if (EPI == GV_F32 || EPI == GV_F32_ATOMIC) {
-#pragma unroll
-            for (int r = 0; r < ROWS; ++r)
-                if (row0 + r < N)
-#pragma unroll
-                    for (int b = 0; b < NB; ++b) {
-                        if (EPI == GV_F32) y[(long long)b * N + row0 + r] = acc[r][b];
-                        else atomicAdd(&y[(long long)b * N + row0 + r], acc[r][b]);
-                    }
-        } else {  // rows are (gate, up) pairs: act[b, n/2] = silu(gate) * up   (LlamaTTS.swift:282-284)
-#pragma unroll
-            for (int r = 0; r < ROWS; r += 2)
-                if (row0 + r + 1 < N)
-#pragma unroll
-                    for (int b = 0; b < NB; ++b) {
-                        const float g = acc[r][b], u = acc[r + 1][b];
-                        tc::store_hilo(act, N / 2, b, (row0 + r) / 2, g / (1.0f + __expf(-g)) * u, LO_ROW);
-                    }
-        }
+        if (i < H) tc::store_hilo(xn, H, b, i, v[j] * r * w[i], half);
     }
 }
 
@@ -940,11 +840,9 @@ struct b2a_tts {
     // activations: fp32 residual stream; GEMM inputs as [16, K] bf16 hi/lo pairs
     DBuf<float> x, y, qkv, logits, probs;
     DBuf<bf16> xn, attn, act;
-    DBuf<float> sk_ws;       // stream-K partial tiles of the decode GEMMs (qkv / o / down), see tc::Args::part_ws
+    DBuf<float> sk_ws;       // stream-K partial tiles of the q|k|v GEMM when it runs stream-K (qkv_cluster == 0), see tc::Args::part_ws
     DBuf<unsigned> sk_cnt;
     int sk_slots = 0;
-    // wgmma / TMA path
-    bool use_tc = true;
     int num_sms = 132;
     std::vector<CUtensorMap> tm_qkv, tm_o, tm_gu, tm_down;
     // weight rows per m-tile for a whole-tile GEMM of M rows (tc::Args::tile_rows): 128 unless that leaves > 1/4 of the SMs idle
@@ -967,25 +865,24 @@ struct b2a_tts {
     DBuf<int> tokens, pos, recent, recent_n, out_tokens, n_gen, done, n_active, ids, forced;
     HBuf<int> h_flag;
     cudaEvent_t ev_poll[2] = {nullptr, nullptr};   // the generate loop's pipelined "rows still active" polls
-    // fused-norm decode step (default on the wgmma path): o_proj / down_proj run as cluster split-K GEMMs whose leader CTA does the
-    // residual add + the next norm's gain + hi/lo split + sum of squares; no stand-alone add_rmsnorm launches (tc_gemm.cuh).  q|k|v runs
-    // on the same kernel in store mode (qkv_gemm)
-    bool fused = false;
+    // fused-norm decode step: o_proj / down_proj run as cluster split-K GEMMs whose leader CTA does the residual add + the next
+    // norm's gain + hi/lo split + sum of squares; one add_rmsnorm launch per step, for the first norm (tc_gemm.cuh).  q|k|v runs on
+    // the same kernel in store mode (qkv_gemm)
     static constexpr int fused_cluster = 5;   // 5 CTAs per 128-row tile: 120 of 132 SMs for hidden 3072, one wave
     int qkv_cluster = 0;                      // CTAs per 128-row tile of the q|k|v split-K GEMM (pick_qkv_cluster); 0: stream-K
     int qkv_sk_ctas = 0;                      // the stream-K CTA count whose cut of the k-blocks that GEMM reproduces
     // ring depths of the decode step's GEMMs.  With them tc::Smem<16>::bytes, tc::SmemSplit::bytes and attn_smem_bytes() are sized so
     // that any two kernels that follow each other in the fused step fit on one SM together (b2a_debug_step_smem reports the three)
     static constexpr int gemm_stages = 6, splitk_stages = 5;
-    int fused_parts = 0;
-    DBuf<float> ss_a, ss_b;          // [H / 128, 8] partial sums of squares: ss_a feeds the post-attention norm, ss_b the input norm
+    int fused_parts = 0;             // m-tiles of H (the last one may be partly filled): partial sums of squares per row
+    DBuf<float> ss_a, ss_b;          // [fused_parts <= 64, 8] partial sums of squares: ss_a feeds the post-attention norm, ss_b the input norm
     StackSpec spec;                  // which keys / features this stack was built with
     const float* x_ext = nullptr;    // row N1: when set, a step starts from these embeddings [8, H] instead of embed(tokens)
-    float* normed_out = nullptr;     // row N1: when set, the final RMSNorm also writes its fp32 output here [8, H]
+    float* normed_out = nullptr;     // row N1: when set, run_final_norm writes the final RMSNorm's fp32 output here [8, H]
     std::atomic<int> cancel{0};
     int bench_mask_eos = 0, bench_wrap_codes = 0;   // b2a_tts_set_bench_flags (include/b200audio_internal.h): fixed-work benchmark switches
     int nb_pad = 0;   // rows rounded up to 1/2/4/8
-    bool trace_on = false;       // debug: residual stream at every RMSNorm input (eager forward only)
+    bool trace_on = false;       // debug: residual stream at every RMSNorm input (eager forward only, trace_x)
     DBuf<float> trace;           // [2*layers + 1][8][H]
     // CUDA graphs for the two step flavours (captured per (nb_pad, params) configuration)
     cudaGraphExec_t g_step = nullptr, g_prefill = nullptr;
@@ -1041,7 +938,12 @@ struct b2a_tts {
     void check_config() {
         const b2a_llama_config& c = cfg;
         B2A_CHECK(c.head_dim == HD, B2A_ERR_INVALID_INPUT, "llama: head_dim must be 128");
-        B2A_CHECK(c.hidden_size % 8 == 0 && c.intermediate_size % 8 == 0, B2A_ERR_INVALID_INPUT, "llama: sizes must be multiples of 8");
+        // every GEMM's K is a whole number of 64-wide k-blocks (tc::BK); the fused step's 1024-thread first norm holds a row in
+        // registers (RN_MAXV values per thread)
+        B2A_CHECK(c.hidden_size > 0 && c.hidden_size % 64 == 0 && c.hidden_size <= RN_THREADS * RN_MAXV, B2A_ERR_INVALID_INPUT,
+                  "llama: hidden_size must be a multiple of 64 (<= 8192)");
+        B2A_CHECK(c.intermediate_size > 0 && c.intermediate_size % 64 == 0, B2A_ERR_INVALID_INPUT,
+                  "llama: intermediate_size must be a multiple of 64");
         {
             const int g = c.num_key_value_heads > 0 && c.num_attention_heads % c.num_key_value_heads == 0
                               ? c.num_attention_heads / c.num_key_value_heads : 0;
@@ -1058,7 +960,6 @@ struct b2a_tts {
         const b2a_llama_config& c = cfg;
         const int H = c.hidden_size, I = c.intermediate_size, nq = c.num_attention_heads, nkv = c.num_key_value_heads;
         const int NQ = nq * HD, NKV = nkv * HD;
-        B2A_CHECK(H <= RN_THREADS * RN_MAXV, B2A_ERR_INVALID_INPUT, "llama: hidden_size above 8192 is not supported");
         std::vector<float> fr = llama3_freqs(c);
         freqs.upload(fr.data(), fr.size());
         const size_t kv = (size_t)c.num_hidden_layers * c.max_batch * nkv * c.max_context * HD;
@@ -1082,55 +983,41 @@ struct b2a_tts {
         B2A_CUDA(cudaMemset(pos.p, 0, B * sizeof(int)));
         h_flag.alloc(16);
         // process-wide kernel attributes: always the same (largest) value, several handles may coexist
-        gemv_attrs<1>(); gemv_attrs<2>(); gemv_attrs<4>(); gemv_attrs<8>();
         attn_cluster_attr<1>(); attn_cluster_attr<2>(); attn_cluster_attr<3>(); attn_cluster_attr<4>(); attn_cluster_attr<6>(); attn_cluster_attr<8>();
-        // wgmma / TMA path: needs every GEMM K to be a multiple of 64; B2A_GEMM=simt forces the SIMT fallback
-        const char* env = getenv("B2A_GEMM");
-        use_tc = !(env && std::string(env) == "simt") && H % tc::BK == 0 && NQ % tc::BK == 0 && I % tc::BK == 0;
-        fused_parts = H / tc::BM;
-        fused = use_tc && H % tc::BM == 0 && fused_parts <= 64;
+        tc::set_attributes();
+        fused_parts = cdiv(H, tc::BM);          // <= 64: H <= 8192 (check_config)
         ss_a.alloc((size_t)64 * 8); ss_b.alloc((size_t)64 * 8);
         B2A_CUDA(cudaMemset(ss_a.p, 0, 64 * 8 * sizeof(float)));
         B2A_CUDA(cudaMemset(ss_b.p, 0, 64 * 8 * sizeof(float)));
         B2A_CUDA(cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, device));
-        {   // stream-K workspace for the decode GEMMs that split K ranges across CTAs: qkv, o, down (BN = 16)
-            const int ops[3][2] = {{NQ + 2 * NKV, H}, {H, NQ}, {H, I}};
-            int mt_max = 0;
-            for (const auto& op : ops) {
-                const int mt = cdiv(op[0], tc::BM), kb = op[1] / tc::BK;
-                if (kb == 0) continue;
-                const int ctas = (int)std::min<long long>(num_sms, (long long)mt * kb);
-                sk_slots = std::max(sk_slots, tc::stream_k_slots(mt, kb, ctas));
-                mt_max = std::max(mt_max, mt);
+        {   // q|k|v as clusters when they fit in one wave; otherwise the stream-K GEMM, with its workspace (BN = 16)
+            const int mt = cdiv(NQ + 2 * NKV, tc::BM), kb = H / tc::BK;
+            qkv_cluster = pick_qkv_cluster(mt, kb, num_sms, &qkv_sk_ctas);
+            if (qkv_cluster == 0) {
+                sk_slots = tc::stream_k_slots(mt, kb, qkv_sk_ctas);
+                sk_ws.alloc((size_t)mt * sk_slots * 16 * tc::BM);
+                sk_cnt.alloc(mt);
+                B2A_CUDA(cudaMemset(sk_cnt.p, 0, (size_t)mt * sizeof(unsigned)));
             }
-            sk_ws.alloc((size_t)std::max(1, mt_max) * std::max(1, sk_slots) * 16 * tc::BM);
-            sk_cnt.alloc((size_t)std::max(1, mt_max));
-            B2A_CUDA(cudaMemset(sk_cnt.p, 0, (size_t)std::max(1, mt_max) * sizeof(unsigned)));
         }
         const char* envp = getenv("B2A_PREFILL");
         use_batched_prefill = !(envp && std::string(envp) == "step");
-        if (use_tc) {
-            tc::set_attributes();
-            if (fused) {
-                qkv_cluster = pick_qkv_cluster(cdiv(NQ + 2 * NKV, tc::BM), H / tc::BK, num_sms, &qkv_sk_ctas);
+        for (auto& L : layers) {
+            tm_qkv.push_back(tc::make_tmap_bf16(L.wqkv.p, NQ + 2 * NKV, H, tc::BM));
+            tm_o.push_back(tc::make_tmap_bf16(L.wo.p, H, NQ, tc::BM));
+            tm_gu.push_back(tc::make_tmap_bf16(L.wgu.p, 2 * I, H, tc::BM));
+            {   // decode step: when 128-row tiles would leave more than a quarter of the SMs idle (Qwen3-TTS: 6144 rows = 48 tiles), use
+                // as many m-tiles as SMs (rows per tile a multiple of 8).  Orpheus (128 tiles on 132 SMs) keeps 128.
+                gu_tile_rows = pick_tile_rows(2 * I, num_sms);
+                tm_gu_dec.push_back(tc::make_tmap_bf16(L.wgu.p, 2 * I, H, gu_tile_rows));
             }
-            for (auto& L : layers) {
-                tm_qkv.push_back(tc::make_tmap_bf16(L.wqkv.p, NQ + 2 * NKV, H, tc::BM));
-                tm_o.push_back(tc::make_tmap_bf16(L.wo.p, H, NQ, tc::BM));
-                tm_gu.push_back(tc::make_tmap_bf16(L.wgu.p, 2 * I, H, tc::BM));
-                {   // decode step: when 128-row tiles would leave more than a quarter of the SMs idle (Qwen3-TTS: 6144 rows = 48 tiles), use
-                    // as many m-tiles as SMs (rows per tile a multiple of 8).  Orpheus (128 tiles on 132 SMs) keeps 128.
-                    gu_tile_rows = pick_tile_rows(2 * I, num_sms);
-                    tm_gu_dec.push_back(tc::make_tmap_bf16(L.wgu.p, 2 * I, H, gu_tile_rows));
-                }
-                tm_down.push_back(tc::make_tmap_bf16(L.wdown.p, H, I, tc::BM));
-            }
-            lm_tile_rows = pick_tile_rows(c.vocab_size, num_sms);
-            if (lm_head) tm_lm = tc::make_tmap_bf16(lm_head, c.vocab_size, H, lm_tile_rows);
-            tmx_xn = tc::make_tmap_bf16(xn.p, R16, H, 16);
-            tmx_attn = tc::make_tmap_bf16(attn.p, R16, NQ, 16);
-            tmx_act = tc::make_tmap_bf16(act.p, R16, I, 16);
+            tm_down.push_back(tc::make_tmap_bf16(L.wdown.p, H, I, tc::BM));
         }
+        lm_tile_rows = pick_tile_rows(c.vocab_size, num_sms);
+        if (lm_head) tm_lm = tc::make_tmap_bf16(lm_head, c.vocab_size, H, lm_tile_rows);
+        tmx_xn = tc::make_tmap_bf16(xn.p, R16, H, 16);
+        tmx_attn = tc::make_tmap_bf16(attn.p, R16, NQ, 16);
+        tmx_act = tc::make_tmap_bf16(act.p, R16, I, 16);
         B2A_CUDA(cudaDeviceSynchronize());
     }
 
@@ -1232,46 +1119,7 @@ struct b2a_tts {
         alloc_state();
     }
 
-    template <int NB, int ROWS, int EPI>
-    void gemv_launch(const bf16* W, const bf16* xin, float* yout, bf16* actout, int N, int K, int warps, int ksplit,
-                     cudaStream_t s) {
-        const size_t sm = (size_t)2 * NB * (K / ksplit) * sizeof(bf16);
-        dim3 grid(cdiv(N, warps * ROWS), ksplit);
-        launch_pdl(gemv_bf16_kernel<NB, ROWS, EPI>, grid, dim3(warps * 32), sm, s, W, xin, yout, actout, N, K);
-    }
-    template <int NB, int ROWS, int EPI>
-    static void gemv_attr() {
-        B2A_CUDA(cudaFuncSetAttribute(gemv_bf16_kernel<NB, ROWS, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    }
-    template <int NB>
-    static void gemv_attrs() {
-        gemv_attr<NB, 2, GV_F32>(); gemv_attr<NB, 2, GV_SWIGLU>(); gemv_attr<NB, 2, GV_F32_ATOMIC>();
-    }
-    enum { OP_QKV, OP_O, OP_GU, OP_DOWN, OP_LM };
-    template <int NB>
-    void gemv_op(int op, const bf16* W, const bf16* xin, float* yout, bf16* actout, int N, int K, cudaStream_t s) {
-        const bool split = (K / 8) % 2 == 0 && (size_t)2 * NB * K * sizeof(bf16) > 96 * 1024;
-        switch (op) {
-            case OP_GU: gemv_launch<NB, 2, GV_SWIGLU>(W, xin, yout, actout, N, K, 8, 1, s); break;
-            case OP_DOWN:
-            case OP_O:
-                if (split) gemv_launch<NB, 2, GV_F32_ATOMIC>(W, xin, yout, actout, N, K, 4, 2, s);
-                else gemv_launch<NB, 2, GV_F32>(W, xin, yout, actout, N, K, 4, 1, s);
-                break;
-            default: gemv_launch<NB, 2, GV_F32>(W, xin, yout, actout, N, K, 8, 1, s); break;
-        }
-    }
-    void gemv_nb(int op, const bf16* W, const bf16* xin, float* yout, bf16* actout, int N, int K, cudaStream_t s) {
-        B2A_CHECK((size_t)2 * nb_pad * K * sizeof(bf16) <= 200 * 1024 * ((op == OP_DOWN || op == OP_O) ? 2 : 1),
-                  B2A_ERR_INVALID_INPUT, "llama: layer too wide for the shared-memory activation tile");
-        switch (nb_pad) {
-            case 1: gemv_op<1>(op, W, xin, yout, actout, N, K, s); break;
-            case 2: gemv_op<2>(op, W, xin, yout, actout, N, K, s); break;
-            case 4: gemv_op<4>(op, W, xin, yout, actout, N, K, s); break;
-            default: gemv_op<8>(op, W, xin, yout, actout, N, K, s); break;
-        }
-    }
-
+    enum { OP_QKV, OP_GU, OP_LM };
     // D[tokens, M] = X[tokens, K] * W[M, K]^T on the wgmma path (hi/lo activations, BN = 16)
     void tc_gemm(const CUtensorMap& tmW, const CUtensorMap& tmX, int op, float* yout, bf16* actout, int B, int M, int K,
                  cudaStream_t s, const float* rstd_ss = nullptr) {
@@ -1290,40 +1138,12 @@ struct b2a_tts {
             a.ldo = M; a.epi_full = tc::EPI_STORE; a.epi_partial = -1; a.lo_rows = 0;
             a.tile_rows = head_rows_now > 0 ? head_rows_now : lm_tile_rows; a.m_tiles = cdiv(M, a.tile_rows);
             ctas = std::min(num_sms, a.m_tiles);
-        } else {   // qkv / o / down: stream-K, partial tiles summed in slot order and stored into the fp32 output
+        } else {   // OP_QKV when its clusters do not fit (qkv_gemm): stream-K, partial tiles summed in slot order and stored
             a.ldo = M; a.epi_full = tc::EPI_STORE; a.epi_partial = tc::EPI_PARTIAL; a.lo_rows = 0;
             ctas = (int)std::min<long long>(num_sms, (long long)a.m_tiles * a.k_blocks);
             a.part_ws = sk_ws.p; a.part_cnt = sk_cnt.p; a.part_slots = sk_slots;
         }
         tc::launch<16>(tmW, tmX, a, ctas, 1, s);
-    }
-
-    void gemm(int op, int layer, int B, cudaStream_t s) {
-        const int H = cfg.hidden_size, I = cfg.intermediate_size, NQ = cfg.num_attention_heads * HD,
-                  NKV = cfg.num_key_value_heads * HD;
-        LayerW* L = layer >= 0 ? &layers[layer] : nullptr;
-        switch (op) {
-            case OP_QKV:
-                if (use_tc) tc_gemm(tm_qkv[layer], tmx_xn, op, qkv.p, nullptr, B, NQ + 2 * NKV, H, s);
-                else gemv_nb(op, L->wqkv.p, xn.p, qkv.p, nullptr, NQ + 2 * NKV, H, s);
-                break;
-            case OP_O:
-                if (use_tc) tc_gemm(tm_o[layer], tmx_attn, op, y.p, nullptr, B, H, NQ, s);
-                else gemv_nb(op, L->wo.p, attn.p, y.p, nullptr, H, NQ, s);
-                break;
-            case OP_GU:
-                if (use_tc) tc_gemm(tm_gu_dec[layer], tmx_xn, op, nullptr, act.p, B, 2 * I, H, s);
-                else gemv_nb(op, L->wgu.p, xn.p, nullptr, act.p, 2 * I, H, s);
-                break;
-            case OP_DOWN:
-                if (use_tc) tc_gemm(tm_down[layer], tmx_act, op, y.p, nullptr, B, H, I, s);
-                else gemv_nb(op, L->wdown.p, act.p, y.p, nullptr, H, I, s);
-                break;
-            default:
-                if (use_tc) tc_gemm(tm_lm, tmx_xn, op, logits.p, nullptr, B, cfg.vocab_size, H, s);
-                else gemv_nb(op, lm_head, xn.p, logits.p, nullptr, cfg.vocab_size, H, s);
-                break;
-        }
     }
 
     // o_proj / down_proj as a cluster split-K GEMM with the residual add and the next norm fused into the leader's epilogue
@@ -1359,13 +1179,14 @@ struct b2a_tts {
     // The fused-norm step: embed -> raw norm -> L x [qkv gemm (rstd in the epilogue) -> attention -> o split-K (+ residual, norm 2)
     // -> gate/up gemm (rstd, SwiGLU) -> down split-K (+ residual, next layer's norm 1 / the final norm)].  Leaves the residual
     // stream in x, xn = hi/lo of x * final_norm_gain and its sums of squares in ss_b: the lm head GEMM applies rstd itself.
-    void run_layers_fused(int B, cudaStream_t s) {
+    void run_layers(int B, cudaStream_t s) {
         const int H = cfg.hidden_size, I = cfg.intermediate_size, nq = cfg.num_attention_heads, nkv = cfg.num_key_value_heads;
         const int NQ = nq * HD, L = cfg.num_hidden_layers;
         if (x_ext) launch_pdl(ext_embed_kernel, dim3(B), dim3(256), 0, s, x_ext, x.p, y.p, H);
         else launch_pdl(embed_kernel, dim3(B), dim3(256), 0, s, tokens.p, embed.p, x.p, y.p, H, cfg.vocab_size);
+        trace_x(0, B, s);
         launch_pdl(add_rmsnorm_kernel, dim3(B), dim3(RN_THREADS), 0, s, x.p, (float*)nullptr, layers[0].ln1.p, xn.p, H, cfg.rms_norm_eps,
-                   (float*)nullptr, LO_ROW, (float*)nullptr, ss_b.p, fused_parts);
+                   LO_ROW, ss_b.p, fused_parts);
         const size_t kv_layer = (size_t)cfg.max_batch * nkv * cfg.max_context * HD;
         for (int l = 0; l < L; ++l) {
             LayerW& Lw = layers[l];
@@ -1374,65 +1195,41 @@ struct b2a_tts {
                         1.0f / sqrtf((float)HD), spec.qk_norm ? Lw.qnorm.p : nullptr, spec.qk_norm ? Lw.knorm.p : nullptr, cfg.rms_norm_eps};
             attn_launch(aa, B, s);
             splitk_gemm(tm_o[l], tmx_attn, H, NQ, Lw.ln2.p, ss_a.p, B, s);
+            trace_x(2 * l + 1, B, s);
             tc_gemm(tm_gu_dec[l], tmx_xn, OP_GU, nullptr, act.p, B, 2 * I, H, s, ss_a.p);
             splitk_gemm(tm_down[l], tmx_act, H, I, l + 1 < L ? layers[l + 1].ln1.p : final_ln.p, ss_b.p, B, s);
+            trace_x(2 * l + 2, B, s);
         }
     }
-    int launches_layers_fused() const { return 2 + cfg.num_hidden_layers * 5; }
-
-    // embed(tokens) -> all layers; leaves the residual stream in x and the last MLP output in y
-    void run_layers(int B, cudaStream_t s) {
-        if (fused && !trace_on) { run_layers_fused(B, s); return; }
-        const int H = cfg.hidden_size, nq = cfg.num_attention_heads, nkv = cfg.num_key_value_heads;
-        const int G = nq / nkv;
-        if (x_ext) launch_pdl(ext_embed_kernel, dim3(B), dim3(256), 0, s, x_ext, x.p, y.p, H);
-        else launch_pdl(embed_kernel, dim3(B), dim3(256), 0, s, tokens.p, embed.p, x.p, y.p, H, cfg.vocab_size);
-        const size_t kv_layer = (size_t)cfg.max_batch * nkv * cfg.max_context * HD;
-        for (int l = 0; l < cfg.num_hidden_layers; ++l) {
-            LayerW& L = layers[l];
-            launch_pdl(add_rmsnorm_kernel, dim3(B), dim3(RN_THREADS), 0, s, x.p, l == 0 ? (float*)nullptr : y.p, L.ln1.p, xn.p, H,
-                       cfg.rms_norm_eps, trace_on ? trace.p + (size_t)(2 * l) * 8 * H : (float*)nullptr, LO_ROW,
-                       (float*)nullptr, (float*)nullptr, 0);
-            gemm(OP_QKV, l, B, s);
-            AttnArgs aa{qkv.p, pos.p, freqs.p, kcache.p + l * kv_layer, vcache.p + l * kv_layer, attn.p, nq, nkv, cfg.max_context,
-                        1.0f / sqrtf((float)HD), spec.qk_norm ? L.qnorm.p : nullptr, spec.qk_norm ? L.knorm.p : nullptr, cfg.rms_norm_eps};
-            attn_launch(aa, B, s);
-            gemm(OP_O, l, B, s);
-            launch_pdl(add_rmsnorm_kernel, dim3(B), dim3(RN_THREADS), 0, s, x.p, y.p, L.ln2.p, xn.p, H, cfg.rms_norm_eps,
-                       trace_on ? trace.p + (size_t)(2 * l + 1) * 8 * H : (float*)nullptr, LO_ROW, (float*)nullptr, (float*)nullptr, 0);
-            gemm(OP_GU, l, B, s);
-            gemm(OP_DOWN, l, B, s);
-        }
-        (void)G;
+    int launches_layers() const { return 2 + cfg.num_hidden_layers * 5; }
+    // b2a_tts_debug_trace: the residual stream x [B, H] into slot i of the record, i.e. the input of the i-th RMSNorm.  Tracing is
+    // for eager forwards (b2a_tts_forward_logits); tts_generate_impl turns it off before it captures its graphs
+    void trace_x(int i, int B, cudaStream_t s) {
+        if (trace_on)
+            B2A_CUDA(cudaMemcpyAsync(trace.p + (size_t)i * 8 * cfg.hidden_size, x.p, (size_t)B * cfg.hidden_size * sizeof(float),
+                                     cudaMemcpyDeviceToDevice, s));
     }
 
+    // x, xn (un-normalised) and ss_b are final after run_layers: only row N1 needs the fp32 normalised hidden state
     void run_final_norm(int B, cudaStream_t s) {
-        if (fused && !trace_on) {   // x, xn (un-normalised) and ss_b are already final: only row N1 needs the fp32 normalised hidden
-            if (normed_out)
-                launch_pdl(finalize_norm_kernel, dim3(B), dim3(256), 0, s, (const float*)x.p, (const float*)final_ln.p, (const float*)ss_b.p, fused_parts,
-                           normed_out, cfg.hidden_size, cfg.rms_norm_eps);
-            return;
-        }
-        launch_pdl(add_rmsnorm_kernel, dim3(B), dim3(RN_THREADS), 0, s, x.p, y.p, final_ln.p, xn.p, cfg.hidden_size, cfg.rms_norm_eps,
-                   trace_on ? trace.p + (size_t)(2 * cfg.num_hidden_layers) * 8 * cfg.hidden_size : (float*)nullptr, LO_ROW,
-                   normed_out, (float*)nullptr, 0);
+        if (normed_out)
+            launch_pdl(finalize_norm_kernel, dim3(B), dim3(256), 0, s, (const float*)x.p, (const float*)final_ln.p, (const float*)ss_b.p, fused_parts,
+                       normed_out, cfg.hidden_size, cfg.rms_norm_eps);
     }
     void run_lm_head(int B, cudaStream_t s) {
         run_final_norm(B, s);
-        if (fused && !trace_on) tc_gemm(tm_lm, tmx_xn, OP_LM, logits.p, nullptr, B, cfg.vocab_size, cfg.hidden_size, s, ss_b.p);
-        else gemm(OP_LM, -1, B, s);
+        tc_gemm(tm_lm, tmx_xn, OP_LM, logits.p, nullptr, B, cfg.vocab_size, cfg.hidden_size, s, ss_b.p);
     }
-    // after prefill_batched's gather_last (x, y hold the last position un-added): always the stand-alone norm + plain GEMM
+    // after prefill_batched's gather_last (x, y hold the last position un-added): the stand-alone norm + plain GEMM
     void run_lm_head_after_prefill(int B, cudaStream_t s) {
         launch_pdl(add_rmsnorm_kernel, dim3(B), dim3(RN_THREADS), 0, s, x.p, y.p, final_ln.p, xn.p, cfg.hidden_size, cfg.rms_norm_eps,
-                   (float*)nullptr, LO_ROW, (float*)nullptr, (float*)nullptr, 0);
-        gemm(OP_LM, -1, B, s);
+                   LO_ROW, (float*)nullptr, 0);
+        tc_gemm(tm_lm, tmx_xn, OP_LM, logits.p, nullptr, B, cfg.vocab_size, cfg.hidden_size, s);
     }
-    // a head the caller owns (row N1: the code predictor's 15 lm heads): logits_out[b, :M] = W[M, H] * normed hidden
-    void run_head(const CUtensorMap& tmW, const bf16* W, int M, float* logits_out, int B, cudaStream_t s, int tile_rows = 0) {
+    // a head the caller owns (row N1: the code predictor's 15 lm heads): logits_out[b, :M] = W[M, H] * normed hidden, tmW a map of W
+    void run_head(const CUtensorMap& tmW, int M, float* logits_out, int B, cudaStream_t s, int tile_rows = 0) {
         head_rows_now = tile_rows;              // tmW's box rows (0: this stack's own lm_tile_rows)
-        if (use_tc) tc_gemm(tmW, tmx_xn, OP_LM, logits_out, nullptr, B, M, cfg.hidden_size, s, (fused && !trace_on) ? ss_b.p : nullptr);
-        else gemv_nb(OP_LM, W, xn.p, logits_out, nullptr, M, cfg.hidden_size, s);
+        tc_gemm(tmW, tmx_xn, OP_LM, logits_out, nullptr, B, M, cfg.hidden_size, s, ss_b.p);
         head_rows_now = 0;
     }
     // logits are [8, V] row-major.
@@ -1449,7 +1246,7 @@ struct b2a_tts {
     // what they were), the wgmma kernel beyond
     bool simt_prompt_attn(int L) const { return L <= PA_MAXL && pattn_smem(L) <= 220 * 1024; }
     bool can_batch_prefill(int L) const {
-        return use_tc && use_batched_prefill && spec.has_embed && !spec.qk_norm && L >= 2 && L <= cfg.max_context;
+        return use_batched_prefill && spec.has_embed && !spec.qk_norm && L >= 2 && L <= cfg.max_context;
     }
 
     // D[T, M] = X[T, K] W^T for all prompt tokens: 128-column tiles (64 tokens as hi/lo), CTAs own whole tiles
@@ -1500,7 +1297,7 @@ struct b2a_tts {
         for (int l = 0; l < cfg.num_hidden_layers; ++l) {
             LayerW& Lw = layers[l];
             launch_pdl(add_rmsnorm_kernel, dim3(T), dim3(RN_THREADS), 0, s, xp.p, l == 0 ? (float*)nullptr : yp.p, Lw.ln1.p, xnp.p, H,
-                       cfg.rms_norm_eps, (float*)nullptr, PF_HALF, (float*)nullptr, (float*)nullptr, 0);
+                       cfg.rms_norm_eps, PF_HALF, (float*)nullptr, 0);
             pf_gemm(tm_qkv[l], tmp_xn, tc::EPI_STORE, qkvp.p, nullptr, T, QKV_N, H, s);
             if (simt_attn) {
                 PrefillAttnArgs pa{qkvp.p, rope_tab.p, kcache.p + l * kv_layer, vcache.p + l * kv_layer, attnp.p, nq, nkv,
@@ -1520,8 +1317,8 @@ struct b2a_tts {
                 pfa_ops.run(qkvp.p, rope_tab.p, kcache.p + l * kv_layer, vcache.p + l * kv_layer, attnp.p, L, cfg.max_context, s);
             }
             pf_gemm(tm_o[l], tmp_attn, tc::EPI_STORE, yp.p, nullptr, T, H, NQ, s);
-            launch_pdl(add_rmsnorm_kernel, dim3(T), dim3(RN_THREADS), 0, s, xp.p, yp.p, Lw.ln2.p, xnp.p, H, cfg.rms_norm_eps,
-                       (float*)nullptr, PF_HALF, (float*)nullptr, (float*)nullptr, 0);
+            launch_pdl(add_rmsnorm_kernel, dim3(T), dim3(RN_THREADS), 0, s, xp.p, yp.p, Lw.ln2.p, xnp.p, H, cfg.rms_norm_eps, PF_HALF,
+                       (float*)nullptr, 0);
             pf_gemm(tm_gu[l], tmp_xn, tc::EPI_SWIGLU, nullptr, actp.p, T, 2 * I, H, s);
             pf_gemm(tm_down[l], tmp_act, tc::EPI_STORE, yp.p, nullptr, T, H, I, s);
         }
@@ -1563,8 +1360,8 @@ struct b2a_tts {
         B2A_CUDA(cudaGraphInstantiate(&g_prefill, g, 0));
         cudaGraphDestroy(g);
         g_nb = B; g_args = sa; g_L = L;
-        launches_step = fused ? launches_layers_fused() + 1 + 1 : 1 + cfg.num_hidden_layers * 7 + 2 + 1;
-        launches_prefill = fused ? launches_layers_fused() + 1 : 1 + cfg.num_hidden_layers * 7 + 1;
+        launches_step = launches_layers() + 1 + 1;
+        launches_prefill = launches_layers() + 1;
     }
     int g_L = 0, launches_step = 0, launches_prefill = 0;
 };
@@ -1650,7 +1447,7 @@ static void tts_generate_impl(b2a_tts* h, const int32_t* input_ids, bool ids_on_
                                       h->recent_n.p, h->n_gen.p, h->done.p, h->n_active.p, 0);
     count_launch();
     // prefill.  Batched: every prompt token through each layer at once (wgmma GEMMs, 64 tokens per tile), then
-    // lm head + sampler on the last position.  Fallback (B2A_PREFILL=step, SIMT mode, q/k norm): replay the decode
+    // lm head + sampler on the last position.  Fallback (B2A_PREFILL=step, q/k norm): replay the decode
     // step per position -- positions 0..L-2 need no logits, position L-1 runs the full step.
     int steps = 0;
     if (h->can_batch_prefill(L)) {
@@ -1983,8 +1780,6 @@ int32_t b2a_tts_prepare_input_ids_ref(const int32_t* const* prompt_ids, const in
     });
 }
 
-// Debug / parity hook: residual stream seen by every RMSNorm (2 per layer + final) for the LAST position of
-// the last b2a_tts_forward_logits call made while tracing was enabled; out is [2*layers+1, batch, hidden].
 int32_t b2a_debug_step_smem(int32_t gqa, int32_t* out) {
     return guarded([&] {
         B2A_CHECK(out && (gqa == 1 || gqa == 2 || gqa == 3 || gqa == 4 || gqa == 6 || gqa == 8), B2A_ERR_INVALID_INPUT,
@@ -2031,6 +1826,8 @@ int32_t b2a_prompt_attn_test(const float* qkv, const float* freqs, float* kcache
     });
 }
 
+// Debug / parity hook: residual stream seen by every RMSNorm (2 per layer + final) for the LAST position of
+// the last b2a_tts_forward_logits call made while tracing was enabled; out is [2*layers+1, batch, hidden].
 int32_t b2a_tts_debug_trace(b2a_tts* h, int32_t enable, int32_t batch, float* out) {
     return guarded([&] {
         B2A_CHECK(h, B2A_ERR_INVALID_INPUT, "b2a_tts_debug_trace: null handle");
@@ -2347,11 +2144,9 @@ struct b2a_qwen3_talker {
         std::vector<const bf16*> ptrs;
         for (auto& e : cp_emb) ptrs.push_back(e.p);
         cp_emb_ptrs.upload(ptrs.data(), ptrs.size());
-        if (pred->use_tc) {
-            tm_cp_head.clear();
-            cp_head_rows = b2a_tts::pick_tile_rows(cfg.cp_vocab_size, pred->num_sms);
-            for (auto& hd : cp_head) tm_cp_head.push_back(tc::make_tmap_bf16(hd.p, cfg.cp_vocab_size, Hh, cp_head_rows));
-        } else tm_cp_head.resize(cp_head.size());
+        tm_cp_head.clear();
+        cp_head_rows = b2a_tts::pick_tile_rows(cfg.cp_vocab_size, pred->num_sms);
+        for (auto& hd : cp_head) tm_cp_head.push_back(tc::make_tmap_bf16(hd.p, cfg.cp_vocab_size, Hh, cp_head_rows));
         talker->x_ext = x_in.p; talker->normed_out = hid.p;
         pred->x_ext = px.p;
         talker->set_batch(8); pred->set_batch(8);
@@ -2458,7 +2253,7 @@ struct b2a_qwen3_talker {
             else launch_pdl(q3_gather_kernel, dim3(B), dim3(256), 0, s, (const bf16*)cp_emb[k - 1].p, cfg.cp_vocab_size, (const int*)codes.p, G(), k, px.p, H(), pred->pos.p, k + 1);
             pred->run_layers(B, s);
             pred->run_final_norm(B, s);
-            pred->run_head(tm_cp_head[k], cp_head[k].p, cfg.cp_vocab_size, pred->logits.p, B, s, cp_head_rows);
+            pred->run_head(tm_cp_head[k], cfg.cp_vocab_size, pred->logits.p, B, s, cp_head_rows);
             q3s::Args a = sampler_args(p, false, k + 1);
             a.tokens = codes.p + (k + 1); a.tokens_stride = G();
             q3s::launch(a, B, s);

@@ -154,20 +154,6 @@ def test_end_to_end_tokens_to_waveform_and_errors(b2a):
     assert all(len(t) <= 5 for t in toks3)
 
 
-def test_simt_fallback_matches_wgmma_path(b2a, tiny, monkeypatch):
-    """B2A_GEMM=simt selects the CUDA-core GEMV fallback (same hi/lo numerics): both paths agree to fp32 noise."""
-    cfg, W, m = tiny
-    ids = np.random.default_rng(17).integers(0, 2048, size=(3, 9)).astype(np.int32)
-    a = m(ids)
-    monkeypatch.setenv("B2A_GEMM", "simt")
-    m2 = b2a.LlamaTTSModel(hf_config(cfg), W, max_batch=4, max_context=64)
-    monkeypatch.delenv("B2A_GEMM")
-    b = m2(ids)
-    assert rel_err(b, a) < 3e-5                                   # the fused-norm step applies rstd behind the GEMM: fp32 rounding differs
-    ref = ol.LlamaOracle(cfg, W, round_acts=False).forward(torch.as_tensor(ids)).numpy()
-    assert rel_err(b, ref) < 1e-4
-
-
 def test_long_context_attention_splits(b2a):
     """Context over many 64-key attention chunks against the oracle: positions on both sides of chunk boundaries, where the
     chunks alternate between the two CTAs of the cluster and their softmax states are merged."""
@@ -190,8 +176,8 @@ LONG_CONTEXT_HEADS = [(128, 1, 1), (128, 2, 1), (128, 4, 1), (128, 6, 1), (128, 
 def test_long_context_attention_every_gqa_ratio(b2a, hidden, nq, nkv):
     """test_long_context_attention_splits for the other GQA ratios.  330 positions (more than one prompt tile of 128) go through the
     decode step one position at a time, so each runs attn_decode_cluster_kernel<G>; at G = 8 the K/V ring is 2 chunks deep and
-    wraps many times.  Hidden 192 is not a multiple of 128, which selects the unfused step (stand-alone RMSNorm kernels, stream-K
-    o_proj / down_proj)."""
+    wraps many times.  Hidden 192 is not a multiple of 128: the fused step's last m-tile of o_proj / down_proj is half filled, and
+    its partial sums of squares cover those 64 rows only."""
     cfg = ol.LlamaConfig(hidden_size=hidden, num_hidden_layers=1, intermediate_size=256, num_attention_heads=nq,
                          num_key_value_heads=nkv, head_dim=128, vocab_size=512)
     W = ol.init_weights(cfg, 5, std=0.1)
@@ -201,6 +187,44 @@ def test_long_context_attention_every_gqa_ratio(b2a, hidden, nq, nkv):
     ref = ol.LlamaOracle(cfg, W, round_acts=False).forward(torch.as_tensor(ids)).numpy()
     for pos in (0, 63, 64, 65, 127, 128, 143, 144, 145, 191, 192, 255, 256, 287, 288, 329):
         assert rel_err(lg[:, pos], ref[:, pos]) < 1e-4, pos
+
+
+@pytest.mark.parametrize("hidden", [256, 192])
+def test_debug_trace_matches_oracle_residual_stream(b2a, hidden):
+    """b2a_tts_debug_trace (tools/diag_llama.py): the residual stream of the last position at every RMSNorm input -- the embedding,
+    then after each layer's o_proj and down_proj, the last being the final norm's input -- as the fused step leaves it in x.  Hidden
+    192 has a half-filled last m-tile."""
+    cfg = ol.LlamaConfig(**{**TINY, "hidden_size": hidden})
+    W = ol.init_weights(cfg, 1234, std=0.08)
+    m = b2a.LlamaTTSModel(hf_config(cfg), W, max_batch=8, max_context=64)
+    ids = np.random.default_rng(3).integers(0, 2048, size=(2, 12)).astype(np.int32)
+    for L in (1, 12):
+        m.debug_trace(True)
+        lg = m(ids[:, :L])
+        tr = m.debug_trace(False, batch=2, read=True)
+        ref_tr = []
+        ref = ol.LlamaOracle(cfg, W, round_acts=False).forward(torch.as_tensor(ids[:, :L], dtype=torch.long), trace=ref_tr).numpy()
+        assert len(ref_tr) == tr.shape[0] == 2 * cfg.num_hidden_layers + 1
+        for i, t in enumerate(ref_tr):
+            assert rel_err(tr[i], t.numpy()) < 1e-4, (L, i, rel_err(tr[i], t.numpy()))
+        assert rel_err(lg, ref) < 1e-4, (L, rel_err(lg, ref))
+
+
+@pytest.mark.parametrize("hidden,inter", [(200, 512), (256, 520)], ids=["hidden200", "intermediate520"])
+def test_widths_off_the_64_grid_are_rejected_at_creation(b2a, hidden, inter):
+    """Every GEMM of the Llama and Qwen3 stacks takes K in whole 64-wide k-blocks, so other widths fail at creation, as Whisper's do
+    (both constructors of each handle run the same check before touching the weights)."""
+    llama = {**hf_config(ol.LlamaConfig(**TINY)), "hidden_size": hidden, "intermediate_size": inter}
+    with pytest.raises(b2a.AudioGenerationError) as e:
+        b2a.LlamaTTSModel.random_init(llama, max_batch=2, max_context=64)
+    assert e.value.case == "invalidInput" and "multiple of 64" in e.value.message
+    cp = b2a.Qwen3CodePredictorConfig(vocab_size=2048, hidden_size=hidden, intermediate_size=inter, num_hidden_layers=2,
+                                      num_attention_heads=2, num_key_value_heads=1, num_code_groups=4)
+    talker = b2a.Qwen3TalkerConfig(vocab_size=3072, hidden_size=hidden, intermediate_size=inter, num_hidden_layers=2, num_attention_heads=2,
+                                   num_key_value_heads=1, num_code_groups=4, text_hidden_size=128, text_vocab_size=200, code_predictor=cp)
+    with pytest.raises(b2a.AudioGenerationError) as e:
+        b2a.Qwen3TTSTalker.random_init(talker, max_batch=2, max_context=64)
+    assert e.value.case == "invalidInput" and "multiple of 64" in e.value.message
 
 
 # (B, L, q heads, kv heads).  The batched prompt pass runs when its attention tile fits: 1024 L + 16384 G bytes <= 220 KB, so

@@ -6,7 +6,7 @@ b2a_tc_gemm_splitk_store_test).  Each CTA of a tile's cluster streams the piece 
 
 is bit-identical to the stream-K launch, and within float64 bounds; rows t >= N of out are untouched.  Also: the launch plan the
 engine picks (one CTA per piece, all clusters resident at once), its neighbours in the step fitting on one SM, and the stream-K
-GEMM (the fallback, and the non-fused trace path) storing into an output that was not zeroed first."""
+GEMM (the fallback) storing into an output that was not zeroed first."""
 import ctypes as C
 
 import numpy as np
@@ -127,7 +127,7 @@ def test_qkv_neighbours_fit_on_one_sm(b2a, G):
 
 def test_streamk_store_needs_no_zeroed_output(b2a):
     """Stream-K with EPI_STORE: the CTA that completes a tile stores the sum of its partials, so the output may hold anything before
-    (the step's stream-K fallback and the trace path no longer clear q|k|v)."""
+    (the step's stream-K fallback does not clear q|k|v)."""
     M, K, N = 512, 256, 8
     g = torch.Generator(device="cuda").manual_seed(5)
     W = (torch.randn(M, K, device="cuda", generator=g) * 0.02).to(torch.bfloat16)
@@ -140,8 +140,8 @@ def test_streamk_store_needs_no_zeroed_output(b2a):
 
 
 def test_trace_after_fused_steps_matches_oracle(b2a):
-    """The fused step leaves q|k|v holding the last layer's projection; a traced (non-fused, stream-K) forward after it must not
-    add onto it."""
+    """The fused step leaves q|k|v holding the last layer's projection; a traced forward after it (the same step, recording the
+    residual stream) must not add onto it."""
     cfg = ol.LlamaConfig(hidden_size=256, num_hidden_layers=2, intermediate_size=512, num_attention_heads=2, num_key_value_heads=1,
                          head_dim=128, vocab_size=512)
     W = ol.init_weights(cfg, 3, std=0.05)
