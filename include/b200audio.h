@@ -354,8 +354,13 @@ void b2a_vocos_destroy(b2a_vocos* h);
  * time), audio_scales [n_chunks, B] float32 or NULL (nil scales); the waveform is [B, samples, audio_channels] with
  * samples = b2a_encodec_output_length(n_chunks, T) (T*hop un-chunked; stride*(n_chunks-1) + T*hop with linearOverlapAdd).
  * The padding-mask truncation (:397-399) is a host-side slice of the result.  The reference's fatalError on
- * "Expected one frame" (:375-377) is B2A_ERR_AUDIO_DECODING_FAILED here.  Only norm_type "weight_norm" (plain folded
- * conv weights, no norm layer: EncodecLayers.swift:133-137) is implemented; "time_group_norm" -> invalidInput. */
+ * "Expected one frame" (:375-377) is B2A_ERR_AUDIO_DECODING_FAILED here.  norm_type 0 is "weight_norm" (plain folded conv
+ * weights, no norm layer: EncodecLayers.swift:133-137); 1 is "time_group_norm" (the 48 kHz stereo model): plain conv weights,
+ * each conv followed by GroupNorm(1, C_out) with eps 1e-5 whose affine is the checkpoint's <conv prefix>norm.weight / norm.bias
+ * [C_out] (EncodecLayers.swift:128-132, 244-248); statistics are per chunk and clip, so no output is causal.  Any other value
+ * is B2A_ERR_INVALID_INPUT, and so is norm_type 1 over a checkpoint with no norm layers (no decoder.layers.0.norm.weight):
+ * config.json does not describe those weights.  A checkpoint with norm layers that lacks one of them is
+ * B2A_ERR_MODEL_NOT_INITIALIZED naming the tensor (stricter than the reference's loader, which would keep gamma 1, beta 0). */
 typedef struct b2a_encodec_config {
     int32_t audio_channels;
     int32_t num_filters;
@@ -369,7 +374,7 @@ typedef struct b2a_encodec_config {
     int32_t residual_kernel_size;
     int32_t use_causal_conv;
     int32_t pad_mode_reflect;       /* 1 = "reflect" (clamped indices, EncodecLayers.swift:160-186), 0 = zero padding */
-    int32_t norm_type;              /* 0 = weight_norm; anything else -> invalidInput */
+    int32_t norm_type;              /* 0 = weight_norm, 1 = time_group_norm; anything else -> invalidInput */
     int32_t last_kernel_size;
     int32_t compress;
     int32_t n_upsampling_ratios;

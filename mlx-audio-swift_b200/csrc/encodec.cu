@@ -23,6 +23,12 @@
 //     the 2s contiguous input rows of an output (src = q*s + tap - padL), the right padding through the same edge rule.  New
 //     kernels sit only at the edges: the stem from 1-2 audio channels (reading each chunk of the waveform in place), the
 //     per-chunk RMS scale, and the residual code search in ordered fp32 (DESIGN.md §3.6b).
+//   * norm_type time_group_norm (the 48 kHz stereo model; EncodecLayers.swift:128-132, 244-248) puts a GroupNorm(1, C_out) after
+//     every conv.  Each such conv is its usual launch followed by gn_stats_kernel (per-row mean / rstd over all T x C_out
+//     elements, so every chunk of every clip has its own) and gn_apply_kernel.  The transposed conv writes its untrimmed output
+//     and the apply trims (the reference norms before the trim); the resnet's shortcut and block.3 run as two GEMMs whose normed
+//     outputs one apply sums; the decoder's last apply carries the chunk scale.  The norm affines are required: a checkpoint with
+//     norm layers that lacks one is modelNotInitialized, where the reference's loader would keep gamma = 1, beta = 0.
 #include "common.cuh"
 #include "seanet.cuh"
 
@@ -287,6 +293,111 @@ __global__ void __launch_bounds__(256) chunk_scale_kernel(const float* __restric
     if (threadIdx.x == 0) scale[n] = (float)sqrt(red[0] / (double)Lc) + 1e-8f;
 }
 
+// ================================================================== time_group_norm (GroupNorm(1, C) after every conv)
+// Statistics of batch row n over all E = rows * C contiguous elements of x [N, rows, C]: GN_PARTS(E) CTAs per row each sum a
+// fixed slice in double (thread t takes elements t, t + 256, ...; a fixed tree across the CTA), and the row's last CTA to finish
+// combines the partials in index order into stats[n] = (mean, rstd).  The slices depend on E only, so a row's statistics do not
+// depend on how many rows share the launch: batched == serial bit for bit.  cnt[n] is zero before a launch and after it.
+constexpr int GN_SLICE = 16384, GN_MAX_PARTS = 2048;
+inline int gn_parts(long long E) { return (int)std::min<long long>(std::max<long long>((E + GN_SLICE - 1) / GN_SLICE, 1), GN_MAX_PARTS); }
+
+__global__ void __launch_bounds__(256) gn_stats_kernel(const float* __restrict__ x, long long E, double2* __restrict__ part,
+                                                       unsigned* __restrict__ cnt, float2* __restrict__ stats, float eps) {
+    __shared__ double rs[256], rq[256];
+    __shared__ bool last;
+    const int n = blockIdx.y, p = blockIdx.x, P = gridDim.x, tid = threadIdx.x;
+    const long long slice = (E + P - 1) / P, e0 = (long long)p * slice, e1 = min(E, e0 + slice);
+    const float* xn = x + (long long)n * E;
+    double s = 0.0, q = 0.0;
+    long long e = e0 + tid;
+    for (; e + 3 * 256 < e1; e += 4 * 256) {      // four loads in flight per thread; the same per-thread order as one at a time
+        const float v0 = xn[e], v1 = xn[e + 256], v2 = xn[e + 512], v3 = xn[e + 768];
+        s += (double)v0; q += (double)v0 * v0;
+        s += (double)v1; q += (double)v1 * v1;
+        s += (double)v2; q += (double)v2 * v2;
+        s += (double)v3; q += (double)v3 * v3;
+    }
+    for (; e < e1; e += 256) { const double v = xn[e]; s += v; q += v * v; }
+    rs[tid] = s; rq[tid] = q;
+    __syncthreads();
+    for (int o = 128; o; o >>= 1) {
+        if (tid < o) { rs[tid] += rs[tid + o]; rq[tid] += rq[tid + o]; }
+        __syncthreads();
+    }
+    if (tid == 0) {
+        part[(long long)n * P + p] = make_double2(rs[0], rq[0]);
+        __threadfence();
+        last = atomicAdd(cnt + n, 1u) == (unsigned)(P - 1);
+    }
+    __syncthreads();
+    if (!last || tid >= 32) return;
+    __threadfence();
+    // warp 0 of the last CTA: lane l sums partials l, l + 32, ... in order, then a fixed xor tree
+    double S = 0.0, Q = 0.0;
+    for (int i = tid; i < P; i += 32) {
+        const double2 v = __ldcg(part + (long long)n * P + i);
+        S += v.x; Q += v.y;
+    }
+#pragma unroll
+    for (int o = 16; o; o >>= 1) { S += __shfl_xor_sync(0xffffffffu, S, o); Q += __shfl_xor_sync(0xffffffffu, Q, o); }
+    if (tid == 0) {
+        const double mean = S / (double)E, var = fmax(Q / (double)E - mean * mean, 0.0);
+        stats[n] = make_float2((float)mean, (float)(1.0 / sqrt(var + (double)eps)));
+        cnt[n] = 0u;
+    }
+}
+
+// y = GN_a(xa) [+ GN_b(xb) | + xb] [* scale[n]] over out [N, L, C].  xa has rows_a rows per batch row and is read from row off_a
+// on (the transposed conv's left trim); xb is [N, L, C].  GN(x)[c] = (x - mean) * rstd * gamma[c] + beta[c].  VEC: float4 along
+// channels (C % 4 == 0); the scalar path serves the final wave's 1 or 2 channels.  out may be xa (one source, off_a = 0) or xb:
+// every element is read before it is written by the same thread.
+struct GnApplyArgs {
+    const float* xa; const float2* sa; const float* ga; const float* ba; long long rows_a, off_a;
+    const float* xb; const float2* sb; const float* gb; const float* bb;    // sb null: plain addend (identity shortcut)
+    const float* scale;                                                      // [N] or null
+    float* out; long long L; int C;
+};
+
+template <bool VEC>
+__global__ void __launch_bounds__(256) gn_apply_kernel(GnApplyArgs a) {
+    const int n = blockIdx.y;
+    const long long per = a.L * a.C;
+    const long long i = ((long long)blockIdx.x * blockDim.x + threadIdx.x) * (VEC ? 4 : 1);
+    if (i >= per) return;
+    const int c = (int)(i % a.C);
+    const float2 sa = a.sa[n];
+    const float sc = a.scale ? a.scale[n] : 1.f;
+    const float* xa = a.xa + (long long)n * a.rows_a * a.C + a.off_a * a.C + i;
+    const long long o = (long long)n * per + i;
+    if constexpr (VEC) {
+        const float4 v = *reinterpret_cast<const float4*>(xa);
+        const float4 g = *reinterpret_cast<const float4*>(a.ga + c), b = *reinterpret_cast<const float4*>(a.ba + c);
+        float r[4] = {(v.x - sa.x) * sa.y * g.x + b.x, (v.y - sa.x) * sa.y * g.y + b.y,
+                      (v.z - sa.x) * sa.y * g.z + b.z, (v.w - sa.x) * sa.y * g.w + b.w};
+        if (a.xb) {
+            const float4 u = *reinterpret_cast<const float4*>(a.xb + o);
+            float w[4] = {u.x, u.y, u.z, u.w};
+            if (a.sb) {
+                const float2 sb = a.sb[n];
+                const float4 gb = *reinterpret_cast<const float4*>(a.gb + c), bb = *reinterpret_cast<const float4*>(a.bb + c);
+                w[0] = (w[0] - sb.x) * sb.y * gb.x + bb.x; w[1] = (w[1] - sb.x) * sb.y * gb.y + bb.y;
+                w[2] = (w[2] - sb.x) * sb.y * gb.z + bb.z; w[3] = (w[3] - sb.x) * sb.y * gb.w + bb.w;
+            }
+#pragma unroll
+            for (int k = 0; k < 4; ++k) r[k] += w[k];
+        }
+        *reinterpret_cast<float4*>(a.out + o) = make_float4(r[0] * sc, r[1] * sc, r[2] * sc, r[3] * sc);
+    } else {
+        float r = (*xa - sa.x) * sa.y * a.ga[c] + a.ba[c];
+        if (a.xb) {
+            float w = a.xb[o];
+            if (a.sb) { const float2 sb = a.sb[n]; w = (w - sb.x) * sb.y * a.gb[c] + a.bb[c]; }
+            r += w;
+        }
+        a.out[o] = r * sc;
+    }
+}
+
 }  // namespace ec
 }  // namespace b2a
 
@@ -298,10 +409,17 @@ struct EcLstm {
     DBuf<float> Wh[ec::LSTM_MAX_LAYERS], Wx[ec::LSTM_MAX_LAYERS], b[ec::LSTM_MAX_LAYERS];
 };
 
+// a GroupNorm(1, C)'s affine (time_group_norm only)
+struct EcNorm {
+    DBuf<float> g, b;
+};
+
 // an EncodecResnetBlock: r1 = k-tap conv dim -> hid (ELU of its input), r2 = [shortcut | block.3] over K = dim + hid, or
-// block.3 plus the identity residual without a conv shortcut
+// block.3 plus the identity residual without a conv shortcut.  Under time_group_norm the two addends have statistics of their
+// own, so r2 is block.3 alone, sc the shortcut alone, and n1 / n3 / ns the norms after block.1 / block.3 / the shortcut.
 struct EcRes {
-    ec::Conv r1, r2;
+    ec::Conv r1, r2, sc;
+    EcNorm n1, n3, ns;
 };
 
 struct b2a_encodec {
@@ -310,24 +428,34 @@ struct b2a_encodec {
     cudaStream_t stream = nullptr;
     int n_q = 0;
     DBuf<float> books;                       // [n_q][size][dim]
+    bool gn = false;                         // norm_type time_group_norm: a GroupNorm(1, C_out) after every conv
     ec::Conv conv0;
+    EcNorm norm0;
     EcLstm lstm;
-    struct Stage { int ratio, cin, cout, taps; ec::Conv up; EcRes res; };
+    struct Stage { int ratio, cin, cout, taps; ec::Conv up; EcNorm nup; EcRes res; };
     std::vector<Stage> stages;
     DBuf<float> wlast, blast;
+    EcNorm nlast;
     // encoder (only when the checkpoint has encoder.* tensors)
     bool has_enc = false;
     std::string enc_error = "encodec encode: the checkpoint has no encoder weights";
     DBuf<float> wstem, bstem;                // [num_filters, kernel_size, audio_channels]
-    struct EStage { int ratio, cin, cout; EcRes res; ec::Conv down; };
+    EcNorm nstem;
+    struct EStage { int ratio, cin, cout; EcRes res; ec::Conv down; EcNorm ndown; };
     std::vector<EStage> estages;
     EcLstm elstm;
     ec::Conv elast;
+    EcNorm nelast;
     DBuf<float> book_sq;                     // [n_q][size] |e|^2 in search order
     // workspaces
     DBuf<float> bufA, bufB, bufC, xp, hseq[ec::LSTM_MAX_LAYERS], chunks, scales, wave, zbuf, audio;
     DBuf<int> codes;
     DBuf<unsigned> bar;
+    // time_group_norm workspaces: the shortcut's output, per-CTA partial sums, per-row arrival counters, two rows of statistics
+    DBuf<float> bufD;
+    DBuf<double2> gn_part;
+    DBuf<unsigned> gn_cnt;
+    DBuf<float2> gn_sa, gn_sb;
     int dim0 = 0;
 
     static void up(DBuf<float>& d, const std::vector<float>& v) { d.upload(v.data(), v.size()); }
@@ -340,10 +468,23 @@ struct b2a_encodec {
         up(cv.A, tt.f32(p + "conv.weight", (int64_t)cout * k * cin));      // [out, k, in] == [M, tap*Cin + ci]
         up(cv.bias, tt.f32(p + "conv.bias", cout));
     }
+    // GroupNorm affine [C] of the conv at prefix p (time_group_norm only)
+    void load_norm(const TensorTable& tt, EcNorm& nm, const std::string& p, int C) const {
+        if (!gn) return;
+        up(nm.g, tt.f32(p + "norm.weight", C));
+        up(nm.b, tt.f32(p + "norm.bias", C));
+    }
     void load_resnet(const TensorTable& tt, EcRes& r, const std::string& p, int dim) const {
         const int hid = dim / cfg.compress;
         chan_ok(hid);
         plain(tt, r.r1, p + "block.1.", hid, cfg.residual_kernel_size, dim);
+        if (gn) {
+            plain(tt, r.r2, p + "block.3.", dim, 1, hid);
+            load_norm(tt, r.n1, p + "block.1.", hid);
+            load_norm(tt, r.n3, p + "block.3.", dim);
+            if (cfg.use_conv_shortcut) { plain(tt, r.sc, p + "shortcut.", dim, 1, dim); load_norm(tt, r.ns, p + "shortcut.", dim); }
+            return;
+        }
         // second launch: [shortcut | block.3] over K = dim + hid (x raw, hidden through ELU)
         std::vector<float> w1 = tt.f32(p + "block.3.conv.weight", (int64_t)dim * hid), b1 = tt.f32(p + "block.3.conv.bias", dim);
         if (cfg.use_conv_shortcut) {
@@ -379,7 +520,11 @@ struct b2a_encodec {
         cudaDeviceProp prop{};
         B2A_CUDA(cudaGetDeviceProperties(&prop, dev));
         num_sms = prop.multiProcessorCount;
-        B2A_CHECK(c.norm_type == 0, B2A_ERR_INVALID_INPUT, "encodec: only norm_type weight_norm (folded weights) is implemented");
+        B2A_CHECK(c.norm_type == 0 || c.norm_type == 1, B2A_ERR_INVALID_INPUT, "encodec: norm_type must be 0 (weight_norm) or 1 (time_group_norm)");
+        gn = c.norm_type == 1;
+        // config.json does not describe the norm layers: a time_group_norm config over a checkpoint without them is a config error
+        B2A_CHECK(!gn || tt.find("decoder.layers.0.norm.weight"), B2A_ERR_INVALID_INPUT,
+                  "encodec: norm_type time_group_norm but the checkpoint has no norm layers (decoder.layers.0.norm.weight)");
         B2A_CHECK(c.n_upsampling_ratios >= 1 && c.n_upsampling_ratios <= 8, B2A_ERR_INVALID_INPUT, "encodec: bad upsampling_ratios");
         B2A_CHECK(c.num_residual_layers == 1 || c.dilation_growth_rate == 1, B2A_ERR_INVALID_INPUT,
                   "encodec: dilated residual layers change the frame count in the reference (EncodecLayers.swift:117); not implemented");
@@ -403,7 +548,8 @@ struct b2a_encodec {
         int idx = 0;
         auto key = [&](int i, const char* rest) { return "decoder.layers." + std::to_string(i) + "." + rest; };
         dim0 = scaling * c.num_filters;
-        plain(tt, conv0, key(idx, ""), dim0, c.kernel_size, c.hidden_size); ++idx;
+        plain(tt, conv0, key(idx, ""), dim0, c.kernel_size, c.hidden_size);
+        load_norm(tt, norm0, key(idx, ""), dim0); ++idx;
         load_lstm(tt, lstm, key(idx, ""), dim0);
         ++idx;   // the LSTM block occupies a slot even when it has no layers
         for (int i = 0; i < c.n_upsampling_ratios; ++i) {
@@ -429,6 +575,7 @@ struct b2a_encodec {
                     }
                 st.up.M = s * st.cout; st.up.K = st.taps * st.cin;
                 up(st.up.A, A); up(st.up.bias, bb);
+                load_norm(tt, st.nup, key(idx, ""), st.cout);
                 ++idx;
             }
             for (int j = 0; j < c.num_residual_layers; ++j) {
@@ -443,6 +590,7 @@ struct b2a_encodec {
         chan_ok(c.num_filters);
         up(wlast, tt.f32(key(idx, "conv.weight"), (int64_t)c.audio_channels * c.last_kernel_size * c.num_filters));
         up(blast, tt.f32(key(idx, "conv.bias"), c.audio_channels));
+        load_norm(tt, nlast, key(idx, ""), c.audio_channels);
         bar.alloc(1);
         if (tt.find("encoder.layers.0.conv.weight")) {
             // a malformed encoder leaves a working decoder: encode then reports why (B2A_ERR_MODEL_NOT_INITIALIZED)
@@ -461,6 +609,7 @@ struct b2a_encodec {
         int idx = 0;
         up(wstem, tt.f32(key(idx) + "conv.weight", (int64_t)F * k * CH));
         up(bstem, tt.f32(key(idx) + "conv.bias", F));
+        load_norm(tt, nstem, key(idx), F);
         ++idx;
         int scaling = 1;
         for (int i = cfg.n_upsampling_ratios - 1; i >= 0; --i) {
@@ -469,13 +618,15 @@ struct b2a_encodec {
             st.cin = scaling * F; st.cout = 2 * st.cin;
             for (int j = 0; j < cfg.num_residual_layers; ++j) { load_resnet(tt, st.res, key(idx), st.cin); ++idx; }
             ++idx;                                    // ELU slot
-            plain(tt, st.down, key(idx), st.cout, 2 * st.ratio, st.cin); ++idx;
+            plain(tt, st.down, key(idx), st.cout, 2 * st.ratio, st.cin);
+            load_norm(tt, st.ndown, key(idx), st.cout); ++idx;
             estages.push_back(std::move(st));
             scaling *= 2;
         }
         load_lstm(tt, elstm, key(idx), scaling * F); ++idx;
         ++idx;                                        // ELU slot
         plain(tt, elast, key(idx), cfg.hidden_size, cfg.last_kernel_size, scaling * F);
+        load_norm(tt, nelast, key(idx), cfg.hidden_size);
         // |e|^2 of every codebook row, in the search's summation order
         const long long rows = (long long)n_q * cfg.codebook_size;
         book_sq.alloc((size_t)rows);
@@ -512,6 +663,65 @@ struct b2a_encodec {
     void run_resnet(const EcRes& r, float*& x, float*& y, float* z, int N, long long L, int dim, cudaStream_t s) {
         int padL; pads(cfg.residual_kernel_size, padL);
         ec::resnet_block(r.r1, r.r2, cfg.use_conv_shortcut != 0, cfg.residual_kernel_size, padL, cfg.pad_mode_reflect, x, y, z, N, L, dim, s);
+    }
+
+    // ---- time_group_norm: GroupNorm(1, C) with eps 1e-5 (EncodecLayers.swift:128-132, 244-248) as statistics then apply
+    // per-row (mean, rstd) of x [N, rows, C] into st
+    void gn_stats(const float* x, int N, long long rows, int C, float2* st, cudaStream_t s) {
+        const long long E = rows * C;
+        const int P = ec::gn_parts(E);
+        gn_part.alloc((size_t)N * P);
+        if (gn_cnt.n < (size_t)N) {
+            gn_cnt.alloc((size_t)N);
+            B2A_CUDA(cudaMemsetAsync(gn_cnt.p, 0, (size_t)N * sizeof(unsigned), s));
+        }
+        ec::gn_stats_kernel<<<dim3(P, N), 256, 0, s>>>(x, E, gn_part.p, gn_cnt.p, st, 1e-5f);
+        count_launch();
+    }
+    void gn_apply(const ec::GnApplyArgs& a, int N, cudaStream_t s) {
+        const long long per = a.L * a.C;
+        if (a.C % 4 == 0) ec::gn_apply_kernel<true><<<dim3((unsigned)cdiv(per / 4, 256), N), 256, 0, s>>>(a);
+        else ec::gn_apply_kernel<false><<<dim3((unsigned)cdiv(per, 256), N), 256, 0, s>>>(a);
+        count_launch();
+    }
+    // x [N, L, C] = GN(x) [* scale[n]], in place
+    void gn_inplace(float* x, const EcNorm& nm, int N, long long L, int C, const float* scale, cudaStream_t s) {
+        gn_stats(x, N, L, C, gn_sa.p, s);
+        ec::GnApplyArgs a{};
+        a.xa = x; a.sa = gn_sa.p; a.ga = nm.g.p; a.ba = nm.b.p; a.rows_a = L; a.scale = scale; a.out = x; a.L = L; a.C = C;
+        gn_apply(a, N, s);
+    }
+    void gn_alloc(int N) {
+        gn_sa.alloc((size_t)N); gn_sb.alloc((size_t)N);
+    }
+
+    // EncodecResnetBlock under time_group_norm (EncodecLayers.swift:319-336): GN_s(shortcut(x)) + GN_3(block.3(ELU(GN_1(block.1(ELU(x)))))),
+    // or x + GN_3(...) without a conv shortcut.  z [N, L, hid] and w [N, L, dim] are scratch; the result lands in y and x / y swap.
+    void run_resnet_gn(const EcRes& r, float*& x, float*& y, float* z, float* w, int N, long long L, int dim, cudaStream_t s) {
+        const int hid = r.r1.M;
+        ec::ConvArgs a{};
+        a.xa = x; a.La = (int)L; a.Ca = dim; a.taps = cfg.residual_kernel_size; pads(cfg.residual_kernel_size, a.padL);
+        a.reflect = cfg.pad_mode_reflect; a.elu_a = 1;
+        a.A = r.r1.A.p; a.bias = r.r1.bias.p; a.M = hid; a.K = r.r1.K; a.Lq = (int)L; a.N = N; a.out = z; a.out_per_n = L * hid;
+        ec::launch_conv(a, s);
+        gn_inplace(z, r.n1, N, L, hid, nullptr, s);
+        ec::ConvArgs b{};
+        b.xa = z; b.La = (int)L; b.Ca = hid; b.taps = 1; b.elu_a = 1;
+        b.A = r.r2.A.p; b.bias = r.r2.bias.p; b.M = dim; b.K = r.r2.K; b.Lq = (int)L; b.N = N; b.out = y; b.out_per_n = L * dim;
+        ec::launch_conv(b, s);
+        gn_stats(y, N, L, dim, gn_sa.p, s);
+        ec::GnApplyArgs g{};
+        g.xa = y; g.sa = gn_sa.p; g.ga = r.n3.g.p; g.ba = r.n3.b.p; g.rows_a = L; g.xb = x; g.out = y; g.L = L; g.C = dim;
+        if (cfg.use_conv_shortcut) {
+            ec::ConvArgs c{};
+            c.xa = x; c.La = (int)L; c.Ca = dim; c.taps = 1;
+            c.A = r.sc.A.p; c.bias = r.sc.bias.p; c.M = dim; c.K = r.sc.K; c.Lq = (int)L; c.N = N; c.out = w; c.out_per_n = L * dim;
+            ec::launch_conv(c, s);
+            gn_stats(w, N, L, dim, gn_sb.p, s);
+            g.xb = w; g.sb = gn_sb.p; g.gb = r.ns.g.p; g.bb = r.ns.b.p;
+        }
+        gn_apply(g, N, s);
+        std::swap(x, y);
     }
 
     // EncodecLSTMBlock (EncodecLayers.swift:72-88) on x [N, T, H]: the stack plus its skip; result in x
@@ -564,9 +774,14 @@ struct b2a_encodec {
         size_t big = (size_t)N * T * std::max(dim0, 4 * dim0);
         {
             long long L = T;
-            for (auto& st : stages) { L *= st.ratio; big = std::max(big, (size_t)((long long)N * L * st.cout)); }
+            for (auto& st : stages) {
+                // under time_group_norm the transposed conv writes its untrimmed (L + taps - 1) * s rows
+                if (gn) big = std::max(big, (size_t)((long long)N * (L + st.taps - 1) * st.ratio * st.cout));
+                L *= st.ratio; big = std::max(big, (size_t)((long long)N * L * st.cout));
+            }
         }
         bufA.alloc(big); bufB.alloc(big); bufC.alloc(big);
+        if (gn) { bufD.alloc(big); gn_alloc(N); }
         float* x = bufA.p; float* y = bufB.p; float* z = bufC.p;
         // 1. RVQ decode
         ec::rvq_sum_kernel<<<(unsigned)((long long)N * T), 128, 0, s>>>(d_codes, books.p, x, nq, T, cfg.codebook_size, cfg.codebook_dim);
@@ -577,6 +792,7 @@ struct b2a_encodec {
             a.xa = x; a.La = T; a.Ca = cfg.hidden_size; a.taps = cfg.kernel_size; pads(cfg.kernel_size, a.padL); a.reflect = cfg.pad_mode_reflect;
             a.A = conv0.A.p; a.bias = conv0.bias.p; a.M = conv0.M; a.K = conv0.K; a.Lq = T; a.N = N; a.out = y; a.out_per_n = (long long)T * dim0;
             ec::launch_conv(a, s);
+            if (gn) gn_inplace(y, norm0, N, T, dim0, nullptr, s);
             std::swap(x, y);
         }
         // 3. LSTM block
@@ -593,12 +809,26 @@ struct b2a_encodec {
                 ec::ConvArgs a{};
                 a.xa = x; a.La = (int)L; a.Ca = st.cin; a.taps = st.taps; a.backward = 1; a.elu_a = 1;
                 a.A = st.up.A.p; a.bias = st.up.bias.p; a.M = st.up.M; a.K = st.up.K; a.Lq = (int)L + st.taps - 1; a.N = N;
-                a.out = y; a.out_per_n = Lo * st.cout; a.shift = (long long)pl * st.cout;
-                ec::launch_conv(a, s);
-                std::swap(x, y);
+                if (gn) {
+                    // conv, then norm over all (L + taps - 1) * s rows, then trim (EncodecLayers.swift:251-272): the conv writes
+                    // untrimmed into y and the apply reads from row pl into x
+                    const long long Lfull = (L + st.taps - 1) * s_;
+                    a.out = y; a.out_per_n = Lfull * st.cout; a.shift = 0;
+                    ec::launch_conv(a, s);
+                    gn_stats(y, N, Lfull, st.cout, gn_sa.p, s);
+                    ec::GnApplyArgs g{};
+                    g.xa = y; g.sa = gn_sa.p; g.ga = st.nup.g.p; g.ba = st.nup.b.p; g.rows_a = Lfull; g.off_a = pl;
+                    g.out = x; g.L = Lo; g.C = st.cout;
+                    gn_apply(g, N, s);
+                } else {
+                    a.out = y; a.out_per_n = Lo * st.cout; a.shift = (long long)pl * st.cout;
+                    ec::launch_conv(a, s);
+                    std::swap(x, y);
+                }
             }
             L = Lo;
-            run_resnet(st.res, x, y, z, N, L, st.cout, s);
+            if (gn) run_resnet_gn(st.res, x, y, z, bufD.p, N, L, st.cout, s);
+            else run_resnet(st.res, x, y, z, N, L, st.cout, s);
         }
         // 5. ELU -> last conv (+ per-chunk scale), 6. overlap-add when chunked
         const bool chunked = chunk_length() != 0;
@@ -610,8 +840,11 @@ struct b2a_encodec {
             const size_t smem = ((size_t)(256 + k - 1) * (C + 1) + (size_t)CH * k * C) * sizeof(float);
             B2A_CHECK(smem <= 200 * 1024, B2A_ERR_INVALID_INPUT, "encodec: last conv too wide");
             B2A_CUDA(cudaFuncSetAttribute(ec::final_conv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            ec::final_conv_kernel<<<dim3(cdiv(L, 256), N), 256, smem, s>>>(x, wlast.p, blast.p, d_scales, dst, (int)L, C, k, CH, padL, cfg.pad_mode_reflect);
+            // under time_group_norm the chunk scale follows the last conv's norm (decodeFrame, Encodec.swift:294-301)
+            ec::final_conv_kernel<<<dim3(cdiv(L, 256), N), 256, smem, s>>>(x, wlast.p, blast.p, gn ? nullptr : d_scales, dst, (int)L, C, k, CH,
+                                                                          padL, cfg.pad_mode_reflect);
             count_launch();
+            if (gn) gn_inplace(dst, nlast, N, L, CH, d_scales, s);
         }
         if (chunked) {
             const long long total = out_len(n_chunks, T);
@@ -669,6 +902,7 @@ struct b2a_encodec {
             for (auto& st : estages) { l = conv_out_len(l, 2 * st.ratio, st.ratio); big = std::max(big, (size_t)((long long)N * l * st.cout)); }
         }
         bufA.alloc(big); bufB.alloc(big); bufC.alloc(big);
+        if (gn) { bufD.alloc(big); gn_alloc(N); }
         float* x = bufA.p; float* y = bufB.p; float* z = bufC.p;
         // 1. per-chunk scale (normalize), 2. stem on the waveform in place
         const float* sc = nullptr;
@@ -688,10 +922,14 @@ struct b2a_encodec {
             ec::stem_conv_kernel<<<dim3(cdiv(L, ec::STEM_T), N), 256, smem, s>>>(d_audio, wstem.p, bstem.p, sc, x, B, samples, CH, sh.chunk_len,
                                                                                 sh.chunk_stride, F, k, padL, cfg.pad_mode_reflect);
             count_launch();
+            if (gn) gn_inplace(x, nstem, N, L, F, nullptr, s);
         }
         // 3. downsampling stages: resnet, ELU + conv k = 2r stride r (one implicit-GEMM launch; ELU fused on its input)
         for (auto& st : estages) {
-            if (cfg.num_residual_layers > 0) run_resnet(st.res, x, y, z, N, L, st.cin, s);
+            if (cfg.num_residual_layers > 0) {
+                if (gn) run_resnet_gn(st.res, x, y, z, bufD.p, N, L, st.cin, s);
+                else run_resnet(st.res, x, y, z, N, L, st.cin, s);
+            }
             const int r = st.ratio, k = 2 * r;
             const long long Lo = conv_out_len(L, k, r);
             ec::ConvArgs a{};
@@ -700,6 +938,7 @@ struct b2a_encodec {
             a.A = st.down.A.p; a.bias = st.down.bias.p; a.M = st.down.M; a.K = st.down.K; a.Lq = (int)Lo; a.N = N;
             a.out = y; a.out_per_n = Lo * st.cout;
             ec::launch_conv(a, s);
+            if (gn) gn_inplace(y, st.ndown, N, Lo, st.cout, nullptr, s);
             std::swap(x, y);
             L = Lo;
         }
@@ -712,6 +951,7 @@ struct b2a_encodec {
             a.xa = x; a.La = T; a.Ca = H; a.taps = cfg.last_kernel_size; pads(cfg.last_kernel_size, a.padL); a.reflect = cfg.pad_mode_reflect; a.elu_a = 1;
             a.A = elast.A.p; a.bias = elast.bias.p; a.M = elast.M; a.K = elast.K; a.Lq = T; a.N = N; a.out = zbuf.p; a.out_per_n = (long long)T * D;
             ec::launch_conv(a, s);
+            if (gn) gn_inplace(zbuf.p, nelast, N, T, D, nullptr, s);
         }
         // 6. residual VQ encode
         {

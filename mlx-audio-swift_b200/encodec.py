@@ -61,7 +61,7 @@ class Encodec:
             setattr(c, name, int(getattr(config, name)))
         c.use_causal_conv, c.use_conv_shortcut = int(config.use_causal_conv), int(config.use_conv_shortcut)
         c.pad_mode_reflect = int(config.pad_mode == "reflect")
-        c.norm_type = 0 if config.norm_type == "weight_norm" else 1
+        c.norm_type = {"weight_norm": 0, "time_group_norm": 1}.get(config.norm_type, 2)    # 2: the library's invalidInput
         c.n_upsampling_ratios = len(config.upsampling_ratios)
         for i, r in enumerate(config.upsampling_ratios[:8]):
             c.upsampling_ratios[i] = int(r)
@@ -76,7 +76,9 @@ class Encodec:
 
     @classmethod
     def from_model_directory(cls, model_dir, device: int = 0) -> "Encodec":
-        """fromModelDirectory (Encodec.swift:423-440): config.json + model.safetensors, keys as shipped (the library's reader)."""
+        """fromModelDirectory (Encodec.swift:423-440): config.json + model.safetensors, keys as shipped (the library's reader).
+        The mlx-community layout is the library's own: ``*.conv.weight [out, k, in]`` and, for time_group_norm checkpoints such
+        as encodec-48khz, ``*.norm.weight`` / ``*.norm.bias [C_out]`` after every conv."""
         import json
         from pathlib import Path
         from .loading import Weights
@@ -123,9 +125,14 @@ class Encodec:
     @staticmethod
     def random_init_weights(config: EncodecConfig, seed: int = 1234, n_codebooks: int = 8, encoder: bool = False) -> Dict[str, np.ndarray]:
         """Random-init weights with the checkpoint's keys / MLX layouts (benchmarks): U(+-1/sqrt(fan_in)), N(0,1) codebooks.
-        encoder=True appends the encoder's weights (drawn after everything else, so the decoder / codebooks do not change)."""
+        encoder=True appends the encoder's weights (drawn after everything else, so the decoder / codebooks do not change).
+        time_group_norm adds every conv's ``norm.weight`` / ``norm.bias`` from a generator of their own (the other tensors are
+        those of the same config under weight_norm), gamma = +-U(0.5, 1.5) and beta = +-U(0.1, 0.5): away from 1 and 0, so a
+        dropped or swapped affine shows."""
         rng = np.random.default_rng(seed)
+        nrng = np.random.default_rng([seed, 1])
         w: Dict[str, np.ndarray] = {}
+        gn = config.norm_type == "time_group_norm"
 
         def u(shape, fan):
             s = (1.0 / fan) ** 0.5
@@ -134,6 +141,10 @@ class Encodec:
         def conv(pre, cout, k, cin):
             w[pre + "conv.weight"] = u((cout, k, cin), k * cin)
             w[pre + "conv.bias"] = u((cout,), k * cin)
+            if gn:
+                sign = np.where(nrng.random(cout) < 0.5, -1.0, 1.0)
+                w[pre + "norm.weight"] = (sign * nrng.uniform(0.5, 1.5, cout)).astype(np.float32)
+                w[pre + "norm.bias"] = (np.where(nrng.random(cout) < 0.5, -1.0, 1.0) * nrng.uniform(0.1, 0.5, cout)).astype(np.float32)
 
         for q in range(n_codebooks):
             w[f"quantizer.layers.{q}.codebook.embed"] = rng.standard_normal((config.codebook_size, config.codebook_dim)).astype(np.float32)

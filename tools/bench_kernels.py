@@ -1,7 +1,7 @@
 """Per-stage measurements for the other BASELINE.json configs (not the driver's bench line): CUDA events on the
 library's streams, inputs resident in HBM, roofline numerators from SURVEY.md section 8d.
 
-    python tools/bench_kernels.py [mel] [snac] [whisper]      -> one JSON line per stage
+    python tools/bench_kernels.py [mel] [snac] [whisper] [encodec] [encodec48] [speech_tokenizer]      -> one JSON line per stage
 """
 import json
 import sys
@@ -101,6 +101,29 @@ def bench_encodec():
                       "note": "fp32 implicit-GEMM convs + persistent wavefront LSTM (T + 1 grid barriers)"}))
 
 
+def bench_encodec48():
+    """The 48 kHz stereo model (time_group_norm, 1 s chunks, 1 % overlap): decode of 8 clips x 31 chunks x 150 frames at 24 kbps
+    (16 codebooks) with per-chunk scales -> 8 x 1 473 600 samples (30.7 s), the clips tools/bench_encodec_encode.py --model 48khz
+    encodes."""
+    import subprocess
+    sys.path.insert(0, str(Path(__file__).resolve().parent))
+    from bench_encodec_encode import config_48khz
+    cfg = config_48khz()
+    codec = m.Encodec(cfg, weights=m.Encodec.random_init_weights(cfg, 1234, n_codebooks=16, encoder=True))
+    B, nc, T = 8, 31, 150
+    rng = np.random.default_rng(2)
+    codes = torch.from_numpy(rng.integers(0, 1024, size=(nc, B, 16, T), dtype=np.int32)).cuda()
+    scales = torch.from_numpy(rng.uniform(0.05, 0.5, size=(nc, B)).astype(np.float32)).cuda()
+    n = codec.output_length(nc, T)
+    wave = torch.empty((B, n, 2), device="cuda")
+    ms = timed(lambda: codec.decode_dev(codes, wave, scales, stream=codec.stream), codec.stream, iters=5, warmup=2)
+    gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True,
+                         check=True).stdout.strip().splitlines()[0]
+    print(json.dumps({"stage": "encodec48_decode", "workload": f"Encodec-48kHz decode, {B} clips x {nc} chunks x {T} frames (16 codebooks) -> {B} x {n / 48000:.1f} s stereo",
+                      "ms": ms, "x_realtime": B * n / 48000 / (ms * 1e-3), "gpu": gpu,
+                      "note": "time_group_norm: every conv followed by gn_stats_kernel + gn_apply_kernel"}))
+
+
 def bench_speech_tokenizer():
     """Qwen3-TTS speech-tokenizer decoder, shipped geometry, 4 rows x 16 streaming chunks of 64 code frames (bench.py's qwen3 block)."""
     import importlib
@@ -131,4 +154,5 @@ def bench_speech_tokenizer():
 if __name__ == "__main__":
     which = sys.argv[1:] or ["mel", "snac", "whisper", "encodec"]
     for w in which:
-        {"mel": bench_mel, "snac": bench_snac, "whisper": bench_whisper, "encodec": bench_encodec, "speech_tokenizer": bench_speech_tokenizer}[w]()
+        {"mel": bench_mel, "snac": bench_snac, "whisper": bench_whisper, "encodec": bench_encodec, "encodec48": bench_encodec48,
+         "speech_tokenizer": bench_speech_tokenizer}[w]()
