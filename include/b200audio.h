@@ -117,10 +117,13 @@ void b2a_logmel_destroy(b2a_logmel* h);
  *   quantizer(z) (ResidualVectorQuantize.callAsFunction, SNAC/VQ.swift:150-163), the
  *   encode-side code search                      -> b2a_snac_quantize
  *   encode(_ audioData:) :120-125 / encodeAudio :197-199 -> b2a_snac_encode (preprocess -> Encoder -> quantizer)
- * codes[i] is [B, T_i] int32 with T_i = t_latent / vq_strides[i]; wave is [B, 1, t_latent*hop].
+ * codes[i] is [B, T_i] int32 with T_i = t_latent / vq_strides[i]; wave is [B, 1, b2a_snac_decoded_length(h, t_latent)].
  * noise[i] (nullable array of nullable pointers) is the [B, 1, T] Gaussian draw of decoder
- * block i's NoiseBlock (Layers.swift:263-279); NULL = draw on device from `seed`
- * (noise_mode 0) or use zero noise (noise_mode 1).                                          */
+ * block i's NoiseBlock (Layers.swift:263-279), T the length of stage i's output (the decoded length of the stages up to i);
+ * NULL = draw on device from `seed` (noise_mode 0) or use zero noise (noise_mode 1).
+ * Both are sized by the decoded length, not by t_latent * hop: like the reference, a stage of odd stride s yields s T - 1
+ * frames (DecoderBlock's outputPadding is dropped), so the 32 / 44 kHz models (decoder_rates [8, 8, 3, 2]) decode t_latent
+ * frames to 384 t_latent - 2 samples.  With attn_window_size > 0, t_latent must be a multiple of it (B2A_ERR_INVALID_INPUT). */
 typedef struct b2a_snac_config {
     int32_t sampling_rate;
     int32_t encoder_dim;
@@ -130,7 +133,8 @@ typedef struct b2a_snac_config {
     int32_t decoder_dim;
     int32_t n_decoder_rates;
     int32_t decoder_rates[8];
-    int32_t attn_window_size; /* 0 => none (only value supported) */
+    int32_t attn_window_size; /* 0 => none (24 kHz); > 0 => LocalMHA over windows of this many frames (32 / 44 kHz models: 32),
+                                 1 .. 64, latent_dim and decoder_dim multiples of 64 (heads of 64); no B2A_SNAC=simt path */
     int32_t codebook_size;
     int32_t codebook_dim;
     int32_t n_vq_strides;
@@ -143,6 +147,9 @@ typedef struct b2a_snac b2a_snac;
 int32_t b2a_snac_create(int32_t device, const b2a_snac_config* cfg, const b2a_tensor* tensors,
                         int32_t n_tensors, b2a_snac** out);
 int64_t b2a_snac_hop_length(const b2a_snac* h);
+/* samples decoded from t_latent frames: t_latent * hop when every decoder rate is even, less by one per odd-stride stage
+ * (scaled by the later strides) otherwise; 0 for a null handle or t_latent <= 0 */
+int64_t b2a_snac_decoded_length(const b2a_snac* h, int64_t t_latent);
 void* b2a_snac_stream(b2a_snac* h); /* the handle's cudaStream_t, for event timing */
 int32_t b2a_snac_decode(b2a_snac* h, const int32_t* const* codes, int32_t batch, int64_t t_latent,
                         const float* const* noise, int32_t noise_mode, uint64_t seed, float* wave);
@@ -153,7 +160,7 @@ int32_t b2a_snac_decode_dev(b2a_snac* h, const int32_t* const* d_codes, int32_t 
 int32_t b2a_snac_quantize(b2a_snac* h, const float* z, int32_t batch, int64_t t_latent,
                           int32_t* const* codes, float* z_q);
 /* SNAC.encode (SNACDecoder.swift:86-105,120-125): wave [B, 1, n_samples] float32 is zero right-padded to a multiple of
- * hop * lcm(vq_strides) (2048 for the 24 kHz model), run through the encoder (Layers.swift:236-259,319-360) and the residual
+ * hop * lcm(vq_strides, attn_window_size) (2048 for the 24 kHz model, 12288 for the 32 / 44 kHz ones), run through the encoder (Layers.swift:236-259,319-360) and the residual
  * quantizer; codes[i] [B, t_latent / vq_strides[i]] int32 with t_latent = b2a_snac_encoded_length(h, n_samples).
  * Needs the checkpoint's encoder.* tensors (a decoder-only handle returns B2A_ERR_MODEL_NOT_INITIALIZED); empty audio is
  * B2A_ERR_AUDIO_ENCODING_FAILED; an encoder geometry the device path does not run (a stride < 2, latent_dim other than

@@ -153,6 +153,10 @@ int32_t b2a_snac_convt_test(const float* x, float* y, const float* alpha, const 
 /* tests/test_gpu_snac_encode.py: the SNAC encoder's latent before the code search (what b2a_snac_encode quantizes) on HOST data:
  * wave [B, n_samples] -> z [B, latent, t_latent] float32, t_latent as b2a_snac_encoded_length gives it.  Errors as b2a_snac_encode. */
 int32_t b2a_snac_encode_latent_test(b2a_snac* h, const float* wave, int32_t batch, int64_t n_samples, float* z);
+/* tests/test_gpu_snac_44khz.py: one launch of SNAC LocalMHA's window core (local_attn_kernel, csrc/snac.cu) on HOST data:
+ * qkv float32 [B * T, 3 dim] (q | k | v before the rotary rotation), inv_freq [32] -> out float32 [B * T, dim], the hi + lo pair it
+ * writes for to_out.  T % window == 0, window 1 .. 64, dim a multiple of 64. */
+int32_t b2a_snac_local_attn_test(const float* qkv, const float* inv_freq, int32_t B, int32_t T, int32_t dim, int32_t window, float* out);
 /* tests/test_gpu_encodec_encode.py: the Encodec encoder's latent before the code search (what b2a_encodec_encode quantizes) on HOST
  * data: audio [B, samples, audio_channels] -> z [n_chunks, B, frames, hidden_size] float32, shapes as b2a_encodec_encoded_shape
  * gives them.  Errors as b2a_encodec_encode. */

@@ -175,6 +175,7 @@ SIGNATURES = {
     "b2a_logmel_destroy": (None, [_P]),
     "b2a_snac_create": (C.c_int32, [C.c_int32, C.POINTER(SnacConfig), C.POINTER(Tensor), C.c_int32, C.POINTER(_P)]),
     "b2a_snac_hop_length": (C.c_int64, [_P]),
+    "b2a_snac_decoded_length": (C.c_int64, [_P, C.c_int64]),
     "b2a_snac_decode": (C.c_int32, [_P, C.POINTER(_P), C.c_int32, C.c_int64, C.POINTER(_P), C.c_int32, C.c_uint64, _P]),
     "b2a_snac_decode_dev": (C.c_int32, [_P, C.POINTER(_P), C.c_int32, C.c_int64, C.POINTER(_P), C.c_int32, C.c_uint64, _P, _P]),
     "b2a_snac_quantize": (C.c_int32, [_P, _P, C.c_int32, C.c_int64, C.POINTER(_P), _P]),
@@ -182,6 +183,7 @@ SIGNATURES = {
     "b2a_snac_encode": (C.c_int32, [_P, _P, C.c_int32, C.c_int64, C.POINTER(_P)]),
     "b2a_snac_encode_dev": (C.c_int32, [_P, _P, C.c_int32, C.c_int64, C.POINTER(_P), _P]),
     "b2a_snac_encode_latent_test": (C.c_int32, [_P, _P, C.c_int32, C.c_int64, _P]),
+    "b2a_snac_local_attn_test": (C.c_int32, [_P, _P] + [C.c_int32] * 4 + [_P]),
     "b2a_snac_destroy": (None, [_P]),
     "b2a_tts_create": (C.c_int32, [C.c_int32, C.POINTER(LlamaConfig), C.POINTER(Tensor), C.c_int32, _P, C.POINTER(_P)]),
     "b2a_tts_debug_trace": (C.c_int32, [_P, C.c_int32, C.c_int32, _P]),

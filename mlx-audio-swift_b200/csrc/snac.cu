@@ -17,6 +17,7 @@
 #include "common.cuh"
 #include "conv_gemm.cuh"
 #include "snac_fused.cuh"
+#include "layernorm.cuh"
 
 #include <algorithm>
 #include <cmath>
@@ -505,56 +506,62 @@ enc_final_dw_kernel(const float* __restrict__ x, float* __restrict__ z, const fl
     }
 }
 
-// final Snake -> conv k7 (C -> 1) -> tanh in NLC (Layers.swift:411-415), C == 64.
-// 256 tokens per CTA; the Snake'd tile (+3 halo rows each side) is staged in shared memory.  Thread (tg, cg) owns 8 consecutive
-// tokens x 8 channels (two float4 column groups {4cg..4cg+3} and {32+4cg..}, so a quarter-warp's LDS.128 covers 128 contiguous
-// bytes): 14 row reads feed 8 x 7 x 8 FMAs against weights held in registers; the 8 channel groups are then reduced by shuffles.
-constexpr int FN_TT = 256, FN_THREADS = 256, FN_MAXC = 64;
+// final Snake -> conv k7 (C -> 1) -> tanh in NLC (Layers.swift:411-415), C == FC (64, or 128 for the zero-padded 96 of the 32 / 44 kHz
+// models).  256 tokens per CTA; the Snake'd tile (+3 halo rows each side) is staged in shared memory.  Thread (tg, cg) owns 8 consecutive
+// tokens x 8 channels of each 64-channel half (two float4 column groups {4cg..4cg+3} and {32+4cg..}, so a quarter-warp's LDS.128 covers
+// 128 contiguous bytes): 14 row reads feed 8 x 7 x 8 FMAs against weights held in registers; the 8 channel groups are then reduced by
+// shuffles.
+constexpr int FN_TT = 256, FN_THREADS = 256;
+template <int FC>
 __global__ void __launch_bounds__(FN_THREADS)
 final_nlc_kernel(const float* __restrict__ x, float* __restrict__ wave, const float* __restrict__ w /*[C,7]*/,
                  const float* __restrict__ alpha, float bias, int T, int C) {
-    extern __shared__ __align__(16) float fsm[];     // [(256 + 6)][64]
+    extern __shared__ __align__(16) float fsm[];     // [(256 + 6)][FC]
+    constexpr int CQ = FC / 4;                       // float4 column groups per row; FN_THREADS % CQ == 0
     const int t0 = blockIdx.x * FN_TT, b = blockIdx.y;
-    const float* xb = x + (long long)b * T * FN_MAXC;
-    {   // FN_THREADS is a multiple of 16: a thread always stages the same 4 channels
-        const int c = (threadIdx.x & 15) * 4;
+    const float* xb = x + (long long)b * T * FC;
+    {   // a thread always stages the same 4 channels
+        const int c = (threadIdx.x % CQ) * 4;
         const float4 al = *reinterpret_cast<const float4*>(alpha + c);
         const float4 iv = make_float4(1.0f / (al.x + 1e-9f), 1.0f / (al.y + 1e-9f), 1.0f / (al.z + 1e-9f), 1.0f / (al.w + 1e-9f));
-        for (int i = threadIdx.x; i < (FN_TT + 6) * 16; i += FN_THREADS) {
-            const int r = i >> 4;
+        for (int i = threadIdx.x; i < (FN_TT + 6) * CQ; i += FN_THREADS) {
+            const int r = i / CQ;
             const int t = t0 + r - 3;
             float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
             if (t >= 0 && t < T) {
-                v = *reinterpret_cast<const float4*>(xb + (long long)t * FN_MAXC + c);
+                v = *reinterpret_cast<const float4*>(xb + (long long)t * FC + c);
                 v.x = cg::snake_inv(v.x, al.x, iv.x); v.y = cg::snake_inv(v.y, al.y, iv.y); v.z = cg::snake_inv(v.z, al.z, iv.z); v.w = cg::snake_inv(v.w, al.w, iv.w);
             }
-            *reinterpret_cast<float4*>(fsm + r * FN_MAXC + c) = v;
+            *reinterpret_cast<float4*>(fsm + r * FC + c) = v;
         }
     }
     const int cgp = threadIdx.x & 7, tg = threadIdx.x >> 3;     // 8 channel groups x 32 token groups
-    float wk[8][7];
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-        const int c = (i < 4 ? 0 : 28) + cgp * 4 + i;            // i >= 4 -> 32 + 4*cgp + (i - 4)
-#pragma unroll
-        for (int k = 0; k < 7; ++k) wk[i][k] = w[c * 7 + k];
-    }
-    __syncthreads();
     float acc[8];
 #pragma unroll
     for (int j = 0; j < 8; ++j) acc[j] = 0.f;
-    const float* base = fsm + (tg * 8) * FN_MAXC + cgp * 4;
 #pragma unroll
-    for (int r = 0; r < 14; ++r) {
-        const float4 lo = *reinterpret_cast<const float4*>(base + r * FN_MAXC);
-        const float4 hi = *reinterpret_cast<const float4*>(base + r * FN_MAXC + 32);
-        const float xv[8] = {lo.x, lo.y, lo.z, lo.w, hi.x, hi.y, hi.z, hi.w};
+    for (int h = 0; h < FC / 64; ++h) {
+        float wk[8][7];
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {
-            const int k = r - j;
-            if (k >= 0 && k < 7) {
+        for (int i = 0; i < 8; ++i) {
+            const int c = h * 64 + (i < 4 ? 0 : 28) + cgp * 4 + i;   // i >= 4 -> 32 + 4*cgp + (i - 4)
 #pragma unroll
-                for (int i = 0; i < 8; ++i) acc[j] = fmaf(wk[i][k], xv[i], acc[j]);
+            for (int k = 0; k < 7; ++k) wk[i][k] = w[c * 7 + k];
+        }
+        if (h == 0) __syncthreads();
+        const float* base = fsm + (tg * 8) * FC + h * 64 + cgp * 4;
+#pragma unroll
+        for (int r = 0; r < 14; ++r) {
+            const float4 lo = *reinterpret_cast<const float4*>(base + r * FC);
+            const float4 hi = *reinterpret_cast<const float4*>(base + r * FC + 32);
+            const float xv[8] = {lo.x, lo.y, lo.z, lo.w, hi.x, hi.y, hi.z, hi.w};
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+                const int k = r - j;
+                if (k >= 0 && k < 7) {
+#pragma unroll
+                    for (int i = 0; i < 8; ++i) acc[j] = fmaf(wk[i][k], xv[i], acc[j]);
+                }
             }
         }
     }
@@ -571,6 +578,64 @@ final_nlc_kernel(const float* __restrict__ x, float* __restrict__ wave, const fl
 #pragma unroll
     for (int j = 1; j < 8; ++j) out = cgp == j ? acc[j] : out;
     if (t < T) wave[(long long)b * T + t] = tanhf(out + bias);
+}
+
+// ------------------------------------------------------------------------------------------------
+// LocalMHA (Attention.swift:14-95) core: windowed non-causal attention of one head over qkv fp32 [B*T, 3*dim] (q | k | v, head h at
+// columns h*64 .. +63 of each), rotary (rotate-half, [freqs, freqs]) applied to q and k as they are loaded, softmax(q k^T / 8) v in fp32.
+// CTA = (window, head, clip), 8 warps; K and V of the window live in shared memory, warp w takes query rows w, w + 8, ...: lane j
+// scores keys j and j + 32, lane d accumulates output channels d and d + 32.  The output goes straight into the hi/lo operand rows
+// [tokens, dim] of to_out.  rope: cos [W][64] then sin [W][64] (angle n * inv_freq[d % 32], position n within the window).
+constexpr int LA_THREADS = 256, LA_MAXW = 64, LA_D = 64;
+__global__ void __launch_bounds__(LA_THREADS)
+local_attn_kernel(const float* __restrict__ qkv, const float* __restrict__ rope, __nv_bfloat16* __restrict__ out, int T, int dim, int W) {
+    __shared__ float Ks[LA_MAXW][LA_D + 1], Vs[LA_MAXW][LA_D];
+    const int win = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const long long tok0 = (long long)b * T + (long long)win * W;
+    const long long ld = 3ll * dim;
+    const float* cs = rope;
+    const float* sn = rope + W * LA_D;
+    for (int n = warp; n < W; n += LA_THREADS / 32) {
+        const float* row = qkv + (tok0 + n) * ld + h * LA_D;
+        const float k0 = row[dim + lane], k1 = row[dim + lane + 32];
+        Ks[n][lane] = k0 * cs[n * LA_D + lane] - k1 * sn[n * LA_D + lane];
+        Ks[n][lane + 32] = k1 * cs[n * LA_D + lane + 32] + k0 * sn[n * LA_D + lane + 32];
+        Vs[n][lane] = row[2 * dim + lane];
+        Vs[n][lane + 32] = row[2 * dim + lane + 32];
+    }
+    __syncthreads();
+    for (int n = warp; n < W; n += LA_THREADS / 32) {
+        const float* row = qkv + (tok0 + n) * ld + h * LA_D;
+        const float x0 = row[lane], x1 = row[lane + 32];
+        const float q0 = 0.125f * (x0 * cs[n * LA_D + lane] - x1 * sn[n * LA_D + lane]);          // 1 / sqrt(64) folded into q
+        const float q1 = 0.125f * (x1 * cs[n * LA_D + lane + 32] + x0 * sn[n * LA_D + lane + 32]);
+        float s0 = 0.f, s1 = 0.f;
+        const int j1 = min(lane + 32, LA_MAXW - 1);
+#pragma unroll 8
+        for (int d = 0; d < 32; ++d) {
+            const float qa = __shfl_sync(0xffffffffu, q0, d), qb = __shfl_sync(0xffffffffu, q1, d);
+            s0 = fmaf(qa, Ks[lane][d], s0); s0 = fmaf(qb, Ks[lane][d + 32], s0);
+            s1 = fmaf(qa, Ks[j1][d], s1); s1 = fmaf(qb, Ks[j1][d + 32], s1);
+        }
+        if (lane >= W) s0 = -INFINITY;
+        if (lane + 32 >= W) s1 = -INFINITY;
+        float mx = fmaxf(s0, s1);
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+        const float p0 = lane < W ? expf(s0 - mx) : 0.f, p1 = lane + 32 < W ? expf(s1 - mx) : 0.f;
+        float sum = p0 + p1;
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+        float o0 = 0.f, o1 = 0.f;
+        for (int j = 0; j < W; ++j) {
+            const float p = __shfl_sync(0xffffffffu, j < 32 ? p0 : p1, j & 31);
+            o0 = fmaf(p, Vs[j][lane], o0); o1 = fmaf(p, Vs[j][lane + 32], o1);
+        }
+        const float inv = 1.0f / sum;
+        tc::store_hilo(out, dim, tok0 + n, h * LA_D + lane, o0 * inv, cg::HALF);
+        tc::store_hilo(out, dim, tok0 + n, h * LA_D + lane + 32, o1 * inv, cg::HALF);
+    }
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -654,13 +719,48 @@ static std::vector<float> block_diag2(const std::vector<float>& w) {
     return d;
 }
 
-static void load_bias(const TensorTable& tt, const std::string& prefix, int n, ConvW& c) {
+static void load_bias(const TensorTable& tt, const std::string& prefix, int n, ConvW& c, int np = 0) {
     if (tt.find(prefix + ".bias")) {
-        std::vector<float> b = tt.f32(prefix + ".bias", n);
-        c.bias.upload(b.data(), n);
+        std::vector<float> b = pad2(tt.f32(prefix + ".bias", n), 1, n, 1, std::max(n, np));
+        c.bias.upload(b.data(), b.size());
         c.has_bias = true;
     }
 }
+
+// the 32 / 44 kHz models' LocalMHA (Attention.swift:14-95) at `dim` channels: LayerNorm(eps 1e-5) -> to_qkv -> windowed attention
+// (local_attn_kernel) -> to_out + residual.  Keys <prefix>.norm.weight|bias, .to_qkv.weight [3 dim, dim], .to_out.weight [dim, dim]
+// (both without bias) and .rel_pos.inv_freq [32].
+constexpr int SN_LN_MAXV = 8;      // LayerNorm channel slots: dim <= 2048
+struct LocalAttn {
+    int dim = 0, window = 0;
+    DBuf<float> ln_w, ln_b, rope;   // rope: cos [window][64] | sin [window][64]
+    TcW qkv, out;
+};
+// local_attn_kernel's rotary table: cos [window][64] | sin [window][64] of n * inv_freq[d % 32] (SinusoidalEmbeddings, xpos off)
+static std::vector<float> rope_table(const float* inv, int window) {
+    std::vector<float> r((size_t)2 * window * LA_D);
+    for (int n = 0; n < window; ++n)
+        for (int d = 0; d < LA_D; ++d) {
+            const double ang = n * (double)inv[d % (LA_D / 2)];
+            r[(size_t)n * LA_D + d] = (float)std::cos(ang);
+            r[((size_t)window + n) * LA_D + d] = (float)std::sin(ang);
+        }
+    return r;
+}
+static void load_attn(const TensorTable& tt, const std::string& p, int dim, int window, LocalAttn& A) {
+    std::vector<float> g = tt.f32(p + ".norm.weight", dim), be = tt.f32(p + ".norm.bias", dim);
+    std::vector<float> wqkv = tt.f32(p + ".to_qkv.weight", 3ll * dim * dim), wo = tt.f32(p + ".to_out.weight", (int64_t)dim * dim);
+    std::vector<float> inv = tt.f32(p + ".rel_pos.inv_freq", LA_D / 2);
+    A.ln_w.upload(g.data(), g.size()); A.ln_b.upload(be.data(), be.size());
+    A.qkv.build(wqkv, 3 * dim, 1, dim);
+    A.out.build(wo, dim, 1, dim);
+    std::vector<float> r = rope_table(inv.data(), window);
+    A.rope.upload(r.data(), r.size());
+    A.dim = dim; A.window = window;
+}
+// frames out of a decoder stage of stride s over t frames: the reference drops DecoderBlock's outputPadding (stride % 2), so a
+// transposed conv with k = 2 s, pad = ceil(s / 2) yields s t - (s mod 2) frames (DESIGN.md, SURVEY.md section 8(c) trap 7)
+static long long stage_len(long long t, int s) { return t * s - s % 2; }
 
 }  // namespace b2a
 
@@ -678,6 +778,8 @@ struct b2a_snac {
     ConvW dw0, pw0, conv0;   // depthwise: dw0 + pw0 ; otherwise conv0 (k7 dense, unsupported on device)
     TcW pw0_tc;
     bool use_tc = true;      // wgmma / NLC path (B2A_SNAC=simt selects the fp32 CUDA-core path)
+    LocalAttn dec_attn, enc_attn;        // LocalMHA of the 32 / 44 kHz models (dim 0: none)
+    DBuf<float> d_qkv;                   // LocalMHA q | k | v, fp32 [tokens, 3 dim]
     int num_sms = 132;
     DBuf<float> xs, xs2;                 // NLC fp32 activations of the current stage (ping-pong for the fused units)
     DBuf<__nv_bfloat16> hA, x2;          // hi/lo tiles: GEMM input of the stage / 2-tap im2col of the next transposed conv
@@ -699,8 +801,6 @@ struct b2a_snac {
     ~b2a_snac() { if (stream) cudaStreamDestroy(stream); }
 
     b2a_snac(int dev, const b2a_snac_config& c, const TensorTable& tt) : device(dev), cfg(c) {
-        B2A_CHECK(c.attn_window_size == 0, B2A_ERR_INVALID_INPUT,
-                  "SNAC: attn_window_size (LocalMHA) is only used by the 32/44 kHz models and is not implemented");
         B2A_CHECK(c.depthwise != 0, B2A_ERR_INVALID_INPUT, "SNAC: only depthwise=true decoders are implemented");
         B2A_CHECK(c.n_vq_strides >= 1 && c.n_vq_strides <= 4 && c.n_decoder_rates >= 1 && c.n_decoder_rates <= 8,
                   B2A_ERR_INVALID_INPUT, "SNAC: unsupported number of codebooks / decoder stages");
@@ -708,6 +808,11 @@ struct b2a_snac {
         require_device(dev);
         B2A_CUDA(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
         latent = c.latent_dim > 0 ? c.latent_dim : c.encoder_dim << c.n_encoder_rates;
+        const int win = c.attn_window_size;
+        B2A_CHECK(win == 0 || (win >= 1 && win <= LA_MAXW && latent % LA_D == 0 && c.decoder_dim % LA_D == 0 &&
+                               latent <= DL_THREADS * SN_LN_MAXV && c.decoder_dim <= DL_THREADS * SN_LN_MAXV),
+                  B2A_ERR_INVALID_INPUT, "SNAC: LocalMHA (attn_window_size > 0) needs a window of 1 .. 64 frames and latent_dim / decoder_dim "
+                  "multiples of 64 (whole heads of 64) up to 2048");
         hop = 1;
         for (int i = 0; i < c.n_decoder_rates; ++i) hop *= c.decoder_rates[i];
         const int D = c.codebook_dim, N = c.codebook_size;
@@ -745,24 +850,32 @@ struct b2a_snac {
             load_bias(tt, p + "1", C, pw0);
         }
         int li = 2;
+        if (win > 0) load_attn(tt, p + "2", C, win, dec_attn);      // decoder.model.layers.2 (Layers.swift:395-397)
+        if (win > 0) li = 3;
+        // stages whose width is not a multiple of 64 (the 96 and 48 of the 32 / 44 kHz models' last stages) run at the encoder's padded
+        // widths: the extra channels carry exact zeros (weights and biases 0, Snake alpha 1)
         blocks.resize(c.n_decoder_rates);
         for (int i = 0; i < c.n_decoder_rates; ++i, ++li) {
             DecBlock& B = blocks[i];
-            B.cin = C >> i; B.cout = C >> (i + 1); B.stride = c.decoder_rates[i];
+            const int ci_ = C >> i, co_ = C >> (i + 1);
+            B.cin = enc_padded(ci_); B.cout = enc_padded(co_); B.stride = c.decoder_rates[i];
             B.pad = (B.stride + 1) / 2;  // Int(ceil(stride/2)), Layers.swift:295
+            B2A_CHECK(B.stride >= 1, B2A_ERR_INVALID_INPUT, "SNAC: decoder stride");
             const std::string b = p + std::to_string(li) + ".block.layers.";
-            std::vector<float> a = tt.f32(b + "0.alpha", B.cin);
+            std::vector<float> a = pad2(tt.f32(b + "0.alpha", ci_), 1, ci_, 1, B.cin, 1.f);
             B.alpha.upload(a.data(), a.size());
             const int s = B.stride, k = 2 * s;
-            std::vector<float> wt = fold_wn(tt, b + "1", B.cin, k, B.cout, false);  // [ci, k, co]
+            std::vector<float> wt0 = fold_wn(tt, b + "1", ci_, k, co_, false);  // [ci, k, co]
+            std::vector<float> wt = pad2(wt0, ci_ * k, co_, ci_ * k, B.cout);
+            wt.resize((size_t)B.cin * k * B.cout, 0.f);
             std::vector<float> A = convt_gemm_rows(wt, B.cin, B.cout, s);
             B.ct.w.upload(A.data(), A.size());
             host_ct.push_back(convt_phase_major(A, B.cin, B.cout, s));
-            load_bias(tt, b + "1", B.cout, B.ct);
+            load_bias(tt, b + "1", co_, B.ct, B.cout);
             int j = 2;
             B.has_noise = c.noise != 0;
             if (B.has_noise) {
-                std::vector<float> wn_ = fold_wn(tt, b + "2.linear", B.cout, 1, B.cout, true);
+                std::vector<float> wn_ = pad2(fold_wn(tt, b + "2.linear", co_, 1, co_, true), co_, co_, B.cout, B.cout);
                 B.noise.w.upload(wn_.data(), wn_.size());
                 host_noise.push_back(wn_);
                 j = 3;
@@ -772,26 +885,27 @@ struct b2a_snac {
                 ResUnit& R = B.ru[u];
                 R.dil = dils[u];
                 const std::string r = b + std::to_string(j) + ".block.layers.";
-                std::vector<float> a0 = tt.f32(r + "0.alpha", B.cout), a2 = tt.f32(r + "2.alpha", B.cout);
+                std::vector<float> a0 = pad2(tt.f32(r + "0.alpha", co_), 1, co_, 1, B.cout, 1.f), a2 = pad2(tt.f32(r + "2.alpha", co_), 1, co_, 1, B.cout, 1.f);
                 R.a0.upload(a0.data(), a0.size());
                 R.a2.upload(a2.data(), a2.size());
-                std::vector<float> wd = fold_wn(tt, r + "1", B.cout, 7, 1, true);
+                std::vector<float> wd = pad2(fold_wn(tt, r + "1", co_, 7, 1, true), co_, 7, B.cout, 7);
                 R.dw.w.upload(wd.data(), wd.size());
-                load_bias(tt, r + "1", B.cout, R.dw);
-                std::vector<float> wp = fold_wn(tt, r + "3", B.cout, 1, B.cout, true);
+                load_bias(tt, r + "1", co_, R.dw, B.cout);
+                std::vector<float> wp = pad2(fold_wn(tt, r + "3", co_, 1, co_, true), co_, co_, B.cout, B.cout);
                 R.pw.w.upload(wp.data(), wp.size());
                 host_pw.push_back(wp);
-                load_bias(tt, r + "3", B.cout, R.pw);
+                load_bias(tt, r + "3", co_, R.pw, B.cout);
             }
         }
-        final_c = C >> c.n_decoder_rates;
         {
-            std::vector<float> a = tt.f32(p + std::to_string(li) + ".alpha", final_c);
+            const int fc = C >> c.n_decoder_rates;
+            final_c = enc_padded(fc);
+            std::vector<float> a = pad2(tt.f32(p + std::to_string(li) + ".alpha", fc), 1, fc, 1, final_c, 1.f);
             alpha_final.upload(a.data(), a.size());
-            std::vector<float> w = fold_wn(tt, p + std::to_string(li + 1), 1, 7, final_c, true);  // [1,7,C]
-            std::vector<float> wt((size_t)final_c * 7);
+            std::vector<float> w = fold_wn(tt, p + std::to_string(li + 1), 1, 7, fc, true);  // [1,7,C]
+            std::vector<float> wt((size_t)final_c * 7, 0.f);
             for (int k = 0; k < 7; ++k)
-                for (int ci = 0; ci < final_c; ++ci) wt[(size_t)ci * 7 + k] = w[(size_t)k * final_c + ci];
+                for (int ci = 0; ci < fc; ++ci) wt[(size_t)ci * 7 + k] = w[(size_t)k * fc + ci];
             final_conv.w.upload(wt.data(), wt.size());
             if (tt.find(p + std::to_string(li + 1) + ".bias")) final_bias = tt.f32(p + std::to_string(li + 1) + ".bias", 1)[0];
         }
@@ -799,14 +913,19 @@ struct b2a_snac {
         B2A_CUDA(cudaGetLastError());
         B2A_CUDA(cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, device));
         const char* env = getenv("B2A_SNAC");
-        bool shapes_ok = latent % 64 == 0 && C % 64 == 0 && final_c == FN_MAXC && c.noise != 0;
+        bool shapes_ok = latent % 64 == 0 && C % 64 == 0 && (final_c == 64 || final_c == 128) && c.noise != 0;
         for (auto& B : blocks) shapes_ok = shapes_ok && B.cin % 64 == 0 && B.cout % 64 == 0;
-        use_tc = shapes_ok && !(env && std::string(env) == "simt");
+        const bool simt = env && std::string(env) == "simt";
+        // the fp32 NCT decoder is the 24 kHz model's cross-check: it has no LocalMHA
+        B2A_CHECK(win == 0 || (shapes_ok && !simt), B2A_ERR_INVALID_INPUT,
+                  "SNAC: a LocalMHA model runs on the tensor-core path only (B2A_SNAC=simt, or a geometry it does not run)");
+        use_tc = shapes_ok && !simt;
         if (use_tc) {
             B2A_CUDA(cudaFuncSetAttribute(dw7_nlc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
             fused_attrs<64>(); fused_attrs<128>();
             B2A_CUDA(cudaFuncSetAttribute(rf::convt_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rf::convt_smem_bytes()));
-            B2A_CUDA(cudaFuncSetAttribute(final_nlc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (FN_TT + 6) * FN_MAXC * (int)sizeof(float)));
+            B2A_CUDA(cudaFuncSetAttribute(final_nlc_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (FN_TT + 6) * 64 * (int)sizeof(float)));
+            B2A_CUDA(cudaFuncSetAttribute(final_nlc_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (FN_TT + 6) * 128 * (int)sizeof(float)));
             pw0_tc.build(host_pw0, C, 1, latent);
             size_t ip = 0;
             for (size_t i = 0; i < blocks.size(); ++i) {
@@ -883,7 +1002,8 @@ struct b2a_snac {
             std::vector<float> bb = pad2(tt.f32(b + "4.bias", E.cout), 1, E.cout, 1, E.cp_out);
             E.down_b.bias.upload(bb.data(), bb.size()); E.down_b.has_bias = true;
         }
-        const std::string f = p + std::to_string(n + 1);
+        if (cfg.attn_window_size > 0) load_attn(tt, p + std::to_string(n + 1), c, cfg.attn_window_size, enc_attn);   // Layers.swift:339-341
+        const std::string f = p + std::to_string(n + (cfg.attn_window_size > 0 ? 2 : 1));
         std::vector<float> w = fold_wn(tt, f, c, 7, 1, true);                            // depthwise [C, 7, 1]
         enc_final.w.upload(w.data(), w.size());
         std::vector<float> b = tt.f32(f + ".bias", c);
@@ -922,7 +1042,9 @@ struct b2a_snac {
     bool convt_fused_ok(size_t i) const {
         if (i == 0 || i >= blocks.size()) return false;
         const DecBlock& B = blocks[i];
-        return B.cin == 128 && B.stride * B.cout == 128 && block_fused(blocks[i - 1]) && block_fused(B);
+        bool even = true;                     // lengths s * t: no odd stride up to here (stage_len)
+        for (size_t j = 0; j <= i; ++j) even = even && blocks[j].stride % 2 == 0;
+        return even && B.cin == 128 && B.stride * B.cout == 128 && block_fused(blocks[i - 1]) && block_fused(B);
     }
     template <int CC>
     static void fused_c(const TcW& W, const rf::Args& a, dim3 g, size_t sm, cudaStream_t s) {
@@ -950,20 +1072,53 @@ struct b2a_snac {
         launch_pdl(rf::convt_fused_kernel, dim3((unsigned)ctas), dim3(rf::THREADS), rf::convt_smem_bytes(), s, W.th, W.tl, a);
     }
 
-    void decode_dev_tc(const int* const* d_codes_in, int batch, long long T, const float* const* d_noise_in, int noise_mode,
-                       unsigned long long seed, float* d_wave_out, cudaStream_t s) {
+    // LocalMHA on the fp32 residual stream x [batch * T, dim]: LayerNorm -> hi/lo hA -> to_qkv (fp32 d_qkv) -> windowed attention ->
+    // hi/lo hA -> to_out, whose epilogue `o` (E_ADD, or E_ADD_HILO into the next transposed conv's operand) adds it into x
+    void local_mha(const LocalAttn& A, float* x, int batch, long long T, cg::Args o, cudaStream_t s) {
+        const long long ntok = (long long)batch * T;
+        d_qkv.alloc((size_t)ntok * 3 * A.dim);
+        dw_layernorm_kernel<SN_LN_MAXV><<<(unsigned)ntok, DL_THREADS, 0, s>>>(x, nullptr, nullptr, A.ln_w.p, A.ln_b.p, nullptr, hA.p, (int)T,
+                                                                             A.dim, 1, 1e-5f);
+        count_launch();
+        cg::Args a{};
+        a.N = (int)ntok; a.epi = cg::E_STORE_F32; a.x = d_qkv.p; a.ldx = 3 * A.dim;
+        cg::launch(A.qkv, hA.p, 2 * pad64(ntok), a, num_sms, s);
+        local_attn_kernel<<<dim3((unsigned)(T / A.window), A.dim / LA_D, batch), LA_THREADS, 0, s>>>(d_qkv.p, A.rope.p, hA.p, (int)T, A.dim,
+                                                                                                  A.window);
+        count_launch();
+        o.N = (int)ntok; o.x = x; o.ldx = A.dim;
+        cg::launch(A.out, hA.p, 2 * pad64(ntok), o, num_sms, s);
+    }
+
+    // largest workspace of a tensor-core decode of `batch` clips of T latent frames (elements); sets the buffer sizes when asked
+    size_t dec_workspace(int batch, long long T, size_t* mx = nullptr, size_t* mh = nullptr, size_t* mx2 = nullptr) const {
         const int C = cfg.decoder_dim;
-        // buffer sizes over all stages
         size_t max_x = (size_t)batch * T * std::max(latent, C), max_h = (size_t)(2 * pad64((long long)batch * T)) * (size_t)std::max(latent, C), max_x2 = 0;
-        {
-            long long t = T;
-            for (auto& B : blocks) {
-                max_x2 = std::max<size_t>(max_x2, (size_t)(2 * pad64((long long)batch * (t + 1))) * 2 * B.cin);
-                t *= B.stride;
-                max_x = std::max<size_t>(max_x, (size_t)batch * t * B.cout);
-                max_h = std::max<size_t>(max_h, (size_t)(2 * pad64((long long)batch * t)) * B.cout);
-            }
+        long long t = T;
+        for (auto& B : blocks) {
+            max_x2 = std::max<size_t>(max_x2, (size_t)(2 * pad64((long long)batch * (t + 1))) * 2 * B.cin);
+            t = stage_len(t, B.stride);
+            max_x = std::max<size_t>(max_x, (size_t)batch * t * B.cout);
+            max_h = std::max<size_t>(max_h, (size_t)(2 * pad64((long long)batch * t)) * B.cout);
         }
+        if (mx) { *mx = max_x; *mh = max_h; *mx2 = max_x2; }
+        return std::max(max_x, std::max(max_h, max_x2));
+    }
+    // clips per call so that every workspace stays below 2^31 elements (32-bit element indices and tensor-map extents): a batch is
+    // decoded / encoded in slices of whole clips, which gives exactly the batched result
+    template <class F>
+    static int clips_per_slice(int batch, F workspace) {
+        int nb = batch;
+        while (nb > 1 && workspace(nb) >= (size_t)1 << 31) nb = (nb + 1) / 2;
+        return nb;
+    }
+
+    // clip0: index of this call's first clip in the caller's batch (the seeded noise is drawn per (clip, frame) of the whole batch)
+    void decode_dev_tc(const int* const* d_codes_in, int batch, long long T, const float* const* d_noise_in, int noise_mode,
+                       unsigned long long seed, float* d_wave_out, cudaStream_t s, long long clip0 = 0) {
+        const int C = cfg.decoder_dim;
+        size_t max_x, max_h, max_x2;
+        dec_workspace(batch, T, &max_x, &max_h, &max_x2);
         xs.alloc(max_x); xs2.alloc(max_x); hA.alloc(max_h); x2.alloc(max_x2);
         // RVQ lookup -> z (NLC) ; depthwise k7 -> hi/lo ; 1x1 (768 -> 1024) + Snake(block 0) -> 2-tap im2col of block 0
         RvqArgs ra{};
@@ -977,14 +1132,23 @@ struct b2a_snac {
             x2_zero_edges_kernel<<<batch, 256, 0, s>>>(x2.p, (int)T, C);
             count_launch();
             cg::Args a{};
-            a.N = (int)(batch * T); a.epi = cg::E_STORE_HILO; a.bias = pw0.has_bias ? pw0.bias.p : nullptr; a.alpha = blocks[0].alpha.p;
-            a.hl = x2.p; a.ldh = 2 * C; a.dual = 1; a.T = (int)T;
+            a.N = (int)(batch * T); a.bias = pw0.has_bias ? pw0.bias.p : nullptr;
+            cg::Args o{};        // the epilogue that writes Snake(block 0) into block 0's 2-tap im2col
+            o.epi = cg::E_STORE_HILO; o.alpha = blocks[0].alpha.p; o.hl = x2.p; o.ldh = 2 * C; o.dual = 1; o.T = (int)T;
+            if (dec_attn.dim) { a.epi = cg::E_STORE_F32; a.x = xs.p; a.ldx = C; }
+            else { a.epi = o.epi; a.alpha = o.alpha; a.hl = o.hl; a.ldh = o.ldh; a.dual = o.dual; a.T = o.T; }
             cg::launch(pw0_tc, hA.p, 2 * pad64((long long)batch * T), a, num_sms, s);
+            if (dec_attn.dim) {      // LocalMHA (Layers.swift:395-397), its residual add carrying block 0's Snake into the im2col
+                o.epi = cg::E_ADD_HILO;
+                local_mha(dec_attn, xs.p, batch, T, o, s);
+            }
         }
         long long t = T;
         for (size_t i = 0; i < blocks.size(); ++i) {
             DecBlock& B = blocks[i];
-            const long long tout = t * B.stride, ntok = (long long)batch * tout;
+            const long long tout = stage_len(t, B.stride), ntok = (long long)batch * tout;
+            // NoiseBlock seed of this stage, shifted so that a slice of clips draws what the whole batch would (cg::gauss(seed, idx))
+            const unsigned long long nseed = seed + 0x1000193ull * (i + 1) + 0x9E3779B97F4A7C15ull * (unsigned long long)(clip0 * tout);
             if (convt_fused_ok(i)) {
                 // last block: Snake + transposed conv straight from the previous block's fp32 output (no 2-tap im2col round trip)
                 rf::ConvtArgs a{};
@@ -1008,7 +1172,7 @@ struct b2a_snac {
                 if (B.has_noise && (nz || noise_mode == 0)) {
                     rf::Args a{};
                     a.x = cur; a.y = oth; a.C = B.cout; a.mode = rf::MODE_NOISE; a.dil = 0; a.noise = nz;
-                    a.seed = seed + 0x1000193ull * (i + 1);
+                    a.seed = nseed;
                     fused(B.cout == 64 ? B.noise_bd : B.noise_tc, a, batch, tout, s);
                     std::swap(cur, oth);
                 }
@@ -1018,12 +1182,15 @@ struct b2a_snac {
                     a.x = cur; a.y = oth; a.C = B.cout; a.mode = rf::MODE_RU; a.dil = R.dil;
                     a.dw_w = R.dw.w.p; a.dw_b = R.dw.has_bias ? R.dw.bias.p : nullptr; a.a_in = R.a0.p; a.a_mid = R.a2.p;
                     a.pw_bias = R.pw.has_bias ? R.pw.bias.p : nullptr;
-                    if (u == 2 && i + 1 < blocks.size() && !convt_fused_ok(i + 1)) {
+                    const bool to_x2 = u == 2 && i + 1 < blocks.size() && !convt_fused_ok(i + 1);
+                    if (to_x2) { a.hl = x2.p; a.a_next = blocks[i + 1].alpha.p; }
+                    fused(B.cout == 64 ? R.pw_bd : R.pw_tc, a, batch, tout, s);
+                    if (to_x2) {
+                        // after the unit (it writes other positions of x2): a plain launch between the last fused unit and the next
+                        // transposed conv's GEMM, whose TMA producer reads x2 without waiting on the programmatic dependency
                         x2_zero_edges_kernel<<<batch, 256, 0, s>>>(x2.p, (int)tout, B.cout);
                         count_launch();
-                        a.hl = x2.p; a.a_next = blocks[i + 1].alpha.p;
                     }
-                    fused(B.cout == 64 ? R.pw_bd : R.pw_tc, a, batch, tout, s);
                     std::swap(cur, oth);
                 }
                 if (cur != xs.p) { std::swap(xs.p, xs2.p); std::swap(xs.n, xs2.n); }       // the live activation is always xs
@@ -1033,7 +1200,7 @@ struct b2a_snac {
             if (B.has_noise && (nz || noise_mode == 0)) {
                 cg::Args a{};
                 a.N = (int)ntok; a.epi = cg::E_NOISE; a.x = xs.p; a.ldx = B.cout; a.noise = nz;
-                a.seed = seed + 0x1000193ull * (i + 1); a.T = (int)tout;
+                a.seed = nseed; a.T = (int)tout;
                 cg::launch(B.noise_tc, hA.p, 2 * pad64(ntok), a, num_sms, s);
             }
             for (int u = 0; u < 3; ++u) {
@@ -1052,8 +1219,12 @@ struct b2a_snac {
             }
             t = tout;
         }
-        final_nlc_kernel<<<dim3(cdiv(t, FN_TT), batch), FN_THREADS, (FN_TT + 6) * FN_MAXC * sizeof(float), s>>>(xs.p, d_wave_out, final_conv.w.p, alpha_final.p, final_bias,
-                                                                            (int)t, final_c);
+        if (final_c == 64)
+            final_nlc_kernel<64><<<dim3(cdiv(t, FN_TT), batch), FN_THREADS, (FN_TT + 6) * 64 * sizeof(float), s>>>(xs.p, d_wave_out, final_conv.w.p, alpha_final.p,
+                                                                                                              final_bias, (int)t, final_c);
+        else
+            final_nlc_kernel<128><<<dim3(cdiv(t, FN_TT), batch), FN_THREADS, (FN_TT + 6) * 128 * sizeof(float), s>>>(xs.p, d_wave_out, final_conv.w.p, alpha_final.p,
+                                                                                                                final_bias, (int)t, final_c);
         count_launch();
         B2A_CUDA(cudaGetLastError());
     }
@@ -1095,9 +1266,26 @@ struct b2a_snac {
         for (auto& L : levels)
             B2A_CHECK(T % L.stride == 0, B2A_ERR_INVALID_INPUT, "snac decode: t_latent must be a multiple of every vq stride");
         B2A_CHECK(T * hop < (1ll << 31) / 2, B2A_ERR_INVALID_INPUT, "snac decode: sequence too long");
+        B2A_CHECK(dec_attn.window == 0 || T % dec_attn.window == 0, B2A_ERR_INVALID_INPUT,
+                  "snac decode: t_latent must be a multiple of attn_window_size (LocalMHA windows)");
         B2A_CUDA(cudaSetDevice(device));
-        if (use_tc && (long long)batch * T * hop < (1ll << 31) - 64) {
-            decode_dev_tc(d_codes_in, batch, T, d_noise_in, noise_mode, seed, d_wave_out, s);
+        const bool tc_fits = (long long)batch * T * hop < (1ll << 31) - 64;
+        B2A_CHECK(dec_attn.dim == 0 || tc_fits, B2A_ERR_INVALID_INPUT, "snac decode: batch * t_latent * hop must be < 2^31");
+        if (use_tc && tc_fits) {
+            const int nb = clips_per_slice(batch, [&](int n) { return dec_workspace(n, T); });
+            const long long tw = decoded_length(T);
+            for (int b0 = 0; b0 < batch; b0 += nb) {
+                const int n = std::min(nb, batch - b0);
+                const int* dc[8];
+                const float* dn[8];
+                for (size_t i = 0; i < levels.size(); ++i) dc[i] = d_codes_in[i] + (long long)b0 * (T / levels[i].stride);
+                long long t = T;
+                for (size_t i = 0; i < blocks.size(); ++i) {
+                    t = stage_len(t, blocks[i].stride);
+                    dn[i] = d_noise_in && d_noise_in[i] ? d_noise_in[i] + (long long)b0 * t : nullptr;
+                }
+                decode_dev_tc(dc, n, T, d_noise_in ? dn : nullptr, noise_mode, seed, d_wave_out + (long long)b0 * tw, s, b0);
+            }
             return;
         }
         const size_t need = max_act(batch, T);
@@ -1120,7 +1308,7 @@ struct b2a_snac {
         long long t = T;
         for (size_t i = 0; i < blocks.size(); ++i) {
             DecBlock& B = blocks[i];
-            const long long tout = t * B.stride;
+            const long long tout = stage_len(t, B.stride);
             // transposed conv: X [cin, t] (already Snake-activated) -> Y [cout, tout]
             gemm(EPI_CONVT, B.ct, X, Y, nullptr, nullptr, nullptr, batch, B.cout * B.stride, (int)t + 1, 2 * B.cin, B.cin,
                  (int)t, B.cout, (int)tout, B.stride, B.pad, 0, 0, s);
@@ -1149,11 +1337,18 @@ struct b2a_snac {
         B2A_CUDA(cudaGetLastError());
     }
 
+    // samples out of t_latent frames: every stage's length is stage_len's
+    long long decoded_length(long long T) const {
+        for (auto& B : blocks) T = stage_len(T, B.stride);
+        return T;
+    }
+
     // ---- encode (SNACDecoder.swift:86-105,120-125) ----------------------------------------------------------------------------
-    // padded length: a multiple of hop * lcm(vq_strides) (SNACDecoder.swift:86-100)
+    // padded length: a multiple of hop * lcm(vq_strides, attn_window_size) (SNACDecoder.swift:86-100)
     long long enc_pad_multiple() const {
         long long l = 1;
         for (auto& L : levels) l = std::lcm(l, (long long)L.stride);
+        if (cfg.attn_window_size > 0) l = std::lcm(l, (long long)cfg.attn_window_size);
         return (long long)enc_hop * l;
     }
     long long encoded_length(long long n) const {
@@ -1173,22 +1368,37 @@ struct b2a_snac {
     }
     // stages at the fused unit's widths; the others run dw7_nlc_kernel + the conv GEMM through the hi/lo operand hA
     static bool enc_fused(const EncBlock& E) { return E.cp == 64 || E.cp == 128; }
-    // d_wave [B, n] -> z [B, latent, T_lat] fp32 NCT in d_zenc (returned); channels-last fp32 stream + bf16 hi/lo GEMM operands
+    // largest workspace of encoding `batch` clips of T0 padded samples (elements); sets the buffer sizes when asked
+    size_t enc_workspace(int batch, long long T0, size_t* mx = nullptr, size_t* mh = nullptr, size_t* mx2 = nullptr) const {
+        size_t max_x = 0, max_h = 0, max_x2 = 0;
+        long long t = T0;
+        for (auto& E : eblocks) {
+            max_x = std::max<size_t>(max_x, (size_t)batch * t * E.cp);
+            if (!enc_fused(E)) max_h = std::max<size_t>(max_h, (size_t)(2 * pad64((long long)batch * t)) * E.cp);   // dw7 -> GEMM operand
+            t /= E.stride;
+            max_x2 = std::max<size_t>(max_x2, (size_t)(2 * pad64((long long)batch * (t + 1))) * 2 * E.stride * E.cp);
+            max_x = std::max<size_t>(max_x, (size_t)batch * t * E.cp_out);
+        }
+        if (enc_attn.dim) max_h = std::max<size_t>(max_h, (size_t)(2 * pad64((long long)batch * t)) * latent);   // LocalMHA operands
+        if (mx) { *mx = max_x; *mh = max_h; *mx2 = max_x2; }
+        return std::max(max_x, std::max(max_h, max_x2));
+    }
+    // d_wave [B, n] -> z [B, latent, T_lat] fp32 NCT in d_zenc (returned), in slices of whole clips (clips_per_slice)
     float* encode_latent_dev(const float* d_wave_in, int batch, long long n, cudaStream_t s) {
         const long long tl = encoded_length(n), T0 = tl * enc_hop;
-        size_t max_x = (size_t)batch * tl * latent, max_h = 0, max_x2 = 0;
-        {
-            long long t = T0;
-            for (auto& E : eblocks) {
-                max_x = std::max<size_t>(max_x, (size_t)batch * t * E.cp);
-                if (!enc_fused(E)) max_h = std::max<size_t>(max_h, (size_t)(2 * pad64((long long)batch * t)) * E.cp);   // dw7 -> GEMM operand
-                t /= E.stride;
-                max_x2 = std::max<size_t>(max_x2, (size_t)(2 * pad64((long long)batch * (t + 1))) * 2 * E.stride * E.cp);
-                max_x = std::max<size_t>(max_x, (size_t)batch * t * E.cp_out);
-            }
-        }
-        xs.alloc(max_x); xs2.alloc(max_x); hA.alloc(max_h); x2.alloc(max_x2);
         d_zenc.alloc((size_t)batch * latent * tl);
+        const int nb = clips_per_slice(batch, [&](int c) { return enc_workspace(c, T0); });
+        for (int b0 = 0; b0 < batch; b0 += nb)
+            encode_latent_slice(d_wave_in + (long long)b0 * n, std::min(nb, batch - b0), n, d_zenc.p + (long long)b0 * latent * tl, s);
+        return d_zenc.p;
+    }
+    // channels-last fp32 stream + bf16 hi/lo GEMM operands
+    void encode_latent_slice(const float* d_wave_in, int batch, long long n, float* d_z, cudaStream_t s) {
+        const long long tl = encoded_length(n), T0 = tl * enc_hop;
+        size_t max_x, max_h, max_x2;
+        enc_workspace(batch, T0, &max_x, &max_h, &max_x2);
+        max_x = std::max<size_t>(max_x, (size_t)batch * tl * latent);
+        xs.alloc(max_x); xs2.alloc(max_x); hA.alloc(max_h); x2.alloc(max_x2);
         {
             const int cp0 = eblocks[0].cp;
             const long long nthr = (long long)batch * T0 * (cp0 / 4);
@@ -1234,11 +1444,15 @@ struct b2a_snac {
             }
             t = tout;
         }
-        enc_final_dw_kernel<<<dim3(cdiv(t, 32), cdiv(latent, 32), batch), dim3(32, 8), 0, s>>>(xs.p, d_zenc.p, enc_final.w.p, enc_final.bias.p,
+        if (enc_attn.dim) {          // LocalMHA (Layers.swift:339-341) adds into the last block's output, ld = cp_out = latent
+            cg::Args o{};
+            o.epi = cg::E_ADD;
+            local_mha(enc_attn, xs.p, batch, t, o, s);
+        }
+        enc_final_dw_kernel<<<dim3(cdiv(t, 32), cdiv(latent, 32), batch), dim3(32, 8), 0, s>>>(xs.p, d_z, enc_final.w.p, enc_final.bias.p,
                                                                                              (int)t, latent, eblocks.back().cp_out);
         count_launch();
         B2A_CUDA(cudaGetLastError());
-        return d_zenc.p;
     }
     // residual VQ (VQ.swift:47-120,150-163) of d_res = z [B, latent, T] fp32 on the device (left holding the final residual):
     // codes of level i -> d_codes_out[i] [B, T / stride_i]; z_q accumulated into d_zq_out when non-null
@@ -1292,6 +1506,7 @@ int32_t b2a_snac_create(int32_t device, const b2a_snac_config* cfg, const b2a_te
 }
 
 int64_t b2a_snac_hop_length(const b2a_snac* h) { return h ? h->hop : 0; }
+int64_t b2a_snac_decoded_length(const b2a_snac* h, int64_t t_latent) { return h && t_latent > 0 ? h->decoded_length(t_latent) : 0; }
 void* b2a_snac_stream(b2a_snac* h) { return h ? (void*)h->stream : nullptr; }
 
 int32_t b2a_snac_decode_dev(b2a_snac* h, const int32_t* const* d_codes, int32_t batch, int64_t T,
@@ -1322,7 +1537,7 @@ int32_t b2a_snac_decode(b2a_snac* h, const int32_t* const* codes, int32_t batch,
         bool any_noise = false;
         long long t = T;
         for (size_t i = 0; i < h->blocks.size(); ++i) {
-            t *= h->blocks[i].stride;
+            t = stage_len(t, h->blocks[i].stride);
             if (noise && noise[i]) {
                 h->d_noise[i].alloc((size_t)batch * t);
                 B2A_CUDA(cudaMemcpyAsync(h->d_noise[i].p, noise[i], (size_t)batch * t * sizeof(float), cudaMemcpyHostToDevice, s));
@@ -1513,6 +1728,33 @@ extern "C" int32_t b2a_snac_convt_test(const float* x, float* y, const float* al
         b2a_snac::launch_convt(W, a, hook_ctas(ctas), s);
         B2A_CUDA(cudaGetLastError());
         B2A_CUDA(cudaStreamSynchronize(s));
+    });
+}
+
+// One launch of LocalMHA's window core (local_attn_kernel) on HOST data: qkv fp32 [B * T, 3 dim] (q | k | v, rotary not yet applied),
+// inv_freq [32] -> out fp32 [B * T, dim] (the hi + lo pair the kernel writes for to_out), T a multiple of the window.
+extern "C" int32_t b2a_snac_local_attn_test(const float* qkv, const float* inv_freq, int32_t B, int32_t T, int32_t dim, int32_t window,
+                                            float* out) {
+    return guarded([&] {
+        B2A_CHECK(qkv && inv_freq && out && B >= 1 && T >= 1 && dim >= LA_D && dim % LA_D == 0 && window >= 1 && window <= LA_MAXW &&
+                      T % window == 0 && (long long)B * T * 3 * dim < (1ll << 31),
+                  B2A_ERR_INVALID_INPUT, "b2a_snac_local_attn_test: bad argument");
+        require_device(0);
+        const long long ntok = (long long)B * T, rows = 2 * b2a_snac::pad64(ntok);
+        DBuf<float> dq, dr;
+        DBuf<__nv_bfloat16> dh;
+        dq.upload(qkv, (size_t)ntok * 3 * dim);
+        dh.alloc((size_t)rows * dim);
+        const std::vector<float> r = rope_table(inv_freq, window);
+        dr.upload(r.data(), r.size());
+        local_attn_kernel<<<dim3(T / window, dim / LA_D, B), LA_THREADS>>>(dq.p, dr.p, dh.p, T, dim, window);
+        B2A_CUDA(cudaGetLastError());
+        std::vector<uint16_t> hl((size_t)rows * dim);
+        B2A_CUDA(cudaMemcpy(hl.data(), dh.p, hl.size() * sizeof(uint16_t), cudaMemcpyDeviceToHost));
+        for (long long t = 0; t < ntok; ++t) {
+            const long long rr = (t / 64) * 128 + t % 64;
+            for (int c = 0; c < dim; ++c) out[t * dim + c] = cg::join16(hl[rr * dim + c], hl[(rr + 64) * dim + c], 0);
+        }
     });
 }
 

@@ -10,6 +10,7 @@
 // leaves the device and the result is deterministic.
 #include "common.cuh"
 #include "conv_gemm.cuh"
+#include "layernorm.cuh"
 
 #include <algorithm>
 #include <cmath>
@@ -34,56 +35,7 @@ __global__ void im2colk_kernel(const float* __restrict__ in, bf16* __restrict__ 
     }
 }
 
-// (optional depthwise conv k over time) -> LayerNorm(eps) over channels.  One CTA per token, one thread per channel slot.
-// out_f32 (nullable): normalised row as fp32 (residual stream) ; out_hl (nullable): hi/lo tiles (GEMM input).
-constexpr int DL_THREADS = 256, DL_MAXV = 4;    // channels <= 1024
-__global__ void __launch_bounds__(DL_THREADS)
-dw_layernorm_kernel(const float* __restrict__ x, const float* __restrict__ dw_w /*[C,k] or null*/, const float* __restrict__ dw_b,
-                    const float* __restrict__ ln_w, const float* __restrict__ ln_b, float* __restrict__ out_f32,
-                    bf16* __restrict__ out_hl, int L, int C, int k, float eps, int ln_batch_stride = 0) {
-    __shared__ float red[DL_THREADS / 32];
-    const long long tok = blockIdx.x;
-    const int b = (int)(tok / L), t = (int)(tok - (long long)b * L);
-    ln_w += (long long)b * ln_batch_stride;     // AdaLayerNorm: the gain / shift rows of this utterance's conditioning (0 = shared LayerNorm)
-    ln_b += (long long)b * ln_batch_stride;
-    float v[DL_MAXV];
-    float s = 0.f;
-#pragma unroll
-    for (int j = 0; j < DL_MAXV; ++j) {
-        const int c = threadIdx.x + j * DL_THREADS;
-        float val = 0.f;
-        if (c < C) {
-            if (dw_w) {
-                val = dw_b ? dw_b[c] : 0.f;
-                for (int kk = 0; kk < k; ++kk) {
-                    const int ti = t + kk - k / 2;
-                    if (ti >= 0 && ti < L) val = fmaf(dw_w[c * k + kk], x[((long long)b * L + ti) * C + c], val);
-                }
-            } else {
-                val = x[tok * C + c];
-            }
-        }
-        v[j] = val;
-        s += val;
-    }
-    const float mean = block_sum<DL_THREADS>(s, red) / (float)C;
-    float q = 0.f;
-#pragma unroll
-    for (int j = 0; j < DL_MAXV; ++j) {
-        const int c = threadIdx.x + j * DL_THREADS;
-        if (c < C) { const float d = v[j] - mean; q += d * d; }
-    }
-    const float r = rsqrtf(block_sum<DL_THREADS>(q, red) / (float)C + eps);
-#pragma unroll
-    for (int j = 0; j < DL_MAXV; ++j) {
-        const int c = threadIdx.x + j * DL_THREADS;
-        if (c < C) {
-            const float o = (v[j] - mean) * r * ln_w[c] + ln_b[c];
-            if (out_f32) out_f32[tok * C + c] = o;
-            if (out_hl) tc::store_hilo(out_hl, C, tok, c, o, cg::HALF);
-        }
-    }
-}
+constexpr int DL_MAXV = 4;    // channels <= 1024 (dw_layernorm_kernel, layernorm.cuh)
 
 // AdaLayerNorm's conditioning (Vocos.swift:31-33): for every norm n and utterance b,  gain[n, b, :] = Ws_n cond_b + bs_n  and
 // shift[n, b, :] = Wh_n cond_b + bh_n.  W [norms][dim][E] (scale then shift stacked: [2][norms][dim][E]), cond [B][E].
@@ -260,12 +212,12 @@ struct b2a_vocos {
             cg::Args a{}; a.N = (int)T; a.epi = cg::E_STORE_F32; a.bias = embed_b.p; a.x = spec.p; a.ldx = D;      // spec doubles as scratch [T, D]
             cg::launch(embed, xa.p, 2 * Tp, a, num_sms, s);
         }
-        dw_layernorm_kernel<<<(unsigned)T, DL_THREADS, 0, s>>>(spec.p, nullptr, nullptr, g0, b0, h.p, nullptr, L, D, 1, 1e-6f, bs);
+        dw_layernorm_kernel<DL_MAXV><<<(unsigned)T, DL_THREADS, 0, s>>>(spec.p, nullptr, nullptr, g0, b0, h.p, nullptr, L, D, 1, 1e-6f, bs);
         count_launch();
         int li = 0;
         for (auto& Bk : blocks) {
             ++li;
-            dw_layernorm_kernel<<<(unsigned)T, DL_THREADS, 0, s>>>(h.p, Bk.dw_w.p, Bk.dw_b.p, gain(li, Bk.ln_w.p), shift(li, Bk.ln_b.p), nullptr, xa.p, L, D,
+            dw_layernorm_kernel<DL_MAXV><<<(unsigned)T, DL_THREADS, 0, s>>>(h.p, Bk.dw_w.p, Bk.dw_b.p, gain(li, Bk.ln_w.p), shift(li, Bk.ln_b.p), nullptr, xa.p, L, D,
                                                                    cfg.dw_kernel_size, 1e-6f, bs);
             count_launch();
             cg::Args a1{}; a1.N = (int)T; a1.epi = cg::E_STORE_HILO; a1.bias = Bk.pw1_b.p; a1.gelu = 1; a1.hl = xb.p; a1.ldh = I; a1.T = L;
@@ -273,7 +225,7 @@ struct b2a_vocos {
             cg::Args a2{}; a2.N = (int)T; a2.epi = cg::E_ADD; a2.bias = Bk.pw2_b.p; a2.x = h.p; a2.ldx = D; a2.gamma = Bk.gamma.p;      // h += gamma * pw2(...)
             cg::launch(Bk.pw2, xb.p, 2 * Tp, a2, num_sms, s);
         }
-        dw_layernorm_kernel<<<(unsigned)T, DL_THREADS, 0, s>>>(h.p, nullptr, nullptr, nf_w.p, nf_b.p, nullptr, xa.p, L, D, 1, 1e-6f);
+        dw_layernorm_kernel<DL_MAXV><<<(unsigned)T, DL_THREADS, 0, s>>>(h.p, nullptr, nullptr, nf_w.p, nf_b.p, nullptr, xa.p, L, D, 1, 1e-6f);
         count_launch();
         {
             cg::Args a{}; a.N = (int)T; a.epi = cg::E_STORE_F32; a.bias = head_b.p; a.x = spec.p; a.ldx = N + 2;

@@ -40,15 +40,23 @@ class SNAC:
         _ffi.check(_ffi.lib().b2a_snac_create(device, C.byref(cfg), table, len(weights), C.byref(self._h)))
         del keep
         self.hop_length = int(_ffi.lib().b2a_snac_hop_length(self._h))
+        self.attn_window_size = attn_window_size or 0
+
+    def decoded_length(self, t_latent: int) -> int:
+        """Samples decoded from t_latent frames: t_latent * hop_length, less one frame per odd-stride decoder stage (the reference
+        drops DecoderBlock's outputPadding), e.g. 384 t_latent - 2 for the 32 / 44 kHz models."""
+        return int(_ffi.lib().b2a_snac_decoded_length(self._h, t_latent))
 
     @staticmethod
     def random_init_weights(seed: int = 1234, latent: int = 768, decoder_dim: int = 1024,
                             decoder_rates: Sequence[int] = (8, 8, 4, 2), vq_strides: Sequence[int] = (4, 2, 1),
                             codebook_size: int = 4096, codebook_dim: int = 8, encoder: bool = False, encoder_dim: int = 48,
-                            encoder_rates: Sequence[int] = (2, 4, 8, 8)) -> Dict[str, np.ndarray]:
+                            encoder_rates: Sequence[int] = (2, 4, 8, 8), attn_window_size: Optional[int] = None) -> Dict[str, np.ndarray]:
         """Random-init snac_24khz-shaped weights (benchmarks): conv v ~ U(+-1/sqrt(fan_in)) as
         Layers.swift:81-86, g = ||v||, zero biases, Snake alpha = 1.  encoder=True appends the encoder's
-        weights (drawn after everything else, so the decoder / quantizer weights do not change)."""
+        weights (drawn after everything else, so the decoder / quantizer weights do not change).
+        attn_window_size adds the 32 / 44 kHz models' LocalMHA blocks (decoder.model.layers.2 and, with the encoder,
+        encoder.block.layers.{n+1}), drawn from a generator of their own (seed + 1), so every other tensor is unchanged."""
         rng = np.random.default_rng(seed)
         w: Dict[str, np.ndarray] = {}
 
@@ -65,10 +73,23 @@ class SNAC:
             wn(q + ".in_proj", (codebook_dim, 1, latent), latent, codebook_dim)
             wn(q + ".out_proj", (latent, 1, codebook_dim), codebook_dim, latent)
             w[q + ".codebook.weight"] = rng.standard_normal((codebook_size, codebook_dim)).astype(np.float32)
+        arng = np.random.default_rng(seed + 1)
+
+        def attn(prefix, dim):       # LocalMHA (Attention.swift:14-95): LayerNorm, to_qkv / to_out without bias, rotary inv_freq
+            s = (1.0 / dim) ** 0.5
+            w[prefix + ".norm.weight"] = np.ones(dim, dtype=np.float32)
+            w[prefix + ".norm.bias"] = np.zeros(dim, dtype=np.float32)
+            w[prefix + ".to_qkv.weight"] = arng.uniform(-s, s, size=(3 * dim, dim)).astype(np.float32)
+            w[prefix + ".to_out.weight"] = arng.uniform(-s, s, size=(dim, dim)).astype(np.float32)
+            w[prefix + ".rel_pos.inv_freq"] = (1.0 / 10000.0 ** (np.arange(0, 64, 2) / 64.0)).astype(np.float32)
+
         p = "decoder.model.layers"
         wn(f"{p}.0", (latent, 7, 1), 7 * latent, latent)
         wn(f"{p}.1", (decoder_dim, 1, latent), latent, decoder_dim)
         li = 2
+        if attn_window_size:
+            attn(f"{p}.2", decoder_dim)
+            li = 3
         for i, s in enumerate(decoder_rates):
             cin, cout = decoder_dim // 2 ** i, decoder_dim // 2 ** (i + 1)
             b = f"{p}.{li}.block.layers"
@@ -99,7 +120,9 @@ class SNAC:
                 w[f"{b}.3.alpha"] = np.ones((1, d, 1), dtype=np.float32)
                 wn(f"{b}.4", (2 * d, 2 * s, d), 2 * s * d, 2 * d)
                 d *= 2
-            wn(f"{p}.{len(encoder_rates) + 1}", (d, 7, 1), 7, d)
+            if attn_window_size:
+                attn(f"{p}.{len(encoder_rates) + 1}", d)
+            wn(f"{p}.{len(encoder_rates) + 1 + bool(attn_window_size)}", (d, 7, 1), 7, d)
         return w
 
     # -- loading (SNACDecoder.swift:135-189) ------------------------------------------------------
@@ -130,8 +153,8 @@ class SNAC:
 
     def decode(self, codes: List[np.ndarray], noise: Optional[List[Optional[np.ndarray]]] = None,
                zero_noise: bool = False, seed: int = 0, out: Optional[np.ndarray] = None) -> np.ndarray:
-        """SNAC.decode (:127-131): codes[i] [B, T_i] int -> waveform [B, 1, T*hop] float32.
-        `noise[i]` supplies NoiseBlock i's Gaussian draw explicitly (SURVEY.md F6)."""
+        """SNAC.decode (:127-131): codes[i] [B, T_i] int -> waveform [B, 1, decoded_length(T)] float32.
+        `noise[i]` supplies NoiseBlock i's Gaussian draw explicitly (SURVEY.md F6), [B, 1, length of stage i's output]."""
         cs = [np.ascontiguousarray(c, dtype=np.int32) for c in codes]
         if len(cs) != self.n_codebooks:
             raise _ffi.AudioGenerationError(_ffi.ERR_INVALID_INPUT, f"expected {self.n_codebooks} code layers")
@@ -145,8 +168,9 @@ class SNAC:
         if noise is not None:
             nz = [None if n is None else np.ascontiguousarray(n, dtype=np.float32) for n in noise]
             np_ = (C.c_void_p * len(self.decoder_rates))(*[None if n is None else n.ctypes.data for n in nz])
-        wave = out if out is not None else np.empty((B, 1, T * self.hop_length), dtype=np.float32)   # `out`: a caller-owned (e.g. pinned) buffer
-        assert wave.shape == (B, 1, T * self.hop_length) and wave.dtype == np.float32 and wave.flags["C_CONTIGUOUS"]
+        n_out = self.decoded_length(T)
+        wave = out if out is not None else np.empty((B, 1, n_out), dtype=np.float32)   # `out`: a caller-owned (e.g. pinned) buffer
+        assert wave.shape == (B, 1, n_out) and wave.dtype == np.float32 and wave.flags["C_CONTIGUOUS"]
         _ffi.check(_ffi.lib().b2a_snac_decode(self._h, cp, B, T, np_, int(zero_noise), seed, _ffi.ptr(wave)))
         return wave
 
@@ -170,14 +194,15 @@ class SNAC:
             self._check_dev(c, "int32", (B, T // s), f"code layer {i}")
 
     def decode_dev(self, d_codes, d_wave, zero_noise: bool = False, seed: int = 0, stream: int = 0) -> None:
-        """Device-resident decode: torch CUDA int32 tensors [B, T_i] -> d_wave [B, 1, T*hop]."""
+        """Device-resident decode: torch CUDA int32 tensors [B, T_i] -> d_wave [B, 1, decoded_length(T)]."""
         if len(d_codes) != self.n_codebooks or d_codes[0].dim() != 2:
             raise _ffi.AudioGenerationError(_ffi.ERR_INVALID_INPUT, f"expected {self.n_codebooks} code layers [B, T_i]")
         B = d_codes[0].shape[0]
         T = d_codes[0].shape[1] * self.vq_strides[0]
         self._check_code_list(d_codes, B, T)
-        n_out = B * T * self.hop_length          # any contiguous layout of [B, 1, T*hop], as before
-        self._check_dev(d_wave, "float32", tuple(d_wave.shape) if getattr(d_wave, "numel", lambda: -1)() == n_out else (B, 1, T * self.hop_length), "d_wave")
+        n_wave = self.decoded_length(T)
+        n_out = B * n_wave                       # any contiguous layout of [B, 1, decoded_length(T)], as before
+        self._check_dev(d_wave, "float32", tuple(d_wave.shape) if getattr(d_wave, "numel", lambda: -1)() == n_out else (B, 1, n_wave), "d_wave")
         cp = (C.c_void_p * len(d_codes))(*[c.data_ptr() for c in d_codes])
         _ffi.check(_ffi.lib().b2a_snac_decode_dev(self._h, cp, B, T, None, int(zero_noise), seed, _ffi.ptr(d_wave),
                                                   C.c_void_p(stream)))
