@@ -622,8 +622,12 @@ int32_t b2a_speech_tokenizer_create_from_directory(const char* dir, int32_t devi
  * Weights: the reference's keys after sanitize strips "talker." (model.layers.N.*, model.codec_embedding.weight,
  * model.text_embedding.weight, text_projection.linear_fc{1,2}.{weight,bias}, codec_head.weight, code_predictor.model.layers.N.*,
  * code_predictor.model.codec_embedding.I.weight, code_predictor.lm_head.I.weight), bf16 or f32 (rounded to bf16: the engine holds
- * bf16 matrices; an MLX affine-quantised (8-bit) checkpoint is expanded by b2a_weights_dequantize first).  head_dim must be 128
- * and the predictor's hidden size must equal the talker's (no small_to_mtp_projection) -- true of the shipped 0.6B geometry.   */
+ * bf16 matrices; an MLX affine-quantised (8-bit) checkpoint is expanded by b2a_weights_dequantize first).  head_dim must be 128.
+ * When cp_hidden_size != hidden_size (the 1.7B checkpoints: 2048 -> 1024) the checkpoint must also hold
+ * code_predictor.small_to_mtp_projection.{weight [cp_hidden, hidden], bias [cp_hidden]} (else B2A_ERR_MODEL_NOT_INITIALIZED), applied
+ * to every predictor input as the reference does (Qwen3TTSCodePredictor.swift:200-238); the lm heads are [cp_vocab, cp_hidden] and
+ * the predictor's codec_embedding.I stay [cp_vocab, hidden].  The projected embedding tables are precomputed at creation in fp32:
+ * (vocab + (num_code_groups - 2) * cp_vocab) * cp_hidden * 4 bytes of device memory, about 130 MB at 1.7B.                    */
 typedef struct b2a_qwen3_talker_config {
     int32_t vocab_size;            /* codec vocabulary (3072) */
     int32_t hidden_size;

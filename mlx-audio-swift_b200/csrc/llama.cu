@@ -1122,8 +1122,9 @@ struct b2a_tts {
     enum { OP_QKV, OP_GU, OP_LM };
     // D[tokens, M] = X[tokens, K] * W[M, K]^T on the wgmma path (hi/lo activations, BN = 16)
     void tc_gemm(const CUtensorMap& tmW, const CUtensorMap& tmX, int op, float* yout, bf16* actout, int B, int M, int K,
-                 cudaStream_t s, const float* rstd_ss = nullptr) {
+                 cudaStream_t s, const float* rstd_ss = nullptr, const float* bias = nullptr) {
         tc::Args a{};
+        a.bias = bias;
         a.rstd_ss = rstd_ss; a.rstd_parts = fused_parts; a.rstd_inv_h = 1.0f / (float)cfg.hidden_size; a.rstd_eps = cfg.rms_norm_eps;
         a.out_f32 = yout; a.out_bf16 = actout; a.M = M; a.N = B; a.K = K;
         a.m_tiles = cdiv(M, tc::BM); a.k_blocks = K / tc::BK;
@@ -1226,10 +1227,11 @@ struct b2a_tts {
                    LO_ROW, (float*)nullptr, 0);
         tc_gemm(tm_lm, tmx_xn, OP_LM, logits.p, nullptr, B, cfg.vocab_size, cfg.hidden_size, s);
     }
-    // a head the caller owns (row N1: the code predictor's 15 lm heads): logits_out[b, :M] = W[M, H] * normed hidden, tmW a map of W
-    void run_head(const CUtensorMap& tmW, int M, float* logits_out, int B, cudaStream_t s, int tile_rows = 0) {
+    // a head the caller owns (row N1: the code predictor's 15 lm heads, and the talker's small_to_mtp_projection with its bias):
+    // logits_out[b, :M] = W[M, H] * normed hidden (+ bias), tmW a map of W
+    void run_head(const CUtensorMap& tmW, int M, float* logits_out, int B, cudaStream_t s, int tile_rows = 0, const float* bias = nullptr) {
         head_rows_now = tile_rows;              // tmW's box rows (0: this stack's own lm_tile_rows)
-        tc_gemm(tmW, tmx_xn, OP_LM, logits_out, nullptr, B, M, cfg.hidden_size, s, ss_b.p);
+        tc_gemm(tmW, tmx_xn, OP_LM, logits_out, nullptr, B, M, cfg.hidden_size, s, ss_b.p, bias);
         head_rows_now = 0;
     }
     // logits are [8, V] row-major.
@@ -1966,15 +1968,19 @@ void b2a_tts_destroy(b2a_tts* h) { delete h; }
 // ================================================================================================
 namespace b2a {
 
-// dst[b, :] = float(table[ids[b * id_stride + id_col], :]);  optionally pos[b] = pos_value (the predictor's cache position)
-__global__ void q3_gather_kernel(const bf16* __restrict__ table, int rows, const int* __restrict__ ids, int id_stride, int id_col,
+__device__ __forceinline__ float q3_f32(bf16 v) { return __bfloat162float(v); }
+__device__ __forceinline__ float q3_f32(float v) { return v; }
+// dst[b, :] = float(table[ids[b * id_stride + id_col], :]);  optionally pos[b] = pos_value (the predictor's cache position).
+// T = bf16: an embedding table; T = float: a table already projected to the predictor's width (b2a_qwen3_talker::proj_tab)
+template <typename T>
+__global__ void q3_gather_kernel(const T* __restrict__ table, int rows, const int* __restrict__ ids, int id_stride, int id_col,
                                  float* __restrict__ dst, int H, int* pos, int pos_value) {
     const int b = blockIdx.x;
     if (!pos) pdl_trigger();     // a kernel that writes pos[] must not trigger early (see attn_decode_cluster_kernel)
     pdl_wait();
     int t = ids[b * id_stride + id_col];
     t = min(max(t, 0), rows - 1);
-    for (int i = threadIdx.x; i < H; i += blockDim.x) dst[(long long)b * H + i] = __bfloat162float(table[(long long)t * H + i]);
+    for (int i = threadIdx.x; i < H; i += blockDim.x) dst[(long long)b * H + i] = q3_f32(table[(long long)t * H + i]);
     if (pos && threadIdx.x == 0) pos[b] = pos_value;
 }
 // dst[b, :] = src[b * src_stride + :]; optionally pos[b] = pos_value (pos_value < 0: pos untouched)
@@ -2079,6 +2085,13 @@ struct b2a_qwen3_talker {
     std::vector<CUtensorMap> tm_cp_head;
     int cp_head_rows = 128;
     DBuf<const bf16*> cp_emb_ptrs;
+    // code_predictor.small_to_mtp_projection [cpH, H] + bias, present iff the predictor is narrower or wider than the talker
+    // (Qwen3TTSCodePredictor.swift:200-238: 1.7B, 2048 -> 1024).  proj_tab holds every embedding row the predictor can be fed,
+    // already projected (fp32): codec_embedding's [vocab, cpH], then codec_embedding[k]'s [cp_vocab, cpH] for k = 0 .. G-3
+    DBuf<bf16> proj_w;
+    DBuf<float> proj_b, proj_tab;
+    CUtensorMap tm_proj{};
+    int proj_rows = 128;
     DBuf<float> x_in, hid, px, trailing, pad, embeds, tmp_a, tmp_b;
     DBuf<int> codes, out_codes, n_frames, done, n_active, row_frame, n_trailing, ids;
     DBuf<unsigned> seen;
@@ -2098,6 +2111,11 @@ struct b2a_qwen3_talker {
     }
     int G() const { return cfg.num_code_groups; }
     int H() const { return cfg.hidden_size; }
+    int PH() const { return cfg.cp_hidden_size; }
+    bool projected() const { return cfg.cp_hidden_size != cfg.hidden_size; }
+    const float* proj_table(int k) const {   // the projected table position k + 1 gathers from: 0 = codec_embedding, k = codec_embedding[k-1]
+        return proj_tab.p + (k == 0 ? 0 : ((size_t)cfg.vocab_size + (size_t)(k - 1) * cfg.cp_vocab_size) * PH());
+    }
 
     static b2a_llama_config stack_cfg(const b2a_qwen3_talker_config& c, bool predictor) {
         b2a_llama_config l{};
@@ -2123,20 +2141,42 @@ struct b2a_qwen3_talker {
     void check() {
         const b2a_qwen3_talker_config& c = cfg;
         B2A_CHECK(c.head_dim == HD && c.cp_head_dim == HD, B2A_ERR_INVALID_INPUT, "qwen3 talker: head_dim must be 128");
-        B2A_CHECK(c.cp_hidden_size == c.hidden_size, B2A_ERR_INVALID_INPUT,
-                  "qwen3 talker: code predictor hidden size must equal the talker's (small_to_mtp_projection is not implemented)");
         B2A_CHECK(c.vocab_size >= 1 && c.vocab_size <= q3s::SLOTS && c.cp_vocab_size >= 1 && c.cp_vocab_size <= q3s::SLOTS, B2A_ERR_INVALID_INPUT,
                   "qwen3 talker: codec vocabularies must be <= 4096");
         B2A_CHECK(c.num_code_groups >= 2 && c.num_code_groups <= 32, B2A_ERR_INVALID_INPUT, "qwen3 talker: num_code_groups must be in 2..32");
         B2A_CHECK(c.max_batch >= 1 && c.max_batch <= 8, B2A_ERR_INVALID_INPUT, "qwen3 talker: max_batch must be in 1..8");
     }
+    // proj_tab: every table row through the projection, once.  The tables are bf16, so the GEMM reads them without a lo half
+    // (hilo = 0); each row is the same linear map the reference applies per position (Qwen3TTS.swift:433-451), to fp32 rounding
+    void build_proj_tables() {
+        const int Hh = H(), P = PH(), G2 = G() - 2;
+        proj_tab.alloc(((size_t)cfg.vocab_size + (size_t)G2 * cfg.cp_vocab_size) * P);
+        const CUtensorMap tw = tc::make_tmap_bf16(proj_w.p, P, Hh, tc::BM);
+        for (int k = 0; k <= G2; ++k) {
+            const bf16* e = k == 0 ? codec_emb.p : cp_emb[k - 1].p;
+            const int rows = k == 0 ? cfg.vocab_size : cfg.cp_vocab_size;
+            tc::Args a{};
+            a.out_f32 = const_cast<float*>(proj_table(k)); a.M = P; a.N = rows; a.K = Hh; a.ldo = P;
+            a.m_tiles = cdiv(P, tc::BM); a.k_blocks = Hh / tc::BK; a.stages = tc::Smem<128>::max_stages(); a.hilo = 0;
+            a.epi_full = tc::EPI_STORE; a.epi_partial = -1; a.bias = proj_b.p;
+            const int n_tiles = cdiv(rows, 128);
+            tc::launch<128>(tw, tc::make_tmap_bf16(e, rows, Hh, 128), a, std::max(1, std::min(a.m_tiles, talker->num_sms / n_tiles)), n_tiles,
+                            stream);
+        }
+        B2A_CUDA(cudaStreamSynchronize(stream));
+    }
     void alloc_state() {
         stream = talker->stream;
-        const int Hh = H();
-        x_in.alloc((size_t)8 * Hh); hid.alloc((size_t)8 * Hh); px.alloc((size_t)8 * Hh); pad.alloc(Hh);
+        const int Hh = H(), P = PH();
+        x_in.alloc((size_t)8 * Hh); hid.alloc((size_t)8 * Hh); px.alloc((size_t)8 * P); pad.alloc(Hh);
         B2A_CUDA(cudaMemset(x_in.p, 0, (size_t)8 * Hh * sizeof(float)));
         B2A_CUDA(cudaMemset(hid.p, 0, (size_t)8 * Hh * sizeof(float)));
-        B2A_CUDA(cudaMemset(px.p, 0, (size_t)8 * Hh * sizeof(float)));
+        B2A_CUDA(cudaMemset(px.p, 0, (size_t)8 * P * sizeof(float)));
+        if (projected()) {
+            build_proj_tables();
+            proj_rows = b2a_tts::pick_tile_rows(P, talker->num_sms);
+            tm_proj = tc::make_tmap_bf16(proj_w.p, P, Hh, proj_rows);
+        }
         codes.alloc((size_t)8 * G()); n_frames.alloc(8); done.alloc(8); n_active.alloc(1); row_frame.alloc(8); n_trailing.alloc(8);
         B2A_CUDA(cudaMemset(codes.p, 0, (size_t)8 * G() * sizeof(int)));
         seen.alloc((size_t)8 * cdiv(cfg.vocab_size, 32));
@@ -2146,7 +2186,7 @@ struct b2a_qwen3_talker {
         cp_emb_ptrs.upload(ptrs.data(), ptrs.size());
         tm_cp_head.clear();
         cp_head_rows = b2a_tts::pick_tile_rows(cfg.cp_vocab_size, pred->num_sms);
-        for (auto& hd : cp_head) tm_cp_head.push_back(tc::make_tmap_bf16(hd.p, cfg.cp_vocab_size, Hh, cp_head_rows));
+        for (auto& hd : cp_head) tm_cp_head.push_back(tc::make_tmap_bf16(hd.p, cfg.cp_vocab_size, P, cp_head_rows));
         talker->x_ext = x_in.p; talker->normed_out = hid.p;
         pred->x_ext = px.p;
         talker->set_batch(8); pred->set_batch(8);
@@ -2165,11 +2205,17 @@ struct b2a_qwen3_talker {
         std::vector<float> b1 = tt.f32("text_projection.linear_fc1.bias", TH), b2 = tt.f32("text_projection.linear_fc2.bias", Hh);
         fc1_b.upload(b1.data(), TH); fc2_b.upload(b2.data(), Hh);
         cp_emb.resize(G() - 1); cp_head.resize(G() - 1);
+        const int P = PH();
         for (int i = 0; i < G() - 1; ++i) {
             b2a_tts::upload_bf16(tt, "code_predictor.model.codec_embedding." + std::to_string(i) + ".weight", (int64_t)c.cp_vocab_size * Hh, cp_emb[i], 0,
                                  (size_t)c.cp_vocab_size * Hh);
-            b2a_tts::upload_bf16(tt, "code_predictor.lm_head." + std::to_string(i) + ".weight", (int64_t)c.cp_vocab_size * Hh, cp_head[i], 0,
-                                 (size_t)c.cp_vocab_size * Hh);
+            b2a_tts::upload_bf16(tt, "code_predictor.lm_head." + std::to_string(i) + ".weight", (int64_t)c.cp_vocab_size * P, cp_head[i], 0,
+                                 (size_t)c.cp_vocab_size * P);
+        }
+        if (projected()) {
+            b2a_tts::upload_bf16(tt, "code_predictor.small_to_mtp_projection.weight", (int64_t)P * Hh, proj_w, 0, (size_t)P * Hh);
+            std::vector<float> pb = tt.f32("code_predictor.small_to_mtp_projection.bias", P);
+            proj_b.upload(pb.data(), P);
         }
         alloc_state();
     }
@@ -2191,7 +2237,12 @@ struct b2a_qwen3_talker {
         B2A_CUDA(cudaMemsetAsync(fc1_b.p, 0, TH * sizeof(float), talker->stream));
         B2A_CUDA(cudaMemsetAsync(fc2_b.p, 0, Hh * sizeof(float), talker->stream));
         cp_emb.resize(G() - 1); cp_head.resize(G() - 1);
-        for (int i = 0; i < G() - 1; ++i) { rnd(cp_emb[i], (size_t)c.cp_vocab_size * Hh); rnd(cp_head[i], (size_t)c.cp_vocab_size * Hh); }
+        for (int i = 0; i < G() - 1; ++i) { rnd(cp_emb[i], (size_t)c.cp_vocab_size * Hh); rnd(cp_head[i], (size_t)c.cp_vocab_size * PH()); }
+        if (projected()) {
+            rnd(proj_w, (size_t)PH() * Hh);
+            proj_b.alloc(PH());
+            B2A_CUDA(cudaMemsetAsync(proj_b.p, 0, PH() * sizeof(float), talker->stream));
+        }
         B2A_CUDA(cudaStreamSynchronize(talker->stream));
         alloc_state();
     }
@@ -2245,12 +2296,23 @@ struct b2a_qwen3_talker {
             q3s::launch(a, B, s);
         }
         // 2. code predictor: position 0 = the talker's hidden state, position 1 = codec_embed(c0) -> head 0 -> c1, then
-        //    position k + 1 = predictor_embed_{k-1}(c_k) -> head k -> c_{k+1}
-        launch_pdl(q3_copy_rows_kernel, dim3(B), dim3(256), 0, s, (const float*)hid.p, (long long)H(), px.p, H(), pred->pos.p, 0);
+        //    position k + 1 = predictor_embed_{k-1}(c_k) -> head k -> c_{k+1}.  With a projection every position goes through it:
+        //    position 0 is projected here from the talker's final-norm operand (rstd and bias in the GEMM's epilogue), the others
+        //    are rows of the projected tables; the zero-width copy then only sets the predictor's cache position
+        if (projected()) {
+            talker->run_head(tm_proj, PH(), px.p, B, s, proj_rows, proj_b.p);
+            launch_pdl(q3_copy_rows_kernel, dim3(B), dim3(256), 0, s, (const float*)nullptr, 0ll, px.p, 0, pred->pos.p, 0);
+        } else {
+            launch_pdl(q3_copy_rows_kernel, dim3(B), dim3(256), 0, s, (const float*)hid.p, (long long)H(), px.p, H(), pred->pos.p, 0);
+        }
         pred->run_layers(B, s);
         for (int k = 0; k < G() - 1; ++k) {
-            if (k == 0) launch_pdl(q3_gather_kernel, dim3(B), dim3(256), 0, s, (const bf16*)codec_emb.p, cfg.vocab_size, (const int*)codes.p, G(), 0, px.p, H(), pred->pos.p, 1);
-            else launch_pdl(q3_gather_kernel, dim3(B), dim3(256), 0, s, (const bf16*)cp_emb[k - 1].p, cfg.cp_vocab_size, (const int*)codes.p, G(), k, px.p, H(), pred->pos.p, k + 1);
+            const int id_rows = k == 0 ? cfg.vocab_size : cfg.cp_vocab_size;
+            if (projected())
+                launch_pdl(q3_gather_kernel<float>, dim3(B), dim3(256), 0, s, proj_table(k), id_rows, (const int*)codes.p, G(), k, px.p, PH(), pred->pos.p, k + 1);
+            else
+                launch_pdl(q3_gather_kernel<bf16>, dim3(B), dim3(256), 0, s, (const bf16*)(k == 0 ? codec_emb.p : cp_emb[k - 1].p), id_rows,
+                           (const int*)codes.p, G(), k, px.p, H(), pred->pos.p, k + 1);
             pred->run_layers(B, s);
             pred->run_final_norm(B, s);
             pred->run_head(tm_cp_head[k], cfg.cp_vocab_size, pred->logits.p, B, s, cp_head_rows);
