@@ -283,6 +283,51 @@ int32_t b2a_tts_interleave(const int32_t* codes0, const int32_t* codes1, const i
                            int32_t n_frames, int32_t* code_list);
 void b2a_tts_destroy(b2a_tts* h);
 
+/* ------------------------------------------------------------------ VyvoTTS (Qwen3 language model + SNAC 24 kHz)
+ * Replaces class Qwen3Model (Sources/MLXAudioTTS/Models/Qwen3/Qwen3.swift:305-931), model_type "qwen3" / "qwen".  The constructors return a
+ * b2a_tts handle: b2a_tts_generate / _stream / _dev, b2a_tts_forward_logits, b2a_tts_cancel and b2a_tts_destroy serve it unchanged, with
+ * VyvoTTS's token layout (Qwen3.swift:18-29): generation stops on 151671 (not kept), a row's codes start after its last start-of-speech
+ * 151670 or, without one, at its first audio token (>= 151679) after the last start-of-AI 151674 (parseOutputRow, :333-358), and a row of
+ * more than 50 frames is decoded as independent 50-frame SNAC chunks whose waveforms are concatenated (decodeAudioFromCodes, :47-83).
+ * The stack is Qwen3 (:145-303): per-head q/k RMSNorm before RoPE, rotate-half RoPE with base rope_theta; head_dim must be 128. */
+typedef struct b2a_qwen3_lm_config {     /* Qwen3Configuration, Config.swift:15-73 */
+    int32_t hidden_size;
+    int32_t num_hidden_layers;
+    int32_t intermediate_size;
+    int32_t num_attention_heads;
+    int32_t num_key_value_heads;
+    int32_t head_dim;
+    int32_t vocab_size;
+    float rms_norm_eps;
+    float rope_theta;          /* default 1e6 */
+    float rope_linear_factor;  /* rope_scaling {"type": "linear", "factor": f}: f; any other rope_scaling (or none): 1 */
+    int32_t tie_word_embeddings;   /* default 0 */
+    int32_t max_position_embeddings;   /* default 32768 (informational) */
+    int32_t sample_rate;       /* default 24000 */
+    int32_t eos_token_id;      /* default 151645 (informational: generation stops on end-of-speech 151671) */
+    int32_t max_batch;         /* KV-cache rows */
+    int32_t max_context;       /* KV-cache positions per row */
+} b2a_qwen3_lm_config;
+
+int32_t b2a_qwen3_lm_create(int32_t device, const b2a_qwen3_lm_config* cfg, const b2a_tensor* tensors, int32_t n_tensors,
+                            b2a_snac* snac /* borrowed, may be NULL */, b2a_tts** out);
+/* config.json -> the struct with Qwen3Configuration's defaults; quant_* (nullable) from its "quantization" block (0 = none) */
+int32_t b2a_qwen3_lm_config_from_json(const char* config_path, int32_t max_batch, int32_t max_context, b2a_qwen3_lm_config* cfg,
+                                      int32_t* quant_group_size, int32_t* quant_bits);
+/* Qwen3Model.fromModelDirectory (:892-930) without tokenizer / SNAC download: config.json + every *.safetensors ->
+ * b2a_weights_sanitize_llama_config (lm_head.weight dropped when tied, MLX 2/4/8-bit layers expanded to bf16) -> b2a_qwen3_lm_create */
+int32_t b2a_qwen3_lm_create_from_directory(const char* model_dir, int32_t device, int32_t max_batch, int32_t max_context, b2a_snac* snac,
+                                           b2a_tts** out);
+/* prepareInputIds (:377-474) on token ids: [151676 padding] [151672] prompt [151645, 151673]; with a reference
+ * [151676 padding] [151672] ref_text_ids [151645, 151673] [151674, 151670] ref_code_list + 151679 [151671, 151675] [151672] prompt [151645, 151673].
+ * Arguments and errors as b2a_tts_prepare_input_ids(_ref). */
+int32_t b2a_qwen3_lm_prepare_input_ids(const int32_t* const* prompt_ids, const int32_t* lens, int32_t batch, int32_t* out, int32_t* out_len);
+int32_t b2a_qwen3_lm_prepare_input_ids_ref(const int32_t* const* prompt_ids, const int32_t* lens, int32_t batch, const int32_t* ref_text_ids,
+                                           int32_t ref_text_len, const int32_t* ref_code_list, int32_t ref_code_len, int32_t* out,
+                                           int32_t* out_len);
+/* parseOutputRow (:333-358) for every row of tokens [B, n]; code_lists_out [B, n], code_lens [B] */
+int32_t b2a_qwen3_lm_parse_output(const int32_t* tokens, int32_t batch, int32_t n, int32_t* code_lists_out, int32_t* code_lens);
+
 /* ------------------------------------------------------------------ weight / format plumbing (SURVEY.md 8f, row N4)
  * Host-only.  Replaces MLX.loadArrays on *.safetensors (llamaTTSLoadWeights, LlamaTTS.swift:982-994: every file of a directory, later
  * files win), WhisperModel.detectFormat / sanitize / remapMlxWhisperKey / whisperSinusoids (WhisperModel.swift:315-480),

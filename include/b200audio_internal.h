@@ -17,7 +17,7 @@ extern "C" {
 /* ------------------------------------------------------------------ benchmark constructors / switches
  *   b2a_tts_create_random / b2a_stt_create_random : same as b2a_tts_create / b2a_stt_create but the weights are drawn ON THE
  *       DEVICE (N(0, std^2) bf16 from a counter-based generator, norm gains 1).
- *   b2a_tts_set_bench_flags : mask_eos != 0 -> never stop on 128258 (fixed work per call); wrap_codes != 0 -> audio codes are
+ *   b2a_tts_set_bench_flags : mask_eos != 0 -> never stop on the handle's stop token (fixed work per call); wrap_codes != 0 -> audio codes are
  *       taken mod 4096 per slot so that random-init tokens index the SNAC codebooks.  Both default to 0 (reference behaviour).
  *   b2a_stt_set_bench_flags : mask_eot != 0 -> a clip never stops on end-of-text (fixed work).
  *   b2a_tts_time_steps : runs `iters` captured decode steps for `batch` rows at context `ctx` (greedy, no host sync inside)
@@ -25,6 +25,9 @@ extern "C" {
 int32_t b2a_tts_create_random(int32_t device, const b2a_llama_config* cfg, float std, uint64_t seed,
                               b2a_snac* snac, b2a_tts** out);
 int32_t b2a_stt_create_random(int32_t device, const b2a_whisper_config* cfg, float std, uint64_t seed, b2a_stt** out);
+/*   b2a_qwen3_lm_create_random : the same for a VyvoTTS handle (b2a_qwen3_lm_create); q/k norm gains are 1 too.               */
+int32_t b2a_qwen3_lm_create_random(int32_t device, const b2a_qwen3_lm_config* cfg, float std, uint64_t seed, b2a_snac* snac,
+                                   b2a_tts** out);
 int32_t b2a_tts_set_bench_flags(b2a_tts* h, int32_t mask_eos, int32_t wrap_codes);
 int32_t b2a_stt_set_bench_flags(b2a_stt* h, int32_t mask_eot);
 int32_t b2a_tts_time_steps(b2a_tts* h, int32_t batch, int32_t ctx, int32_t iters, float* ms_per_step);

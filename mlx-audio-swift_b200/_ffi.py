@@ -49,6 +49,14 @@ class LlamaConfig(C.Structure):
                 ("max_context", C.c_int32)]
 
 
+class Qwen3LMConfig(C.Structure):
+    _fields_ = ([(n, C.c_int32) for n in ("hidden_size", "num_hidden_layers", "intermediate_size", "num_attention_heads",
+                                           "num_key_value_heads", "head_dim", "vocab_size")]
+                + [("rms_norm_eps", C.c_float), ("rope_theta", C.c_float), ("rope_linear_factor", C.c_float)]
+                + [(n, C.c_int32) for n in ("tie_word_embeddings", "max_position_embeddings", "sample_rate", "eos_token_id", "max_batch",
+                                             "max_context")])
+
+
 class GenParams(C.Structure):
     _fields_ = [("max_tokens", C.c_int32), ("temperature", C.c_float), ("top_p", C.c_float),
                 ("repetition_penalty", C.c_float), ("repetition_context_size", C.c_int32), ("seed", C.c_uint64)]
@@ -208,6 +216,15 @@ SIGNATURES = {
     "b2a_tts_deinterleave": (C.c_int32, [_P, C.c_int32, _P, _P, _P, C.POINTER(C.c_int32)]),
     "b2a_tts_interleave": (C.c_int32, [_P, _P, _P, C.c_int32, _P]),
     "b2a_tts_destroy": (None, [_P]),
+    "b2a_qwen3_lm_create": (C.c_int32, [C.c_int32, C.POINTER(Qwen3LMConfig), C.POINTER(Tensor), C.c_int32, _P, C.POINTER(_P)]),
+    "b2a_qwen3_lm_create_random": (C.c_int32, [C.c_int32, C.POINTER(Qwen3LMConfig), C.c_float, C.c_uint64, _P, C.POINTER(_P)]),
+    "b2a_qwen3_lm_config_from_json": (C.c_int32, [C.c_char_p, C.c_int32, C.c_int32, C.POINTER(Qwen3LMConfig), C.POINTER(C.c_int32),
+                                                  C.POINTER(C.c_int32)]),
+    "b2a_qwen3_lm_create_from_directory": (C.c_int32, [C.c_char_p, C.c_int32, C.c_int32, C.c_int32, _P, C.POINTER(_P)]),
+    "b2a_qwen3_lm_prepare_input_ids": (C.c_int32, [C.POINTER(_P), _P, C.c_int32, _P, C.POINTER(C.c_int32)]),
+    "b2a_qwen3_lm_prepare_input_ids_ref": (C.c_int32, [C.POINTER(_P), _P, C.c_int32, _P, C.c_int32, _P, C.c_int32, _P,
+                                                       C.POINTER(C.c_int32)]),
+    "b2a_qwen3_lm_parse_output": (C.c_int32, [_P, C.c_int32, C.c_int32, _P, _P]),
     "b2a_vocos_create": (C.c_int32, [C.c_int32, C.POINTER(VocosConfig), C.POINTER(Tensor), C.c_int32, C.POINTER(_P)]),
     "b2a_vocos_output_length": (C.c_int64, [_P, C.c_int32]),
     "b2a_vocos_stream": (C.c_void_p, [_P]),

@@ -23,15 +23,25 @@
 #include <cstring>
 #include <chrono>
 #include <cmath>
+#include <memory>
 
 namespace b2a {
 
 typedef __nv_bfloat16 bf16;
 
-constexpr int TOK_START_OF_HUMAN = 128259, TOK_END_OF_HUMAN = 128260, TOK_END_OF_TEXT = 128009;
-constexpr int TOK_START_OF_SPEECH = 128257, TOK_END_OF_SPEECH = 128258, TOK_PAD = 128263;
-constexpr int TOK_AUDIO_OFFSET = 128266;
-constexpr int TOK_AUDIO_START = 128261, TOK_AUDIO_END = 128262;        // LlamaTTS.swift:27-28
+// The special tokens of a TTS language model's vocabulary, how a generated row is parsed into SNAC codes and how the codes are decoded.
+// A b2a_tts handle carries one; the prompt framing is [pad..] [SOH] text [EOT, EOH], a reference clip's block
+// [SOH] transcript [EOT, EOH] [SOAI, SOS] codes + audio_offset [EOS, EOAI].
+struct TokenLayout {
+    int start_of_human, end_of_human, end_of_text;
+    int start_of_ai, end_of_ai;                 // Orpheus: 128261 / 128262, the tokens around its reference codes (LlamaTTS.swift:27-28)
+    int start_of_speech, end_of_speech;         // end_of_speech is the stop token: generation ends there and the token is not kept
+    int pad, audio_offset;
+    bool ai_fallback;   // parse: a row without start-of-speech starts at its first audio token after the last start-of-AI
+    int decode_chunk;   // frames per independent SNAC decode of a row (0: the whole row at once)
+};
+constexpr TokenLayout ORPHEUS_TOKENS{128259, 128260, 128009, 128261, 128262, 128257, 128258, 128263, 128266, false, 0};
+constexpr TokenLayout VYVO_TOKENS{151672, 151673, 151645, 151674, 151675, 151670, 151671, 151676, 151679, true, 50};   // Qwen3.swift:18-29, :47
 
 __device__ __forceinline__ float bf16_round(float x) { return __bfloat162float(__float2bfloat16_rn(x)); }
 
@@ -410,12 +420,16 @@ struct PrefillAttnArgs {
     bf16* out;            // [2 * T_pad, nq * 128] hi/lo, 64-token tiles
     int nq, nkv, max_ctx, L;
     float scale;
+    const float* qnorm;   // nullable [128]: per-head RMSNorm gains of q and k before RoPE, as in AttnArgs
+    const float* knorm;
+    float qk_eps;
 };
 
 template <int G>
 __global__ void __launch_bounds__(PA_THREADS)
 prefill_attn_kernel(PrefillAttnArgs a) {
     extern __shared__ __align__(16) uint8_t pa_smem[];
+    __shared__ float s_rk[PA_MAXL], s_rq[G * PA_QT];           // q/k norm: rstd of every key / query vector of this tile
     const int h = blockIdx.x, b = blockIdx.y, q0 = blockIdx.z * PA_QT;
     const int nqt = min(PA_QT, a.L - q0), kmax = q0 + nqt;     // causal: keys 0 .. q0 + nqt - 1
     float* sK = reinterpret_cast<float*>(pa_smem);              // [kmax][128]
@@ -427,12 +441,27 @@ prefill_attn_kernel(PrefillAttnArgs a) {
     float* kc = a.kcache + (((long long)b * a.nkv + h) * a.max_ctx) * HD;
     float* vc = a.vcache + (((long long)b * a.nkv + h) * a.max_ctx) * HD;
 
+    if (a.qnorm) {
+        // per-head RMSNorm x * rsqrt(mean(x^2) + eps) * w before RoPE: one warp per 128-vector (keys, then the tile's queries g * nqt + qi),
+        // the same reduction as attn_decode_cluster_kernel's, so a prompt position normalises exactly as a decode step does
+        for (int v = warp; v < kmax + G * nqt; v += PA_THREADS / 32) {
+            const int qv = v - kmax;
+            const float* src = v < kmax ? base + (long long)v * ld + (a.nq + h) * HD
+                                        : base + (long long)(q0 + qv % nqt) * ld + (h * G + qv / nqt) * HD;
+            const float4 x = reinterpret_cast<const float4*>(src)[lane];
+            const float ss = warp_sum(x.x * x.x + x.y * x.y + x.z * x.z + x.w * x.w);
+            const float r = rsqrtf(ss * (1.0f / HD) + a.qk_eps);
+            if (lane == 0) { if (v < kmax) s_rk[v] = r; else s_rq[qv] = r; }
+        }
+        __syncthreads();
+    }
     // K (RoPE) and V of keys [0, kmax) -> shared memory; this tile's own keys also go to the cache
     for (int i = tid; i < kmax * (HD / 2); i += PA_THREADS) {
         const int t = i / (HD / 2), d = i - t * (HD / 2);
         const float2 cs = a.rope[t * (HD / 2) + d];
         const float* k = base + (long long)t * ld + (a.nq + h) * HD;
-        const float x1 = k[d], x2 = k[d + HD / 2];
+        float x1 = k[d], x2 = k[d + HD / 2];
+        if (a.knorm) { x1 = x1 * s_rk[t] * a.knorm[d]; x2 = x2 * s_rk[t] * a.knorm[d + HD / 2]; }
         const float k1 = x1 * cs.x - x2 * cs.y, k2 = x2 * cs.x + x1 * cs.y;
         sK[t * HD + d] = k1; sK[t * HD + d + HD / 2] = k2;
         if (t >= q0) { kc[(long long)t * HD + d] = k1; kc[(long long)t * HD + d + HD / 2] = k2; }
@@ -447,7 +476,8 @@ prefill_attn_kernel(PrefillAttnArgs a) {
         const int g = i / (nqt * (HD / 2)), r = i - g * nqt * (HD / 2), qi = r / (HD / 2), d = r - qi * (HD / 2);
         const float2 cs = a.rope[(q0 + qi) * (HD / 2) + d];
         const float* q = base + (long long)(q0 + qi) * ld + (h * G + g) * HD;
-        const float x1 = q[d], x2 = q[d + HD / 2];
+        float x1 = q[d], x2 = q[d + HD / 2];
+        if (a.qnorm) { const float r = s_rq[g * nqt + qi]; x1 = x1 * r * a.qnorm[d]; x2 = x2 * r * a.qnorm[d + HD / 2]; }
         sQ[(g * PA_QT + qi) * HD + d] = x1 * cs.x - x2 * cs.y;
         sQ[(g * PA_QT + qi) * HD + d + HD / 2] = x2 * cs.x + x1 * cs.y;
     }
@@ -523,10 +553,12 @@ struct PromptAttnOps {
         tv = tc::make_tmap_f16_3d(vt.p, Lp, pfa::OPW, (long long)B * nkv, 64, pfa::HDIM);
         B2A_CUDA(cudaFuncSetAttribute(pfa::prompt_attn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pfa::SMEM_BYTES));
     }
-    // qkv [B * L, (nq + 2 nkv) * 128] fp32; rope [>= L][64]; caches [B][nkv][max_ctx][128]; out: 64-token hi/lo tiles [.., nq * 128]
-    void run(const float* qkv, const float2* rope, float* kcache, float* vcache, bf16* out, int L, int max_ctx, cudaStream_t s) {
+    // qkv [B * L, (nq + 2 nkv) * 128] fp32; rope [>= L][64]; caches [B][nkv][max_ctx][128]; out: 64-token hi/lo tiles [.., nq * 128];
+    // qnorm / knorm nullable (per-head q/k RMSNorm before RoPE)
+    void run(const float* qkv, const float2* rope, float* kcache, float* vcache, bf16* out, int L, int max_ctx, cudaStream_t s,
+             const float* qnorm = nullptr, const float* knorm = nullptr, float qk_eps = 0.f) {
         pfa::pack_prompt_kernel<<<dim3(Lp / 64, B, nq + nkv), 256, 0, s>>>(qkv, rope, q.p, k.p, vt.p, kcache, vcache, L, Lp, nq, nkv,
-                                                                         max_ctx);
+                                                                         max_ctx, qnorm, knorm, qk_eps);
         const pfa::Args a{out, L, Lp, nq, nkv, 1.0f / sqrtf((float)HD)};
         pfa::prompt_attn_kernel<<<dim3(Lp / pfa::BQ, nq, B), pfa::THREADS, pfa::SMEM_BYTES, s>>>(tq, tk, tv, a);
         count_launch(2);
@@ -565,7 +597,8 @@ struct SampleArgs {
     int V, R, max_tokens;
     float temperature, top_p, rep_penalty;
     unsigned long long seed;
-    int mask_eos;
+    int mask_eos;         // bench only: the stop token can never be sampled
+    int stop_token;       // ends a row and is not recorded (TokenLayout::end_of_speech)
 };
 
 // Logits processors + sampler (deterministic for a given seed, no atomics):
@@ -647,7 +680,7 @@ sample_kernel(SampleArgs a) {
                 lg[tok] = l < 0.f ? l * a.rep_penalty : l / a.rep_penalty;
             }
         }
-        if (a.mask_eos && t == 0 && TOK_END_OF_SPEECH >= i0 && TOK_END_OF_SPEECH < i1) lg[TOK_END_OF_SPEECH] = -INFINITY;
+        if (a.mask_eos && t == 0 && a.stop_token >= i0 && a.stop_token < i1) lg[a.stop_token] = -INFINITY;
         __syncthreads();
 
         // max (and argmax, lowest index wins ties)
@@ -726,7 +759,7 @@ sample_kernel(SampleArgs a) {
             a.recent_n[b] = rn + 1;
         }
         if (a.forced == nullptr && !a.done[b]) {
-            if (tok == TOK_END_OF_SPEECH) {      // LlamaTTS.swift:734-736: stop, token not appended
+            if (tok == a.stop_token) {           // LlamaTTS.swift:734-736, Qwen3.swift:675-681: stop, token not appended
                 a.done[b] = 1;
                 atomicSub(a.n_active, 1);
             } else {
@@ -784,6 +817,13 @@ __global__ void fill_f32_kernel(float* p, int n, float v) {
 // ------------------------------------------------------------------------------------------------
 // Host side
 // ------------------------------------------------------------------------------------------------
+// Qwen3Attention's RoPE (Qwen3.swift:177-192): MLXFast.RoPE(base: theta, scale: 1 / factor), i.e. angle = pos / (theta^(2i/d) * factor)
+static std::vector<float> linear_freqs(const b2a_llama_config& c, float factor) {
+    std::vector<float> f(c.head_dim / 2);
+    for (int i = 0; i < c.head_dim / 2; ++i) f[i] = powf(c.rope_theta, (float)(2 * i) / (float)c.head_dim) * factor;
+    return f;
+}
+
 static std::vector<float> llama3_freqs(const b2a_llama_config& c) {
     // LlamaTTS.swift:121-156 in Float
     const int d = c.head_dim;
@@ -821,6 +861,7 @@ struct StackSpec {
     bool has_embed = true;                     // "<prefix>embed_tokens.weight" (false: inputs are embeddings)
     std::string head;                          // "" = tied to the embedding / none; else an untied [vocab, hidden] matrix
     bool has_head = true;
+    float linear_rope = 0.f;                   // > 0: Qwen3Attention's RoPE with this linear factor (linear_freqs); 0: Llama3ScaledRoPE
 };
 
 }  // namespace b2a
@@ -877,6 +918,7 @@ struct b2a_tts {
     int fused_parts = 0;             // m-tiles of H (the last one may be partly filled): partial sums of squares per row
     DBuf<float> ss_a, ss_b;          // [fused_parts <= 64, 8] partial sums of squares: ss_a feeds the post-attention norm, ss_b the input norm
     StackSpec spec;                  // which keys / features this stack was built with
+    TokenLayout tok = ORPHEUS_TOKENS;  // special tokens, parse rule and decode chunking of generate (VYVO_TOKENS: b2a_qwen3_lm_create)
     const float* x_ext = nullptr;    // row N1: when set, a step starts from these embeddings [8, H] instead of embed(tokens)
     float* normed_out = nullptr;     // row N1: when set, run_final_norm writes the final RMSNorm's fp32 output here [8, H]
     std::atomic<int> cancel{0};
@@ -960,7 +1002,7 @@ struct b2a_tts {
         const b2a_llama_config& c = cfg;
         const int H = c.hidden_size, I = c.intermediate_size, nq = c.num_attention_heads, nkv = c.num_key_value_heads;
         const int NQ = nq * HD, NKV = nkv * HD;
-        std::vector<float> fr = llama3_freqs(c);
+        std::vector<float> fr = spec.linear_rope > 0.f ? linear_freqs(c, spec.linear_rope) : llama3_freqs(c);
         freqs.upload(fr.data(), fr.size());
         const size_t kv = (size_t)c.num_hidden_layers * c.max_batch * nkv * c.max_context * HD;
         kcache.alloc(kv);
@@ -1247,8 +1289,9 @@ struct b2a_tts {
     // the prompt attention for L positions: the SIMT kernel while its K/V rows fit in shared memory (the outputs of short prompts stay
     // what they were), the wgmma kernel beyond
     bool simt_prompt_attn(int L) const { return L <= PA_MAXL && pattn_smem(L) <= 220 * 1024; }
+    // a stack whose inputs are embeddings (the Qwen3-TTS talker and code predictor) replays the decode step per prompt position
     bool can_batch_prefill(int L) const {
-        return use_batched_prefill && spec.has_embed && !spec.qk_norm && L >= 2 && L <= cfg.max_context;
+        return use_batched_prefill && spec.has_embed && L >= 2 && L <= cfg.max_context;
     }
 
     // D[T, M] = X[T, K] W^T for all prompt tokens: 128-column tiles (64 tokens as hi/lo), CTAs own whole tiles
@@ -1298,12 +1341,14 @@ struct b2a_tts {
         const size_t kv_layer = (size_t)cfg.max_batch * nkv * cfg.max_context * HD;
         for (int l = 0; l < cfg.num_hidden_layers; ++l) {
             LayerW& Lw = layers[l];
+            const float* qn = spec.qk_norm ? Lw.qnorm.p : nullptr;
+            const float* kn = spec.qk_norm ? Lw.knorm.p : nullptr;
             launch_pdl(add_rmsnorm_kernel, dim3(T), dim3(RN_THREADS), 0, s, xp.p, l == 0 ? (float*)nullptr : yp.p, Lw.ln1.p, xnp.p, H,
                        cfg.rms_norm_eps, PF_HALF, (float*)nullptr, 0);
             pf_gemm(tm_qkv[l], tmp_xn, tc::EPI_STORE, qkvp.p, nullptr, T, QKV_N, H, s);
             if (simt_attn) {
                 PrefillAttnArgs pa{qkvp.p, rope_tab.p, kcache.p + l * kv_layer, vcache.p + l * kv_layer, attnp.p, nq, nkv,
-                                   cfg.max_context, L, 1.0f / sqrtf((float)HD)};
+                                   cfg.max_context, L, 1.0f / sqrtf((float)HD), qn, kn, cfg.rms_norm_eps};
                 const dim3 grid(nkv, B, cdiv(L, PA_QT));
                 const size_t sm = pattn_smem(L);
                 switch (G) {
@@ -1316,7 +1361,8 @@ struct b2a_tts {
                 }
                 count_launch();
             } else {
-                pfa_ops.run(qkvp.p, rope_tab.p, kcache.p + l * kv_layer, vcache.p + l * kv_layer, attnp.p, L, cfg.max_context, s);
+                pfa_ops.run(qkvp.p, rope_tab.p, kcache.p + l * kv_layer, vcache.p + l * kv_layer, attnp.p, L, cfg.max_context, s, qn, kn,
+                            cfg.rms_norm_eps);
             }
             pf_gemm(tm_o[l], tmp_attn, tc::EPI_STORE, yp.p, nullptr, T, H, NQ, s);
             launch_pdl(add_rmsnorm_kernel, dim3(T), dim3(RN_THREADS), 0, s, xp.p, yp.p, Lw.ln2.p, xnp.p, H, cfg.rms_norm_eps, PF_HALF,
@@ -1341,7 +1387,7 @@ struct b2a_tts {
     static bool same_args(const SampleArgs& a, const SampleArgs& b) {
         return a.V == b.V && a.R == b.R && a.max_tokens == b.max_tokens && a.temperature == b.temperature &&
                a.top_p == b.top_p && a.rep_penalty == b.rep_penalty && a.seed == b.seed && a.mask_eos == b.mask_eos &&
-               a.out_tokens == b.out_tokens;
+               a.stop_token == b.stop_token && a.out_tokens == b.out_tokens;
     }
 
     void capture(int B, const SampleArgs& sa, int L) {
@@ -1371,14 +1417,28 @@ struct b2a_tts {
 // ------------------------------------------------------------------------------------------------
 // host-side token plumbing (ints; the reference does these on the host too)
 // ------------------------------------------------------------------------------------------------
-static std::vector<int> parse_row(const int* row, int n, int crop_after) {
-    // LlamaTTS.swift:400-431 for one row: crop, drop 128258, trim to a multiple of 7, subtract 128266
+static std::vector<int> parse_row(const TokenLayout& tl, const int* row, int n, int crop_after) {
+    // LlamaTTS.swift:400-431 / Qwen3.swift:346-357 for one row: crop, drop the stop token, trim to a multiple of 7, subtract the audio offset
     std::vector<int> r;
     for (int j = crop_after + 1; j < n; ++j)
-        if (row[j] != TOK_END_OF_SPEECH) r.push_back(row[j]);
+        if (row[j] != tl.end_of_speech) r.push_back(row[j]);
     r.resize((r.size() / 7) * 7);
-    for (auto& t : r) t -= TOK_AUDIO_OFFSET;
+    for (auto& t : r) t -= tl.audio_offset;
     return r;
+}
+
+// where a row's codes start (parse_row's crop_after): its last start-of-speech; failing that, with ai_fallback, just before the first audio
+// token after its last start-of-AI (Qwen3.swift:336-344); -1 keeps the whole row
+static int codes_start(const TokenLayout& tl, const int* row, int n) {
+    int last = -1, soa = -1;
+    for (int j = 0; j < n; ++j) {
+        if (row[j] == tl.start_of_speech) last = j;
+        if (row[j] == tl.start_of_ai) soa = j;
+    }
+    if (last < 0 && tl.ai_fallback && soa >= 0)
+        for (int j = soa + 1; j < n; ++j)
+            if (row[j] >= tl.audio_offset) { last = j - 1; break; }
+    return last;
 }
 
 static void deinterleave(const int* cl, int n, std::vector<int>& l1, std::vector<int>& l2, std::vector<int>& l3) {
@@ -1440,7 +1500,7 @@ static void tts_generate_impl(b2a_tts* h, const int32_t* input_ids, bool ids_on_
     sa.n_active = h->n_active.p; sa.forced = nullptr; sa.V = h->cfg.vocab_size; sa.R = gp->repetition_context_size > 0 ? R : 0;
     sa.max_tokens = MT; sa.temperature = gp->temperature; sa.top_p = gp->top_p;
     sa.rep_penalty = gp->repetition_context_size > 0 ? gp->repetition_penalty : 1.0f;
-    sa.seed = gp->seed; sa.mask_eos = h->bench_mask_eos;
+    sa.seed = gp->seed; sa.mask_eos = h->bench_mask_eos; sa.stop_token = h->tok.end_of_speech;
     if (sa.R == 0) { sa.R = 1; }
     h->capture(B, sa, L);
 
@@ -1484,9 +1544,7 @@ static void tts_generate_impl(b2a_tts* h, const int32_t* input_ids, bool ids_on_
             const int ng = std::min(s_ng[b], MT);
             std::vector<int> all(s_prompt.begin() + (size_t)b * L, s_prompt.begin() + (size_t)(b + 1) * L);
             all.insert(all.end(), s_tok.begin() + (size_t)b * MT, s_tok.begin() + (size_t)b * MT + ng);
-            int last = -1;
-            for (int j = 0; j < (int)all.size(); ++j) if (all[j] == TOK_START_OF_SPEECH) last = j;
-            std::vector<int> cl = parse_row(all.data(), (int)all.size(), last);
+            std::vector<int> cl = parse_row(h->tok, all.data(), (int)all.size(), codes_start(h->tok, all.data(), (int)all.size()));
             if (h->bench_wrap_codes)
                 for (size_t i = 0; i < cl.size(); ++i) cl[i] = ((cl[i] % 4096) + 4096) % 4096 + 4096 * (int)(i % 7);
             const int total = (int)cl.size() / 7;
@@ -1583,15 +1641,14 @@ static void tts_generate_impl(b2a_tts* h, const int32_t* input_ids, bool ids_on_
     if (wave_out) {
         const double c0 = now_s();
         // per row: generatedTokens = prompt + generated (LlamaTTS.swift:705-707,738) -> parseOutput -> frames
+        const TokenLayout& tl = h->tok;
         std::vector<std::vector<int>> l1(B), l2(B), l3(B);
         std::vector<int> frames(B, 0);
         bool any = false;
         for (int b = 0; b < B; ++b) {
             std::vector<int> all(prompt.begin() + (size_t)b * L, prompt.begin() + (size_t)(b + 1) * L);
             all.insert(all.end(), toks.begin() + (size_t)b * MT, toks.begin() + (size_t)b * MT + ng[b]);
-            int last = -1;
-            for (int j = 0; j < (int)all.size(); ++j) if (all[j] == TOK_START_OF_SPEECH) last = j;
-            std::vector<int> cl = parse_row(all.data(), (int)all.size(), last);
+            std::vector<int> cl = parse_row(tl, all.data(), (int)all.size(), codes_start(tl, all.data(), (int)all.size()));
             if (h->bench_wrap_codes)   // benchmark only: fold random-init tokens into each slot's 4096-code range
                 for (size_t i = 0; i < cl.size(); ++i) cl[i] = ((cl[i] % 4096) + 4096) % 4096 + 4096 * (int)(i % 7);
             deinterleave(cl.data(), (int)cl.size(), l1[b], l2[b], l3[b]);
@@ -1600,19 +1657,32 @@ static void tts_generate_impl(b2a_tts* h, const int32_t* input_ids, bool ids_on_
             if (wave_len) wave_len[b] = 0;
         }
         B2A_CHECK(any, B2A_ERR_GENERATION_FAILED, "No audio codes generated");   // LlamaTTS.swift:752-754
-        const int64_t hop = b2a_snac_hop_length(h->snac);
-        // group rows with equal frame counts into one batched codec call
-        std::vector<bool> used(B, false);
+        const int64_t hop = b2a_snac_hop_length(h->snac), frame_samples = 4 * hop;
+        // A row is decoded whole, or -- longer than the layout's decode_chunk -- as decode_chunk-frame chunks decoded independently and
+        // concatenated (decodeAudioFromCodes, Qwen3.swift:47-83).  Pieces (row, first frame, frames) of equal length share one batched
+        // codec call: every full chunk of every row in one, trailing pieces grouped by length.
+        struct Piece { int row, f0, nf; };
+        std::vector<Piece> pieces;
         for (int b = 0; b < B; ++b) {
-            if (used[b] || frames[b] == 0) continue;
-            std::vector<int> grp;
-            for (int c = b; c < B; ++c) if (!used[c] && frames[c] == frames[b]) { grp.push_back(c); used[c] = true; }
-            const int F = frames[b], nb = (int)grp.size();
+            if (frames[b] == 0) continue;
+            B2A_CHECK(frames[b] * frame_samples <= wave_cap, B2A_ERR_INVALID_INPUT, "tts generate: wave buffer too small");
+            const int chunk = tl.decode_chunk > 0 ? tl.decode_chunk : frames[b];
+            for (int f0 = 0; f0 < frames[b]; f0 += chunk) pieces.push_back({b, f0, std::min(chunk, frames[b] - f0)});
+        }
+        std::vector<bool> used(pieces.size(), false);
+        for (size_t i = 0; i < pieces.size(); ++i) {
+            if (used[i]) continue;
+            std::vector<Piece> grp;
+            for (size_t j = i; j < pieces.size(); ++j)
+                if (!used[j] && pieces[j].nf == pieces[i].nf) { grp.push_back(pieces[j]); used[j] = true; }
+            const int F = pieces[i].nf, nb = (int)grp.size();
             const int64_t T = 4ll * F, wl = T * hop;
-            B2A_CHECK(wl <= wave_cap, B2A_ERR_INVALID_INPUT, "tts generate: wave buffer too small");
             std::vector<int> c0v, c1v, c2v;
-            for (int r : grp) { c0v.insert(c0v.end(), l1[r].begin(), l1[r].end()); c1v.insert(c1v.end(), l2[r].begin(), l2[r].end());
-                                c2v.insert(c2v.end(), l3[r].begin(), l3[r].end()); }
+            for (const Piece& p : grp) {
+                c0v.insert(c0v.end(), l1[p.row].begin() + p.f0, l1[p.row].begin() + p.f0 + F);
+                c1v.insert(c1v.end(), l2[p.row].begin() + 2 * p.f0, l2[p.row].begin() + 2 * (p.f0 + F));
+                c2v.insert(c2v.end(), l3[p.row].begin() + 4 * p.f0, l3[p.row].begin() + 4 * (p.f0 + F));
+            }
             h->d_codes[0].upload(c0v.data(), c0v.size(), s);
             h->d_codes[1].upload(c1v.data(), c1v.size(), s);
             h->d_codes[2].upload(c2v.data(), c2v.size(), s);
@@ -1621,11 +1691,11 @@ static void tts_generate_impl(b2a_tts* h, const int32_t* input_ids, bool ids_on_
             B2A_CUDA(cudaStreamSynchronize(s));   // host vectors above go out of scope after the copy
             const int32_t st = b2a_snac_decode_dev(h->snac, dc, nb, T, nullptr, 0, gp->seed, h->d_wave.p, s);
             B2A_CHECK(st == B2A_OK, B2A_ERR_AUDIO_DECODING_FAILED, std::string("SNAC decode failed: ") + b2a_last_error());
-            for (int i = 0; i < nb; ++i) {
-                const int r = grp[i];
-                B2A_CUDA(cudaMemcpyAsync(wave_out + (size_t)r * wave_cap, h->d_wave.p + (size_t)i * wl, wl * sizeof(float),
-                                         wave_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, s));
-                if (wave_len) wave_len[r] = wl;
+            for (int k = 0; k < nb; ++k) {
+                const Piece& p = grp[k];
+                B2A_CUDA(cudaMemcpyAsync(wave_out + (size_t)p.row * wave_cap + (size_t)p.f0 * frame_samples, h->d_wave.p + (size_t)k * wl,
+                                         wl * sizeof(float), wave_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, s));
+                if (wave_len) wave_len[p.row] = (int64_t)frames[p.row] * frame_samples;
             }
             B2A_CUDA(cudaStreamSynchronize(s));
         }
@@ -1641,6 +1711,47 @@ static void tts_generate_impl(b2a_tts* h, const int32_t* input_ids, bool ids_on_
         size_t fr = 0, tot = 0;
         cudaMemGetInfo(&fr, &tot);
         info->peak_memory_gb = (double)(tot - fr) / 1e9;
+    }
+}
+
+// prepareInputIds on token ids (LlamaTTS.swift:499-543, Qwen3.swift:417-464): every row is [pad..] [SOH] prompt [EOT, EOH], and with a
+// reference (with_ref) [pad..] [SOH] ref_text [EOT, EOH] [SOAI, SOS] ref_codes + audio_offset [EOS, EOAI] [SOH] prompt [EOT, EOH], the
+// padding in front to the longest prompt.  out NULL: only *out_len.
+static void prepare_ids(const TokenLayout& tl, const int32_t* const* prompt_ids, const int32_t* lens, int32_t batch, const int32_t* ref_text_ids,
+                        int32_t ref_text_len, const int32_t* ref_code_list, int32_t ref_code_len, int32_t* out, int32_t* out_len,
+                        bool with_ref = false) {
+    B2A_CHECK(prompt_ids && lens && out_len && batch > 0, B2A_ERR_INVALID_INPUT, "prepare_input_ids: null argument");
+    B2A_CHECK(ref_code_len % 7 == 0, B2A_ERR_INVALID_INPUT, "prepare_input_ids: ref_code_len must be a multiple of 7");
+    for (int i = 0; i < ref_code_len; ++i)
+        B2A_CHECK(ref_code_list[i] >= 0 && ref_code_list[i] < 7 * 4096, B2A_ERR_INVALID_INPUT,
+                  "prepare_input_ids: reference code out of range [0, 7 * 4096)");
+    int mx = 0;
+    for (int b = 0; b < batch; ++b) {
+        B2A_CHECK(lens[b] >= 0 && (prompt_ids[b] || lens[b] == 0), B2A_ERR_INVALID_INPUT, "prepare_input_ids: bad prompt");
+        mx = std::max(mx, lens[b]);
+    }
+    const int ref = with_ref ? 1 + ref_text_len + 2 + 2 + ref_code_len + 2 : 0;
+    *out_len = mx + ref + 3;
+    if (!out) return;
+    for (int b = 0; b < batch; ++b) {
+        int32_t* r = out + (size_t)b * (mx + ref + 3);
+        int j = 0;
+        for (; j < mx - lens[b]; ++j) r[j] = tl.pad;
+        if (with_ref) {
+            r[j++] = tl.start_of_human;
+            for (int i = 0; i < ref_text_len; ++i) r[j++] = ref_text_ids[i];
+            r[j++] = tl.end_of_text;
+            r[j++] = tl.end_of_human;
+            r[j++] = tl.start_of_ai;
+            r[j++] = tl.start_of_speech;
+            for (int i = 0; i < ref_code_len; ++i) r[j++] = ref_code_list[i] + tl.audio_offset;
+            r[j++] = tl.end_of_speech;
+            r[j++] = tl.end_of_ai;
+        }
+        r[j++] = tl.start_of_human;
+        for (int i = 0; i < lens[b]; ++i) r[j++] = prompt_ids[b][i];
+        r[j++] = tl.end_of_text;
+        r[j++] = tl.end_of_human;
     }
 }
 
@@ -1697,7 +1808,7 @@ int32_t b2a_tts_time_steps(b2a_tts* h, int32_t B, int32_t ctx, int32_t iters, fl
         sa.logits = h->logits.p; sa.probs = h->probs.p; sa.tokens = h->tokens.p; sa.pos = h->pos.p; sa.recent = h->recent.p;
         sa.recent_n = h->recent_n.p; sa.out_tokens = h->out_tokens.p; sa.n_gen = h->n_gen.p; sa.done = h->done.p;
         sa.n_active = h->n_active.p; sa.forced = nullptr; sa.V = h->cfg.vocab_size; sa.R = 1; sa.max_tokens = MT;
-        sa.temperature = 0.f; sa.top_p = 1.f; sa.rep_penalty = 1.f; sa.seed = 0; sa.mask_eos = 1;
+        sa.temperature = 0.f; sa.top_p = 1.f; sa.rep_penalty = 1.f; sa.seed = 0; sa.mask_eos = 1; sa.stop_token = h->tok.end_of_speech;
         h->capture(B, sa, 1);
         B2A_CUDA(cudaMemsetAsync(h->ids.p, 0, (size_t)B * sizeof(int), s));
         init_rows_kernel<<<1, 32, 0, s>>>(h->ids.p, 1, B, 0, h->tokens.p, h->pos.p, h->recent.p, h->recent_n.p, h->n_gen.p,
@@ -1724,61 +1835,16 @@ int32_t b2a_tts_time_steps(b2a_tts* h, int32_t B, int32_t ctx, int32_t iters, fl
 
 int32_t b2a_tts_prepare_input_ids(const int32_t* const* prompt_ids, const int32_t* lens, int32_t batch, int32_t* out,
                                   int32_t* out_len) {
-    return guarded([&] {
-        B2A_CHECK(prompt_ids && lens && out_len && batch > 0, B2A_ERR_INVALID_INPUT, "b2a_tts_prepare_input_ids: null argument");
-        int mx = 0;
-        for (int b = 0; b < batch; ++b) mx = std::max(mx, lens[b]);
-        *out_len = mx + 3;
-        if (!out) return;
-        for (int b = 0; b < batch; ++b) {   // LlamaTTS.swift:499-543
-            int32_t* r = out + (size_t)b * (mx + 3);
-            int j = 0;
-            for (; j < mx - lens[b]; ++j) r[j] = TOK_PAD;
-            r[j++] = TOK_START_OF_HUMAN;
-            for (int i = 0; i < lens[b]; ++i) r[j++] = prompt_ids[b][i];
-            r[j++] = TOK_END_OF_TEXT;
-            r[j++] = TOK_END_OF_HUMAN;
-        }
-    });
+    return guarded([&] { prepare_ids(ORPHEUS_TOKENS, prompt_ids, lens, batch, nullptr, 0, nullptr, 0, out, out_len); });
 }
 
 int32_t b2a_tts_prepare_input_ids_ref(const int32_t* const* prompt_ids, const int32_t* lens, int32_t batch, const int32_t* ref_text_ids,
                                       int32_t ref_text_len, const int32_t* ref_code_list, int32_t ref_code_len, int32_t* out,
                                       int32_t* out_len) {
     return guarded([&] {
-        B2A_CHECK(prompt_ids && lens && out_len && batch > 0 && ref_text_len >= 0 && ref_code_len >= 0 && (ref_text_ids || ref_text_len == 0) &&
-                      (ref_code_list || ref_code_len == 0),
+        B2A_CHECK(ref_text_len >= 0 && ref_code_len >= 0 && (ref_text_ids || ref_text_len == 0) && (ref_code_list || ref_code_len == 0),
                   B2A_ERR_INVALID_INPUT, "b2a_tts_prepare_input_ids_ref: null argument");
-        B2A_CHECK(ref_code_len % 7 == 0, B2A_ERR_INVALID_INPUT, "b2a_tts_prepare_input_ids_ref: ref_code_len must be a multiple of 7");
-        for (int i = 0; i < ref_code_len; ++i)
-            B2A_CHECK(ref_code_list[i] >= 0 && ref_code_list[i] < 7 * 4096, B2A_ERR_INVALID_INPUT,
-                      "b2a_tts_prepare_input_ids_ref: reference code out of range [0, 7 * 4096)");
-        int mx = 0;
-        for (int b = 0; b < batch; ++b) {
-            B2A_CHECK(lens[b] >= 0 && (prompt_ids[b] || lens[b] == 0), B2A_ERR_INVALID_INPUT, "b2a_tts_prepare_input_ids_ref: bad prompt");
-            mx = std::max(mx, lens[b]);
-        }
-        const int ref = 1 + ref_text_len + 2 + 2 + ref_code_len + 2;        // LlamaTTS.swift:520-527
-        *out_len = mx + ref + 3;
-        if (!out) return;
-        for (int b = 0; b < batch; ++b) {   // LlamaTTS.swift:499-543: padding, reference block, prompt
-            int32_t* r = out + (size_t)b * (mx + ref + 3);
-            int j = 0;
-            for (; j < mx - lens[b]; ++j) r[j] = TOK_PAD;
-            r[j++] = TOK_START_OF_HUMAN;
-            for (int i = 0; i < ref_text_len; ++i) r[j++] = ref_text_ids[i];
-            r[j++] = TOK_END_OF_TEXT;
-            r[j++] = TOK_END_OF_HUMAN;
-            r[j++] = TOK_AUDIO_START;
-            r[j++] = TOK_START_OF_SPEECH;
-            for (int i = 0; i < ref_code_len; ++i) r[j++] = ref_code_list[i] + TOK_AUDIO_OFFSET;
-            r[j++] = TOK_END_OF_SPEECH;
-            r[j++] = TOK_AUDIO_END;
-            r[j++] = TOK_START_OF_HUMAN;
-            for (int i = 0; i < lens[b]; ++i) r[j++] = prompt_ids[b][i];
-            r[j++] = TOK_END_OF_TEXT;
-            r[j++] = TOK_END_OF_HUMAN;
-        }
+        prepare_ids(ORPHEUS_TOKENS, prompt_ids, lens, batch, ref_text_ids, ref_text_len, ref_code_list, ref_code_len, out, out_len, true);
     });
 }
 
@@ -1916,9 +1982,9 @@ int32_t b2a_tts_parse_output(const int32_t* tokens, int32_t batch, int32_t n, in
         int last = -1;   // LlamaTTS.swift:391-398: last match in row-major visiting order
         for (int i = 0; i < batch; ++i)
             for (int j = 0; j < n; ++j)
-                if (tokens[(size_t)i * n + j] == TOK_START_OF_SPEECH) last = j;
+                if (tokens[(size_t)i * n + j] == ORPHEUS_TOKENS.start_of_speech) last = j;
         for (int i = 0; i < batch; ++i) {
-            std::vector<int> r = parse_row(tokens + (size_t)i * n, n, last);
+            std::vector<int> r = parse_row(ORPHEUS_TOKENS, tokens + (size_t)i * n, n, last);
             code_lens[i] = (int)r.size();
             memcpy(code_lists_out + (size_t)i * n, r.data(), r.size() * sizeof(int));
         }
@@ -1951,6 +2017,75 @@ int32_t b2a_tts_interleave(const int32_t* c0, const int32_t* c1, const int32_t* 
             o[4] = c1[2 * i + 1] + 4 * 4096;
             o[5] = c2[4 * i + 2] + 5 * 4096;
             o[6] = c2[4 * i + 3] + 6 * 4096;
+        }
+    });
+}
+
+// ------------------------------------------------------------------------------------------------ VyvoTTS (Qwen3Model, Qwen3.swift:305-931)
+static b2a_llama_config qwen3_lm_stack_cfg(const b2a_qwen3_lm_config& c) {
+    B2A_CHECK(c.rope_linear_factor > 0.f, B2A_ERR_INVALID_INPUT, "qwen3 lm: rope_linear_factor must be positive");
+    b2a_llama_config l{};
+    l.hidden_size = c.hidden_size; l.num_hidden_layers = c.num_hidden_layers; l.intermediate_size = c.intermediate_size;
+    l.num_attention_heads = c.num_attention_heads; l.num_key_value_heads = c.num_key_value_heads; l.head_dim = c.head_dim;
+    l.vocab_size = c.vocab_size; l.rms_norm_eps = c.rms_norm_eps; l.rope_theta = c.rope_theta;
+    l.rope_factor = 1.f; l.rope_low_freq_factor = 1.f; l.rope_high_freq_factor = 4.f; l.rope_old_context_len = 8192.f;   // unused: linear_rope
+    l.tie_word_embeddings = c.tie_word_embeddings; l.max_batch = c.max_batch; l.max_context = c.max_context;
+    return l;
+}
+// "model.embed_tokens", q/k norm, "lm_head.weight" unless tied
+static StackSpec qwen3_lm_spec(const b2a_qwen3_lm_config& c) {
+    StackSpec s;
+    s.qk_norm = true;
+    s.linear_rope = c.rope_linear_factor;
+    return s;
+}
+
+int32_t b2a_qwen3_lm_create(int32_t device, const b2a_qwen3_lm_config* cfg, const b2a_tensor* tensors, int32_t n, b2a_snac* snac,
+                            b2a_tts** out) {
+    return guarded([&] {
+        B2A_CHECK(out, B2A_ERR_INVALID_INPUT, "b2a_qwen3_lm_create: null out");
+        *out = nullptr;
+        B2A_CHECK(cfg && tensors && n > 0, B2A_ERR_MODEL_NOT_INITIALIZED, "b2a_qwen3_lm_create: missing config or weights");
+        TensorTable tt(tensors, n);
+        std::unique_ptr<b2a_tts> h(new b2a_tts(device, qwen3_lm_stack_cfg(*cfg), tt, snac, qwen3_lm_spec(*cfg)));
+        h->tok = VYVO_TOKENS;
+        *out = h.release();
+    });
+}
+
+int32_t b2a_qwen3_lm_create_random(int32_t device, const b2a_qwen3_lm_config* cfg, float std, uint64_t seed, b2a_snac* snac, b2a_tts** out) {
+    return guarded([&] {
+        B2A_CHECK(out, B2A_ERR_INVALID_INPUT, "b2a_qwen3_lm_create_random: null out");
+        *out = nullptr;
+        B2A_CHECK(cfg && std > 0.f, B2A_ERR_MODEL_NOT_INITIALIZED, "b2a_qwen3_lm_create_random: missing config");
+        std::unique_ptr<b2a_tts> h(new b2a_tts(device, qwen3_lm_stack_cfg(*cfg), std, seed, snac, qwen3_lm_spec(*cfg)));
+        h->tok = VYVO_TOKENS;
+        *out = h.release();
+    });
+}
+
+int32_t b2a_qwen3_lm_prepare_input_ids(const int32_t* const* prompt_ids, const int32_t* lens, int32_t batch, int32_t* out, int32_t* out_len) {
+    return guarded([&] { prepare_ids(VYVO_TOKENS, prompt_ids, lens, batch, nullptr, 0, nullptr, 0, out, out_len); });
+}
+
+int32_t b2a_qwen3_lm_prepare_input_ids_ref(const int32_t* const* prompt_ids, const int32_t* lens, int32_t batch, const int32_t* ref_text_ids,
+                                           int32_t ref_text_len, const int32_t* ref_code_list, int32_t ref_code_len, int32_t* out,
+                                           int32_t* out_len) {
+    return guarded([&] {
+        B2A_CHECK(ref_text_len >= 0 && ref_code_len >= 0 && (ref_text_ids || ref_text_len == 0) && (ref_code_list || ref_code_len == 0),
+                  B2A_ERR_INVALID_INPUT, "b2a_qwen3_lm_prepare_input_ids_ref: null argument");
+        prepare_ids(VYVO_TOKENS, prompt_ids, lens, batch, ref_text_ids, ref_text_len, ref_code_list, ref_code_len, out, out_len, true);
+    });
+}
+
+int32_t b2a_qwen3_lm_parse_output(const int32_t* tokens, int32_t batch, int32_t n, int32_t* code_lists_out, int32_t* code_lens) {
+    return guarded([&] {
+        B2A_CHECK(tokens && code_lists_out && code_lens && batch > 0 && n >= 0, B2A_ERR_INVALID_INPUT, "b2a_qwen3_lm_parse_output: bad argument");
+        for (int i = 0; i < batch; ++i) {
+            const int32_t* row = tokens + (size_t)i * n;
+            std::vector<int> r = parse_row(VYVO_TOKENS, row, n, codes_start(VYVO_TOKENS, row, n));
+            code_lens[i] = (int)r.size();
+            memcpy(code_lists_out + (size_t)i * n, r.data(), r.size() * sizeof(int));
         }
     });
 }

@@ -194,11 +194,14 @@ prompt_attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
 // [B][nkv][max_ctx][128] at positions 0 .. L-1 (rows >= L are not touched).  One CTA per (64-position tile, row, head), heads
 // [0, nq) = queries, [nq, nq + nkv) = keys and values.  rope [max_ctx][64] = (cos, sin) of position / freqs[d] (rope_table_kernel).
 // V goes through shared memory so that the transposed rows are written 128 bytes at a time.  Positions in [L, Lp) are zeros.
+// qnorm / knorm (nullable, [128] each): per-head RMSNorm x * rsqrt(mean(x^2) + eps) * w of q and k before RoPE (Qwen3 stacks); the cache
+// then holds the normalised, rotated K, as the decode step writes it.
 __global__ void __launch_bounds__(256)
 pack_prompt_kernel(const float* __restrict__ qkv, const float2* __restrict__ rope, __half* __restrict__ Qp, __half* __restrict__ Kp,
                    __half* __restrict__ Vt, float* __restrict__ kcache, float* __restrict__ vcache, int L, int Lp, int nq, int nkv,
-                   int max_ctx) {
+                   int max_ctx, const float* __restrict__ qnorm, const float* __restrict__ knorm, float qk_eps) {
     __shared__ __half sv[2][64][HDIM + 2];
+    __shared__ float srs[64];                                      // q/k norm: rstd of each position's vector
     const int b = blockIdx.y, hd = blockIdx.z, t0 = blockIdx.x * 64;
     const bool is_q = hd < nq;
     const int h = is_q ? hd : hd - nq, ld = (nq + 2 * nkv) * HDIM;
@@ -207,13 +210,26 @@ pack_prompt_kernel(const float* __restrict__ qkv, const float2* __restrict__ rop
     const int col = is_q ? h * HDIM : (nq + h) * HDIM;
     float* kc = kcache + (((long long)b * nkv + h) * max_ctx) * HDIM;
     float* vc = vcache + (((long long)b * nkv + h) * max_ctx) * HDIM;
+    const float* gain = is_q ? qnorm : knorm;
+    if (gain) {   // one warp per position, the decode step's reduction (attn_decode_cluster_kernel)
+        const int lane = threadIdx.x & 31;
+        for (int r = threadIdx.x >> 5; r < 64; r += 8) {
+            const int t = t0 + r;
+            if (t >= L) continue;
+            const float4 x = reinterpret_cast<const float4*>(base + (long long)t * ld + col)[lane];
+            const float ss = warp_sum(x.x * x.x + x.y * x.y + x.z * x.z + x.w * x.w);
+            if (lane == 0) srs[r] = rsqrtf(ss * (1.0f / HDIM) + qk_eps);
+        }
+        __syncthreads();
+    }
     for (int i = threadIdx.x; i < 64 * (HDIM / 2); i += 256) {
         const int r = i / (HDIM / 2), d = i - r * (HDIM / 2), t = t0 + r;
         float y1 = 0.f, y2 = 0.f;
         if (t < L) {
             const float2 cs = rope[t * (HDIM / 2) + d];
             const float* x = base + (long long)t * ld + col;
-            const float x1 = x[d], x2 = x[d + HDIM / 2];
+            float x1 = x[d], x2 = x[d + HDIM / 2];
+            if (gain) { x1 = x1 * srs[r] * gain[d]; x2 = x2 * srs[r] * gain[d + HDIM / 2]; }
             y1 = x1 * cs.x - x2 * cs.y; y2 = x2 * cs.x + x1 * cs.y;
             if (!is_q) { kc[(long long)t * HDIM + d] = y1; kc[(long long)t * HDIM + d + HDIM / 2] = y2; }
         }

@@ -901,6 +901,64 @@ int32_t b2a_tts_create_from_directory(const char* model_dir, int32_t device, int
     });
 }
 
+// config.json -> b2a_qwen3_lm_config (Qwen3Configuration.init(from:), Config.swift:50-73): the eight decode()d keys are required, the rest
+// take the reference's defaults; rope_scaling counts only as {"type": "linear", "factor": f} (Qwen3Attention, Qwen3.swift:177-188)
+int32_t b2a_qwen3_lm_config_from_json(const char* config_path, int32_t max_batch, int32_t max_context, b2a_qwen3_lm_config* cfg,
+                                      int32_t* quant_group_size, int32_t* quant_bits) {
+    return guarded([&] {
+        B2A_CHECK(config_path && cfg, B2A_ERR_INVALID_INPUT, "b2a_qwen3_lm_config_from_json: null argument");
+        const Json j = read_json_file(config_path);
+        B2A_CHECK(j.kind == Json::Obj, B2A_ERR_MODEL_NOT_INITIALIZED, "config.json is not an object");
+        for (const char* k : {"hidden_size", "num_hidden_layers", "intermediate_size", "num_attention_heads", "rms_norm_eps", "vocab_size",
+                              "num_key_value_heads", "head_dim"})
+            B2A_CHECK(j.has(k), B2A_ERR_MODEL_NOT_INITIALIZED, std::string("config.json: missing ") + k);
+        b2a_qwen3_lm_config c{};
+        c.hidden_size = (int)j.number("hidden_size", 0); c.num_hidden_layers = (int)j.number("num_hidden_layers", 0);
+        c.intermediate_size = (int)j.number("intermediate_size", 0); c.num_attention_heads = (int)j.number("num_attention_heads", 0);
+        c.num_key_value_heads = (int)j.number("num_key_value_heads", 0); c.head_dim = (int)j.number("head_dim", 0);
+        c.vocab_size = (int)j.number("vocab_size", 0); c.rms_norm_eps = (float)j.number("rms_norm_eps", 0.0);
+        c.rope_theta = (float)j.number("rope_theta", 1000000.0);
+        c.rope_linear_factor = 1.f;
+        if (const Json* rs = j.find("rope_scaling"); rs && rs->kind == Json::Obj) {
+            const Json* ty = rs->find("type");
+            if (ty && ty->kind == Json::Str && ty->str == "linear" && rs->has("factor")) {
+                const Json* f = rs->find("factor");
+                B2A_CHECK(f->kind == Json::Num && f->num > 0, B2A_ERR_MODEL_NOT_INITIALIZED, "rope_scaling.factor must be a positive number");
+                c.rope_linear_factor = (float)f->num;
+            }
+        }
+        c.tie_word_embeddings = (int)j.number("tie_word_embeddings", 0);
+        c.max_position_embeddings = (int)j.number("max_position_embeddings", 32768);
+        c.sample_rate = (int)j.number("sample_rate", 24000);
+        c.eos_token_id = (int)j.number("eos_token_id", 151645);
+        c.max_batch = max_batch; c.max_context = max_context;
+        *cfg = c;
+        int gs = 0, bits = 0;
+        if (const Json* q = j.find("quantization"); q && q->kind == Json::Obj) { gs = (int)q->number("group_size", 64); bits = (int)q->number("bits", 4); }
+        if (quant_group_size) *quant_group_size = gs;
+        if (quant_bits) *quant_bits = bits;
+    });
+}
+
+// Qwen3Model.fromModelDirectory (Qwen3.swift:892-930): config.json + every *.safetensors -> sanitize -> (de)quantise -> create
+int32_t b2a_qwen3_lm_create_from_directory(const char* model_dir, int32_t device, int32_t max_batch, int32_t max_context, b2a_snac* snac,
+                                           b2a_tts** out) {
+    return guarded([&] {
+        B2A_CHECK(model_dir && out, B2A_ERR_INVALID_INPUT, "b2a_qwen3_lm_create_from_directory: null argument");
+        *out = nullptr;
+        b2a_qwen3_lm_config cfg{};
+        const std::string dir = model_dir;
+        int32_t st = b2a_qwen3_lm_config_from_json((dir + "/config.json").c_str(), max_batch, max_context, &cfg, nullptr, nullptr);
+        if (st != B2A_OK) throw Error(st, b2a_last_error());
+        std::unique_ptr<b2a_weights> w(new b2a_weights());
+        w->load(dir);
+        w->sanitize_llama(cfg.tie_word_embeddings != 0, parse_quant(read_json_file(dir + "/config.json")));
+        const std::vector<b2a_tensor> tab = w->table();
+        st = b2a_qwen3_lm_create(device, &cfg, tab.data(), (int32_t)tab.size(), snac, out);
+        if (st != B2A_OK) throw Error(st, b2a_last_error());
+    });
+}
+
 // config.json -> b2a_qwen3_talker_config: "talker_config" with its nested "code_predictor_config" (Qwen3TTSConfig.swift:45-63,268-292; the
 // same defaults), max_batch / max_context from the caller.
 static b2a_qwen3_talker_config qwen3_talker_config_of(const Json& root, int max_batch, int max_context) {

@@ -49,6 +49,8 @@ class AudioGenerationInfo:
 class LlamaTTSModel:
     sample_rate = 24000
     default_generation_parameters = GenerateParameters()
+    _abi = "b2a_tts"            # prefix of the constructors, prompt framing and parse entry points of this model's token layout
+    _pad_token = PAD_TOKEN
 
     @staticmethod
     def _c_config(config: dict, max_batch: int, max_context: int) -> _ffi.LlamaConfig:
@@ -70,8 +72,8 @@ class LlamaTTSModel:
         c = cls._c_config(config, max_batch, max_context)
         self.config, self.vocab_size, self._snac_model = config, config["vocab_size"], snac
         self._h = C.c_void_p()
-        _ffi.check(_ffi.lib().b2a_tts_create_random(device, C.byref(c), std, seed, snac._h if snac else None,
-                                                    C.byref(self._h)))
+        _ffi.check(getattr(_ffi.lib(), cls._abi + "_create_random")(device, C.byref(c), std, seed, snac._h if snac else None,
+                                                                    C.byref(self._h)))
         return self
 
     @property
@@ -94,23 +96,15 @@ class LlamaTTSModel:
 
     def __init__(self, config: dict, weights: Dict, snac: Optional[SNAC] = None, device: int = 0,
                  max_batch: int = 8, max_context: int = 2048):
-        rs = config.get("rope_scaling") or {}
-        nh = config["num_attention_heads"]
-        c = _ffi.LlamaConfig(
-            config["hidden_size"], config["num_hidden_layers"], config["intermediate_size"], nh,
-            config.get("num_key_value_heads", nh), config.get("head_dim") or config["hidden_size"] // nh,
-            config["vocab_size"], config["rms_norm_eps"], config.get("rope_theta", 10000.0),
-            float(rs.get("factor", 32.0)), float(rs.get("low_freq_factor", 1.0)), float(rs.get("high_freq_factor", 4.0)),
-            float(rs.get("original_max_position_embeddings", 8192.0)), int(config.get("tie_word_embeddings", True)),
-            max_batch, max_context)
+        c = self._c_config(config, max_batch, max_context)
         self.config, self.vocab_size, self._snac_model = config, config["vocab_size"], snac
         weights = {k: v for k, v in weights.items() if "rotary_emb.inv_freq" not in k}      # sanitize (:583-593)
         if c.tie_word_embeddings:
             weights.pop("lm_head.weight", None)
         table, keep = _ffi.make_tensor_table(weights)
         self._h = C.c_void_p()
-        _ffi.check(_ffi.lib().b2a_tts_create(device, C.byref(c), table, len(weights), snac._h if snac else None,
-                                             C.byref(self._h)))
+        _ffi.check(getattr(_ffi.lib(), self._abi + "_create")(device, C.byref(c), table, len(weights), snac._h if snac else None,
+                                                              C.byref(self._h)))
         del keep
 
     @classmethod
@@ -125,13 +119,13 @@ class LlamaTTSModel:
         self.config = json.loads((Path(model_dir) / "config.json").read_text())
         self.vocab_size, self._snac_model = self.config.get("vocab_size", 0), snac      # a bad config.json is the library's error to raise
         self._h = C.c_void_p()
-        _ffi.check(_ffi.lib().b2a_tts_create_from_directory(str(model_dir).encode(), device, max_batch, max_context,
-                                                            snac._h if snac else None, C.byref(self._h)))
+        _ffi.check(getattr(_ffi.lib(), cls._abi + "_create_from_directory")(str(model_dir).encode(), device, max_batch, max_context,
+                                                                            snac._h if snac else None, C.byref(self._h)))
         return self
 
     # -- token plumbing -------------------------------------------------------------------------
-    @staticmethod
-    def prepare_input_ids(prompt_token_ids: Sequence[Sequence[int]], ref_code_list: Optional[Sequence[int]] = None,
+    @classmethod
+    def prepare_input_ids(cls, prompt_token_ids: Sequence[Sequence[int]], ref_code_list: Optional[Sequence[int]] = None,
                           ref_text_ids: Optional[Sequence[int]] = None) -> Tuple[np.ndarray, np.ndarray]:
         """prepareInputIds (:446-553) on already-tokenised prompts.  With both `ref_code_list` (the 7-token interleaved codes
         of a reference clip, `encode_audio_to_code_list`) and `ref_text_ids` (its tokenised transcript) every row gets the
@@ -142,15 +136,15 @@ class LlamaTTSModel:
         pp = (C.c_void_p * B)(*[r.ctypes.data for r in rows])
         n = C.c_int32(0)
         if ref_code_list is None or ref_text_ids is None:
-            fn, extra = _ffi.lib().b2a_tts_prepare_input_ids, ()
+            fn, extra = getattr(_ffi.lib(), cls._abi + "_prepare_input_ids"), ()
         else:
             rc = np.ascontiguousarray(ref_code_list, dtype=np.int32).reshape(-1)
             rt = np.ascontiguousarray(ref_text_ids, dtype=np.int32).reshape(-1)
-            fn, extra = _ffi.lib().b2a_tts_prepare_input_ids_ref, (_ffi.ptr(rt), len(rt), _ffi.ptr(rc), len(rc))
+            fn, extra = getattr(_ffi.lib(), cls._abi + "_prepare_input_ids_ref"), (_ffi.ptr(rt), len(rt), _ffi.ptr(rc), len(rc))
         _ffi.check(fn(pp, _ffi.ptr(lens), B, *extra, None, C.byref(n)))
         out = np.empty((B, n.value), dtype=np.int32)
         _ffi.check(fn(pp, _ffi.ptr(lens), B, *extra, _ffi.ptr(out), C.byref(n)))
-        return out, out != PAD_TOKEN
+        return out, out != cls._pad_token
 
     def encode_audio_to_code_list(self, audio) -> List[int]:
         """llamaEncodeAudioToCodes (:72-98): a 1-D reference clip at 24 kHz -> SNAC codes on the device -> 7-token interleave."""
@@ -165,14 +159,14 @@ class LlamaTTSModel:
             return self.prepare_input_ids([list(prompt_token_ids)], self.encode_audio_to_code_list(ref_audio), ref_text_ids)[0]
         return self.prepare_input_ids([list(prompt_token_ids)])[0]
 
-    @staticmethod
-    def parse_output(input_ids) -> List[List[int]]:
+    @classmethod
+    def parse_output(cls, input_ids) -> List[List[int]]:
         """parseOutput (:383-434)."""
         ids = np.ascontiguousarray(input_ids, dtype=np.int32)
         B, n = ids.shape
         out = np.empty((B, max(n, 1)), dtype=np.int32)
         lens = np.empty(B, dtype=np.int32)
-        _ffi.check(_ffi.lib().b2a_tts_parse_output(_ffi.ptr(ids), B, n, _ffi.ptr(out), _ffi.ptr(lens)))
+        _ffi.check(getattr(_ffi.lib(), cls._abi + "_parse_output")(_ffi.ptr(ids), B, n, _ffi.ptr(out), _ffi.ptr(lens)))
         return [out[b, :lens[b]].tolist() for b in range(B)]
 
     @staticmethod

@@ -8,8 +8,12 @@ With --ref-seconds S every row carries a voice-cloning reference block (prepareI
 a synthetic S-second clip encoded by SNAC on the device and a 16-token stand-in transcript.  The encode runs before the timed call;
 prompts of any length take the batched prefill (longer than 128 tokens with the wgmma prompt attention, csrc/prompt_attn_tc.cuh).
 
-    python tools/tts_benchmark.py [--batch 1] [--prompt 64] [--max-tokens 512] [--model-dir DIR] [--stream] [--interval 0.32]
-                                  [--ref-seconds S]"""
+--model qwen3 runs VyvoTTS (Qwen3Model, Qwen3.swift) instead: QWEN3_06B below, Qwen3-0.6B's layer shapes with VyvoTTS's 180 352-token
+vocabulary -- an assumed geometry, as the published checkpoint's config.json is not at hand -- and the same prompts framed by its
+prepareInputIds, ending in its start-of-speech 151670.
+
+    python tools/tts_benchmark.py [--model orpheus|qwen3] [--batch 1] [--prompt 64] [--max-tokens 512] [--model-dir DIR] [--stream]
+                                  [--interval 0.32] [--ref-seconds S]"""
 import argparse
 import sys
 import time
@@ -21,7 +25,11 @@ sys.path.insert(0, str(Path(__file__).resolve().parents[1]))
 import mlx_audio_swift_b200 as m  # noqa: E402
 from bench import ORPHEUS, make_prompts  # noqa: E402
 
+QWEN3_06B = dict(hidden_size=1024, num_hidden_layers=28, intermediate_size=3072, num_attention_heads=16, num_key_value_heads=8, head_dim=128,
+                 vocab_size=180352, rms_norm_eps=1e-6, rope_theta=1000000.0, tie_word_embeddings=True)
+
 ap = argparse.ArgumentParser()
+ap.add_argument("--model", default="orpheus", choices=["orpheus", "qwen3"])
 ap.add_argument("--batch", type=int, default=1)
 ap.add_argument("--prompt", type=int, default=64)
 ap.add_argument("--max-tokens", type=int, default=512)
@@ -36,19 +44,23 @@ if a.ref_seconds > 0:
     n_ref = int(a.ref_seconds * 24000)
     ref_len = 7 * codec.encoded_length(n_ref) // 4 + 16 + 9            # codes + transcript + the block's framing tokens
 ctx = a.prompt + ref_len + a.max_tokens + 16
+Model, geometry, sos = (m.Qwen3Model, QWEN3_06B, 151670) if a.model == "qwen3" else (m.LlamaTTSModel, ORPHEUS, 128257)
 if a.model_dir:
-    tts = m.LlamaTTSModel.from_model_directory(a.model_dir, snac=codec, max_batch=a.batch, max_context=ctx)
+    tts = Model.from_model_directory(a.model_dir, snac=codec, max_batch=a.batch, max_context=ctx)
 else:
-    tts = m.LlamaTTSModel.random_init(ORPHEUS, snac=codec, max_batch=a.batch, max_context=ctx)
+    tts = Model.random_init(geometry, snac=codec, max_batch=a.batch, max_context=ctx)
+# the untruncated make_prompts rows are [SOH] body [EOT, EOH, SOS]: a body of prompt - 4 tokens keeps the framed prompt at --prompt
+body = [r[1:-3][:max(a.prompt - 4, 1)].tolist() for r in make_prompts(0)[:a.batch]]
 ids = make_prompts(0)[:a.batch, :a.prompt]
+if a.model == "qwen3":
+    ids, _ = tts.prepare_input_ids(body)
+    ids = np.concatenate([ids, np.full((ids.shape[0], 1), sos, dtype=np.int32)], axis=1)
 if a.ref_seconds > 0:
     t = np.arange(n_ref) / 24000.0
     clip = (0.5 * np.sin(2 * np.pi * 220.0 * t) + 0.1 * np.random.default_rng(0).standard_normal(n_ref)).astype(np.float32)
     ref_text = make_prompts(1)[0, 1:17].tolist()
-    # the untruncated make_prompts rows are [SOH] body [EOT, EOH, SOS]: a body of prompt - 4 tokens keeps the framed prompt at --prompt
-    body = [r[1:-3][:max(a.prompt - 4, 1)].tolist() for r in make_prompts(0)[:a.batch]]
     ids, _ = tts.prepare_input_ids(body, tts.encode_audio_to_code_list(clip), ref_text)
-    ids = np.concatenate([ids, np.full((ids.shape[0], 1), 128257, dtype=np.int32)], axis=1)
+    ids = np.concatenate([ids, np.full((ids.shape[0], 1), sos, dtype=np.int32)], axis=1)
     print(f"Cloning prompt: {a.ref_seconds:g}s reference -> {ids.shape[1]} tokens per row")
 P = m.GenerateParameters(max_tokens=a.max_tokens, temperature=0.6, top_p=0.8, repetition_penalty=1.3, repetition_context_size=20,
                          mask_eos=True, wrap_codes=True)
