@@ -328,6 +328,71 @@ int32_t b2a_qwen3_lm_prepare_input_ids_ref(const int32_t* const* prompt_ids, con
 /* parseOutputRow (:333-358) for every row of tokens [B, n]; code_lists_out [B, n], code_lens [B] */
 int32_t b2a_qwen3_lm_parse_output(const int32_t* tokens, int32_t batch, int32_t n, int32_t* code_lists_out, int32_t* code_lens);
 
+/* ------------------------------------------------------------------ Soprano (Qwen3 language model + Vocos decoder of its hidden states)
+ * Replaces class SopranoModel (Sources/MLXAudioTTS/Models/Soprano/Soprano.swift:184-977) and SopranoDecoder (SopranoDecoder.swift:222-285).
+ * The constructors return a b2a_tts handle that owns a Vocos decoder: b2a_tts_generate / _dev, b2a_tts_forward_logits, b2a_tts_cancel and
+ * b2a_tts_destroy serve it.  Soprano decodes the final-RMSNorm hidden state of the last prompt position and of every generated token that
+ * is fed back (forwardWithHiddenStates, :254-275; streamGenerate, :801-885) -- 1 + n_tokens states per row, none for the stop token --
+ * into audio; the step captures them on the device.  Sampling is Soprano's own (:836-901, :996-1059): the repetition penalty looks at the
+ * last repetition_context_size GENERATED tokens and applies once per occurrence (l > 0 ? l / p : l * p), also at temperature 0; top-p
+ * keeps token i iff the ascending cumulative sum of exp(l) (unnormalised) through i exceeds 1 - top_p, and the temperature divides the
+ * filtered logits afterwards.  When no token passes (sum exp(l) <= 1 - top_p) the argmax is returned, where the reference would sample
+ * an all -inf row.  Generation stops on stop_token_id (the tokenizer's EOS, :972), which is not kept.
+ * Waveform of a row with n states: interpolate1d(align_corners) to upscale (n - 1) + 1 frames, the Vocos backbone and ISTFT head, then its
+ * last (n - 1) token_size samples (:664-671); for n = 1 the untrimmed n_fft samples of a one-frame overlap-add (SopranoDecoder.swift:191-196).
+ * Rows of one call decode as they would one by one.  head_dim must be 128; prompt + max_tokens + 1 must fit max_context. */
+typedef struct b2a_soprano_config {     /* SopranoConfiguration, SopranoConfig.swift:65-176, with its defaults */
+    int32_t hidden_size;
+    int32_t num_hidden_layers;
+    int32_t intermediate_size;
+    int32_t num_attention_heads;
+    int32_t num_key_value_heads;
+    int32_t head_dim;
+    int32_t vocab_size;
+    float rms_norm_eps;              /* 1e-6 */
+    float rope_theta;                /* 1e4 */
+    int32_t tie_word_embeddings;     /* 0 */
+    int32_t max_position_embeddings; /* 512 (informational) */
+    int32_t bos_token_id;            /* 1 (informational) */
+    int32_t eos_token_id;            /* 2 (informational: generation stops on stop_token_id) */
+    int32_t pad_token_id;            /* 0 (informational) */
+    int32_t stop_token_id;           /* the tokenizer's EOS; 3 when it has none */
+    int32_t sample_rate;             /* 32000 */
+    int32_t decoder_num_layers;      /* 8 */
+    int32_t decoder_dim;             /* 768 */
+    int32_t decoder_intermediate_dim;/* 2304 */
+    int32_t hop_length;              /* 512 */
+    int32_t n_fft;                   /* 2048 */
+    int32_t upscale;                 /* 4 */
+    int32_t input_kernel;            /* 1 */
+    int32_t dw_kernel;               /* 3 */
+    int32_t token_size;              /* 2048 */
+    int32_t receptive_field;         /* 4 (informational: audio is decoded once per call) */
+    int32_t max_batch;               /* KV-cache rows */
+    int32_t max_context;             /* KV-cache positions per row */
+} b2a_soprano_config;
+
+/* tensors in SopranoModel.sanitize's layout (:314-361): model.* (the Qwen3 stack), lm_head.weight unless tied, decoder.decoder.* (the
+ * Vocos backbone: embed, norm, convnext.N.*, final_layer_norm) and decoder.head.out.*; conv weights in the MLX [out, k, in] layout */
+int32_t b2a_soprano_create(int32_t device, const b2a_soprano_config* cfg, const b2a_tensor* tensors, int32_t n_tensors, b2a_tts** out);
+/* config.json -> the struct with SopranoConfiguration's defaults.  Unless repo_hint contains "soprano-1.1" (case-insensitive) the
+ * decoder is the older one: decoder_dim 512, decoder_intermediate_dim 1536 and input_kernel 3, whatever config.json says
+ * (fromModelDirectory, :934-941).  repo_hint NULL: the config file's directory name.  quant_* (nullable) from "quantization" (0 = none) */
+int32_t b2a_soprano_config_from_json(const char* config_path, const char* repo_hint, int32_t max_batch, int32_t max_context,
+                                     b2a_soprano_config* cfg, int32_t* quant_group_size, int32_t* quant_bits);
+/* fromModelDirectory (:928-976) without the tokenizer: config.json (+ the repo rule above; repo_hint NULL = the directory name) + every
+ * *.safetensors -> sanitize (a leading "model." stripped, language_model.lm_head -> lm_head, language_model.* and bare keys -> model.*,
+ * lm_head.weight dropped when tied) -> MLX 2/4/8-bit layers expanded -> b2a_soprano_create.  stop_token_id is 3 unless the directory's
+ * tokenizer_config.json names an eos_token that tokenizer.json's added_tokens resolve. */
+int32_t b2a_soprano_create_from_directory(const char* model_dir, const char* repo_hint, int32_t device, int32_t max_batch,
+                                          int32_t max_context, b2a_tts** out);
+/* SopranoDecoder.callAsFunction + the cut on its own: hidden [B, n, hidden_size] float32 (host) -> wave_out [B, wave_cap], wave_len[B]
+ * (all rows the same length).  n >= 1. */
+int32_t b2a_soprano_decode_hidden(b2a_tts* h, const float* hidden, int32_t batch, int32_t n, float* wave_out, int64_t wave_cap,
+                                  int64_t* wave_len);
+/* samples of the waveform of n hidden states (0 for a handle that is not Soprano's) */
+int64_t b2a_soprano_wave_length(const b2a_tts* h, int32_t n);
+
 /* ------------------------------------------------------------------ weight / format plumbing (SURVEY.md 8f, row N4)
  * Host-only.  Replaces MLX.loadArrays on *.safetensors (llamaTTSLoadWeights, LlamaTTS.swift:982-994: every file of a directory, later
  * files win), WhisperModel.detectFormat / sanitize / remapMlxWhisperKey / whisperSinusoids (WhisperModel.swift:315-480),
@@ -350,6 +415,8 @@ int32_t b2a_weights_sanitize_llama(b2a_weights* w, int32_t tie_word_embeddings, 
  * mlx-swift-lm's PerLayerQuantization): "quantization": {"group_size", "bits", "<layer path>": false | {"group_size", "bits"}} --
  * per-layer settings override the default, a layer marked false must not carry .scales.  b2a_tts_create_from_directory uses this. */
 int32_t b2a_weights_sanitize_llama_config(b2a_weights* w, const char* config_path);
+/* SopranoModel.sanitize (Soprano.swift:314-361) + the de-quantisation config.json asks for: the key layout b2a_soprano_create takes */
+int32_t b2a_weights_sanitize_soprano_config(b2a_weights* w, const char* config_path);
 /* MLX affine de-quantisation (to bf16) of every layer that carries "<path>.scales", with one group_size / bits -- what
  * WhisperModel.fromDirectory's quantize(model:groupSize:bits:) implies for a quantised checkpoint (WhisperModel.swift:499-511:
  * every Linear and decoder.embed_tokens; the tied projection then multiplies by the de-quantised embedding,

@@ -165,6 +165,21 @@ int32_t b2a_snac_local_attn_test(const float* qkv, const float* inv_freq, int32_
  * gives them.  Errors as b2a_encodec_encode. */
 int32_t b2a_encodec_encode_latent_test(b2a_encodec* h, const float* audio, int32_t batch, int64_t samples, float* z);
 
+/* ------------------------------------------------------------------ Soprano
+ *   b2a_soprano_create_random : b2a_soprano_create with the language model drawn on the device (as b2a_qwen3_lm_create_random) and the
+ *       decoder from `decoder_tensors` (decoder.decoder.* / decoder.head.* keys; n_decoder_tensors may not be 0).
+ *   b2a_soprano_hidden_states : the hidden states the last b2a_tts_generate captured: out [batch, max_tokens + 1, hidden_size] float32
+ *       (nullable), n_states[batch] = 1 + the row's generated tokens.
+ *   b2a_vocos_decode_upsampled_dev : SopranoDecoder on DEVICE rows: row b of the batch is the n states at d_states + d_rows[b] * row_stride
+ *       (d_rows NULL: b), upsampled x upscale inside the embed conv's operand kernel; d_wave [B, b2a_vocos_upsampled_length].
+ *   b2a_vocos_upsampled_length : (upscale (n - 1)) hop for n >= 2, n_fft (the untrimmed one-frame overlap-add) for n = 1.            */
+int32_t b2a_soprano_create_random(int32_t device, const b2a_soprano_config* cfg, float std, uint64_t seed, const b2a_tensor* decoder_tensors,
+                                  int32_t n_decoder_tensors, b2a_tts** out);
+int32_t b2a_soprano_hidden_states(b2a_tts* h, int32_t batch, float* out, int32_t* n_states);
+int32_t b2a_vocos_decode_upsampled_dev(b2a_vocos* h, const float* d_states, int64_t row_stride, const int32_t* d_rows, int32_t batch, int32_t n,
+                                       int32_t upscale, float* d_wave, void* stream);
+int64_t b2a_vocos_upsampled_length(const b2a_vocos* h, int32_t n, int32_t upscale);
+
 #ifdef __cplusplus
 }
 #endif

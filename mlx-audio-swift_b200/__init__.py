@@ -9,6 +9,7 @@ from .dsp import (IncrementalMelSpectrogram, LogMel, compute_mel_spectrogram, ha
 from .snac import SNAC
 from .llama_tts import AudioGenerationInfo, GenerateParameters, LlamaTTSModel
 from .vyvo_tts import Qwen3Model
+from .soprano_tts import SopranoModel
 from .vocos import Vocos
 from .encodec import Encodec, EncodecConfig, EncodecEncodedAudio
 from .loading import Weights, llama_config_from_json
@@ -17,7 +18,7 @@ from .qwen3_tts import (Qwen3CodePredictorConfig, Qwen3GenerateParameters, Qwen3
                         Qwen3TTSSpeakerEncoder, Qwen3TTSTalker)
 
 __all__ = ["AudioGenerationError", "IncrementalMelSpectrogram", "LogMel", "compute_mel_spectrogram", "hanning_window", "hamming_window", "power_to_db",
-           "mel_filters", "whisper_encoder_features", "SNAC", "LlamaTTSModel", "Qwen3Model", "GenerateParameters",
+           "mel_filters", "whisper_encoder_features", "SNAC", "LlamaTTSModel", "Qwen3Model", "SopranoModel", "GenerateParameters",
            "AudioGenerationInfo", "Vocos", "Weights", "llama_config_from_json", "Encodec", "EncodecConfig", "EncodecEncodedAudio", "WhisperModel", "STTGenerateParameters", "STTOutput",
            "StreamingInferenceSession", "StreamingConfig", "StreamingUpdate",
            "Qwen3TTSTalker", "Qwen3TTSModel", "Qwen3TalkerConfig", "Qwen3CodePredictorConfig", "Qwen3GenerateParameters",

@@ -57,6 +57,16 @@ class Qwen3LMConfig(C.Structure):
                                              "max_context")])
 
 
+class SopranoConfig(C.Structure):
+    _fields_ = ([(n, C.c_int32) for n in ("hidden_size", "num_hidden_layers", "intermediate_size", "num_attention_heads",
+                                           "num_key_value_heads", "head_dim", "vocab_size")]
+                + [("rms_norm_eps", C.c_float), ("rope_theta", C.c_float)]
+                + [(n, C.c_int32) for n in ("tie_word_embeddings", "max_position_embeddings", "bos_token_id", "eos_token_id", "pad_token_id",
+                                             "stop_token_id", "sample_rate", "decoder_num_layers", "decoder_dim", "decoder_intermediate_dim",
+                                             "hop_length", "n_fft", "upscale", "input_kernel", "dw_kernel", "token_size", "receptive_field",
+                                             "max_batch", "max_context")])
+
+
 class GenParams(C.Structure):
     _fields_ = [("max_tokens", C.c_int32), ("temperature", C.c_float), ("top_p", C.c_float),
                 ("repetition_penalty", C.c_float), ("repetition_context_size", C.c_int32), ("seed", C.c_uint64)]
@@ -225,6 +235,15 @@ SIGNATURES = {
     "b2a_qwen3_lm_prepare_input_ids_ref": (C.c_int32, [C.POINTER(_P), _P, C.c_int32, _P, C.c_int32, _P, C.c_int32, _P,
                                                        C.POINTER(C.c_int32)]),
     "b2a_qwen3_lm_parse_output": (C.c_int32, [_P, C.c_int32, C.c_int32, _P, _P]),
+    "b2a_soprano_create": (C.c_int32, [C.c_int32, C.POINTER(SopranoConfig), C.POINTER(Tensor), C.c_int32, C.POINTER(_P)]),
+    "b2a_soprano_create_random": (C.c_int32, [C.c_int32, C.POINTER(SopranoConfig), C.c_float, C.c_uint64, C.POINTER(Tensor), C.c_int32,
+                                              C.POINTER(_P)]),
+    "b2a_soprano_config_from_json": (C.c_int32, [C.c_char_p, C.c_char_p, C.c_int32, C.c_int32, C.POINTER(SopranoConfig),
+                                                 C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
+    "b2a_soprano_create_from_directory": (C.c_int32, [C.c_char_p, C.c_char_p, C.c_int32, C.c_int32, C.c_int32, C.POINTER(_P)]),
+    "b2a_soprano_decode_hidden": (C.c_int32, [_P, _P, C.c_int32, C.c_int32, _P, C.c_int64, _P]),
+    "b2a_soprano_wave_length": (C.c_int64, [_P, C.c_int32]),
+    "b2a_soprano_hidden_states": (C.c_int32, [_P, C.c_int32, _P, _P]),
     "b2a_vocos_create": (C.c_int32, [C.c_int32, C.POINTER(VocosConfig), C.POINTER(Tensor), C.c_int32, C.POINTER(_P)]),
     "b2a_vocos_output_length": (C.c_int64, [_P, C.c_int32]),
     "b2a_vocos_stream": (C.c_void_p, [_P]),
@@ -232,6 +251,8 @@ SIGNATURES = {
     "b2a_vocos_decode_dev": (C.c_int32, [_P, _P, C.c_int32, C.c_int32, _P, _P]),
     "b2a_vocos_decode_cond": (C.c_int32, [_P, _P, _P, C.c_int32, C.c_int32, _P]),
     "b2a_vocos_destroy": (None, [_P]),
+    "b2a_vocos_decode_upsampled_dev": (C.c_int32, [_P, _P, C.c_int64, _P, C.c_int32, C.c_int32, C.c_int32, _P, _P]),
+    "b2a_vocos_upsampled_length": (C.c_int64, [_P, C.c_int32, C.c_int32]),
     "b2a_speech_tokenizer_create": (C.c_int32, [C.c_int32, C.POINTER(SpeechTokenizerConfig), C.POINTER(Tensor), C.c_int32, C.POINTER(_P)]),
     "b2a_speech_tokenizer_total_upsample": (C.c_int32, [_P]),
     "b2a_speech_tokenizer_stream": (C.c_void_p, [_P]),
@@ -301,6 +322,7 @@ SIGNATURES = {
     "b2a_weights_sanitize_whisper": (C.c_int32, [_P, C.POINTER(C.c_int32)]),
     "b2a_weights_sanitize_llama": (C.c_int32, [_P, C.c_int32, C.c_int32, C.c_int32]),
     "b2a_weights_sanitize_llama_config": (C.c_int32, [_P, C.c_char_p]),
+    "b2a_weights_sanitize_soprano_config": (C.c_int32, [_P, C.c_char_p]),
     "b2a_weights_dequantize": (C.c_int32, [_P, C.c_int32, C.c_int32]),
     "b2a_weights_free": (None, [_P]),
     "b2a_tts_config_from_json": (C.c_int32, [C.c_char_p, C.c_int32, C.c_int32, C.POINTER(LlamaConfig), C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),

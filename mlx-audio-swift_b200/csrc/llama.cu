@@ -74,16 +74,28 @@ __global__ void ext_embed_kernel(const float* __restrict__ src, float* __restric
     }
 }
 
-// fused-norm step, row N1 only: the fp32 normalised hidden state  out[b, :] = x[b, :] * rstd[b] * w  from the partial sums of squares
+// fused-norm step: the fp32 normalised hidden state  out[b, :] = x[b, :] * rstd[b] * w  from the partial sums of squares.
+// slot == null (row N1): out is [8, H].  slot != null (Soprano's capture, out [B, slots, H]): row b writes slot k = slot[b] (its n_gen:
+// the state of generated token k, or of the last prompt position for k = 0) only while n_cap[b] == k, then n_cap[b] = k + 1.  A stop
+// token leaves n_gen unchanged, so the step that feeds it finds the slot taken and writes nothing; read on the device, the graph replays.
 __global__ void finalize_norm_kernel(const float* __restrict__ x, const float* __restrict__ w, const float* __restrict__ ss, int parts,
-                                     float* __restrict__ out, int H, float eps) {
+                                     float* __restrict__ out, int H, float eps, const int* __restrict__ slot, int* n_cap, int slots) {
     const int b = blockIdx.x;
     pdl_trigger();
     pdl_wait();
+    long long o = (long long)b * H;
+    if (slot) {
+        const int k = slot[b];
+        const bool take = n_cap[b] == k && k < slots;
+        __syncthreads();                       // every thread has read n_cap[b] before it moves on
+        if (!take) return;
+        if (threadIdx.x == 0) n_cap[b] = k + 1;
+        o = ((long long)b * slots + k) * H;
+    }
     float t = 0.f;
     for (int p = 0; p < parts; ++p) t += ss[p * 8 + b];
     const float r = rsqrtf(t / (float)H + eps);
-    for (int i = threadIdx.x; i < H; i += blockDim.x) out[(long long)b * H + i] = x[(long long)b * H + i] * r * w[i];
+    for (int i = threadIdx.x; i < H; i += blockDim.x) out[o + i] = x[(long long)b * H + i] * r * w[i];
 }
 
 constexpr int LO_ROW = 8;   // activation matrices are [16, K] bf16: row b = hi(x_b), row 8 + b = lo(x_b) = bf16(x_b - hi)
@@ -599,6 +611,7 @@ struct SampleArgs {
     unsigned long long seed;
     int mask_eos;         // bench only: the stop token can never be sampled
     int stop_token;       // ends a row and is not recorded (TokenLayout::end_of_speech)
+    int soprano;          // Soprano's own penalty and top-p (Soprano.swift:836-901, :996-1059), see sample_kernel
 };
 
 // Logits processors + sampler (deterministic for a given seed, no atomics):
@@ -670,8 +683,25 @@ sample_kernel(SampleArgs a) {
     };
 
     if (a.forced == nullptr) {
-        // RepetitionContext.process: once per unique token among the last R; every CTA handles the tokens of its own range
-        if (a.rep_penalty != 1.0f && t < nrec) {
+        if (a.soprano) {
+            // applyRepetitionPenalty (Soprano.swift:888-901) over the last R GENERATED tokens (the prompt never enters the ring: the
+            // caller starts it empty, so nothing is penalised before the first token, Soprano.swift:843).  It runs once per
+            // OCCURRENCE, in sequence: the first occurrence's thread applies l > 0 ? l / p : l * p as many times as the token occurs.
+            // It runs at temperature 0 too, before the argmax.
+            if (a.rep_penalty != 1.0f && t < nrec) {
+                const int tok = a.recent[b * a.R + t];
+                bool first = true;
+                int k = 0;
+                for (int j = 0; j < nrec; ++j)
+                    if (a.recent[b * a.R + j] == tok) { first &= j >= t; ++k; }
+                if (first && tok >= i0 && tok < i1) {
+                    float l = lg[tok];
+                    for (int j = 0; j < k; ++j) l = l > 0.f ? l / a.rep_penalty : l * a.rep_penalty;
+                    lg[tok] = l;
+                }
+            }
+        } else if (a.rep_penalty != 1.0f && t < nrec) {
+            // RepetitionContext.process: once per unique token among the last R; every CTA handles the tokens of its own range
             const int tok = a.recent[b * a.R + t];
             bool dup = false;
             for (int j = 0; j < t; ++j) dup |= (a.recent[b * a.R + j] == tok);
@@ -706,27 +736,36 @@ sample_kernel(SampleArgs a) {
                 const float u = ((float)(z >> 40) + 0.5f) * (1.0f / 16777216.0f);      // (0, 1)
                 return l * inv_t - __logf(-__logf(u));
             };
-            // pass A: Z = sum exp((l - max) / T) and the first draw
+            // Soprano's TopPSampler (Soprano.swift:1002-1059) filters on exp(l) of the penalised logits, NOT on probabilities: token i
+            // is kept iff the ascending cumulative sum of exp(l_j) through i exceeds 1 - top_p, i.e. with g the max-shifted mass of
+            // strictly larger logits and z the shifted total, iff g < z - (1 - top_p) e^(-max).  Its masses are taken at temperature 1;
+            // the temperature divides the FILTERED logits afterwards (categorical(filtered / T)), which is the proposal below.
+            const float zs = a.soprano ? 1.0f : inv_t;
+            // pass A: Z = sum exp((l - max) / T) (Soprano: at T = 1) and the first draw
             float z = 0.f, gv = -INFINITY;
             int gi = 0x7fffffff;
             for (int i = i0 + t; i < i1; i += SM_THREADS) {
                 const float l = lg[i];
-                z += __expf((l - mx) * inv_t);
+                z += __expf((l - mx) * zs);
                 const float k = l == -INFINITY ? -INFINITY : gumbel_key(i, l, 0);
                 if (k > gv) { gv = k; gi = i; }
             }
             exchange(gv, gi, z);
             const float Z = z;
+            const float cut = a.soprano ? Z - (1.0f - a.top_p) * expf(-mx) : a.top_p * Z;
             int cand = gi;
             bool accepted = a.top_p >= 1.0f;
+            // Soprano, sum exp(l) <= 1 - top_p: no token passes and the reference would sample from an all -inf row.  The argmax is
+            // returned instead (a deliberate difference).
+            if (!accepted && a.soprano && !(cut > 0.f)) { cand = tok_final; accepted = true; }
             for (int att = 0; !accepted; ++att) {
-                // nucleus test: the mass of strictly more probable tokens must be below top_p
+                // nucleus test: the mass of strictly more probable tokens must be below top_p (Soprano: below cut)
                 const float lc = lg[cand];
                 float gm = 0.f, dv = -INFINITY;
                 int di = 0x7fffffff;
-                for (int i = i0 + t; i < i1; i += SM_THREADS) { const float l = lg[i]; if (l > lc) gm += __expf((l - mx) * inv_t); }
+                for (int i = i0 + t; i < i1; i += SM_THREADS) { const float l = lg[i]; if (l > lc) gm += __expf((l - mx) * zs); }
                 exchange(dv, di, gm);
-                if (gm < a.top_p * Z) { accepted = true; break; }
+                if (gm < cut) { accepted = true; break; }
                 if (att + 1 >= SM_MAX_ATTEMPTS) { cand = tok_final; break; }      // the argmax is always in the nucleus
                 gv = -INFINITY; gi = 0x7fffffff;
                 float ds = 0.f;
@@ -933,8 +972,17 @@ struct b2a_tts {
     // codec workspaces
     DBuf<int> d_codes[3];
     DBuf<float> d_wave;
+    // Soprano (b2a_soprano_create): the handle owns a Vocos decoder and the step captures every row's final-norm hidden state into
+    // hidden [B, hidden_slots = max_tokens + 1, H] (finalize_norm_kernel); n_cap[b] counts the states row b holds
+    b2a_vocos* vocos = nullptr;
+    int upscale = 0, token_size = 0;
+    DBuf<float> hidden;
+    DBuf<int> n_cap, d_rows;
+    int hidden_slots = 0, hidden_rows = 0;
+    const float* g_hidden = nullptr;   // the capture buffer the step graph was captured with
 
     ~b2a_tts() {
+        if (vocos) b2a_vocos_destroy(vocos);
         if (g_step) cudaGraphExecDestroy(g_step);
         if (g_prefill) cudaGraphExecDestroy(g_prefill);
         for (auto& e : ev_poll) if (e) cudaEventDestroy(e);
@@ -1253,18 +1301,29 @@ struct b2a_tts {
                                      cudaMemcpyDeviceToDevice, s));
     }
 
-    // x, xn (un-normalised) and ss_b are final after run_layers: only row N1 needs the fp32 normalised hidden state
-    void run_final_norm(int B, cudaStream_t s) {
+    // x, xn (un-normalised) and ss_b are final after run_layers: only row N1 and Soprano's capture need the fp32 normalised hidden state
+    void run_final_norm(int B, cudaStream_t s, bool capture) {
         if (normed_out)
             launch_pdl(finalize_norm_kernel, dim3(B), dim3(256), 0, s, (const float*)x.p, (const float*)final_ln.p, (const float*)ss_b.p, fused_parts,
-                       normed_out, cfg.hidden_size, cfg.rms_norm_eps);
+                       normed_out, cfg.hidden_size, cfg.rms_norm_eps, (const int*)nullptr, (int*)nullptr, 0);
+        if (capture)
+            launch_pdl(finalize_norm_kernel, dim3(B), dim3(256), 0, s, (const float*)x.p, (const float*)final_ln.p, (const float*)ss_b.p, fused_parts,
+                       hidden.p, cfg.hidden_size, cfg.rms_norm_eps, (const int*)n_gen.p, n_cap.p, hidden_slots);
     }
-    void run_lm_head(int B, cudaStream_t s) {
-        run_final_norm(B, s);
+    // capture: Soprano's generate (hidden states into `hidden`); forward_logits never captures
+    void run_lm_head(int B, cudaStream_t s, bool capture = false) {
+        run_final_norm(B, s, capture);
         tc_gemm(tm_lm, tmx_xn, OP_LM, logits.p, nullptr, B, cfg.vocab_size, cfg.hidden_size, s, ss_b.p);
     }
-    // after prefill_batched's gather_last (x, y hold the last position un-added): the stand-alone norm + plain GEMM
+    // after prefill_batched's gather_last (x, y hold the last position un-added): the stand-alone norm + plain GEMM.  Soprano runs the
+    // decode step's tail instead (raw norm, then capture + GEMM with rstd), so slot 0 is computed as every later slot is.
     void run_lm_head_after_prefill(int B, cudaStream_t s) {
+        if (vocos) {
+            launch_pdl(add_rmsnorm_kernel, dim3(B), dim3(RN_THREADS), 0, s, x.p, y.p, final_ln.p, xn.p, cfg.hidden_size, cfg.rms_norm_eps,
+                       LO_ROW, ss_b.p, fused_parts);
+            run_lm_head(B, s, true);
+            return;
+        }
         launch_pdl(add_rmsnorm_kernel, dim3(B), dim3(RN_THREADS), 0, s, x.p, y.p, final_ln.p, xn.p, cfg.hidden_size, cfg.rms_norm_eps,
                    LO_ROW, (float*)nullptr, 0);
         tc_gemm(tm_lm, tmx_xn, OP_LM, logits.p, nullptr, B, cfg.vocab_size, cfg.hidden_size, s);
@@ -1387,16 +1446,16 @@ struct b2a_tts {
     static bool same_args(const SampleArgs& a, const SampleArgs& b) {
         return a.V == b.V && a.R == b.R && a.max_tokens == b.max_tokens && a.temperature == b.temperature &&
                a.top_p == b.top_p && a.rep_penalty == b.rep_penalty && a.seed == b.seed && a.mask_eos == b.mask_eos &&
-               a.stop_token == b.stop_token && a.out_tokens == b.out_tokens;
+               a.stop_token == b.stop_token && a.out_tokens == b.out_tokens && a.soprano == b.soprano;
     }
 
     void capture(int B, const SampleArgs& sa, int L) {
-        if (g_step && g_nb == B && same_args(sa, g_args) && g_L == L) return;
+        if (g_step && g_nb == B && same_args(sa, g_args) && g_L == L && g_hidden == hidden.p) return;
         drop_graphs();
         cudaGraph_t g;
         B2A_CUDA(cudaStreamBeginCapture(stream, cudaStreamCaptureModeThreadLocal));
         run_layers(B, stream);
-        run_lm_head(B, stream);
+        run_lm_head(B, stream, sa.soprano != 0);
         launch_pdl(sample_kernel, dim3(B * SM_CLUSTER), dim3(SM_THREADS), 0, stream, sa);
         B2A_CUDA(cudaStreamEndCapture(stream, &g));
         B2A_CUDA(cudaGraphInstantiate(&g_step, g, 0));
@@ -1407,8 +1466,8 @@ struct b2a_tts {
         B2A_CUDA(cudaStreamEndCapture(stream, &g));
         B2A_CUDA(cudaGraphInstantiate(&g_prefill, g, 0));
         cudaGraphDestroy(g);
-        g_nb = B; g_args = sa; g_L = L;
-        launches_step = launches_layers() + 1 + 1;
+        g_nb = B; g_args = sa; g_L = L; g_hidden = hidden.p;
+        launches_step = launches_layers() + 1 + 1 + (sa.soprano ? 1 : 0);
         launches_prefill = launches_layers() + 1;
     }
     int g_L = 0, launches_step = 0, launches_prefill = 0;
@@ -1460,6 +1519,46 @@ static double now_s() {
     return std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count();
 }
 
+// Samples of a Soprano waveform of n hidden states: the decoder's output (upscale (n - 1) hop, or the untrimmed n_fft of a one-frame
+// OLA for n = 1, SopranoDecoder.swift:191-196), cut to its last (n - 1) token_size samples when that is positive (Soprano.swift:664-671).
+// *offset receives the first kept sample.
+static int64_t soprano_wave_len(const b2a_tts* h, int n, int64_t* offset) {
+    const int64_t total = b2a_vocos_upsampled_length(h->vocos, n, h->upscale);
+    const int64_t cut = (int64_t)(n - 1) * h->token_size;
+    const int64_t keep = cut > 0 ? std::min(cut, total) : total;
+    if (offset) *offset = total - keep;
+    return keep;
+}
+
+// SopranoDecoder on rows of d_states (row r at d_states + r * row_stride, n[r] states of H floats): rows with equal counts share one
+// Vocos pass, so a batch decodes exactly as its rows would one by one (no row is padded: the ConvNeXt convolutions would see it).
+// wave_out [B, wave_cap] receives each row's cut waveform, wave_len[B] its length.
+static void soprano_decode(b2a_tts* h, const float* d_states, int64_t row_stride, const std::vector<int>& n, float* wave_out,
+                           bool wave_on_device, int64_t wave_cap, int64_t* wave_len, cudaStream_t s) {
+    const int B = (int)n.size();
+    std::vector<bool> used(B, false);
+    for (int i = 0; i < B; ++i) {
+        if (used[i]) continue;
+        std::vector<int> grp;
+        for (int j = i; j < B; ++j)
+            if (!used[j] && n[j] == n[i]) { grp.push_back(j); used[j] = true; }
+        int64_t off = 0;
+        const int64_t keep = soprano_wave_len(h, n[i], &off), total = off + keep;
+        B2A_CHECK(keep <= wave_cap, B2A_ERR_INVALID_INPUT, "soprano: wave buffer too small");
+        h->d_rows.upload(grp.data(), grp.size(), s);
+        h->d_wave.alloc((size_t)grp.size() * total);
+        const int32_t st = b2a_vocos_decode_upsampled_dev(h->vocos, d_states, row_stride, h->d_rows.p, (int32_t)grp.size(), n[i], h->upscale,
+                                                          h->d_wave.p, s);
+        B2A_CHECK(st == B2A_OK, B2A_ERR_AUDIO_DECODING_FAILED, std::string("Soprano decode failed: ") + b2a_last_error());
+        for (size_t k = 0; k < grp.size(); ++k) {
+            B2A_CUDA(cudaMemcpyAsync(wave_out + (size_t)grp[k] * wave_cap, h->d_wave.p + k * total + off, keep * sizeof(float),
+                                     wave_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, s));
+            if (wave_len) wave_len[grp[k]] = keep;
+        }
+        B2A_CUDA(cudaStreamSynchronize(s));   // grp (the uploaded row list) and d_wave are reused by the next group
+    }
+}
+
 // shared body of b2a_tts_generate / _dev.  ids_on_device: input ids pointer is a device pointer.
 // chunked audio emission during generation (row N2): every `frames_per_chunk` new 7-token frames of a row are decoded with
 // `left_context` already-emitted frames in front (the codec is convolutional: the context absorbs the left edge) and handed to
@@ -1482,7 +1581,11 @@ static void tts_generate_impl(b2a_tts* h, const int32_t* input_ids, bool ids_on_
     B2A_CHECK(gp->repetition_context_size >= 0 && gp->repetition_context_size <= 64, B2A_ERR_INVALID_INPUT,
               "tts generate: repetition_context_size must be in 0..64");
     B2A_CHECK(gp->temperature >= 0.f && gp->top_p > 0.f, B2A_ERR_INVALID_INPUT, "tts generate: bad sampling parameters");
-    if (wave_out) B2A_CHECK(h->snac, B2A_ERR_MODEL_NOT_INITIALIZED, "SNAC model not loaded");   // LlamaTTS.swift:672-674
+    const bool soprano = h->vocos != nullptr;
+    // Soprano feeds its last generated token forward once more (its hidden state is audio): one more cache position
+    if (soprano) B2A_CHECK(L + gp->max_tokens + 1 <= h->cfg.max_context, B2A_ERR_INVALID_INPUT, "soprano generate: prompt + max_tokens + 1 exceeds max_context");
+    if (soprano) B2A_CHECK(ss.frames_per_chunk == 0, B2A_ERR_INVALID_INPUT, "soprano generate: audio is decoded once per call, not in chunks");
+    if (wave_out && !soprano) B2A_CHECK(h->snac, B2A_ERR_MODEL_NOT_INITIALIZED, "SNAC model not loaded");   // LlamaTTS.swift:672-674
     B2A_CUDA(cudaSetDevice(h->device));
     cudaStream_t s = h->stream;
     h->cancel.store(0);
@@ -1501,13 +1604,21 @@ static void tts_generate_impl(b2a_tts* h, const int32_t* input_ids, bool ids_on_
     sa.max_tokens = MT; sa.temperature = gp->temperature; sa.top_p = gp->top_p;
     sa.rep_penalty = gp->repetition_context_size > 0 ? gp->repetition_penalty : 1.0f;
     sa.seed = gp->seed; sa.mask_eos = h->bench_mask_eos; sa.stop_token = h->tok.end_of_speech;
+    sa.soprano = soprano ? 1 : 0;
     if (sa.R == 0) { sa.R = 1; }
+    if (soprano) {
+        h->hidden_slots = MT + 1; h->hidden_rows = B;
+        h->hidden.alloc((size_t)B * h->hidden_slots * h->cfg.hidden_size);
+        h->n_cap.alloc(8);
+    }
     h->capture(B, sa, L);
 
     const double t0 = now_s();
-    init_rows_kernel<<<1, 32, 0, s>>>(h->ids.p, L, B, gp->repetition_context_size > 0 ? R : 0, h->tokens.p, h->pos.p, h->recent.p,
+    // Soprano's penalty sees generated tokens only (Soprano.swift:831,868): its ring starts empty
+    init_rows_kernel<<<1, 32, 0, s>>>(h->ids.p, L, B, gp->repetition_context_size > 0 && !soprano ? R : 0, h->tokens.p, h->pos.p, h->recent.p,
                                       h->recent_n.p, h->n_gen.p, h->done.p, h->n_active.p, 0);
     count_launch();
+    if (soprano) B2A_CUDA(cudaMemsetAsync(h->n_cap.p, 0, 8 * sizeof(int), s));
     // prefill.  Batched: every prompt token through each layer at once (wgmma GEMMs, 64 tokens per tile), then
     // lm head + sampler on the last position.  Fallback (B2A_PREFILL=step, q/k norm): replay the decode
     // step per position -- positions 0..L-2 need no logits, position L-1 runs the full step.
@@ -1619,6 +1730,12 @@ static void tts_generate_impl(b2a_tts* h, const int32_t* input_ids, bool ids_on_
         if (h->cancel.load()) { cancelled = true; break; }
         if (h->h_flag.p[0] <= 0) break;
     }
+    // Soprano: a row that reached max_tokens has its last token fed forward too (the reference's loop forwards every token it keeps,
+    // Soprano.swift:836-879); one more step captures that state.  Its sample is never recorded: every row is done.
+    if (soprano && steps >= MT && !cancelled) {
+        B2A_CUDA(cudaGraphLaunch(h->g_step, s));
+        count_launch(h->launches_step);
+    }
     if (pipelined) { B2A_CUDA(cudaStreamSynchronize(s)); if (h->cancel.load()) cancelled = true; }
     if (streaming && !cancelled) emit_audio(true);
     const double t2 = now_s();
@@ -1638,7 +1755,13 @@ static void tts_generate_impl(b2a_tts* h, const int32_t* input_ids, bool ids_on_
     }
 
     double codec_t = 0;
-    if (wave_out) {
+    if (wave_out && soprano) {
+        const double c0 = now_s();
+        std::vector<int> nc(B);
+        B2A_CUDA(cudaMemcpy(nc.data(), h->n_cap.p, B * sizeof(int), cudaMemcpyDeviceToHost));
+        soprano_decode(h, h->hidden.p, (int64_t)h->hidden_slots * h->cfg.hidden_size, nc, wave_out, wave_on_device, wave_cap, wave_len, s);
+        codec_t = now_s() - c0;
+    } else if (wave_out) {
         const double c0 = now_s();
         // per row: generatedTokens = prompt + generated (LlamaTTS.swift:705-707,738) -> parseOutput -> frames
         const TokenLayout& tl = h->tok;
@@ -2090,6 +2213,106 @@ int32_t b2a_qwen3_lm_parse_output(const int32_t* tokens, int32_t batch, int32_t 
     });
 }
 
+// ------------------------------------------------------------------------------------------------ Soprano (SopranoModel, Soprano.swift:184-977)
+static b2a_llama_config soprano_stack_cfg(const b2a_soprano_config& c) {
+    b2a_qwen3_lm_config q{};
+    q.hidden_size = c.hidden_size; q.num_hidden_layers = c.num_hidden_layers; q.intermediate_size = c.intermediate_size;
+    q.num_attention_heads = c.num_attention_heads; q.num_key_value_heads = c.num_key_value_heads; q.head_dim = c.head_dim;
+    q.vocab_size = c.vocab_size; q.rms_norm_eps = c.rms_norm_eps; q.rope_theta = c.rope_theta; q.rope_linear_factor = 1.f;
+    q.tie_word_embeddings = c.tie_word_embeddings; q.max_batch = c.max_batch; q.max_context = c.max_context;
+    return qwen3_lm_stack_cfg(q);
+}
+
+// the Soprano stack is Qwen3's (Soprano.swift:24-180): q/k norm, rotate-half RoPE with base rope_theta, no scaling
+static StackSpec soprano_spec() {
+    StackSpec s;
+    s.qk_norm = true;
+    s.linear_rope = 1.f;
+    return s;
+}
+
+// the handle's Vocos: decoder.decoder.* -> backbone.*, decoder.head.* -> head.* (the keys b2a_vocos_create reads), Vocos's
+// LayerNorm backbone at the decoder geometry of the config
+static void soprano_attach_decoder(b2a_tts* h, int device, const b2a_soprano_config& c, const b2a_tensor* tensors, int n) {
+    B2A_CHECK(c.upscale >= 1 && c.token_size >= 0, B2A_ERR_INVALID_INPUT, "soprano: upscale must be >= 1 and token_size >= 0");
+    std::vector<std::string> names;
+    std::vector<b2a_tensor> dec;
+    names.reserve(n);
+    for (int i = 0; i < n; ++i) {
+        const std::string k = tensors[i].name ? tensors[i].name : "";
+        if (k.rfind("decoder.decoder.", 0) == 0) names.push_back("backbone." + k.substr(16));
+        else if (k.rfind("decoder.head.", 0) == 0) names.push_back("head." + k.substr(13));
+        else continue;
+        dec.push_back(tensors[i]);
+    }
+    for (size_t i = 0; i < dec.size(); ++i) dec[i].name = names[i].c_str();
+    B2A_CHECK(!dec.empty(), B2A_ERR_MODEL_NOT_INITIALIZED, "soprano: no decoder.decoder.* / decoder.head.* weights");
+    b2a_vocos_config v{};
+    v.input_channels = c.hidden_size; v.dim = c.decoder_dim; v.intermediate_dim = c.decoder_intermediate_dim; v.num_layers = c.decoder_num_layers;
+    v.n_fft = c.n_fft; v.hop_length = c.hop_length; v.input_kernel_size = c.input_kernel; v.dw_kernel_size = c.dw_kernel;
+    v.adanorm_num_embeddings = 0;
+    const int32_t st = b2a_vocos_create(device, &v, dec.data(), (int32_t)dec.size(), &h->vocos);
+    if (st != B2A_OK) throw Error(st, b2a_last_error());
+    h->upscale = c.upscale; h->token_size = c.token_size;
+    h->tok = TokenLayout{-1, -1, -1, -1, -1, -1, c.stop_token_id, -1, 0, false, 0};
+}
+
+int32_t b2a_soprano_create(int32_t device, const b2a_soprano_config* cfg, const b2a_tensor* tensors, int32_t n, b2a_tts** out) {
+    return guarded([&] {
+        B2A_CHECK(out, B2A_ERR_INVALID_INPUT, "b2a_soprano_create: null out");
+        *out = nullptr;
+        B2A_CHECK(cfg && tensors && n > 0, B2A_ERR_MODEL_NOT_INITIALIZED, "b2a_soprano_create: missing config or weights");
+        TensorTable tt(tensors, n);
+        std::unique_ptr<b2a_tts> h(new b2a_tts(device, soprano_stack_cfg(*cfg), tt, nullptr, soprano_spec()));
+        soprano_attach_decoder(h.get(), device, *cfg, tensors, n);
+        *out = h.release();
+    });
+}
+
+int32_t b2a_soprano_create_random(int32_t device, const b2a_soprano_config* cfg, float std, uint64_t seed, const b2a_tensor* decoder_tensors,
+                                  int32_t n_decoder_tensors, b2a_tts** out) {
+    return guarded([&] {
+        B2A_CHECK(out, B2A_ERR_INVALID_INPUT, "b2a_soprano_create_random: null out");
+        *out = nullptr;
+        B2A_CHECK(cfg && std > 0.f && decoder_tensors && n_decoder_tensors > 0, B2A_ERR_MODEL_NOT_INITIALIZED,
+                  "b2a_soprano_create_random: missing config or decoder weights");
+        std::unique_ptr<b2a_tts> h(new b2a_tts(device, soprano_stack_cfg(*cfg), std, seed, nullptr, soprano_spec()));
+        soprano_attach_decoder(h.get(), device, *cfg, decoder_tensors, n_decoder_tensors);
+        *out = h.release();
+    });
+}
+
+int64_t b2a_soprano_wave_length(const b2a_tts* h, int32_t n) {
+    return h && h->vocos && n >= 1 ? soprano_wave_len(h, n, nullptr) : 0;
+}
+
+int32_t b2a_soprano_decode_hidden(b2a_tts* h, const float* hidden, int32_t B, int32_t n, float* wave_out, int64_t wave_cap, int64_t* wave_len) {
+    return guarded([&] {
+        B2A_CHECK(h && hidden && wave_out, B2A_ERR_INVALID_INPUT, "b2a_soprano_decode_hidden: null argument");
+        B2A_CHECK(h->vocos, B2A_ERR_INVALID_INPUT, "b2a_soprano_decode_hidden: not a Soprano handle");
+        B2A_CHECK(B >= 1 && n >= 1, B2A_ERR_INVALID_INPUT, "b2a_soprano_decode_hidden: batch and state count must be positive");
+        B2A_CUDA(cudaSetDevice(h->device));
+        cudaStream_t s = h->stream;
+        const size_t row = (size_t)n * h->cfg.hidden_size;
+        DBuf<float> d;
+        d.upload(hidden, (size_t)B * row, s);
+        soprano_decode(h, d.p, (int64_t)row, std::vector<int>(B, n), wave_out, false, wave_cap, wave_len, s);
+    });
+}
+
+int32_t b2a_soprano_hidden_states(b2a_tts* h, int32_t B, float* out, int32_t* n_states) {
+    return guarded([&] {
+        B2A_CHECK(h && h->vocos && n_states && B >= 1 && B <= 8, B2A_ERR_INVALID_INPUT, "b2a_soprano_hidden_states: bad argument");
+        B2A_CHECK(h->hidden.p && h->n_cap.p && B <= h->hidden_rows, B2A_ERR_INVALID_INPUT,
+                  "b2a_soprano_hidden_states: batch exceeds the last generate call's");
+        B2A_CUDA(cudaSetDevice(h->device));
+        B2A_CUDA(cudaStreamSynchronize(h->stream));
+        B2A_CUDA(cudaMemcpy(n_states, h->n_cap.p, B * sizeof(int), cudaMemcpyDeviceToHost));
+        if (out)
+            B2A_CUDA(cudaMemcpy(out, h->hidden.p, (size_t)B * h->hidden_slots * h->cfg.hidden_size * sizeof(float), cudaMemcpyDeviceToHost));
+    });
+}
+
 void b2a_tts_destroy(b2a_tts* h) { delete h; }
 
 }  // extern "C"
@@ -2449,7 +2672,7 @@ struct b2a_qwen3_talker {
                 launch_pdl(q3_gather_kernel<bf16>, dim3(B), dim3(256), 0, s, (const bf16*)(k == 0 ? codec_emb.p : cp_emb[k - 1].p), id_rows,
                            (const int*)codes.p, G(), k, px.p, H(), pred->pos.p, k + 1);
             pred->run_layers(B, s);
-            pred->run_final_norm(B, s);
+            pred->run_final_norm(B, s, false);
             pred->run_head(tm_cp_head[k], cfg.cp_vocab_size, pred->logits.p, B, s, cp_head_rows);
             q3s::Args a = sampler_args(p, false, k + 1);
             a.tokens = codes.p + (k + 1); a.tokens_stride = G();

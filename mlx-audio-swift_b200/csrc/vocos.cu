@@ -35,6 +35,37 @@ __global__ void im2colk_kernel(const float* __restrict__ in, bf16* __restrict__ 
     }
 }
 
+// SopranoDecoder's interpolate1d(align_corners) x upscale (SopranoDecoder.swift:22-80, :263-275) fused into the embed conv's im2col:
+// u[t] = y[lo] (1 - f) + y[hi] f, x_t = t * ((n-1)/(T-1)) in fp32 in that order, lo = floor(x_t), hi = min(lo + 1, n - 1), f = x_t - lo
+// (u = y when T == n), over the n states of row rows[b] of src (row stride row_stride floats, C channels each); out row (b, t) =
+// [u[t-k/2] | ... | u[t+k/2]] as hi/lo, zero padded.  The T upsampled frames never exist in memory.  Explicit _rn operations: no
+// contraction into fma, the reference rounds every product.
+__global__ void upsample_im2colk_kernel(const float* __restrict__ src, long long row_stride, const int* __restrict__ rows, int n, int T,
+                                        bf16* __restrict__ out, int C, int k, int Kp) {
+    const long long tok = blockIdx.x;
+    const int b = (int)(tok / T), t = (int)(tok - (long long)b * T);
+    const float* y = src + (long long)(rows ? rows[b] : b) * row_stride;
+    const float scale = T > 1 ? (float)(n - 1) / (float)(T - 1) : 0.f;
+    for (int i = threadIdx.x; i < Kp; i += blockDim.x) {
+        float v = 0.f;
+        if (i < k * C) {
+            const int kk = i / C, c = i - kk * C;
+            const int ti = t + kk - k / 2;
+            if (ti >= 0 && ti < T) {
+                if (T == n) {
+                    v = y[(long long)ti * C + c];
+                } else {
+                    const float x = __fmul_rn((float)ti, scale);
+                    const int lo = (int)floorf(x), hi = min(lo + 1, n - 1);
+                    const float f = __fsub_rn(x, (float)lo);
+                    v = __fadd_rn(__fmul_rn(y[(long long)lo * C + c], __fsub_rn(1.0f, f)), __fmul_rn(y[(long long)hi * C + c], f));
+                }
+            }
+        }
+        tc::store_hilo(out, Kp, tok, i, v, cg::HALF);
+    }
+}
+
 constexpr int DL_MAXV = 4;    // channels <= 1024 (dw_layernorm_kernel, layernorm.cuh)
 
 // AdaLayerNorm's conditioning (Vocos.swift:31-33): for every norm n and utterance b,  gain[n, b, :] = Ws_n cond_b + bs_n  and
@@ -66,13 +97,14 @@ __global__ void spec_kernel(const float* __restrict__ h, bf16* __restrict__ out,
     }
 }
 
-// overlap-add as a gather + window-sum normalisation + centre trim (Vocos.swift:123-160)
+// overlap-add as a gather + window-sum normalisation + centre trim (Vocos.swift:123-160): output sample tp is OLA sample tp + trim
+// (trim n_fft / 2; 0 for Soprano's untrimmed one-frame case)
 __global__ void ola_kernel(const float* __restrict__ frames /*[B*L, n_fft] already windowed*/, const float* __restrict__ win,
-                           float* __restrict__ wave, int L, int n_fft, int hop, int out_len) {
+                           float* __restrict__ wave, int L, int n_fft, int hop, int out_len, int trim) {
     const int b = blockIdx.y;
     const int tp = blockIdx.x * blockDim.x + threadIdx.x;     // trimmed index
     if (tp >= out_len) return;
-    const int t = tp + n_fft / 2;
+    const int t = tp + trim;
     int i1 = t / hop;
     if (i1 > L - 1) i1 = L - 1;
     float acc = 0.f, ws = 0.f;
@@ -182,8 +214,11 @@ struct b2a_vocos {
     // d_feats [B, L, input_channels] fp32 (device) -> d_wave [B, (L-1)*hop]
     // d_cond [B, adanorm_num_embeddings] fp32 (device): the conditioning rows AdaLayerNorm's Linears see (one-hot bandwidth ids in the
     // reference's use); required iff the model was built with adanorm_num_embeddings > 0 (the reference fatalErrors without it)
-    void decode_dev(const float* d_feats, int B, int L, float* d_wave, cudaStream_t s, const float* d_cond = nullptr) {
-        B2A_CHECK(B >= 1 && L >= 2, B2A_ERR_INVALID_INPUT, "vocos decode: need at least 2 frames");
+    // up != null (Soprano): the features are up->n hidden states per row, upsampled to L = upscale (n - 1) + 1 frames inside the embed
+    // conv's operand kernel (d_feats unused); L = 1 is allowed there and gives the untrimmed n_fft samples of the one-frame OLA
+    struct Upsample { const float* src; long long row_stride; const int* rows; int n; };
+    void decode_dev(const float* d_feats, int B, int L, float* d_wave, cudaStream_t s, const float* d_cond = nullptr, const Upsample* up = nullptr) {
+        B2A_CHECK(B >= 1 && (L >= 2 || (up && L == 1)), B2A_ERR_INVALID_INPUT, "vocos decode: need at least 2 frames");
         B2A_CUDA(cudaSetDevice(device));
         const int D = cfg.dim, I = cfg.intermediate_dim, N = cfg.n_fft;
         const int E = cfg.adanorm_num_embeddings, norms = 1 + cfg.num_layers;
@@ -206,7 +241,11 @@ struct b2a_vocos {
         xa.alloc((size_t)2 * Tp * kmax); xb.alloc((size_t)2 * Tp * kmax);
         h.alloc((size_t)T * D); spec.alloc((size_t)T * (N + 2)); frames.alloc((size_t)T * N);
         // embed conv (im2col GEMM) -> LayerNorm -> residual stream h
-        im2colk_kernel<<<(unsigned)T, 256, 0, s>>>(d_feats, xa.p, L, cfg.input_channels, cfg.input_kernel_size, kp_embed);
+        if (up)
+            upsample_im2colk_kernel<<<(unsigned)T, 256, 0, s>>>(up->src, up->row_stride, up->rows, up->n, L, xa.p, cfg.input_channels,
+                                                                 cfg.input_kernel_size, kp_embed);
+        else
+            im2colk_kernel<<<(unsigned)T, 256, 0, s>>>(d_feats, xa.p, L, cfg.input_channels, cfg.input_kernel_size, kp_embed);
         count_launch();
         {
             cg::Args a{}; a.N = (int)T; a.epi = cg::E_STORE_F32; a.bias = embed_b.p; a.x = spec.p; a.ldx = D;      // spec doubles as scratch [T, D]
@@ -237,8 +276,8 @@ struct b2a_vocos {
             cg::Args a{}; a.N = (int)T; a.epi = cg::E_STORE_F32; a.x = frames.p; a.ldx = N;
             cg::launch(idft, xb.p, 2 * Tp, a, num_sms, s);
         }
-        const int ol = (int)out_len(L);
-        ola_kernel<<<dim3(cdiv(ol, 256), B), 256, 0, s>>>(frames.p, win.p, d_wave, L, N, cfg.hop_length, ol);
+        const int ol = L == 1 ? N : (int)out_len(L);
+        ola_kernel<<<dim3(cdiv(ol, 256), B), 256, 0, s>>>(frames.p, win.p, d_wave, L, N, cfg.hop_length, ol, L == 1 ? 0 : N / 2);
         count_launch();
         B2A_CUDA(cudaGetLastError());
     }
@@ -295,6 +334,22 @@ int32_t b2a_vocos_decode_cond(b2a_vocos* h, const float* feats, const float* con
         h->decode_dev(h->feats.p, B, L, h->wave.p, s, (cond && E > 0) ? h->cond.p : (cond ? cond : nullptr));
         B2A_CUDA(cudaMemcpyAsync(wave, h->wave.p, nout * sizeof(float), cudaMemcpyDeviceToHost, s));
         B2A_CUDA(cudaStreamSynchronize(s));
+    });
+}
+
+int64_t b2a_vocos_upsampled_length(const b2a_vocos* h, int32_t n, int32_t upscale) {
+    if (!h || n < 1 || upscale < 1) return 0;
+    return n == 1 ? h->cfg.n_fft : h->out_len(upscale * (n - 1) + 1);
+}
+
+int32_t b2a_vocos_decode_upsampled_dev(b2a_vocos* h, const float* d_states, int64_t row_stride, const int32_t* d_rows, int32_t B, int32_t n,
+                                       int32_t upscale, float* d_wave, void* stream) {
+    return guarded([&] {
+        B2A_CHECK(h && d_states && d_wave, B2A_ERR_INVALID_INPUT, "b2a_vocos_decode_upsampled_dev: null argument");
+        B2A_CHECK(n >= 1 && upscale >= 1 && row_stride >= (int64_t)n * h->cfg.input_channels, B2A_ERR_INVALID_INPUT,
+                  "b2a_vocos_decode_upsampled_dev: bad state count, upscale or row stride");
+        const b2a_vocos::Upsample up{d_states, (long long)row_stride, d_rows, n};
+        h->decode_dev(nullptr, B, upscale * (n - 1) + 1, d_wave, stream ? (cudaStream_t)stream : h->stream, nullptr, &up);
     });
 }
 

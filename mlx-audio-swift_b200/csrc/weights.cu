@@ -21,6 +21,7 @@
 
 #include <algorithm>
 #include <cmath>
+#include <cctype>
 #include <memory>
 
 namespace b2a {
@@ -466,6 +467,31 @@ struct b2a_weights {
         }
     }
 
+    // ---- Soprano: SopranoModel.sanitize (Soprano.swift:314-361), then the MLX de-quantisation of every layer with ".scales"
+    // (:950-963).  decoder.* keeps its keys (b2a_soprano_create hands them to the Vocos decoder, which reads them as fp32).
+    void sanitize_soprano(bool tie, const QuantSpec& spec) {
+        std::vector<WItem> out;
+        for (auto& it : items) {
+            WItem t = it;
+            std::string k = it.name;
+            if (k.rfind("model.", 0) == 0) k = k.substr(6);                    // "model.language_model.*" -> "language_model.*"
+            if (k.rfind("decoder.", 0) == 0) {
+            } else if (k.rfind("language_model.lm_head", 0) == 0) {
+                k = k.substr(15);                                               // lm_head sits on SopranoModel itself
+            } else if (k.rfind("language_model.", 0) == 0) {
+                k = "model." + k.substr(15);
+            } else if (k.rfind("lm_head", 0) != 0) {
+                k = "model." + k;                                               // bare inner keys: embed_tokens.*, layers.*, norm.*
+            }
+            if (tie && k == "lm_head.weight") continue;
+            t.name = k;
+            out.push_back(std::move(t));
+        }
+        items.clear();
+        for (auto& t : out) put(std::move(t));
+        dequantize_layers(spec);
+    }
+
     // ---- Qwen3-TTS talker: Qwen3TTSTalkerForConditionalGeneration.sanitize (Qwen3TTSTalker.swift:356-365) keeps "talker.*" and drops
     // the prefix; a quantised checkpoint (config "quantization", Qwen3TTS.swift:1156-1171: every layer that carries ".scales") is
     // expanded to bf16 -- the engine streams bf16 matrices.
@@ -834,6 +860,14 @@ int32_t b2a_weights_sanitize_llama_config(b2a_weights* w, const char* config_pat
         w->sanitize_llama(j.number("tie_word_embeddings", 1) != 0, parse_quant(j));
     });
 }
+int32_t b2a_weights_sanitize_soprano_config(b2a_weights* w, const char* config_path) {
+    return guarded([&] {
+        B2A_CHECK(w && config_path, B2A_ERR_INVALID_INPUT, "b2a_weights_sanitize_soprano_config: null argument");
+        const Json j = read_json_file(config_path);
+        B2A_CHECK(j.kind == Json::Obj, B2A_ERR_MODEL_NOT_INITIALIZED, "config.json is not an object");
+        w->sanitize_soprano(j.number("tie_word_embeddings", 0) != 0, parse_quant(j));
+    });
+}
 int32_t b2a_weights_sanitize_llama(b2a_weights* w, int32_t tie_word_embeddings, int32_t group_size, int32_t bits) {
     return guarded([&] {
         B2A_CHECK(w, B2A_ERR_INVALID_INPUT, "b2a_weights_sanitize_llama: null handle");
@@ -955,6 +989,100 @@ int32_t b2a_qwen3_lm_create_from_directory(const char* model_dir, int32_t device
         w->sanitize_llama(cfg.tie_word_embeddings != 0, parse_quant(read_json_file(dir + "/config.json")));
         const std::vector<b2a_tensor> tab = w->table();
         st = b2a_qwen3_lm_create(device, &cfg, tab.data(), (int32_t)tab.size(), snac, out);
+        if (st != B2A_OK) throw Error(st, b2a_last_error());
+    });
+}
+
+// config.json -> b2a_soprano_config (SopranoConfiguration.init(from:), SopranoConfig.swift:133-175): the seven decode()d keys are required,
+// the rest take the reference's defaults; then fromModelDirectory's decoder rule (Soprano.swift:934-941) on the repo name
+static std::string lower(std::string s) {
+    for (auto& ch : s) ch = (char)std::tolower((unsigned char)ch);
+    return s;
+}
+static std::string base_name(std::string p) {
+    while (p.size() > 1 && p.back() == '/') p.pop_back();
+    const size_t i = p.rfind('/');
+    return i == std::string::npos ? p : p.substr(i + 1);
+}
+int32_t b2a_soprano_config_from_json(const char* config_path, const char* repo_hint, int32_t max_batch, int32_t max_context,
+                                     b2a_soprano_config* cfg, int32_t* quant_group_size, int32_t* quant_bits) {
+    return guarded([&] {
+        B2A_CHECK(config_path && cfg, B2A_ERR_INVALID_INPUT, "b2a_soprano_config_from_json: null argument");
+        const Json j = read_json_file(config_path);
+        B2A_CHECK(j.kind == Json::Obj, B2A_ERR_MODEL_NOT_INITIALIZED, "config.json is not an object");
+        for (const char* k : {"hidden_size", "num_hidden_layers", "intermediate_size", "num_attention_heads", "num_key_value_heads", "head_dim",
+                              "vocab_size"})
+            B2A_CHECK(j.has(k), B2A_ERR_MODEL_NOT_INITIALIZED, std::string("config.json: missing ") + k);
+        b2a_soprano_config c{};
+        c.hidden_size = (int)j.number("hidden_size", 0); c.num_hidden_layers = (int)j.number("num_hidden_layers", 0);
+        c.intermediate_size = (int)j.number("intermediate_size", 0); c.num_attention_heads = (int)j.number("num_attention_heads", 0);
+        c.num_key_value_heads = (int)j.number("num_key_value_heads", 0); c.head_dim = (int)j.number("head_dim", 0);
+        c.vocab_size = (int)j.number("vocab_size", 0);
+        c.max_position_embeddings = (int)j.number("max_position_embeddings", 512);
+        c.rms_norm_eps = (float)j.number("rms_norm_eps", 1e-6); c.rope_theta = (float)j.number("rope_theta", 10000.0);
+        c.tie_word_embeddings = (int)j.number("tie_word_embeddings", 0);
+        c.bos_token_id = (int)j.number("bos_token_id", 1); c.eos_token_id = (int)j.number("eos_token_id", 2);
+        c.pad_token_id = (int)j.number("pad_token_id", 0); c.stop_token_id = 3;
+        c.sample_rate = (int)j.number("sample_rate", 32000);
+        c.decoder_num_layers = (int)j.number("decoder_num_layers", 8); c.decoder_dim = (int)j.number("decoder_dim", 768);
+        c.decoder_intermediate_dim = (int)j.number("decoder_intermediate_dim", 2304); c.hop_length = (int)j.number("hop_length", 512);
+        c.n_fft = (int)j.number("n_fft", 2048); c.upscale = (int)j.number("upscale", 4); c.input_kernel = (int)j.number("input_kernel", 1);
+        c.dw_kernel = (int)j.number("dw_kernel", 3); c.token_size = (int)j.number("token_size", 2048);
+        c.receptive_field = (int)j.number("receptive_field", 4);
+        std::string cp = config_path;
+        const size_t sl = cp.rfind('/');
+        const std::string repo = repo_hint ? std::string(repo_hint) : base_name(sl == std::string::npos ? std::string(".") : cp.substr(0, sl));
+        if (lower(repo).find("soprano-1.1") == std::string::npos) {      // the older decoder, whatever config.json says
+            c.decoder_dim = 512; c.decoder_intermediate_dim = 1536; c.input_kernel = 3;
+        }
+        c.max_batch = max_batch; c.max_context = max_context;
+        *cfg = c;
+        int gs = 0, bits = 0;
+        if (const Json* q = j.find("quantization"); q && q->kind == Json::Obj) { gs = (int)q->number("group_size", 64); bits = (int)q->number("bits", 4); }
+        if (quant_group_size) *quant_group_size = gs;
+        if (quant_bits) *quant_bits = bits;
+    });
+}
+
+// model.stopTokenId = tokenizer.eosTokenId ?? 3 (Soprano.swift:971-973): tokenizer_config.json's eos_token resolved through tokenizer.json's
+// added_tokens or model.vocab; 3 when either file or the token is missing
+static int soprano_stop_token(const std::string& dir) {
+    struct stat st{};
+    if (stat((dir + "/tokenizer_config.json").c_str(), &st) != 0 || stat((dir + "/tokenizer.json").c_str(), &st) != 0) return 3;
+    const Json tc = read_json_file(dir + "/tokenizer_config.json");
+    const Json* e = tc.find("eos_token");
+    std::string eos;
+    if (e && e->kind == Json::Str) eos = e->str;
+    else if (e && e->kind == Json::Obj && e->find("content") && e->find("content")->kind == Json::Str) eos = e->find("content")->str;
+    if (eos.empty()) return 3;
+    const Json tj = read_json_file(dir + "/tokenizer.json");
+    if (const Json* at = tj.find("added_tokens"); at && at->kind == Json::Arr)
+        for (const Json& t : at->arr) {
+            const Json* c = t.find("content");
+            if (c && c->kind == Json::Str && c->str == eos && t.has("id")) return (int)t.number("id", 3);
+        }
+    if (const Json* m = tj.find("model"); m && m->kind == Json::Obj)
+        if (const Json* v = m->find("vocab"); v && v->kind == Json::Obj)
+            if (const Json* id = v->find(eos); id && id->kind == Json::Num) return (int)id->num;
+    return 3;
+}
+
+int32_t b2a_soprano_create_from_directory(const char* model_dir, const char* repo_hint, int32_t device, int32_t max_batch,
+                                          int32_t max_context, b2a_tts** out) {
+    return guarded([&] {
+        B2A_CHECK(model_dir && out, B2A_ERR_INVALID_INPUT, "b2a_soprano_create_from_directory: null argument");
+        *out = nullptr;
+        b2a_soprano_config cfg{};
+        const std::string dir = model_dir;
+        const std::string repo = repo_hint ? std::string(repo_hint) : base_name(dir);
+        int32_t st = b2a_soprano_config_from_json((dir + "/config.json").c_str(), repo.c_str(), max_batch, max_context, &cfg, nullptr, nullptr);
+        if (st != B2A_OK) throw Error(st, b2a_last_error());
+        cfg.stop_token_id = soprano_stop_token(dir);
+        std::unique_ptr<b2a_weights> w(new b2a_weights());
+        w->load(dir);
+        w->sanitize_soprano(cfg.tie_word_embeddings != 0, parse_quant(read_json_file(dir + "/config.json")));
+        const std::vector<b2a_tensor> tab = w->table();
+        st = b2a_soprano_create(device, &cfg, tab.data(), (int32_t)tab.size(), out);
         if (st != B2A_OK) throw Error(st, b2a_last_error());
     });
 }

@@ -12,7 +12,13 @@ prompts of any length take the batched prefill (longer than 128 tokens with the 
 vocabulary -- an assumed geometry, as the published checkpoint's config.json is not at hand -- and the same prompts framed by its
 prepareInputIds, ending in its start-of-speech 151670.
 
-    python tools/tts_benchmark.py [--model orpheus|qwen3] [--batch 1] [--prompt 64] [--max-tokens 512] [--model-dir DIR] [--stream]
+--model soprano runs Soprano (SopranoModel, Soprano.swift) at SOPRANO_ASSUMED below: hidden 512 (the decoder's input channels), 8 layers,
+MLP 2048, 4 query / 1 key-value heads of 128, vocabulary 8192 and the Soprano-1.1 decoder (768 / 2304, 8 ConvNeXt blocks, n_fft 2048, hop
+512, upscale 4, input kernel 1) -- an ASSUMED geometry, as the published config.json is not at hand.  Its language model is drawn on the
+device, its decoder from oracle/vocos.py's seeded init; prompts are random ids; sampling is Soprano's defaults (T 0.7, top-p 0.95, penalty
+1.5 over 30) with the stop token masked, so every row generates --max-tokens tokens.  Audio is 32 kHz and comes once, at the end.
+
+    python tools/tts_benchmark.py [--model orpheus|qwen3|soprano] [--batch 1] [--prompt 64] [--max-tokens 512] [--model-dir DIR] [--stream]
                                   [--interval 0.32] [--ref-seconds S]"""
 import argparse
 import sys
@@ -28,8 +34,40 @@ from bench import ORPHEUS, make_prompts  # noqa: E402
 QWEN3_06B = dict(hidden_size=1024, num_hidden_layers=28, intermediate_size=3072, num_attention_heads=16, num_key_value_heads=8, head_dim=128,
                  vocab_size=180352, rms_norm_eps=1e-6, rope_theta=1000000.0, tie_word_embeddings=True)
 
+SOPRANO_ASSUMED = dict(hidden_size=512, num_hidden_layers=8, intermediate_size=2048, num_attention_heads=4, num_key_value_heads=1, head_dim=128,
+                       vocab_size=8192, tie_word_embeddings=False, decoder_num_layers=8, decoder_dim=768, decoder_intermediate_dim=2304,
+                       hop_length=512, n_fft=2048, upscale=4, input_kernel=1, dw_kernel=3, token_size=2048)
+
+
+def report(elapsed, audio, first_token, started, info, ttfb=None):
+    print(f"Finished generation in {elapsed:0.2f}s")
+    print("Benchmark:")
+    print(f"  Audio duration: {audio:.2f}s")
+    ttfb = elapsed if ttfb is None else ttfb
+    print(f"  TTFB: {ttfb:.3f}s (first token after {first_token[0] - started:.3f}s)" if first_token else "  TTFB: n/a")
+    print(f"  RTFx: {audio / elapsed:.3f}" if audio > 0 else "  RTFx: n/a")
+    print(f"  Tokens/s: {info.tokens_per_second:.2f}")
+
+
+def soprano_benchmark(a):
+    from oracle import soprano as so
+    cfg = so.SopranoConfig(**SOPRANO_ASSUMED)
+    dec = so.decoder_weights_only(cfg, 1234)
+    tts = m.SopranoModel.random_init(cfg.to_json(), dec, max_batch=a.batch, max_context=a.prompt + a.max_tokens + 2)
+    ids = np.random.default_rng(0).integers(4, cfg.vocab_size, size=(a.batch, a.prompt)).astype(np.int32)
+    P = m.GenerateParameters(max_tokens=a.max_tokens, temperature=0.7, top_p=0.95, repetition_penalty=1.5, repetition_context_size=30,
+                             mask_eos=True)
+    tts.generate_batch(ids, P)                   # warm-up (graph capture, allocations)
+    first_token = []
+    started = time.perf_counter()
+    toks, waves, info = tts.generate_batch(ids, P, on_token=lambda b, step, tok: first_token.append(time.perf_counter()) if not first_token else None)
+    elapsed = time.perf_counter() - started
+    print(f"Soprano, assumed geometry {SOPRANO_ASSUMED}, batch {a.batch}, {a.prompt}-token prompt, {a.max_tokens} tokens")
+    report(elapsed, sum(len(w) for w in waves) / float(tts.sample_rate), first_token, started, info)
+
+
 ap = argparse.ArgumentParser()
-ap.add_argument("--model", default="orpheus", choices=["orpheus", "qwen3"])
+ap.add_argument("--model", default="orpheus", choices=["orpheus", "qwen3", "soprano"])
 ap.add_argument("--batch", type=int, default=1)
 ap.add_argument("--prompt", type=int, default=64)
 ap.add_argument("--max-tokens", type=int, default=512)
@@ -38,6 +76,9 @@ ap.add_argument("--stream", action="store_true", help="chunked audio emission du
 ap.add_argument("--interval", type=float, default=0.32, help="streaming interval in seconds (App.swift:137)")
 ap.add_argument("--ref-seconds", type=float, default=0.0, help="voice-cloning prompt with a synthetic reference clip of S seconds")
 a = ap.parse_args()
+if a.model == "soprano":
+    soprano_benchmark(a)
+    sys.exit(0)
 codec = m.SNAC(weights=m.SNAC.random_init_weights(1234, encoder=a.ref_seconds > 0))
 ref_len = 0
 if a.ref_seconds > 0:
@@ -80,10 +121,4 @@ else:
     toks, waves, info = tts.generate_batch(ids, P, on_token=lambda b, step, tok: first_token.append(time.perf_counter()) if not first_token else None)
     elapsed = time.perf_counter() - started
 audio = sum(len(w) for w in waves if w is not None) / 24000.0
-print(f"Finished generation in {elapsed:0.2f}s")
-print("Benchmark:")
-print(f"  Audio duration: {audio:.2f}s")
-ttfb = (first_audio[0] - started) if first_audio else elapsed
-print(f"  TTFB: {ttfb:.3f}s (first token after {first_token[0] - started:.3f}s)" if first_token else "  TTFB: n/a")
-print(f"  RTFx: {audio / elapsed:.3f}" if audio > 0 else "  RTFx: n/a")
-print(f"  Tokens/s: {info.tokens_per_second:.2f}")
+report(elapsed, audio, first_token, started, info, (first_audio[0] - started) if first_audio else None)
