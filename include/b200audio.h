@@ -921,6 +921,94 @@ int32_t b2a_weights_sanitize_qwen3_speaker_encoder(b2a_weights* w);
 int32_t b2a_qwen3_speaker_encoder_config_from_json(const char* config_path, b2a_qwen3_speaker_encoder_config* cfg);
 int32_t b2a_qwen3_speaker_encoder_create_from_directory(const char* model_dir, int32_t device, b2a_qwen3_speaker_encoder** out);
 
+/* ------------------------------------------------------------------ Mimi (24 kHz audio <-> 12.5 Hz codes, streaming decoder)
+ * Replaces Mimi and MimiStreamingDecoder (Sources/MLXAudioCodecs/Mimi/Mimi.swift), the codec Marvis and PocketTTS decode with.
+ *   encode: audio [B, 1, n] float32 -> codes [B, num_codebooks, encoded_length(n)] int32, every level of the split quantizer.
+ *           The same implementation as b2a_speech_tokenizer_encoder: the Qwen3-TTS encoder is Mimi's encoder.
+ *   decode: codes [B, K, T] int32, 1 <= K <= num_codebooks, each in [0, codebook_size) -> waveform [B, 1, T * 1920] float32.  Level 0
+ *           through rvq_first, levels 1 .. K-1 through rvq_rest (Quantization.swift:113-120, 203-210), the depthwise ×2 upsample, the
+ *           decoder transformer over a KV cache and the SEANet decoder (ELU, transposed convs ×8/6/5/4, no output clip).
+ * One code path: decode_step carries the upsample tail, every conv's history and the KV cache across calls (Mimi.decodeStep,
+ * Mimi.swift:196-202); b2a_mimi_reset clears all three (MimiStreamingDecoder.reset, :215-219).  b2a_mimi_decode is a reset followed
+ * by one step.  Unlike the reference's decode(), it therefore also resets the upsample tail, and it leaves its own state behind, so a
+ * decode_step after it continues that clip (the reference's decode() uses the non-streaming convs and leaves their state empty).
+ * Attention keeps, per call, the last T + min(context, p0) keys of the cache (p0 = positions decoded before the call,
+ * Transformer.swift:156-164): query t sees cache positions [max(0, p0 - context), p0 + t].  A one-shot decode is therefore full
+ * causal over the clip; a stream longer than `context` latent positions (10 s) is not, and differs from it.
+ * Errors: K outside 1..num_codebooks, codes outside [0, codebook_size) (host entry points; the _dev ones clamp), batch outside
+ * 1..max_batch, a stream longer than max_cache_frames code frames, a batch size that changes inside a stream, a geometry the
+ * device path does not run -> B2A_ERR_INVALID_INPUT; a missing tensor -> B2A_ERR_MODEL_NOT_INITIALIZED; empty audio ->
+ * B2A_ERR_AUDIO_ENCODING_FAILED.  Deterministic: a batch row's output is bit for bit the row's output alone.                   */
+typedef struct b2a_mimi_config {
+    int32_t sample_rate;           /* 24000 */
+    float frame_rate;              /* 12.5 code frames per second */
+    int32_t channels;              /* audio channels: 1 */
+    /* SEANet (SeanetConfig) */
+    int32_t dimension;             /* 512: latent width, also the transformer's d_model */
+    int32_t n_filters;             /* 64 */
+    int32_t n_residual_layers;     /* 1 (the only value the device path runs) */
+    int32_t num_ratios;
+    int32_t ratios[8];             /* [8, 6, 5, 4]: the decoder order; the encoder runs them reversed */
+    int32_t kernel_size;           /* 7 */
+    int32_t residual_kernel_size;  /* 3 */
+    int32_t last_kernel_size;      /* 3 */
+    int32_t dilation_base;         /* 2 (unused with one residual layer) */
+    int32_t compress;              /* 2 */
+    int32_t causal;                /* 1 (required) */
+    int32_t true_skip;             /* 1 (required: identity residual) */
+    /* transformer (TransformerConfig), used by both the encoder and the decoder transformer */
+    int32_t num_heads;             /* 8 */
+    int32_t num_layers;            /* 8 */
+    int32_t dim_feedforward;       /* 2048 */
+    int32_t context;               /* 250 latent positions */
+    int32_t max_period;            /* 10000: RoPE base */
+    int32_t gating;                /* 0 (required): exact-GELU MLP */
+    int32_t norm_rms;              /* 0 (required): layer_norm, eps 1e-5 */
+    int32_t kv_repeat;             /* 1 (required) */
+    /* quantizer */
+    int32_t num_codebooks;         /* nq */
+    int32_t codebook_size;         /* 2048 */
+    int32_t codebook_dim;          /* 256 */
+    /* device path */
+    int32_t max_batch;             /* decode rows per call */
+    int32_t max_cache_frames;      /* code frames one stream may decode before a reset (KV cache capacity / 2) */
+} b2a_mimi_config;
+
+typedef struct b2a_mimi b2a_mimi;
+/* mimi_202407(num_codebooks) (Mimi.swift:47-97) with the device-path bounds; num_codebooks < 1 or bounds < 1 -> INVALID_INPUT */
+int32_t b2a_mimi_config_default(int32_t num_codebooks, int32_t max_batch, int32_t max_cache_frames, b2a_mimi_config* out);
+/* tensors: b2a_weights_sanitize_mimi's keys in MLX layouts (encoder.*, encoder_transformer.*, downsample.*, quantizer.*, upsample.*,
+ * decoder_transformer.*, decoder.*) */
+int32_t b2a_mimi_create(int32_t device, const b2a_mimi_config* cfg, const b2a_tensor* tensors, int32_t n_tensors, b2a_mimi** out);
+/* Mimi.sanitize (Mimi.swift:337-413) on an open checkpoint, key for key: "_"-prefixed segments lose the "_", encoder.model. /
+ * decoder.model. -> encoder. / decoder., in_proj_weight -> in_proj.weight, linear1 / linear2 -> gating.linear1 / 2, the decoder index
+ * map [2, 5, 8, 11] and the encoder's [1, 4, 7, 10], 0 / 14 -> init_conv1d / final_conv1d, .block.1. / .block.3. -> .block.0. /
+ * .block.1., the last two axes of every .conv / .input_proj / .output_proj weight swapped, and .convtr weights to MLX's [out, k, in]
+ * (depthwise (C, 1, k) -> (C, k, 1)).  No key is dropped.                                                                      */
+int32_t b2a_weights_sanitize_mimi(b2a_weights* w);
+/* Mimi.fromPretrained on a local single-file checkpoint: mimi_202407(num_codebooks), load, sanitize, create.  The codebooks are
+ * embedding_sum / max(cluster_usage, 1e-5), computed once at load. */
+int32_t b2a_mimi_create_from_file(const char* path, int32_t num_codebooks, int32_t device, int32_t max_batch, int32_t max_cache_frames,
+                                  b2a_mimi** out);
+int32_t b2a_mimi_num_codebooks(const b2a_mimi* h);
+/* samples per code frame: prod(ratios) * (sample_rate / prod(ratios) / frame_rate) = 1920 at the shipped geometry (0: null handle) */
+int32_t b2a_mimi_samples_per_frame(const b2a_mimi* h);
+/* code frames for n samples: ceil(ceil(n / 960) / 2) at the shipped geometry (0 for n < 1 or a null handle) */
+int64_t b2a_mimi_encoded_length(const b2a_mimi* h, int64_t n_samples);
+int32_t b2a_mimi_encode(b2a_mimi* h, const float* audio, int32_t batch, int64_t n_samples, int32_t* codes);
+int32_t b2a_mimi_encode_dev(b2a_mimi* h, const float* d_audio, int32_t batch, int64_t n_samples, int32_t* d_codes, void* stream);
+/* one-shot: reset, then one step.  codes [B, K, T] -> wave [B, 1, T * samples_per_frame] */
+int32_t b2a_mimi_decode(b2a_mimi* h, const int32_t* codes, int32_t batch, int32_t K, int32_t T, float* wave);
+int32_t b2a_mimi_decode_dev(b2a_mimi* h, const int32_t* d_codes, int32_t batch, int32_t K, int32_t T, float* d_wave, void* stream);
+/* Mimi.decodeStep: T more code frames of the current stream -> their T * samples_per_frame samples */
+int32_t b2a_mimi_decode_step(b2a_mimi* h, const int32_t* codes, int32_t batch, int32_t K, int32_t T, float* wave);
+int32_t b2a_mimi_decode_step_dev(b2a_mimi* h, const int32_t* d_codes, int32_t batch, int32_t K, int32_t T, float* d_wave, void* stream);
+/* MimiStreamingDecoder.decodeFrames: T single-frame steps of the current stream (no reset), concatenated */
+int32_t b2a_mimi_decode_frames(b2a_mimi* h, const int32_t* codes, int32_t batch, int32_t K, int32_t T, float* wave);
+int32_t b2a_mimi_reset(b2a_mimi* h);
+void* b2a_mimi_stream(b2a_mimi* h);
+void b2a_mimi_destroy(b2a_mimi* h);
+
 #ifdef __cplusplus
 }
 #endif

@@ -12,6 +12,7 @@ from .vyvo_tts import Qwen3Model
 from .soprano_tts import SopranoModel
 from .vocos import Vocos
 from .encodec import Encodec, EncodecConfig, EncodecEncodedAudio
+from .mimi import Mimi, MimiStreamingDecoder
 from .loading import Weights, llama_config_from_json
 from .whisper import STTGenerateParameters, STTOutput, StreamingConfig, StreamingInferenceSession, StreamingUpdate, WhisperModel
 from .qwen3_tts import (Qwen3CodePredictorConfig, Qwen3GenerateParameters, Qwen3SpeakerEncoderConfig, Qwen3TalkerConfig, Qwen3TTSModel,
@@ -19,7 +20,7 @@ from .qwen3_tts import (Qwen3CodePredictorConfig, Qwen3GenerateParameters, Qwen3
 
 __all__ = ["AudioGenerationError", "IncrementalMelSpectrogram", "LogMel", "compute_mel_spectrogram", "hanning_window", "hamming_window", "power_to_db",
            "mel_filters", "whisper_encoder_features", "SNAC", "LlamaTTSModel", "Qwen3Model", "SopranoModel", "GenerateParameters",
-           "AudioGenerationInfo", "Vocos", "Weights", "llama_config_from_json", "Encodec", "EncodecConfig", "EncodecEncodedAudio", "WhisperModel", "STTGenerateParameters", "STTOutput",
+           "AudioGenerationInfo", "Vocos", "Weights", "llama_config_from_json", "Encodec", "EncodecConfig", "EncodecEncodedAudio", "Mimi", "MimiStreamingDecoder", "WhisperModel", "STTGenerateParameters", "STTOutput",
            "StreamingInferenceSession", "StreamingConfig", "StreamingUpdate",
            "Qwen3TTSTalker", "Qwen3TTSModel", "Qwen3TalkerConfig", "Qwen3CodePredictorConfig", "Qwen3GenerateParameters",
            "Qwen3TTSSpeakerEncoder", "Qwen3SpeakerEncoderConfig"]

@@ -114,6 +114,16 @@ class SpeechTokenizerEncoderConfig(C.Structure):
                 + [(n, C.c_int32) for n in ("codebook_size", "codebook_dim", "num_quantizers", "valid_num_quantizers")])
 
 
+class MimiConfig(C.Structure):
+    _fields_ = ([("sample_rate", C.c_int32), ("frame_rate", C.c_float)]
+                + [(n, C.c_int32) for n in ("channels", "dimension", "n_filters", "n_residual_layers", "num_ratios")]
+                + [("ratios", C.c_int32 * 8)]
+                + [(n, C.c_int32) for n in ("kernel_size", "residual_kernel_size", "last_kernel_size", "dilation_base", "compress", "causal",
+                                           "true_skip", "num_heads", "num_layers", "dim_feedforward", "context", "max_period", "gating",
+                                           "norm_rms", "kv_repeat", "num_codebooks", "codebook_size", "codebook_dim", "max_batch",
+                                           "max_cache_frames")])
+
+
 class Qwen3SpeakerEncoderConfig(C.Structure):
     _fields_ = ([(n, C.c_int32) for n in ("mel_dim", "enc_dim", "num_enc_layers")]
                 + [(n, C.c_int32 * 8) for n in ("enc_channels", "enc_kernel_sizes", "enc_dilations")]
@@ -315,6 +325,23 @@ SIGNATURES = {
     "b2a_weights_sanitize_qwen3_speaker_encoder": (C.c_int32, [_P]),
     "b2a_qwen3_speaker_encoder_config_from_json": (C.c_int32, [C.c_char_p, C.POINTER(Qwen3SpeakerEncoderConfig)]),
     "b2a_qwen3_speaker_encoder_create_from_directory": (C.c_int32, [C.c_char_p, C.c_int32, C.POINTER(_P)]),
+    "b2a_mimi_config_default": (C.c_int32, [C.c_int32, C.c_int32, C.c_int32, C.POINTER(MimiConfig)]),
+    "b2a_mimi_create": (C.c_int32, [C.c_int32, C.POINTER(MimiConfig), C.POINTER(Tensor), C.c_int32, C.POINTER(_P)]),
+    "b2a_weights_sanitize_mimi": (C.c_int32, [_P]),
+    "b2a_mimi_create_from_file": (C.c_int32, [C.c_char_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.POINTER(_P)]),
+    "b2a_mimi_num_codebooks": (C.c_int32, [_P]),
+    "b2a_mimi_samples_per_frame": (C.c_int32, [_P]),
+    "b2a_mimi_encoded_length": (C.c_int64, [_P, C.c_int64]),
+    "b2a_mimi_encode": (C.c_int32, [_P, _P, C.c_int32, C.c_int64, _P]),
+    "b2a_mimi_encode_dev": (C.c_int32, [_P, _P, C.c_int32, C.c_int64, _P, _P]),
+    "b2a_mimi_decode": (C.c_int32, [_P, _P, C.c_int32, C.c_int32, C.c_int32, _P]),
+    "b2a_mimi_decode_dev": (C.c_int32, [_P, _P, C.c_int32, C.c_int32, C.c_int32, _P, _P]),
+    "b2a_mimi_decode_step": (C.c_int32, [_P, _P, C.c_int32, C.c_int32, C.c_int32, _P]),
+    "b2a_mimi_decode_step_dev": (C.c_int32, [_P, _P, C.c_int32, C.c_int32, C.c_int32, _P, _P]),
+    "b2a_mimi_decode_frames": (C.c_int32, [_P, _P, C.c_int32, C.c_int32, C.c_int32, _P]),
+    "b2a_mimi_reset": (C.c_int32, [_P]),
+    "b2a_mimi_stream": (C.c_void_p, [_P]),
+    "b2a_mimi_destroy": (None, [_P]),
     "b2a_encodec_destroy": (None, [_P]),
     "b2a_weights_load": (C.c_int32, [C.c_char_p, C.POINTER(_P)]),
     "b2a_weights_count": (C.c_int32, [_P]),

@@ -11,7 +11,7 @@ HERE = Path(__file__).resolve().parent
 CSRC = HERE / "csrc"
 LIBDIR = HERE / "lib"
 LIB = LIBDIR / "libb200audio.so"
-SOURCES = ["api.cu", "mel.cu", "snac.cu", "llama.cu", "tc_gemm.cu", "conv_gemm.cu", "whisper.cu", "vocos.cu", "encodec.cu", "weights.cu", "speech_tokenizer.cu", "qwen3_sampler.cu", "speaker_encoder.cu"]
+SOURCES = ["api.cu", "mel.cu", "snac.cu", "llama.cu", "tc_gemm.cu", "conv_gemm.cu", "whisper.cu", "vocos.cu", "encodec.cu", "weights.cu", "speech_tokenizer.cu", "qwen3_sampler.cu", "speaker_encoder.cu", "mimi.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr",

@@ -246,7 +246,7 @@ implicit_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_const
             const long long fo = (long long)tf * a.up + rho;
             if (a.xo) a.xo[((long long)b * To + fo) * a.Cout + co] = val;
             if (a.hl) {
-                const float hv = a.sa ? snake_inv(val, sa, sb) : val;
+                const float hv = a.sa ? snake_inv(val, sa, sb) : a.elu ? (val > 0.f ? val : expm1f(val)) : val;
                 const long long idx = ((long long)b * (a.Hout + To) + a.Hout + fo) * a.Cout + co;
                 put_hilo16(reinterpret_cast<uint16_t*>(a.hl), plane, idx, hv, a.f16);
             }

@@ -191,6 +191,7 @@ struct Args {
                                   // round-to-nearest bound that bias.
     const float* sa;              // SnakeBeta on the hi/lo copy: v + sb * sin^2(sa * v), sa = exp(alpha), sb = 1 / (exp(beta) + 1e-9)
     const float* sb;
+    int elu;                      // ELU(alpha 1) on the hi/lo copy instead (Mimi's SEANet decoder: the next conv's input activation)
 };
 
 // One implicit convolution of weight W over planes `in` [2][B][in_frames][W.Cin] in W's operand format.  Set here: the weight

@@ -21,6 +21,7 @@
 #include "common.cuh"
 #include "conv_gemm.cuh"
 #include "seanet.cuh"
+#include "codec_transformer.cuh"
 
 #include <algorithm>
 #include <cmath>
@@ -29,34 +30,9 @@
 namespace b2a {
 namespace st {
 
-typedef __nv_bfloat16 bf16;
-
 // ----------------------------------------------------------------------------------------------- SIMT kernels
-__device__ __forceinline__ void put_planes(bf16* base, long long plane, long long idx, float v, int f16) {
-    cg::put_hilo16(reinterpret_cast<uint16_t*>(base), plane, idx, v, f16);
-}
-
-// codes [B, nq, T] -> planes [2][B*T][2*D2]: channels [0, D2) = sum of the semantic codebooks, [D2, 2*D2) = sum of the rest
-__global__ void rvq_gather_kernel(const int* __restrict__ codes, const float* __restrict__ emb /*[nq][bins][D2]*/, bf16* __restrict__ out,
-                                  int B, int T, int nq, int nq_model, int nsem, int bins, int D2, int f16) {
-    const long long n = blockIdx.x;
-    const int b = (int)(n / T), t = (int)(n - (long long)b * T);
-    const long long plane = (long long)B * T * 2 * D2;
-    for (int c = threadIdx.x; c < D2; c += blockDim.x) {
-        float s0 = 0.f, s1 = 0.f;
-        for (int qi = 0; qi < nq && qi < nq_model; ++qi) {
-            int code = codes[((long long)b * nq + qi) * T + t];
-            code = code < 0 ? 0 : (code >= bins ? bins - 1 : code);
-            const float v = emb[((long long)qi * bins + code) * D2 + c];
-            if (qi < nsem) s0 += v; else s1 += v;
-        }
-        put_planes(out, plane, n * 2 * D2 + c, s0, f16);
-        put_planes(out, plane, n * 2 * D2 + D2 + c, s1, f16);
-    }
-}
-
+// (the gathers, LayerNorm, RoPE, attention and history carries shared with Mimi are in codec_transformer.cuh)
 // RMSNorm over channels -> planes [2][N][C]   (DecoderRMSNorm :301-314: w * (x * rsqrt(mean(x^2) + eps)))
-constexpr int RN_THREADS = 128;
 __global__ void __launch_bounds__(RN_THREADS)
 rmsnorm_planes_kernel(const float* __restrict__ x, const float* __restrict__ w, bf16* __restrict__ out, long long N, int C, float eps, int f16) {
     __shared__ float red[RN_THREADS / 32];
@@ -65,110 +41,6 @@ rmsnorm_planes_kernel(const float* __restrict__ x, const float* __restrict__ w, 
     for (int c = threadIdx.x; c < C; c += RN_THREADS) { const float v = x[n * C + c]; ss += v * v; }
     const float r = rsqrtf(block_sum<RN_THREADS>(ss, red) / (float)C + eps);
     for (int c = threadIdx.x; c < C; c += RN_THREADS) put_planes(out, N * C, n * C + c, w[c] * (x[n * C + c] * r), f16);
-}
-
-// RoPE on q (in place) and k (into the cache), v copied into the cache.  qkv [N, (nh + 2 nkv) * hd] fp32.  Frequency i rotates the
-// pair (i, i + hd/2) (rotate-half: the decoder, DecoderTransformer) or (2i, 2i + 1) (INTERLEAVED: the encoder, MLX RoPE traditional:
-// true, Mimi/Transformer.swift:130).
-template <bool INTERLEAVED>
-__global__ void rope_cache_kernel(float* __restrict__ qkv, float* __restrict__ Kc, float* __restrict__ Vc, const float* __restrict__ inv_freq,
-                                  int T, int pos0, int nh, int nkv, int hd, int cap) {
-    const long long n = blockIdx.x;
-    const int b = (int)(n / T), t = (int)(n - (long long)b * T);
-    const int pos = pos0 + t, half = hd / 2, ld = (nh + 2 * nkv) * hd;
-    float* row = qkv + n * ld;
-    for (int idx = threadIdx.x; idx < (nh + nkv) * half; idx += blockDim.x) {
-        const int head = idx / half, i = idx - head * half;
-        float sn, cs;
-        sincosf((float)pos * inv_freq[i], &sn, &cs);
-        const int i1 = INTERLEAVED ? 2 * i : i, i2 = INTERLEAVED ? 2 * i + 1 : i + half;
-        const float x1 = row[head * hd + i1], x2 = row[head * hd + i2];
-        const float o1 = x1 * cs - x2 * sn, o2 = x2 * cs + x1 * sn;
-        if (head < nh) {
-            row[head * hd + i1] = o1;
-            row[head * hd + i2] = o2;
-        } else {
-            float* dst = Kc + (((long long)b * nkv + (head - nh)) * cap + pos) * hd;
-            dst[i1] = o1;
-            dst[i2] = o2;
-        }
-    }
-    for (int idx = threadIdx.x; idx < nkv * hd; idx += blockDim.x) {
-        const int kvh = idx / hd, d = idx - kvh * hd;
-        Vc[(((long long)b * nkv + kvh) * cap + pos) * hd + d] = row[(nh + nkv) * hd + idx];
-    }
-}
-
-// causal attention of the chunk's T queries over cache positions [0, pos0 + t]: one warp per (query, head), each lane
-// owns hd / 32 consecutive dims, online softmax, four keys in flight.  Output -> planes [2][N][nh * hd].
-constexpr int AT_WARPS = 4;
-template <int DPL>
-__global__ void __launch_bounds__(AT_WARPS * 32)
-attn_kernel(const float* __restrict__ qkv, const float* __restrict__ Kc, const float* __restrict__ Vc, bf16* __restrict__ out,
-            int B, int T, int pos0, int nh, int nkv, int cap, float scale, int f16) {
-    constexpr int HD = DPL * 32;
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int t = blockIdx.x * AT_WARPS + warp, h = blockIdx.y, b = blockIdx.z;
-    if (t >= T) return;
-    const long long n = (long long)b * T + t;
-    const int ld = (nh + 2 * nkv) * HD, kvh = h / (nh / nkv);
-    float q[DPL], acc[DPL];
-#pragma unroll
-    for (int d = 0; d < DPL; ++d) { q[d] = qkv[n * ld + h * HD + lane * DPL + d] * scale; acc[d] = 0.f; }
-    const float* Kb = Kc + ((long long)b * nkv + kvh) * cap * HD + lane * DPL;
-    const float* Vb = Vc + ((long long)b * nkv + kvh) * cap * HD + lane * DPL;
-    float m = -INFINITY, l = 0.f;
-    const int nkeys = pos0 + t + 1;
-    for (int p0 = 0; p0 < nkeys; p0 += 4) {
-        float s[4];
-#pragma unroll
-        for (int u = 0; u < 4; ++u) {
-            float d0 = 0.f;
-            if (p0 + u < nkeys) {
-#pragma unroll
-                for (int d = 0; d < DPL; ++d) d0 = fmaf(q[d], Kb[(long long)(p0 + u) * HD + d], d0);
-            }
-            s[u] = d0;
-        }
-#pragma unroll
-        for (int u = 0; u < 4; ++u) s[u] = warp_sum(s[u]);
-        float mx = m;
-#pragma unroll
-        for (int u = 0; u < 4; ++u) if (p0 + u < nkeys) mx = fmaxf(mx, s[u]);
-        const float corr = __expf(m - mx);      // m = -inf on the first pass: exp(-inf) = 0
-        l *= corr;
-#pragma unroll
-        for (int d = 0; d < DPL; ++d) acc[d] *= corr;
-#pragma unroll
-        for (int u = 0; u < 4; ++u) {
-            if (p0 + u < nkeys) {
-                const float e = __expf(s[u] - mx);
-                l += e;
-#pragma unroll
-                for (int d = 0; d < DPL; ++d) acc[d] = fmaf(e, Vb[(long long)(p0 + u) * HD + d], acc[d]);
-            }
-        }
-        m = mx;
-    }
-    const float inv = 1.0f / l;
-    const long long N = (long long)B * T;
-#pragma unroll
-    for (int d = 0; d < DPL; ++d) put_planes(out, N * nh * HD, n * nh * HD + h * HD + lane * DPL + d, acc[d] * inv, f16);
-}
-
-// LayerNorm with bias over channels -> planes [2][N][C]   (MLXNN LayerNorm: (x - mean) * rsqrt(var + eps) * w + b)
-__global__ void __launch_bounds__(RN_THREADS)
-layernorm_planes_kernel(const float* __restrict__ x, const float* __restrict__ w, const float* __restrict__ bias, bf16* __restrict__ out,
-                        long long N, int C, float eps, int f16) {
-    __shared__ float red[RN_THREADS / 32];
-    const long long n = blockIdx.x;
-    float s = 0.f;
-    for (int c = threadIdx.x; c < C; c += RN_THREADS) s += x[n * C + c];
-    const float mean = block_sum<RN_THREADS>(s, red) / (float)C;
-    float q = 0.f;
-    for (int c = threadIdx.x; c < C; c += RN_THREADS) { const float d = x[n * C + c] - mean; q += d * d; }
-    const float r = rsqrtf(block_sum<RN_THREADS>(q, red) / (float)C + eps);
-    for (int c = threadIdx.x; c < C; c += RN_THREADS) put_planes(out, N * C, n * C + c, (x[n * C + c] - mean) * r * w[c] + bias[c], f16);
 }
 
 // The split quantizer's k1 input projections in ordered fp32, so that the code search is a function of z alone:
@@ -249,37 +121,6 @@ dw_ln_kernel(const float* __restrict__ x, const float* __restrict__ st, const fl
     }
 }
 
-// fp32 history: new[b][f] = last H frames of [old | x]
-__global__ void state_update_f32_kernel(const float* __restrict__ x, const float* __restrict__ old, float* __restrict__ nw, int B, int T, int H, int C) {
-    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= (long long)B * H * C) return;
-    const int c = (int)(i % C);
-    const long long bf = i / C;
-    const int f = (int)(bf % H), b = (int)(bf / H);
-    const int src = T + f;        // frame index in [old (H) | x (T)]
-    nw[i] = src < H ? old[((long long)b * H + src) * C + c] : x[((long long)b * T + (src - H)) * C + c];
-}
-
-// bf16 planes with a history prefix: X = [2][B][H + T][C].  Copies the old state into frames [0, H) and saves the last H
-// frames of [old | new] as the new state (old and new are different buffers).  8 channels (16 bytes) per thread.
-__global__ void carry_planes_kernel(bf16* __restrict__ X, const bf16* __restrict__ old, bf16* __restrict__ nw, int B, int T, int H, int C8) {
-    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    const long long per_plane = (long long)B * H * C8;
-    if (i >= 2 * per_plane) return;
-    const int c = (int)(i % C8);
-    long long r = i / C8;
-    const int f = (int)(r % H); r /= H;
-    const int b = (int)(r % B), p = (int)(r / B);
-    const uint4* o4 = reinterpret_cast<const uint4*>(old);
-    uint4* n4 = reinterpret_cast<uint4*>(nw);
-    uint4* x4 = reinterpret_cast<uint4*>(X);
-    const long long xrow = ((long long)p * B + b) * (H + T);
-    const uint4 ov = o4[i];
-    x4[(xrow + f) * C8 + c] = ov;
-    const int src = T + f;
-    n4[i] = src < H ? o4[(((long long)p * B + b) * H + src) * C8 + c] : x4[(xrow + src) * C8 + c];
-}
-
 // SnakeBeta -> causal k-tap conv to ONE channel -> clip(-1, 1)          (DecoderOutputSnake + DecoderOutputConv :693-731, :946)
 // x [B, T, C] fp32 (raw, pre-activation), st [B, k-1, C] raw history.  64 outputs per CTA; the activated tile lives in smem.
 constexpr int FC_TILE = 64, FC_THREADS = 128, FC_MAXK = 8;
@@ -319,8 +160,6 @@ final_conv_kernel(const float* __restrict__ x, const float* __restrict__ st, con
 using cg::TcW;
 
 struct Snake { DBuf<float> a, ib; };                 // a = exp(alpha), ib = 1 / (exp(beta) + 1e-9)
-struct PlaneState { DBuf<bf16> s[2]; int H = 0, C = 0; };      // [2][B][H][C]
-struct F32State { DBuf<float> s[2]; int H = 0, C = 0; };       // [B][H][C]
 
 struct TLayer { TcW qkv, o, gu, down; DBuf<float> ln1, ln2, sc_attn, sc_mlp; DBuf<float> K, V; };
 struct UpLayer { TcW ct, pw1, pw2; DBuf<float> dw_w, dw_b, ln_w, ln_b, gamma; F32State st; int factor = 1; };
@@ -374,16 +213,6 @@ struct b2a_speech_tokenizer {
 
     static std::vector<float> conv_w(const TensorTable& tt, const std::string& name, int out, int k, int in) {
         return tt.f32(name, (int64_t)out * k * in);       // MLX [out, k, in] == [M][taps][Cin] with tap j <-> kernel index j
-    }
-    // transposed conv, MLX [out, k, in], k = n * r: rows m = rho * out + co, tap j <-> input frame q - (n - 1 - j) <-> kernel index rho + (n - 1 - j) * r
-    static std::vector<float> convt_w(const std::vector<float>& w, int out, int k, int in, int r) {
-        const int n = k / r;
-        std::vector<float> g((size_t)r * out * n * in);
-        for (int rho = 0; rho < r; ++rho)
-            for (int co = 0; co < out; ++co)
-                for (int j = 0; j < n; ++j)
-                    memcpy(&g[(((size_t)rho * out + co) * n + j) * in], &w[((size_t)co * k + rho + (size_t)(n - 1 - j) * r) * in], (size_t)in * sizeof(float));
-        return g;
     }
     static void up(DBuf<float>& d, const std::vector<float>& v) { d.upload(v.data(), v.size()); }
     static void load_snake(Snake& s, const TensorTable& tt, const std::string& p, int C) {
@@ -494,7 +323,7 @@ struct b2a_speech_tokenizer {
             U.factor = c.upsampling_ratios[i];
             B2A_CHECK(U.factor >= 1 && U.factor <= 16, B2A_ERR_INVALID_INPUT, "speech tokenizer: bad upsampling ratio");
             total_up *= U.factor;
-            U.ct.build(convt_w(conv_w(tt, p + "0.conv.weight", L, U.factor, L), L, U.factor, L, U.factor), U.factor * L, 1, L, use_f16);
+            U.ct.build(convt_weight(conv_w(tt, p + "0.conv.weight", L, U.factor, L), L, U.factor, L, U.factor), U.factor * L, 1, L, use_f16);
             U.ct.set_bias(tt.f32(p + "0.conv.bias", L));
             up(U.dw_w, tt.f32(p + "1.dwconv.conv.weight", (int64_t)L * 7));
             up(U.dw_b, tt.f32(p + "1.dwconv.conv.bias", L));
@@ -518,7 +347,7 @@ struct b2a_speech_tokenizer {
             Bk.cin = dd >> b; Bk.cout = dd >> (b + 1);
             B2A_CHECK(Bk.cin % 8 == 0 && Bk.cout % 8 == 0, B2A_ERR_INVALID_INPUT, "speech tokenizer: decoder channels must be multiples of 8");
             load_snake(Bk.sn, tt, p + "0", Bk.cin);
-            Bk.ct.build(convt_w(conv_w(tt, p + "1.conv.weight", Bk.cout, 2 * Bk.rate, Bk.cin), Bk.cout, 2 * Bk.rate, Bk.cin, Bk.rate), Bk.rate * Bk.cout, 2, Bk.cin, use_f16);
+            Bk.ct.build(convt_weight(conv_w(tt, p + "1.conv.weight", Bk.cout, 2 * Bk.rate, Bk.cin), Bk.cout, 2 * Bk.rate, Bk.cin, Bk.rate), Bk.rate * Bk.cout, 2, Bk.cin, use_f16);
             Bk.ct.set_bias(tt.f32(p + "1.conv.bias", Bk.cout));
             Bk.st.H = 1; Bk.st.C = Bk.cin;
             const int dil[3] = {1, 3, 9};
@@ -595,9 +424,9 @@ struct b2a_speech_tokenizer {
         const dim3 grid(cdiv(T, AT_WARPS), cfg.num_attention_heads, B), block(AT_WARPS * 32);
         const float scale = 1.0f / sqrtf((float)cfg.head_dim);
         const int nh = cfg.num_attention_heads, nkv = cfg.num_key_value_heads, cap = cfg.max_cache_frames;
-        if (cfg.head_dim == 32) attn_kernel<1><<<grid, block, 0, s>>>(Q.p, L.K.p, L.V.p, out, B, T, cache_len, nh, nkv, cap, scale, use_f16);
-        else if (cfg.head_dim == 64) attn_kernel<2><<<grid, block, 0, s>>>(Q.p, L.K.p, L.V.p, out, B, T, cache_len, nh, nkv, cap, scale, use_f16);
-        else attn_kernel<4><<<grid, block, 0, s>>>(Q.p, L.K.p, L.V.p, out, B, T, cache_len, nh, nkv, cap, scale, use_f16);
+        if (cfg.head_dim == 32) attn_kernel<1><<<grid, block, 0, s>>>(Q.p, L.K.p, L.V.p, out, B, T, cache_len, nh, nkv, cap, scale, use_f16, 0);
+        else if (cfg.head_dim == 64) attn_kernel<2><<<grid, block, 0, s>>>(Q.p, L.K.p, L.V.p, out, B, T, cache_len, nh, nkv, cap, scale, use_f16, 0);
+        else attn_kernel<4><<<grid, block, 0, s>>>(Q.p, L.K.p, L.V.p, out, B, T, cache_len, nh, nkv, cap, scale, use_f16, 0);
         count_launch();
     }
 
@@ -942,9 +771,9 @@ struct b2a_speech_tokenizer_encoder {
             count_launch();
             {
                 const dim3 grid(cdiv(cap, AT_WARPS), nh, B), block(AT_WARPS * 32);
-                if (hd == 32) attn_kernel<1><<<grid, block, 0, s>>>(Q.p, Kc.p, Vc.p, P1.p, B, cap, 0, nh, nh, cap, scale, 1);
-                else if (hd == 64) attn_kernel<2><<<grid, block, 0, s>>>(Q.p, Kc.p, Vc.p, P1.p, B, cap, 0, nh, nh, cap, scale, 1);
-                else attn_kernel<4><<<grid, block, 0, s>>>(Q.p, Kc.p, Vc.p, P1.p, B, cap, 0, nh, nh, cap, scale, 1);
+                if (hd == 32) attn_kernel<1><<<grid, block, 0, s>>>(Q.p, Kc.p, Vc.p, P1.p, B, cap, 0, nh, nh, cap, scale, 1, 0);
+                else if (hd == 64) attn_kernel<2><<<grid, block, 0, s>>>(Q.p, Kc.p, Vc.p, P1.p, B, cap, 0, nh, nh, cap, scale, 1, 0);
+                else attn_kernel<4><<<grid, block, 0, s>>>(Q.p, Kc.p, Vc.p, P1.p, B, cap, 0, nh, nh, cap, scale, 1, 0);
                 count_launch();
             }
             { ic::Args a{}; a.B = B; a.T = cap; a.xo = x; a.add = 1; a.gamma = Ly.ls1.p; ic::launch(Ly.o, P1.p, cap, a, num_sms, s); }
@@ -1104,7 +933,7 @@ int32_t b2a_speech_tokenizer_debug_layout(const float* w, int32_t out, int32_t k
         B2A_CHECK(stride == 0 || k % stride == 0, B2A_ERR_INVALID_INPUT, "b2a_speech_tokenizer_debug_layout: kernel must be a multiple of the stride");
         std::vector<float> src(w, w + (size_t)out * k * in);
         const int M = stride ? stride * out : out, T = stride ? k / stride : k;
-        const std::vector<float> g = TcW::pad_k(stride ? b2a_speech_tokenizer::convt_w(src, out, k, in, stride) : src, M, T, in);
+        const std::vector<float> g = TcW::pad_k(stride ? convt_weight(src, out, k, in, stride) : src, M, T, in);
         B2A_CHECK((int64_t)g.size() <= capacity, B2A_ERR_INVALID_INPUT, "b2a_speech_tokenizer_debug_layout: output buffer too small");
         memcpy(layout_out, g.data(), g.size() * sizeof(float));
         *rows = M; *taps = T; *kpad = cdiv(in, tc::BK) * tc::BK;

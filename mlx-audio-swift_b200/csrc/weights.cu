@@ -803,6 +803,64 @@ struct b2a_weights {
         items = std::move(out);
     }
 
+    // ---- Mimi.sanitize (Mimi/Mimi.swift:337-413), key for key: Swift's replacingOccurrences replaces every occurrence
+    void sanitize_mimi() {
+        auto replace_all = [](std::string& s, const std::string& from, const std::string& to) {
+            for (size_t p = 0; (p = s.find(from, p)) != std::string::npos; p += to.size()) s.replace(p, from.size(), to);
+        };
+        auto ends_with = [](const std::string& s, const std::string& e) { return s.size() >= e.size() && s.compare(s.size() - e.size(), e.size(), e) == 0; };
+        for (auto& t : items) {
+            std::string k, seg;
+            for (size_t a = 0;;) {                      // drop the leading "_" of every dot-separated segment
+                const size_t b = t.name.find('.', a);
+                seg = t.name.substr(a, b == std::string::npos ? std::string::npos : b - a);
+                if (!seg.empty() && seg[0] == '_') seg = seg.substr(1);
+                k += (a ? "." : "") + seg;
+                if (b == std::string::npos) break;
+                a = b + 1;
+            }
+            if (k.rfind("encoder.model.", 0) == 0) replace_all(k, "encoder.model.", "encoder.");
+            if (k.rfind("decoder.model.", 0) == 0) replace_all(k, "decoder.model.", "decoder.");
+            if (ends_with(k, ".in_proj_weight")) replace_all(k, ".in_proj_weight", ".in_proj.weight");
+            if (ends_with(k, ".linear1.weight")) replace_all(k, ".linear1.weight", ".gating.linear1.weight");
+            if (ends_with(k, ".linear2.weight")) replace_all(k, ".linear2.weight", ".gating.linear2.weight");
+            const int dec_idx[4] = {2, 5, 8, 11}, enc_idx[4] = {1, 4, 7, 10};
+            for (int l = 0; l < 4; ++l) {
+                replace_all(k, "decoder." + std::to_string(dec_idx[l]) + ".", "decoder.layers." + std::to_string(l) + ".upsample.");
+                replace_all(k, "decoder." + std::to_string(dec_idx[l] + 1) + ".", "decoder.layers." + std::to_string(l) + ".residuals.0.");
+            }
+            for (int l = 0; l < 4; ++l) {
+                replace_all(k, "encoder." + std::to_string(enc_idx[l]) + ".", "encoder.layers." + std::to_string(l) + ".residuals.0.");
+                replace_all(k, "encoder." + std::to_string(enc_idx[l] + 2) + ".", "encoder.layers." + std::to_string(l) + ".downsample.");
+            }
+            replace_all(k, "decoder.0.", "decoder.init_conv1d.");
+            replace_all(k, "decoder.14.", "decoder.final_conv1d.");
+            replace_all(k, "encoder.0.", "encoder.init_conv1d.");
+            replace_all(k, "encoder.14.", "encoder.final_conv1d.");
+            replace_all(k, ".block.1.", ".block.0.");
+            replace_all(k, ".block.3.", ".block.1.");
+            if ((ends_with(k, ".conv.weight") || ends_with(k, ".output_proj.weight") || ends_with(k, ".input_proj.weight")) && t.ndim >= 2) {
+                if (t.ndim == 3) permute3(t, 0, 2, 1);
+                else if (t.ndim == 2) {
+                    const std::vector<float> v = as_f32(t);
+                    const int64_t r = t.shape[0], c = t.shape[1];
+                    auto o = std::make_shared<std::vector<uint8_t>>((size_t)(r * c) * 4);
+                    float* of = (float*)o->data();
+                    for (int64_t i = 0; i < r; ++i)
+                        for (int64_t j = 0; j < c; ++j) of[j * r + i] = v[i * c + j];
+                    t.owned = o; t.data = of; t.dtype = B2A_DTYPE_F32; t.shape[0] = c; t.shape[1] = r;
+                } else {
+                    throw Error(B2A_ERR_MODEL_NOT_INITIALIZED, "mimi sanitize: cannot swap the last axes of a 4-D tensor: " + t.name);
+                }
+            }
+            if (ends_with(k, ".convtr.weight") && t.ndim == 3) {
+                if (t.shape[1] == 1) permute3(t, 0, 2, 1);      // depthwise (C, 1, k) -> (C, k, 1)
+                else permute3(t, 1, 2, 0);                      // (in, out, k) -> (out, k, in)
+            }
+            t.name = k;
+        }
+    }
+
     std::vector<b2a_tensor> table() const {
         std::vector<b2a_tensor> t(items.size());
         for (size_t i = 0; i < items.size(); ++i) {
@@ -1366,6 +1424,32 @@ int32_t b2a_power_to_db(const float* spectrogram, int64_t n, float amin, float t
         for (int64_t i = 0; i < n; ++i) { out[i] = 10.0f * log10f(std::max(spectrogram[i], amin)); mx = std::max(mx, out[i]); }
         if (top_db >= 0.f)
             for (int64_t i = 0; i < n; ++i) out[i] = std::max(out[i], mx - top_db);
+    });
+}
+
+
+int32_t b2a_weights_sanitize_mimi(b2a_weights* w) {
+    return guarded([&] {
+        B2A_CHECK(w, B2A_ERR_INVALID_INPUT, "b2a_weights_sanitize_mimi: null handle");
+        w->sanitize_mimi();
+    });
+}
+
+// Mimi.fromPretrained (Mimi.swift:236-335) on a local checkpoint file: mimi_202407(num_codebooks) -> load -> sanitize -> create
+int32_t b2a_mimi_create_from_file(const char* path, int32_t num_codebooks, int32_t device, int32_t max_batch, int32_t max_cache_frames,
+                                  b2a_mimi** out) {
+    return guarded([&] {
+        B2A_CHECK(path && out, B2A_ERR_INVALID_INPUT, "b2a_mimi_create_from_file: null argument");
+        *out = nullptr;
+        b2a_mimi_config cfg{};
+        int32_t st = b2a_mimi_config_default(num_codebooks, max_batch, max_cache_frames, &cfg);
+        if (st != B2A_OK) throw Error(st, b2a_last_error());
+        std::unique_ptr<b2a_weights> w(new b2a_weights());
+        w->load_file(path);
+        w->sanitize_mimi();
+        const std::vector<b2a_tensor> tab = w->table();
+        st = b2a_mimi_create(device, &cfg, tab.data(), (int32_t)tab.size(), out);
+        if (st != B2A_OK) throw Error(st, b2a_last_error());
     });
 }
 

@@ -51,6 +51,10 @@ class Weights:
         downsample.*, quantizer.*) in MLX layouts, every other key dropped."""
         _ffi.check(_ffi.lib().b2a_weights_sanitize_speech_tokenizer_encoder(self._h))
 
+    def sanitize_mimi(self) -> None:
+        """Mimi.sanitize (Mimi/Mimi.swift:337-413), key for key; no key is dropped."""
+        _ffi.check(_ffi.lib().b2a_weights_sanitize_mimi(self._h))
+
     def sanitize_qwen3_speaker_encoder(self) -> None:
         """Qwen3TTSSpeakerEncoder.sanitize (Qwen3TTSSpeakerEncoder.swift:324-354): the keys after the "speaker_encoder" component,
         3-D ".weight" tensors that fail checkArrayShapeQwen3 transposed [out, in, k] -> [out, k, in], every other key dropped."""
