@@ -108,13 +108,25 @@ int32_t b2a_debug_qkv_split(int32_t m_tiles, int32_t k_blocks, int32_t* out);
  * DEVICE qkv [B * T, 3 * nh * 64] fp32; out [2 * 64 * cdiv(B * T, 64), nh * 64] bf16: token t = b * T + i at hi row
  * (t / 64) * 128 + t % 64, lo row = hi row + 64.  Rows of tokens >= B * T are not written.                                  */
 int32_t b2a_mha_tc_test(const float* qkv, void* out, int32_t B, int32_t T, int32_t nh, void* stream);
-/* tests/test_gpu_prompt_attention.py: the Orpheus long-prompt attention (csrc/prompt_attn_tc.cuh: rope_table_kernel, pack_prompt_kernel,
- * prompt_attn_kernel) for one layer, all pointers DEVICE.  qkv [B * L, (nq + 2 nkv) * 128] fp32 (q | k | v of token b * L + i), freqs
- * [64] the RoPE frequencies (angle = position / freqs[d]); kcache / vcache fp32 [B][nkv][max_ctx][128] receive the RoPE'd keys and the
- * values at positions 0 .. L-1, rows >= L untouched; out [2 * 64 * cdiv(B * L, 64), nq * 128] bf16: the causal attention of token t at
- * hi row (t / 64) * 128 + t % 64, lo row = hi row + 64.  Rows of tokens >= B * L are not written.                                  */
-int32_t b2a_prompt_attn_test(const float* qkv, const float* freqs, float* kcache, float* vcache, void* out, int32_t B, int32_t L,
-                             int32_t nq, int32_t nkv, int32_t max_ctx, void* stream);
+/* tests/test_gpu_prompt_attention.py: the prompt attention of the batched prefill for one layer, all pointers DEVICE: rope_table_kernel,
+ * then path 1 the SIMT prefill_attn_kernel<G> (only the L the engine gives it: L <= 128 at G <= 4, 124 at G = 6, 92 at G = 8) or path 2
+ * the wgmma pack_prompt_kernel + prompt_attn_kernel (csrc/prompt_attn_tc.cuh), with the engine's launches.  qkv [B * L, (nq + 2 nkv) * 128]
+ * fp32 (q | k | v of token b * L + i), freqs [64] the RoPE frequencies (angle = position / freqs[d]); qnorm / knorm [128] (both or
+ * neither, nullable): per-head RMSNorm x * rsqrt(mean(x^2) + qk_eps) * gain of every q / k head before RoPE; kcache / vcache fp32
+ * [B][nkv][max_ctx][128] receive the (normalised) RoPE'd keys and the values at positions 0 .. L-1, rows >= L untouched;
+ * out [2 * 64 * cdiv(B * L, 64), nq * 128] bf16: the causal attention of token t at hi row (t / 64) * 128 + t % 64, lo row = hi row + 64.
+ * Rows of tokens >= B * L are not written.  q heads per kv head: 1, 2, 3, 4, 6 or 8.                                          */
+int32_t b2a_prompt_attn_test(const float* qkv, const float* freqs, const float* qnorm, const float* knorm, float qk_eps, float* kcache,
+                             float* vcache, void* out, int32_t B, int32_t L, int32_t nq, int32_t nkv, int32_t max_ctx, int32_t path,
+                             void* stream);
+/* tests/test_gpu_decode_attention.py: one decode-step attention launch of the Llama / Qwen3 stacks (attn_decode_cluster_kernel<G>,
+ * csrc/llama.cu) with the step's grid (nkv, B, 2), shared memory and programmatic-dependent launch, all pointers DEVICE.  Row b < B
+ * (B <= 8) with 0 <= pos[b] < max_ctx normalises (qnorm / knorm as above) and rotates its q heads and new key from qkv
+ * [B, (nq + 2 nkv) * 128] fp32 at position pos[b], writes the key and the raw value to row pos[b] of kcache / vcache fp32
+ * [B][nkv][max_ctx][128] and attends to the cached rows 0 .. pos[b] - 1 plus the new one.  out [16, nq * 128] bf16: hi row b, lo row
+ * 8 + b.  Other rows write nothing.  q heads per kv head: 1, 2, 3, 4, 6 or 8.                                                  */
+int32_t b2a_decode_attn_test(const float* qkv, const int32_t* pos, const float* freqs, const float* qnorm, const float* knorm, float qk_eps,
+                             float* kcache, float* vcache, void* out, int32_t B, int32_t nq, int32_t nkv, int32_t max_ctx, void* stream);
 /* tests/test_gpu_whisper_decode_attention.py: one Whisper decoder-step attention launch (mha_decode_kernel, csrc/whisper.cu) with the
  * engine's grid (nh, B, S), all pointers DEVICE.  self_attn != 0: q is the fused q|k|v row [B, 3 * nh * 64] (query, new key, new
  * value), kcache / vcache fp32 [B][nh][max_t][64]; row b with 0 <= pos[b] < max_t writes its new key / value at pos[b] and attends

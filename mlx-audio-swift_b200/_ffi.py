@@ -286,7 +286,8 @@ SIGNATURES = {
     "b2a_tc_gemm_splitk_store_test": (C.c_int32, [_P, _P, _P, _P, C.c_int32, C.c_float] + [C.c_int32] * 6 + [_P]),
     "b2a_debug_qkv_split": (C.c_int32, [C.c_int32, C.c_int32, C.POINTER(C.c_int32)]),
     "b2a_mha_tc_test": (C.c_int32, [_P, _P, C.c_int32, C.c_int32, C.c_int32, _P]),
-    "b2a_prompt_attn_test": (C.c_int32, [_P, _P, _P, _P, _P, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _P]),
+    "b2a_prompt_attn_test": (C.c_int32, [_P, _P, _P, _P, C.c_float, _P, _P, _P] + [C.c_int32] * 6 + [_P]),
+    "b2a_decode_attn_test": (C.c_int32, [_P, _P, _P, _P, _P, C.c_float, _P, _P, _P] + [C.c_int32] * 4 + [_P]),
     "b2a_wh_decode_attn_test": (C.c_int32, [C.c_int32, _P, _P, _P, _P, _P, _P, _P, _P, _P, C.c_int32, C.c_int32, C.c_int32, _P]),
     "b2a_conv_gemm_test": (C.c_int32, [_P, C.c_int32, C.c_int32, _P, C.c_int32, C.c_int32, _P, _P, _P, C.c_int32, _P, C.c_int32, _P,
                                        C.c_int32] + [C.c_int32] * 6 + [_P, C.c_uint64, C.c_int32, _P]),

@@ -146,6 +146,8 @@ add_rmsnorm_kernel(float* __restrict__ x, float* __restrict__ delta, const float
 // ------------------------------------------------------------------------------------------------
 constexpr int HD = 128, AT_THREADS = 256, MAXG = 8, AT_CAP = 64;   // AT_CAP * 4 == AT_THREADS
 constexpr int AT_SLOTS = 3;                                         // ring slots of attn_decode_cluster_kernel, one 64 x 128 fp32 matrix each
+// the q heads per kv head the attention kernels are instantiated for
+constexpr bool gqa_supported(int G) { return G == 1 || G == 2 || G == 3 || G == 4 || G == 6 || G == 8; }
 // Dynamic shared memory of attn_decode_cluster_kernel<G>: the ring (96 KB), q, the new k | v row, the peer's merged state, barriers.
 // 102 528 bytes at G = 3 and 107 648 at G = 8 (plus 512 static): one CTA fits beside a decode GEMM CTA (121 088) or a split-K CTA
 // (109 056) on an SM.  The 8 warp-partial outputs ([8][G][128] fp32) are written over ring slot 0 once the last chunk is consumed.
@@ -548,6 +550,13 @@ prefill_attn_kernel(PrefillAttnArgs a) {
         tc::store_hilo(a.out, ldo, tok, col + 3, o.w * inv, PF_HALF);
     }
 }
+
+// Dynamic shared memory of prefill_attn_kernel<G> for L prompt positions: the K and V rows of the whole prompt and one tile's queries.
+constexpr size_t PA_SMEM_MAX = 220 * 1024;
+constexpr size_t pattn_smem(int L, int G) { return ((size_t)2 * L * HD + (size_t)G * PA_QT * HD) * sizeof(float); }
+// The prompt attention for L positions at G q heads per kv head: the SIMT kernel while its K/V rows fit in shared memory (the outputs
+// of short prompts stay what they were), the wgmma kernel beyond.  The largest SIMT L is 128 for G <= 4, 124 for G = 6, 92 for G = 8.
+constexpr bool simt_prompt_attn(int L, int G) { return L <= PA_MAXL && pattn_smem(L, G) <= PA_SMEM_MAX; }
 
 // pfa::prompt_attn_kernel's operands for B rows of L positions (padded to Lp = a multiple of pfa::BQ) and their tensor maps;
 // grown, never shrunk.  run(): pack_prompt_kernel then prompt_attn_kernel, the attention of one layer.
@@ -1011,7 +1020,8 @@ struct b2a_tts {
         // it shares an SM with a GEMM CTA of the step (see tc::set_attributes)
         B2A_CUDA(cudaFuncSetAttribute(attn_decode_cluster_kernel<G>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
     }
-    void attn_launch(const AttnArgs& aa, int B, cudaStream_t s) {
+    // the decode-step attention for rows 0..B-1 (the caller has checked gqa_supported(nq / nkv))
+    static void attn_launch(const AttnArgs& aa, int B, cudaStream_t s) {
         const int G = aa.nq / aa.nkv;
         const size_t sm = attn_smem_bytes(G);
         const dim3 g3(aa.nkv, B, 2);
@@ -1037,7 +1047,7 @@ struct b2a_tts {
         {
             const int g = c.num_key_value_heads > 0 && c.num_attention_heads % c.num_key_value_heads == 0
                               ? c.num_attention_heads / c.num_key_value_heads : 0;
-            B2A_CHECK(g == 1 || g == 2 || g == 3 || g == 4 || g == 6 || g == 8, B2A_ERR_INVALID_INPUT,
+            B2A_CHECK(gqa_supported(g), B2A_ERR_INVALID_INPUT,
                       "llama: unsupported GQA ratio (q heads per kv head must be 1, 2, 3, 4, 6 or 8)");
         }
         B2A_CHECK(c.max_batch >= 1 && c.max_batch <= 8, B2A_ERR_INVALID_INPUT, "llama: max_batch must be in 1..8");
@@ -1337,17 +1347,26 @@ struct b2a_tts {
     }
     // logits are [8, V] row-major.
 
-    template <int G>
     static void pattn_attr() {
-        B2A_CUDA(cudaFuncSetAttribute(prefill_attn_kernel<G>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
+        for (auto k : {prefill_attn_kernel<1>, prefill_attn_kernel<2>, prefill_attn_kernel<3>, prefill_attn_kernel<4>,
+                       prefill_attn_kernel<6>, prefill_attn_kernel<8>})
+            B2A_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)PA_SMEM_MAX));
     }
-    size_t pattn_smem(int L) const {
-        const int G = cfg.num_attention_heads / cfg.num_key_value_heads;
-        return ((size_t)2 * L * HD + (size_t)G * PA_QT * HD) * sizeof(float);
+    // the SIMT prompt attention of B rows of pa.L positions (the caller has checked simt_prompt_attn(pa.L, G))
+    static void pattn_launch(const PrefillAttnArgs& pa, int B, cudaStream_t s) {
+        const int G = pa.nq / pa.nkv;
+        const dim3 grid(pa.nkv, B, cdiv(pa.L, PA_QT));
+        const size_t sm = pattn_smem(pa.L, G);
+        switch (G) {
+            case 1: prefill_attn_kernel<1><<<grid, PA_THREADS, sm, s>>>(pa); break;
+            case 2: prefill_attn_kernel<2><<<grid, PA_THREADS, sm, s>>>(pa); break;
+            case 3: prefill_attn_kernel<3><<<grid, PA_THREADS, sm, s>>>(pa); break;
+            case 4: prefill_attn_kernel<4><<<grid, PA_THREADS, sm, s>>>(pa); break;
+            case 6: prefill_attn_kernel<6><<<grid, PA_THREADS, sm, s>>>(pa); break;
+            default: prefill_attn_kernel<8><<<grid, PA_THREADS, sm, s>>>(pa); break;
+        }
+        count_launch();
     }
-    // the prompt attention for L positions: the SIMT kernel while its K/V rows fit in shared memory (the outputs of short prompts stay
-    // what they were), the wgmma kernel beyond
-    bool simt_prompt_attn(int L) const { return L <= PA_MAXL && pattn_smem(L) <= 220 * 1024; }
     // a stack whose inputs are embeddings (the Qwen3-TTS talker and code predictor) replays the decode step per prompt position
     bool can_batch_prefill(int L) const {
         return use_batched_prefill && spec.has_embed && L >= 2 && L <= cfg.max_context;
@@ -1380,10 +1399,10 @@ struct b2a_tts {
             tmp_xn = tc::make_tmap_bf16(xnp.p, 2 * Tp, H, 128);
             tmp_attn = tc::make_tmap_bf16(attnp.p, 2 * Tp, NQ, 128);
             tmp_act = tc::make_tmap_bf16(actp.p, 2 * Tp, I, 128);
-            pattn_attr<1>(); pattn_attr<2>(); pattn_attr<3>(); pattn_attr<4>(); pattn_attr<6>(); pattn_attr<8>();
+            pattn_attr();
         }
         rope_tab.alloc((size_t)cfg.max_context * (HD / 2));
-        const bool simt_attn = simt_prompt_attn(L);
+        const bool simt_attn = simt_prompt_attn(L, G);
         if (!simt_attn) pfa_ops.prepare(B, L, nq, nkv);
         // padding tokens of the last tile must read as zero (no kernel writes them): its hi rows T % 64 .. 63 and the lo rows below
         if (const int r0 = T % PF_HALF) {
@@ -1408,17 +1427,7 @@ struct b2a_tts {
             if (simt_attn) {
                 PrefillAttnArgs pa{qkvp.p, rope_tab.p, kcache.p + l * kv_layer, vcache.p + l * kv_layer, attnp.p, nq, nkv,
                                    cfg.max_context, L, 1.0f / sqrtf((float)HD), qn, kn, cfg.rms_norm_eps};
-                const dim3 grid(nkv, B, cdiv(L, PA_QT));
-                const size_t sm = pattn_smem(L);
-                switch (G) {
-                    case 1: prefill_attn_kernel<1><<<grid, PA_THREADS, sm, s>>>(pa); break;
-                    case 2: prefill_attn_kernel<2><<<grid, PA_THREADS, sm, s>>>(pa); break;
-                    case 3: prefill_attn_kernel<3><<<grid, PA_THREADS, sm, s>>>(pa); break;
-                    case 4: prefill_attn_kernel<4><<<grid, PA_THREADS, sm, s>>>(pa); break;
-                    case 6: prefill_attn_kernel<6><<<grid, PA_THREADS, sm, s>>>(pa); break;
-                    default: prefill_attn_kernel<8><<<grid, PA_THREADS, sm, s>>>(pa); break;
-                }
-                count_launch();
+                pattn_launch(pa, B, s);
             } else {
                 pfa_ops.run(qkvp.p, rope_tab.p, kcache.p + l * kv_layer, vcache.p + l * kv_layer, attnp.p, L, cfg.max_context, s, qn, kn,
                             cfg.rms_norm_eps);
@@ -1973,7 +1982,7 @@ int32_t b2a_tts_prepare_input_ids_ref(const int32_t* const* prompt_ids, const in
 
 int32_t b2a_debug_step_smem(int32_t gqa, int32_t* out) {
     return guarded([&] {
-        B2A_CHECK(out && (gqa == 1 || gqa == 2 || gqa == 3 || gqa == 4 || gqa == 6 || gqa == 8), B2A_ERR_INVALID_INPUT,
+        B2A_CHECK(out && gqa_supported(gqa), B2A_ERR_INVALID_INPUT,
                   "b2a_debug_step_smem: q heads per kv head must be 1, 2, 3, 4, 6 or 8");
         out[0] = (int32_t)tc::Smem<16>::bytes(b2a_tts::gemm_stages);
         out[1] = (int32_t)tc::SmemSplit::bytes(b2a_tts::splitk_stages, b2a_tts::fused_cluster);
@@ -1996,22 +2005,54 @@ int32_t b2a_debug_qkv_split(int32_t m_tiles, int32_t k_blocks, int32_t* out) {
     });
 }
 
-// The long-prompt attention on its own (include/b200audio_internal.h): rope_table_kernel + pack_prompt_kernel + prompt_attn_kernel,
-// as prefill_batched runs them for one layer, on DEVICE buffers the caller owns.
-int32_t b2a_prompt_attn_test(const float* qkv, const float* freqs, float* kcache, float* vcache, void* out, int32_t B, int32_t L,
-                             int32_t nq, int32_t nkv, int32_t max_ctx, void* stream) {
+// The decode-step attention on its own (include/b200audio_internal.h): attn_decode_cluster_kernel<G> with the step's launch
+// (b2a_tts::attn_launch), on DEVICE buffers the caller owns.
+int32_t b2a_decode_attn_test(const float* qkv, const int32_t* pos, const float* freqs, const float* qnorm, const float* knorm, float qk_eps,
+                             float* kcache, float* vcache, void* out, int32_t B, int32_t nq, int32_t nkv, int32_t max_ctx, void* stream) {
     return guarded([&] {
-        B2A_CHECK(qkv && freqs && kcache && vcache && out && B >= 1 && L >= 1 && L <= max_ctx && nkv >= 1 && nq >= nkv && nq % nkv == 0,
+        B2A_CHECK(qkv && pos && freqs && kcache && vcache && out && B >= 1 && B <= 8 && max_ctx >= 1 && !qnorm == !knorm,
+                  B2A_ERR_INVALID_INPUT, "b2a_decode_attn_test: bad argument");
+        B2A_CHECK(nkv >= 1 && nq % nkv == 0 && gqa_supported(nq / nkv), B2A_ERR_INVALID_INPUT,
+                  "b2a_decode_attn_test: q heads per kv head must be 1, 2, 3, 4, 6 or 8");
+        require_device(0);
+        b2a_tts::attn_cluster_attr<1>(); b2a_tts::attn_cluster_attr<2>(); b2a_tts::attn_cluster_attr<3>();
+        b2a_tts::attn_cluster_attr<4>(); b2a_tts::attn_cluster_attr<6>(); b2a_tts::attn_cluster_attr<8>();
+        const cudaStream_t s = (cudaStream_t)stream;
+        const AttnArgs aa{qkv, pos, freqs, kcache, vcache, (bf16*)out, nq, nkv, max_ctx, 1.0f / sqrtf((float)HD), qnorm, knorm, qk_eps};
+        b2a_tts::attn_launch(aa, B, s);
+        B2A_CUDA(cudaGetLastError());
+        B2A_CUDA(cudaStreamSynchronize(s));
+    });
+}
+
+// The prompt attention on its own (include/b200audio_internal.h): rope_table_kernel, then path 1 prefill_attn_kernel<G> or path 2
+// pack_prompt_kernel + prompt_attn_kernel, as prefill_batched runs them for one layer, on DEVICE buffers the caller owns.
+int32_t b2a_prompt_attn_test(const float* qkv, const float* freqs, const float* qnorm, const float* knorm, float qk_eps, float* kcache,
+                             float* vcache, void* out, int32_t B, int32_t L, int32_t nq, int32_t nkv, int32_t max_ctx, int32_t path,
+                             void* stream) {
+    return guarded([&] {
+        B2A_CHECK(qkv && freqs && kcache && vcache && out && B >= 1 && L >= 1 && L <= max_ctx && !qnorm == !knorm && (path == 1 || path == 2),
                   B2A_ERR_INVALID_INPUT, "b2a_prompt_attn_test: bad argument");
+        B2A_CHECK(nkv >= 1 && nq % nkv == 0 && gqa_supported(nq / nkv), B2A_ERR_INVALID_INPUT,
+                  "b2a_prompt_attn_test: q heads per kv head must be 1, 2, 3, 4, 6 or 8");
+        B2A_CHECK(path == 2 || simt_prompt_attn(L, nq / nkv), B2A_ERR_INVALID_INPUT,
+                  "b2a_prompt_attn_test: L too long for the SIMT prompt attention at this GQA ratio");
         require_device(0);
         const cudaStream_t s = (cudaStream_t)stream;
         DBuf<float2> rope;
         rope.alloc((size_t)L * (HD / 2));
         rope_table_kernel<<<cdiv(L * (HD / 2), 256), 256, 0, s>>>(freqs, rope.p, L);
         count_launch();
-        PromptAttnOps ops;
-        ops.prepare(B, L, nq, nkv);
-        ops.run(qkv, rope.p, kcache, vcache, (bf16*)out, L, max_ctx, s);
+        PromptAttnOps ops;                          // its buffers outlive the launches (freed after the synchronise)
+        if (path == 1) {
+            b2a_tts::pattn_attr();
+            const PrefillAttnArgs pa{qkv, rope.p, kcache, vcache, (bf16*)out, nq, nkv, max_ctx, L, 1.0f / sqrtf((float)HD), qnorm, knorm,
+                                     qk_eps};
+            b2a_tts::pattn_launch(pa, B, s);
+        } else {
+            ops.prepare(B, L, nq, nkv);
+            ops.run(qkv, rope.p, kcache, vcache, (bf16*)out, L, max_ctx, s, qnorm, knorm, qk_eps);
+        }
         B2A_CUDA(cudaGetLastError());
         B2A_CUDA(cudaStreamSynchronize(s));
     });
