@@ -199,7 +199,7 @@ typedef struct b2a_llama_config {
     float rope_high_freq_factor;
     float rope_old_context_len;
     int32_t tie_word_embeddings;
-    int32_t max_batch;   /* KV-cache rows */
+    int32_t max_batch;   /* KV-cache rows, 1..32 (other values: B2A_ERR_INVALID_INPUT) */
     int32_t max_context; /* KV-cache positions per row */
 } b2a_llama_config;
 
@@ -305,7 +305,7 @@ typedef struct b2a_qwen3_lm_config {     /* Qwen3Configuration, Config.swift:15-
     int32_t max_position_embeddings;   /* default 32768 (informational) */
     int32_t sample_rate;       /* default 24000 */
     int32_t eos_token_id;      /* default 151645 (informational: generation stops on end-of-speech 151671) */
-    int32_t max_batch;         /* KV-cache rows */
+    int32_t max_batch;         /* KV-cache rows, 1..32 */
     int32_t max_context;       /* KV-cache positions per row */
 } b2a_qwen3_lm_config;
 
@@ -368,7 +368,7 @@ typedef struct b2a_soprano_config {     /* SopranoConfiguration, SopranoConfig.s
     int32_t dw_kernel;               /* 3 */
     int32_t token_size;              /* 2048 */
     int32_t receptive_field;         /* 4 (informational: audio is decoded once per call) */
-    int32_t max_batch;               /* KV-cache rows */
+    int32_t max_batch;               /* KV-cache rows, 1..32 */
     int32_t max_context;             /* KV-cache positions per row */
 } b2a_soprano_config;
 
@@ -763,7 +763,7 @@ typedef struct b2a_qwen3_talker_config {
     int32_t cp_head_dim;
     float cp_rms_norm_eps;
     float cp_rope_theta;
-    int32_t max_batch;             /* <= 8 utterances per call */
+    int32_t max_batch;             /* 1..32 utterances per call */
     int32_t max_context;           /* prompt embeddings + frames per utterance */
 } b2a_qwen3_talker_config;
 

@@ -45,6 +45,10 @@ int32_t b2a_tts_debug_trace(b2a_tts* h, int32_t enable, int32_t batch, float* ou
  * q heads per kv head (1, 2, 3, 4, 6 or 8; its 512 static bytes are not included).  tests/test_gpu_step_coresidency.py checks
  * that neighbouring kernels of the step fit on one SM together.                                                              */
 int32_t b2a_debug_step_smem(int32_t gqa, int32_t* out);
+/* Host-only: the same for a call of `rows` rows (1..32), which runs the step at width R = 8, 16 or 32 -- out[0] R, out[1] the decode
+ * GEMM's ring depth, out[2] its bytes (tc_gemm_kernel<2R>), out[3] the split-K ring depth, out[4] its bytes (clusters of 5),
+ * out[5] the attention kernel's.  DESIGN.md section 3.3 states these values.                                                   */
+int32_t b2a_debug_step_smem_rows(int32_t rows, int32_t gqa, int32_t* out);
 
 /* Host-only (no device needed): the GEMM weight matrix the implicit convolution reads for an MLX-layout [out, k, in] weight --
  * stride 0: causal conv, rows = out, taps = k; stride > 0: transposed conv with k = n * stride, rows = stride * out

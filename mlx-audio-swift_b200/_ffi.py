@@ -216,6 +216,7 @@ SIGNATURES = {
     "b2a_tts_create": (C.c_int32, [C.c_int32, C.POINTER(LlamaConfig), C.POINTER(Tensor), C.c_int32, _P, C.POINTER(_P)]),
     "b2a_tts_debug_trace": (C.c_int32, [_P, C.c_int32, C.c_int32, _P]),
     "b2a_debug_step_smem": (C.c_int32, [C.c_int32, C.POINTER(C.c_int32)]),
+    "b2a_debug_step_smem_rows": (C.c_int32, [C.c_int32, C.c_int32, C.POINTER(C.c_int32)]),
     "b2a_tts_create_random": (C.c_int32, [C.c_int32, C.POINTER(LlamaConfig), C.c_float, C.c_uint64, _P, C.POINTER(_P)]),
     "b2a_tts_stream": (C.c_void_p, [_P]),
     "b2a_tts_set_bench_flags": (C.c_int32, [_P, C.c_int32, C.c_int32]),

@@ -8,7 +8,7 @@
 //
 // HBM layout: weights bf16 [out, in] row-major (q|k|v fused into one matrix, gate/up row-
 // interleaved so SwiGLU is a GEMM epilogue); KV cache fp32 [layer][B][kv_head][ctx][128];
-// residual stream fp32 [B, H]; GEMM inputs bf16 hi/lo pairs [16, K] (LO_ROW).
+// residual stream fp32 [B, H]; GEMM inputs bf16 hi/lo pairs [2R, K] at the step's width R (tc::decode_width).
 // The whole decode step (embed -> 28 layers -> lm head -> logits processors -> sampler ->
 // bookkeeping) is captured in one CUDA graph and replayed per token; nothing syncs with the
 // host inside the loop except a poll of the "all rows finished" flag every few steps.
@@ -75,11 +75,11 @@ __global__ void ext_embed_kernel(const float* __restrict__ src, float* __restric
 }
 
 // fused-norm step: the fp32 normalised hidden state  out[b, :] = x[b, :] * rstd[b] * w  from the partial sums of squares.
-// slot == null (row N1): out is [8, H].  slot != null (Soprano's capture, out [B, slots, H]): row b writes slot k = slot[b] (its n_gen:
+// ss is [parts, ss_ld] (ss_ld: the step's width).  slot == null (row N1): out is [B, H].  slot != null (Soprano's capture, out [B, slots, H]): row b writes slot k = slot[b] (its n_gen:
 // the state of generated token k, or of the last prompt position for k = 0) only while n_cap[b] == k, then n_cap[b] = k + 1.  A stop
 // token leaves n_gen unchanged, so the step that feeds it finds the slot taken and writes nothing; read on the device, the graph replays.
 __global__ void finalize_norm_kernel(const float* __restrict__ x, const float* __restrict__ w, const float* __restrict__ ss, int parts,
-                                     float* __restrict__ out, int H, float eps, const int* __restrict__ slot, int* n_cap, int slots) {
+                                     float* __restrict__ out, int H, float eps, const int* __restrict__ slot, int* n_cap, int slots, int ss_ld) {
     const int b = blockIdx.x;
     pdl_trigger();
     pdl_wait();
@@ -93,12 +93,10 @@ __global__ void finalize_norm_kernel(const float* __restrict__ x, const float* _
         o = ((long long)b * slots + k) * H;
     }
     float t = 0.f;
-    for (int p = 0; p < parts; ++p) t += ss[p * 8 + b];
+    for (int p = 0; p < parts; ++p) t += ss[p * ss_ld + b];
     const float r = rsqrtf(t / (float)H + eps);
     for (int i = threadIdx.x; i < H; i += blockDim.x) out[o + i] = x[(long long)b * H + i] * r * w[i];
 }
-
-constexpr int LO_ROW = 8;   // activation matrices are [16, K] bf16: row b = hi(x_b), row 8 + b = lo(x_b) = bf16(x_b - hi)
 
 // x += delta (optional, delta is zeroed afterwards);  xn = hi/lo split of  x * rsqrt(mean(x^2) + eps) * w
 // One 1024-thread CTA per row, the row lives in registers (H <= 8192).
@@ -130,10 +128,11 @@ add_rmsnorm_kernel(float* __restrict__ x, float* __restrict__ delta, const float
     float tot = 0.f;
 #pragma unroll
     for (int i = 0; i < RN_THREADS / 32; ++i) tot += red[i];
-    // ss_out != null ("raw" mode, fused-norm decode step): xn = hi/lo of x * w UN-normalised, the row's sum of squares goes to
-    // ss_out[0, b] (parts 1.. are cleared): the consumer GEMM applies rstd in its epilogue (tc_gemm.cuh, Args::rstd_ss)
+    // ss_out != null ("raw" mode, fused-norm decode step, half = the step's width): xn = hi/lo of x * w UN-normalised, the row's sum
+    // of squares goes to ss_out[0, b] of the [ss_parts, half] array (parts 1.. are cleared): the consumer GEMM applies rstd in its
+    // epilogue (tc_gemm.cuh, Args::rstd_ss)
     const float r = ss_out ? 1.0f : rsqrtf(tot / (float)H + eps);
-    if (ss_out && tid < ss_parts) ss_out[tid * 8 + b] = tid == 0 ? tot : 0.f;
+    if (ss_out && tid < ss_parts) ss_out[tid * half + b] = tid == 0 ? tot : 0.f;
 #pragma unroll
     for (int j = 0; j < RN_MAXV; ++j) {
         const int i = tid + j * RN_THREADS;
@@ -162,12 +161,13 @@ struct AttnArgs {
     const float* freqs;    // [64] llama3 rope divisors
     float* kcache;         // this layer: [B][nkv][max_ctx][128] fp32
     float* vcache;
-    bf16* out;             // [16, nq*128] hi/lo
+    bf16* out;             // [2 lo, nq*128] hi/lo
     int nq, nkv, max_ctx;
     float scale;
     const float* qnorm;    // nullable [128]: per-head RMSNorm gain applied to every q head BEFORE RoPE (Qwen3TTSTalker.swift:127-186)
     const float* knorm;    // nullable [128]: same for the k head
     float qk_eps;
+    int lo;                // the step's width (tc::decode_width): row b's lo half is row lo + b of out
 };
 
 // One thread-block cluster of two CTAs per (kv head, row), grid (kv heads, rows, 2).  Keys 0..pos are cut into 64-key chunks
@@ -394,7 +394,7 @@ attn_decode_cluster_kernel(const __grid_constant__ AttnArgs a) {
             const float M = fmaxf(Ms[g], M1);
             const float w0 = Ms[g] == -INFINITY ? 0.f : __expf(Ms[g] - M), w1 = M1 == -INFINITY ? 0.f : __expf(M1 - M);
             const float L = Ls[g] * w0 + L1 * w1, O = Os[g] * w0 + O1 * w1;
-            tc::store_hilo(a.out, (long long)a.nq * HD, b, (h * G + g) * HD + tid, O / L, LO_ROW);
+            tc::store_hilo(a.out, (long long)a.nq * HD, b, (h * G + g) * HD + tid, O / L, a.lo);
         }
     }
 }
@@ -926,7 +926,7 @@ struct b2a_tts {
     const bf16* lm_head = nullptr;
     DBuf<float> final_ln, freqs;
     DBuf<float> kcache, vcache;   // [layer][B][nkv][ctx][hd] fp32
-    // activations: fp32 residual stream; GEMM inputs as [16, K] bf16 hi/lo pairs
+    // activations: fp32 residual stream [max_batch, H]; GEMM inputs as [2R, K] bf16 hi/lo pairs, R the call's width
     DBuf<float> x, y, qkv, logits, probs;
     DBuf<bf16> xn, attn, act;
     DBuf<float> sk_ws;       // stream-K partial tiles of the q|k|v GEMM when it runs stream-K (qkv_cluster == 0), see tc::Args::part_ws
@@ -942,7 +942,8 @@ struct b2a_tts {
     int lm_tile_rows = 128, head_rows_now = 0;   // head_rows_now: tile rows of the map passed to the current OP_LM launch (0 = lm_tile_rows)
     std::vector<CUtensorMap> tm_gu_dec;     // gate/up with gu_tile_rows-row boxes for the decode step (tc::Args::tile_rows)
     int gu_tile_rows = 0;
-    CUtensorMap tm_lm{}, tmx_xn{}, tmx_attn{}, tmx_act{};
+    CUtensorMap tm_lm{};
+    CUtensorMap tmx_xn[3]{}, tmx_attn[3]{}, tmx_act[3]{};   // per width (tc::decode_width_index): [2R, K] with 2R-row boxes
     // batched prefill workspace (sized for the largest B*L seen so far)
     DBuf<float> xp, yp, qkvp;
     DBuf<bf16> xnp, attnp, actp;
@@ -958,23 +959,26 @@ struct b2a_tts {
     // norm's gain + hi/lo split + sum of squares; one add_rmsnorm launch per step, for the first norm (tc_gemm.cuh).  q|k|v runs on
     // the same kernel in store mode (qkv_gemm)
     static constexpr int fused_cluster = 5;   // 5 CTAs per 128-row tile: 120 of 132 SMs for hidden 3072, one wave
-    int qkv_cluster = 0;                      // CTAs per 128-row tile of the q|k|v split-K GEMM (pick_qkv_cluster); 0: stream-K
-    int qkv_sk_ctas = 0;                      // the stream-K CTA count whose cut of the k-blocks that GEMM reproduces
-    // ring depths of the decode step's GEMMs.  With them tc::Smem<16>::bytes, tc::SmemSplit::bytes and attn_smem_bytes() are sized so
-    // that any two kernels that follow each other in the fused step fit on one SM together (b2a_debug_step_smem reports the three)
-    static constexpr int gemm_stages = 6, splitk_stages = 5;
+    int qkv_cluster[3] = {0, 0, 0};           // per width: CTAs per 128-row tile of the q|k|v split-K GEMM (pick_qkv_cluster); 0: stream-K
+    int qkv_sk_ctas = 0;                      // the stream-K CTA count whose cut of the k-blocks that GEMM reproduces (any width)
+    // ring depths of the decode step's GEMMs per width (8, 16, 32 rows).  At 8 rows tc::Smem<16>::bytes, tc::SmemSplit<8>::bytes and
+    // attn_smem_bytes() are sized so that any two kernels that follow each other in the fused step fit on one SM together
+    // (b2a_debug_step_smem reports the three); DESIGN.md section 3.3 gives the wider widths' choice (b2a_debug_step_smem_rows)
+    static constexpr int GEMM_STAGES[3] = {6, 4, 3}, SPLITK_STAGES[3] = {5, 4, 2};
+    int width = 8, wi = 0;           // the current call's width R (tc::decode_width of its rows) and its index
+    int max_width = 8;               // the width of max_batch rows: activation buffers hold [2 max_width, K]
     int fused_parts = 0;             // m-tiles of H (the last one may be partly filled): partial sums of squares per row
-    DBuf<float> ss_a, ss_b;          // [fused_parts <= 64, 8] partial sums of squares: ss_a feeds the post-attention norm, ss_b the input norm
+    DBuf<float> ss_a, ss_b;          // [fused_parts <= 64, R] partial sums of squares: ss_a feeds the post-attention norm, ss_b the input norm
     StackSpec spec;                  // which keys / features this stack was built with
     TokenLayout tok = ORPHEUS_TOKENS;  // special tokens, parse rule and decode chunking of generate (VYVO_TOKENS: b2a_qwen3_lm_create)
-    const float* x_ext = nullptr;    // row N1: when set, a step starts from these embeddings [8, H] instead of embed(tokens)
-    float* normed_out = nullptr;     // row N1: when set, run_final_norm writes the final RMSNorm's fp32 output here [8, H]
+    const float* x_ext = nullptr;    // row N1: when set, a step starts from these embeddings [max_batch, H] instead of embed(tokens)
+    float* normed_out = nullptr;     // row N1: when set, run_final_norm writes the final RMSNorm's fp32 output here [max_batch, H]
     std::atomic<int> cancel{0};
     int bench_mask_eos = 0, bench_wrap_codes = 0;   // b2a_tts_set_bench_flags (include/b200audio_internal.h): fixed-work benchmark switches
-    int nb_pad = 0;   // rows rounded up to 1/2/4/8
+    int nb_pad = 0;   // rows rounded up to 1/2/4/8 within width 8, else the width
     bool trace_on = false;       // debug: residual stream at every RMSNorm input (eager forward only, trace_x)
-    DBuf<float> trace;           // [2*layers + 1][8][H]
-    // CUDA graphs for the two step flavours (captured per (nb_pad, params) configuration)
+    DBuf<float> trace;           // [2*layers + 1][max_batch][H]
+    // CUDA graphs for the two step flavours (captured per (rows, params) configuration)
     cudaGraphExec_t g_step = nullptr, g_prefill = nullptr;
     SampleArgs g_args{};
     int g_nb = 0;
@@ -1050,7 +1054,7 @@ struct b2a_tts {
             B2A_CHECK(gqa_supported(g), B2A_ERR_INVALID_INPUT,
                       "llama: unsupported GQA ratio (q heads per kv head must be 1, 2, 3, 4, 6 or 8)");
         }
-        B2A_CHECK(c.max_batch >= 1 && c.max_batch <= 8, B2A_ERR_INVALID_INPUT, "llama: max_batch must be in 1..8");
+        B2A_CHECK(c.max_batch >= 1 && c.max_batch <= 32, B2A_ERR_INVALID_INPUT, "llama: max_batch must be in 1..32");
         B2A_CHECK(c.max_context >= 8, B2A_ERR_INVALID_INPUT, "llama: max_context too small");
         require_device(device);
         B2A_CUDA(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
@@ -1067,7 +1071,8 @@ struct b2a_tts {
         vcache.alloc(kv);
         B2A_CUDA(cudaMemset(kcache.p, 0, kv * sizeof(float)));
         B2A_CUDA(cudaMemset(vcache.p, 0, kv * sizeof(float)));
-        const int B = 8, R16 = 16;
+        max_width = tc::decode_width(c.max_batch);
+        const int B = std::max(8, c.max_batch), R16 = 2 * max_width;
         x.alloc((size_t)B * H); y.alloc((size_t)B * H); qkv.alloc((size_t)B * (NQ + 2 * NKV));
         logits.alloc((size_t)B * c.vocab_size); probs.alloc((size_t)B * c.vocab_size);
         xn.alloc((size_t)R16 * H); attn.alloc((size_t)R16 * NQ); act.alloc((size_t)R16 * I);
@@ -1086,20 +1091,11 @@ struct b2a_tts {
         attn_cluster_attr<1>(); attn_cluster_attr<2>(); attn_cluster_attr<3>(); attn_cluster_attr<4>(); attn_cluster_attr<6>(); attn_cluster_attr<8>();
         tc::set_attributes();
         fused_parts = cdiv(H, tc::BM);          // <= 64: H <= 8192 (check_config)
-        ss_a.alloc((size_t)64 * 8); ss_b.alloc((size_t)64 * 8);
-        B2A_CUDA(cudaMemset(ss_a.p, 0, 64 * 8 * sizeof(float)));
-        B2A_CUDA(cudaMemset(ss_b.p, 0, 64 * 8 * sizeof(float)));
+        ss_a.alloc((size_t)64 * max_width); ss_b.alloc((size_t)64 * max_width);
+        B2A_CUDA(cudaMemset(ss_a.p, 0, 64 * max_width * sizeof(float)));
+        B2A_CUDA(cudaMemset(ss_b.p, 0, 64 * max_width * sizeof(float)));
         B2A_CUDA(cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, device));
-        {   // q|k|v as clusters when they fit in one wave; otherwise the stream-K GEMM, with its workspace (BN = 16)
-            const int mt = cdiv(NQ + 2 * NKV, tc::BM), kb = H / tc::BK;
-            qkv_cluster = pick_qkv_cluster(mt, kb, num_sms, &qkv_sk_ctas);
-            if (qkv_cluster == 0) {
-                sk_slots = tc::stream_k_slots(mt, kb, qkv_sk_ctas);
-                sk_ws.alloc((size_t)mt * sk_slots * 16 * tc::BM);
-                sk_cnt.alloc(mt);
-                B2A_CUDA(cudaMemset(sk_cnt.p, 0, (size_t)mt * sizeof(unsigned)));
-            }
-        }
+        pick_qkv_clusters();
         const char* envp = getenv("B2A_PREFILL");
         use_batched_prefill = !(envp && std::string(envp) == "step");
         for (auto& L : layers) {
@@ -1115,9 +1111,12 @@ struct b2a_tts {
         }
         lm_tile_rows = pick_tile_rows(c.vocab_size, num_sms);
         if (lm_head) tm_lm = tc::make_tmap_bf16(lm_head, c.vocab_size, H, lm_tile_rows);
-        tmx_xn = tc::make_tmap_bf16(xn.p, R16, H, 16);
-        tmx_attn = tc::make_tmap_bf16(attn.p, R16, NQ, 16);
-        tmx_act = tc::make_tmap_bf16(act.p, R16, I, 16);
+        for (int w = 0; w < 3 && tc::DECODE_WIDTHS[w] <= max_width; ++w) {
+            const int rows = 2 * tc::DECODE_WIDTHS[w];
+            tmx_xn[w] = tc::make_tmap_bf16(xn.p, rows, H, rows);
+            tmx_attn[w] = tc::make_tmap_bf16(attn.p, rows, NQ, rows);
+            tmx_act[w] = tc::make_tmap_bf16(act.p, rows, I, rows);
+        }
         B2A_CUDA(cudaDeviceSynchronize());
     }
 
@@ -1219,8 +1218,26 @@ struct b2a_tts {
         alloc_state();
     }
 
+    int rows_cap() const { return std::max(8, cfg.max_batch); }   // rows of the per-row state buffers
+    // q|k|v as clusters when they fit in one wave at a width's footprint; otherwise the stream-K GEMM, with its workspace (slots of
+    // [2 max_width, 128])
+    void pick_qkv_clusters() {
+        const int mt = cdiv((cfg.num_attention_heads + 2 * cfg.num_key_value_heads) * HD, tc::BM), kb = cfg.hidden_size / tc::BK;
+        bool stream_k = false;
+        for (int w = 0; w < 3 && tc::DECODE_WIDTHS[w] <= max_width; ++w) {
+            qkv_cluster[w] = pick_qkv_cluster(mt, kb, num_sms, &qkv_sk_ctas, tc::DECODE_WIDTHS[w], SPLITK_STAGES[w]);
+            stream_k |= qkv_cluster[w] == 0;
+        }
+        if (stream_k && !sk_cnt.p) {
+            sk_slots = tc::stream_k_slots(mt, kb, qkv_sk_ctas);
+            sk_ws.alloc((size_t)mt * sk_slots * 2 * max_width * tc::BM);
+            sk_cnt.alloc(mt);
+            B2A_CUDA(cudaMemset(sk_cnt.p, 0, (size_t)mt * sizeof(unsigned)));
+        }
+    }
+
     enum { OP_QKV, OP_GU, OP_LM };
-    // D[tokens, M] = X[tokens, K] * W[M, K]^T on the wgmma path (hi/lo activations, BN = 16)
+    // D[tokens, M] = X[tokens, K] * W[M, K]^T on the wgmma path (hi/lo activations, BN = 2 width)
     void tc_gemm(const CUtensorMap& tmW, const CUtensorMap& tmX, int op, float* yout, bf16* actout, int B, int M, int K,
                  cudaStream_t s, const float* rstd_ss = nullptr, const float* bias = nullptr) {
         tc::Args a{};
@@ -1228,11 +1245,11 @@ struct b2a_tts {
         a.rstd_ss = rstd_ss; a.rstd_parts = fused_parts; a.rstd_inv_h = 1.0f / (float)cfg.hidden_size; a.rstd_eps = cfg.rms_norm_eps;
         a.out_f32 = yout; a.out_bf16 = actout; a.M = M; a.N = B; a.K = K;
         a.m_tiles = cdiv(M, tc::BM); a.k_blocks = K / tc::BK;
-        a.stages = gemm_stages;
+        a.stages = GEMM_STAGES[wi];
         a.hilo = 1;
         int ctas = num_sms;
         if (op == OP_GU) {
-            a.ldo = M / 2; a.epi_full = tc::EPI_SWIGLU; a.epi_partial = -1; a.lo_rows = LO_ROW;
+            a.ldo = M / 2; a.epi_full = tc::EPI_SWIGLU; a.epi_partial = -1; a.lo_rows = width;
             a.tile_rows = gu_tile_rows; a.m_tiles = cdiv(M, gu_tile_rows);      // tmW is tm_gu_dec[layer]
             ctas = std::min(num_sms, a.m_tiles);
         } else if (op == OP_LM) {
@@ -1244,38 +1261,56 @@ struct b2a_tts {
             ctas = (int)std::min<long long>(num_sms, (long long)a.m_tiles * a.k_blocks);
             a.part_ws = sk_ws.p; a.part_cnt = sk_cnt.p; a.part_slots = sk_slots;
         }
-        tc::launch<16>(tmW, tmX, a, ctas, 1, s);
+        if (width == 8) tc::launch<16>(tmW, tmX, a, ctas, 1, s);
+        else if (width == 16) tc::launch<32>(tmW, tmX, a, ctas, 1, s, true);
+        else tc::launch<64>(tmW, tmX, a, ctas, 1, s);
     }
 
     // o_proj / down_proj as a cluster split-K GEMM with the residual add and the next norm fused into the leader's epilogue
     void splitk_gemm(const CUtensorMap& tmW, const CUtensorMap& tmX, int M, int K, const float* gain, float* ss, int B, cudaStream_t s) {
         tc::SplitArgs a{};
-        a.M = M; a.N = B; a.K = K; a.k_blocks = K / tc::BK; a.stages = splitk_stages;
+        a.M = M; a.N = B; a.K = K; a.k_blocks = K / tc::BK; a.stages = SPLITK_STAGES[wi];
         a.h = x.p; a.gain = gain; a.xn = xn.p; a.ss = ss;
         a.rstd_ss = nullptr; a.rstd_parts = 0; a.rstd_inv_h = 0.f; a.rstd_eps = 0.f;
-        tc::launch_splitk(tmW, tmX, a, cdiv(M, tc::BM), std::max(1, std::min(fused_cluster, a.k_blocks)), s);
+        launch_splitk(tmW, tmX, a, cdiv(M, tc::BM), std::max(1, std::min(fused_cluster, a.k_blocks)), s);
+    }
+    void launch_splitk(const CUtensorMap& tmW, const CUtensorMap& tmX, const tc::SplitArgs& a, int m_tiles, int cluster, cudaStream_t s) {
+        if (width == 8) tc::launch_splitk<8>(tmW, tmX, a, m_tiles, cluster, s);
+        else if (width == 16) tc::launch_splitk<16>(tmW, tmX, a, m_tiles, cluster, s);
+        else tc::launch_splitk<32>(tmW, tmX, a, m_tiles, cluster, s);
     }
     // q|k|v projection of the fused step: q|k|v[t] = rstd[t] * Wqkv xn[t] (the input norm's scale from ss_b), stored, in clusters of
     // qkv_cluster CTAs that compute exactly what the stream-K GEMM computes (tc::SplitArgs::sk_ctas); that GEMM itself when the
     // clusters do not fit in one wave
     void qkv_gemm(int layer, int B, cudaStream_t s) {
         const int H = cfg.hidden_size, M = (cfg.num_attention_heads + 2 * cfg.num_key_value_heads) * HD;
-        if (qkv_cluster < 1) { tc_gemm(tm_qkv[layer], tmx_xn, OP_QKV, qkv.p, nullptr, B, M, H, s, ss_b.p); return; }
+        if (qkv_cluster[wi] < 1) { tc_gemm(tm_qkv[layer], tmx_xn[wi], OP_QKV, qkv.p, nullptr, B, M, H, s, ss_b.p); return; }
         tc::SplitArgs a{};
-        a.M = M; a.N = B; a.K = H; a.k_blocks = H / tc::BK; a.stages = splitk_stages; a.sk_ctas = qkv_sk_ctas;
+        a.M = M; a.N = B; a.K = H; a.k_blocks = H / tc::BK; a.stages = SPLITK_STAGES[wi]; a.sk_ctas = qkv_sk_ctas;
         a.out = qkv.p;
         a.rstd_ss = ss_b.p; a.rstd_parts = fused_parts; a.rstd_inv_h = 1.0f / (float)H; a.rstd_eps = cfg.rms_norm_eps;
-        tc::launch_splitk(tm_qkv[layer], tmx_xn, a, cdiv(M, tc::BM), qkv_cluster, s);
+        launch_splitk(tm_qkv[layer], tmx_xn[wi], a, cdiv(M, tc::BM), qkv_cluster[wi], s);
     }
     // The q|k|v split-K launch cuts each tile's k-blocks where the stream-K GEMM over *sk_ctas = min(SMs, units) CTAs cuts them (so
     // its output is bit-identical), one CTA per piece: the cluster size is the most pieces of any tile (tc::stream_k_slots).  It is
     // used when that is at most 8 and all m_tiles clusters are resident at once (cudaOccupancyMaxActiveClusters at the launch's own
-    // shared-memory footprint); 0 otherwise (the stream-K GEMM runs).  Needs tc::set_attributes().
-    static int pick_qkv_cluster(int m_tiles, int k_blocks, int sms, int* sk_ctas) {
+    // shared-memory footprint at this width and ring depth); 0 otherwise (the stream-K GEMM runs).  Needs tc::set_attributes().
+    static int pick_qkv_cluster(int m_tiles, int k_blocks, int sms, int* sk_ctas, int width = 8, int stages = SPLITK_STAGES[0]) {
         *sk_ctas = (int)std::min<long long>(sms, (long long)m_tiles * k_blocks);
         const int c = tc::stream_k_slots(m_tiles, k_blocks, *sk_ctas);
         if (c > tc::SPLIT_MAX_CLUSTER) return 0;
-        return m_tiles <= tc::splitk_active_clusters(c, tc::SmemSplit::bytes(splitk_stages, c)) ? c : 0;
+        return m_tiles <= splitk_active_clusters(width, c, splitk_bytes(width, stages, c)) ? c : 0;
+    }
+    static size_t splitk_bytes(int width, int stages, int cluster) {
+        return width == 8 ? tc::SmemSplit<8>::bytes(stages, cluster) : width == 16 ? tc::SmemSplit<16>::bytes(stages, cluster)
+                                                                                   : tc::SmemSplit<32>::bytes(stages, cluster);
+    }
+    static size_t gemm_bytes(int width, int stages) {
+        return width == 8 ? tc::Smem<16>::bytes(stages) : width == 16 ? tc::Smem<32>::bytes(stages) : tc::Smem<64>::bytes(stages);
+    }
+    static int splitk_active_clusters(int width, int cluster, size_t bytes) {
+        return width == 8 ? tc::splitk_active_clusters<8>(cluster, bytes) : width == 16 ? tc::splitk_active_clusters<16>(cluster, bytes)
+                                                                                        : tc::splitk_active_clusters<32>(cluster, bytes);
     }
     // The fused-norm step: embed -> raw norm -> L x [qkv gemm (rstd in the epilogue) -> attention -> o split-K (+ residual, norm 2)
     // -> gate/up gemm (rstd, SwiGLU) -> down split-K (+ residual, next layer's norm 1 / the final norm)].  Leaves the residual
@@ -1287,18 +1322,19 @@ struct b2a_tts {
         else launch_pdl(embed_kernel, dim3(B), dim3(256), 0, s, tokens.p, embed.p, x.p, y.p, H, cfg.vocab_size);
         trace_x(0, B, s);
         launch_pdl(add_rmsnorm_kernel, dim3(B), dim3(RN_THREADS), 0, s, x.p, (float*)nullptr, layers[0].ln1.p, xn.p, H, cfg.rms_norm_eps,
-                   LO_ROW, ss_b.p, fused_parts);
+                   width, ss_b.p, fused_parts);
         const size_t kv_layer = (size_t)cfg.max_batch * nkv * cfg.max_context * HD;
         for (int l = 0; l < L; ++l) {
             LayerW& Lw = layers[l];
             qkv_gemm(l, B, s);
             AttnArgs aa{qkv.p, pos.p, freqs.p, kcache.p + l * kv_layer, vcache.p + l * kv_layer, attn.p, nq, nkv, cfg.max_context,
-                        1.0f / sqrtf((float)HD), spec.qk_norm ? Lw.qnorm.p : nullptr, spec.qk_norm ? Lw.knorm.p : nullptr, cfg.rms_norm_eps};
+                        1.0f / sqrtf((float)HD), spec.qk_norm ? Lw.qnorm.p : nullptr, spec.qk_norm ? Lw.knorm.p : nullptr, cfg.rms_norm_eps,
+                        width};
             attn_launch(aa, B, s);
-            splitk_gemm(tm_o[l], tmx_attn, H, NQ, Lw.ln2.p, ss_a.p, B, s);
+            splitk_gemm(tm_o[l], tmx_attn[wi], H, NQ, Lw.ln2.p, ss_a.p, B, s);
             trace_x(2 * l + 1, B, s);
-            tc_gemm(tm_gu_dec[l], tmx_xn, OP_GU, nullptr, act.p, B, 2 * I, H, s, ss_a.p);
-            splitk_gemm(tm_down[l], tmx_act, H, I, l + 1 < L ? layers[l + 1].ln1.p : final_ln.p, ss_b.p, B, s);
+            tc_gemm(tm_gu_dec[l], tmx_xn[wi], OP_GU, nullptr, act.p, B, 2 * I, H, s, ss_a.p);
+            splitk_gemm(tm_down[l], tmx_act[wi], H, I, l + 1 < L ? layers[l + 1].ln1.p : final_ln.p, ss_b.p, B, s);
             trace_x(2 * l + 2, B, s);
         }
     }
@@ -1307,7 +1343,7 @@ struct b2a_tts {
     // for eager forwards (b2a_tts_forward_logits); tts_generate_impl turns it off before it captures its graphs
     void trace_x(int i, int B, cudaStream_t s) {
         if (trace_on)
-            B2A_CUDA(cudaMemcpyAsync(trace.p + (size_t)i * 8 * cfg.hidden_size, x.p, (size_t)B * cfg.hidden_size * sizeof(float),
+            B2A_CUDA(cudaMemcpyAsync(trace.p + (size_t)i * rows_cap() * cfg.hidden_size, x.p, (size_t)B * cfg.hidden_size * sizeof(float),
                                      cudaMemcpyDeviceToDevice, s));
     }
 
@@ -1315,37 +1351,37 @@ struct b2a_tts {
     void run_final_norm(int B, cudaStream_t s, bool capture) {
         if (normed_out)
             launch_pdl(finalize_norm_kernel, dim3(B), dim3(256), 0, s, (const float*)x.p, (const float*)final_ln.p, (const float*)ss_b.p, fused_parts,
-                       normed_out, cfg.hidden_size, cfg.rms_norm_eps, (const int*)nullptr, (int*)nullptr, 0);
+                       normed_out, cfg.hidden_size, cfg.rms_norm_eps, (const int*)nullptr, (int*)nullptr, 0, width);
         if (capture)
             launch_pdl(finalize_norm_kernel, dim3(B), dim3(256), 0, s, (const float*)x.p, (const float*)final_ln.p, (const float*)ss_b.p, fused_parts,
-                       hidden.p, cfg.hidden_size, cfg.rms_norm_eps, (const int*)n_gen.p, n_cap.p, hidden_slots);
+                       hidden.p, cfg.hidden_size, cfg.rms_norm_eps, (const int*)n_gen.p, n_cap.p, hidden_slots, width);
     }
     // capture: Soprano's generate (hidden states into `hidden`); forward_logits never captures
     void run_lm_head(int B, cudaStream_t s, bool capture = false) {
         run_final_norm(B, s, capture);
-        tc_gemm(tm_lm, tmx_xn, OP_LM, logits.p, nullptr, B, cfg.vocab_size, cfg.hidden_size, s, ss_b.p);
+        tc_gemm(tm_lm, tmx_xn[wi], OP_LM, logits.p, nullptr, B, cfg.vocab_size, cfg.hidden_size, s, ss_b.p);
     }
     // after prefill_batched's gather_last (x, y hold the last position un-added): the stand-alone norm + plain GEMM.  Soprano runs the
     // decode step's tail instead (raw norm, then capture + GEMM with rstd), so slot 0 is computed as every later slot is.
     void run_lm_head_after_prefill(int B, cudaStream_t s) {
         if (vocos) {
             launch_pdl(add_rmsnorm_kernel, dim3(B), dim3(RN_THREADS), 0, s, x.p, y.p, final_ln.p, xn.p, cfg.hidden_size, cfg.rms_norm_eps,
-                       LO_ROW, ss_b.p, fused_parts);
+                       width, ss_b.p, fused_parts);
             run_lm_head(B, s, true);
             return;
         }
         launch_pdl(add_rmsnorm_kernel, dim3(B), dim3(RN_THREADS), 0, s, x.p, y.p, final_ln.p, xn.p, cfg.hidden_size, cfg.rms_norm_eps,
-                   LO_ROW, (float*)nullptr, 0);
-        tc_gemm(tm_lm, tmx_xn, OP_LM, logits.p, nullptr, B, cfg.vocab_size, cfg.hidden_size, s);
+                   width, (float*)nullptr, 0);
+        tc_gemm(tm_lm, tmx_xn[wi], OP_LM, logits.p, nullptr, B, cfg.vocab_size, cfg.hidden_size, s);
     }
     // a head the caller owns (row N1: the code predictor's 15 lm heads, and the talker's small_to_mtp_projection with its bias):
     // logits_out[b, :M] = W[M, H] * normed hidden (+ bias), tmW a map of W
     void run_head(const CUtensorMap& tmW, int M, float* logits_out, int B, cudaStream_t s, int tile_rows = 0, const float* bias = nullptr) {
         head_rows_now = tile_rows;              // tmW's box rows (0: this stack's own lm_tile_rows)
-        tc_gemm(tmW, tmx_xn, OP_LM, logits_out, nullptr, B, M, cfg.hidden_size, s, ss_b.p, bias);
+        tc_gemm(tmW, tmx_xn[wi], OP_LM, logits_out, nullptr, B, M, cfg.hidden_size, s, ss_b.p, bias);
         head_rows_now = 0;
     }
-    // logits are [8, V] row-major.
+    // logits are [max_batch, V] row-major.
 
     static void pattn_attr() {
         for (auto k : {prefill_attn_kernel<1>, prefill_attn_kernel<2>, prefill_attn_kernel<3>, prefill_attn_kernel<4>,
@@ -1443,8 +1479,11 @@ struct b2a_tts {
         B2A_CUDA(cudaGetLastError());
     }
 
+    // a call of B rows runs the step at width tc::decode_width(B): 8, 16 or 32 token rows per GEMM tile
     void set_batch(int B) {
-        nb_pad = B <= 1 ? 1 : B <= 2 ? 2 : B <= 4 ? 4 : 8;
+        width = tc::decode_width(B);
+        wi = tc::decode_width_index(width);
+        nb_pad = B <= 1 ? 1 : B <= 2 ? 2 : B <= 4 ? 4 : width;
     }
 
     void drop_graphs() {
@@ -1603,7 +1642,7 @@ static void tts_generate_impl(b2a_tts* h, const int32_t* input_ids, bool ids_on_
     const int MT = gp->max_tokens, R = std::max(1, gp->repetition_context_size);
     h->ids.alloc((size_t)B * L);
     h->out_tokens.alloc((size_t)B * MT);
-    h->recent.alloc((size_t)8 * R);
+    h->recent.alloc((size_t)h->rows_cap() * R);
     B2A_CUDA(cudaMemcpyAsync(h->ids.p, input_ids, (size_t)B * L * sizeof(int),
                              ids_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, s));
     SampleArgs sa{};
@@ -1618,7 +1657,7 @@ static void tts_generate_impl(b2a_tts* h, const int32_t* input_ids, bool ids_on_
     if (soprano) {
         h->hidden_slots = MT + 1; h->hidden_rows = B;
         h->hidden.alloc((size_t)B * h->hidden_slots * h->cfg.hidden_size);
-        h->n_cap.alloc(8);
+        h->n_cap.alloc(h->rows_cap());
     }
     h->capture(B, sa, L);
 
@@ -1627,7 +1666,7 @@ static void tts_generate_impl(b2a_tts* h, const int32_t* input_ids, bool ids_on_
     init_rows_kernel<<<1, 32, 0, s>>>(h->ids.p, L, B, gp->repetition_context_size > 0 && !soprano ? R : 0, h->tokens.p, h->pos.p, h->recent.p,
                                       h->recent_n.p, h->n_gen.p, h->done.p, h->n_active.p, 0);
     count_launch();
-    if (soprano) B2A_CUDA(cudaMemsetAsync(h->n_cap.p, 0, 8 * sizeof(int), s));
+    if (soprano) B2A_CUDA(cudaMemsetAsync(h->n_cap.p, 0, h->rows_cap() * sizeof(int), s));
     // prefill.  Batched: every prompt token through each layer at once (wgmma GEMMs, 64 tokens per tile), then
     // lm head + sampler on the last position.  Fallback (B2A_PREFILL=step, q/k norm): replay the decode
     // step per position -- positions 0..L-2 need no logits, position L-1 runs the full step.
@@ -1935,7 +1974,7 @@ int32_t b2a_tts_time_steps(b2a_tts* h, int32_t B, int32_t ctx, int32_t iters, fl
         const int MT = iters + 8;
         h->ids.alloc((size_t)B * 1);
         h->out_tokens.alloc((size_t)B * MT);
-        h->recent.alloc(8);
+        h->recent.alloc(h->rows_cap());
         SampleArgs sa{};
         sa.logits = h->logits.p; sa.probs = h->probs.p; sa.tokens = h->tokens.p; sa.pos = h->pos.p; sa.recent = h->recent.p;
         sa.recent_n = h->recent_n.p; sa.out_tokens = h->out_tokens.p; sa.n_gen = h->n_gen.p; sa.done = h->done.p;
@@ -1984,9 +2023,23 @@ int32_t b2a_debug_step_smem(int32_t gqa, int32_t* out) {
     return guarded([&] {
         B2A_CHECK(out && gqa_supported(gqa), B2A_ERR_INVALID_INPUT,
                   "b2a_debug_step_smem: q heads per kv head must be 1, 2, 3, 4, 6 or 8");
-        out[0] = (int32_t)tc::Smem<16>::bytes(b2a_tts::gemm_stages);
-        out[1] = (int32_t)tc::SmemSplit::bytes(b2a_tts::splitk_stages, b2a_tts::fused_cluster);
+        out[0] = (int32_t)tc::Smem<16>::bytes(b2a_tts::GEMM_STAGES[0]);
+        out[1] = (int32_t)tc::SmemSplit<8>::bytes(b2a_tts::SPLITK_STAGES[0], b2a_tts::fused_cluster);
         out[2] = (int32_t)attn_smem_bytes(gqa);
+    });
+}
+
+int32_t b2a_debug_step_smem_rows(int32_t rows, int32_t gqa, int32_t* out) {
+    return guarded([&] {
+        B2A_CHECK(out && rows >= 1 && rows <= 32 && gqa_supported(gqa), B2A_ERR_INVALID_INPUT,
+                  "b2a_debug_step_smem_rows: rows must be in 1..32 and q heads per kv head 1, 2, 3, 4, 6 or 8");
+        const int w = tc::decode_width(rows), wi = tc::decode_width_index(w);
+        out[0] = w;
+        out[1] = b2a_tts::GEMM_STAGES[wi];
+        out[2] = (int32_t)b2a_tts::gemm_bytes(w, b2a_tts::GEMM_STAGES[wi]);
+        out[3] = b2a_tts::SPLITK_STAGES[wi];
+        out[4] = (int32_t)b2a_tts::splitk_bytes(w, b2a_tts::SPLITK_STAGES[wi], b2a_tts::fused_cluster);
+        out[5] = (int32_t)attn_smem_bytes(gqa);
     });
 }
 
@@ -1998,8 +2051,8 @@ int32_t b2a_debug_qkv_split(int32_t m_tiles, int32_t k_blocks, int32_t* out) {
         int sms = 0, sk_ctas = 0;
         B2A_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0));
         out[0] = b2a_tts::pick_qkv_cluster(m_tiles, k_blocks, sms, &sk_ctas);
-        out[1] = out[0] ? (int32_t)tc::SmemSplit::bytes(b2a_tts::splitk_stages, out[0]) : 0;
-        out[2] = out[0] ? tc::splitk_active_clusters(out[0], (size_t)out[1]) : 0;
+        out[1] = out[0] ? (int32_t)tc::SmemSplit<8>::bytes(b2a_tts::SPLITK_STAGES[0], out[0]) : 0;
+        out[2] = out[0] ? tc::splitk_active_clusters<8>(out[0], (size_t)out[1]) : 0;
         out[3] = sk_ctas;
         out[4] = tc::stream_k_slots(m_tiles, k_blocks, sk_ctas);
     });
@@ -2018,7 +2071,7 @@ int32_t b2a_decode_attn_test(const float* qkv, const int32_t* pos, const float* 
         b2a_tts::attn_cluster_attr<1>(); b2a_tts::attn_cluster_attr<2>(); b2a_tts::attn_cluster_attr<3>();
         b2a_tts::attn_cluster_attr<4>(); b2a_tts::attn_cluster_attr<6>(); b2a_tts::attn_cluster_attr<8>();
         const cudaStream_t s = (cudaStream_t)stream;
-        const AttnArgs aa{qkv, pos, freqs, kcache, vcache, (bf16*)out, nq, nkv, max_ctx, 1.0f / sqrtf((float)HD), qnorm, knorm, qk_eps};
+        const AttnArgs aa{qkv, pos, freqs, kcache, vcache, (bf16*)out, nq, nkv, max_ctx, 1.0f / sqrtf((float)HD), qnorm, knorm, qk_eps, 8};
         b2a_tts::attn_launch(aa, B, s);
         B2A_CUDA(cudaGetLastError());
         B2A_CUDA(cudaStreamSynchronize(s));
@@ -2066,14 +2119,14 @@ int32_t b2a_tts_debug_trace(b2a_tts* h, int32_t enable, int32_t batch, float* ou
         B2A_CUDA(cudaSetDevice(h->device));
         const int H = h->cfg.hidden_size, n = 2 * h->cfg.num_hidden_layers + 1;
         if (out) {
-            B2A_CHECK(h->trace.p && batch >= 1 && batch <= 8, B2A_ERR_INVALID_INPUT, "b2a_tts_debug_trace: nothing traced");
+            B2A_CHECK(h->trace.p && batch >= 1 && batch <= h->rows_cap(), B2A_ERR_INVALID_INPUT, "b2a_tts_debug_trace: nothing traced");
             B2A_CUDA(cudaStreamSynchronize(h->stream));
             for (int i = 0; i < n; ++i)
-                B2A_CUDA(cudaMemcpy(out + (size_t)i * batch * H, h->trace.p + (size_t)i * 8 * H, (size_t)batch * H * sizeof(float),
+                B2A_CUDA(cudaMemcpy(out + (size_t)i * batch * H, h->trace.p + (size_t)i * h->rows_cap() * H, (size_t)batch * H * sizeof(float),
                                     cudaMemcpyDeviceToHost));
         }
         h->trace_on = enable != 0;
-        if (h->trace_on) { h->trace.alloc((size_t)n * 8 * H); h->drop_graphs(); }
+        if (h->trace_on) { h->trace.alloc((size_t)n * h->rows_cap() * H); h->drop_graphs(); }
     });
 }
 
@@ -2085,18 +2138,19 @@ int32_t b2a_tts_forward_logits(b2a_tts* h, const int32_t* ids, int32_t B, int32_
         cudaStream_t s = h->stream;
         h->set_batch(B);
         h->drop_graphs();
-        std::vector<int> hp(8, 0);
-        if (!reset_cache) B2A_CUDA(cudaMemcpy(hp.data(), h->pos.p, 8 * sizeof(int), cudaMemcpyDeviceToHost));
+        const int RC = h->rows_cap();
+        std::vector<int> hp(RC, 0);
+        if (!reset_cache) B2A_CUDA(cudaMemcpy(hp.data(), h->pos.p, RC * sizeof(int), cudaMemcpyDeviceToHost));
         const int start = reset_cache ? 0 : hp[0];
         B2A_CHECK(start + L <= h->cfg.max_context, B2A_ERR_INVALID_INPUT, "b2a_tts_forward_logits: context overflow");
         h->ids.alloc((size_t)B * L);
         B2A_CUDA(cudaMemcpyAsync(h->ids.p, ids, (size_t)B * L * sizeof(int), cudaMemcpyHostToDevice, s));
         const int V = h->cfg.vocab_size;
-        std::vector<int> tk(8, 0), ps(8, -1);
+        std::vector<int> tk(RC, 0), ps(RC, -1);
         for (int p = 0; p < L; ++p) {
             for (int b = 0; b < B; ++b) { tk[b] = ids[(size_t)b * L + p]; ps[b] = start + p; }
-            B2A_CUDA(cudaMemcpyAsync(h->tokens.p, tk.data(), 8 * sizeof(int), cudaMemcpyHostToDevice, s));
-            B2A_CUDA(cudaMemcpyAsync(h->pos.p, ps.data(), 8 * sizeof(int), cudaMemcpyHostToDevice, s));
+            B2A_CUDA(cudaMemcpyAsync(h->tokens.p, tk.data(), RC * sizeof(int), cudaMemcpyHostToDevice, s));
+            B2A_CUDA(cudaMemcpyAsync(h->pos.p, ps.data(), RC * sizeof(int), cudaMemcpyHostToDevice, s));
             h->run_layers(B, s);
             h->run_lm_head(B, s);
             for (int b = 0; b < B; ++b)
@@ -2105,7 +2159,7 @@ int32_t b2a_tts_forward_logits(b2a_tts* h, const int32_t* ids, int32_t B, int32_
             B2A_CUDA(cudaStreamSynchronize(s));
         }
         for (int b = 0; b < B; ++b) ps[b] = start + L;
-        B2A_CUDA(cudaMemcpy(h->pos.p, ps.data(), 8 * sizeof(int), cudaMemcpyHostToDevice));
+        B2A_CUDA(cudaMemcpy(h->pos.p, ps.data(), RC * sizeof(int), cudaMemcpyHostToDevice));
         B2A_CUDA(cudaGetLastError());
     });
 }
@@ -2343,7 +2397,7 @@ int32_t b2a_soprano_decode_hidden(b2a_tts* h, const float* hidden, int32_t B, in
 
 int32_t b2a_soprano_hidden_states(b2a_tts* h, int32_t B, float* out, int32_t* n_states) {
     return guarded([&] {
-        B2A_CHECK(h && h->vocos && n_states && B >= 1 && B <= 8, B2A_ERR_INVALID_INPUT, "b2a_soprano_hidden_states: bad argument");
+        B2A_CHECK(h && h->vocos && n_states && B >= 1 && B <= h->cfg.max_batch, B2A_ERR_INVALID_INPUT, "b2a_soprano_hidden_states: bad argument");
         B2A_CHECK(h->hidden.p && h->n_cap.p && B <= h->hidden_rows, B2A_ERR_INVALID_INPUT,
                   "b2a_soprano_hidden_states: batch exceeds the last generate call's");
         B2A_CUDA(cudaSetDevice(h->device));
@@ -2409,14 +2463,14 @@ struct Q3Feedback {
     const bf16* codec_emb; int codec_rows;
     const bf16* const* cp_emb;   // device array of G-1 tables [cp_vocab, H]
     int cp_rows;
-    const int* codes;            // [8, G] this frame
+    const int* codes;            // [max_batch, G] this frame
     const float* trailing;       // [B, n_max, H]
     const int* n_trailing;       // [B]
     int n_max;
     const float* pad;            // [H]
-    float* x_in;                 // [8, H] next talker input
-    int* talker_pos;             // [8]
-    int* row_frame;              // [8] frames stepped so far (= index of the trailing text row to consume)
+    float* x_in;                 // [max_batch, H] next talker input
+    int* talker_pos;             // [max_batch]
+    int* row_frame;              // [max_batch] frames stepped so far (= index of the trailing text row to consume)
     int* out_codes;              // [B, max_tokens, G]
     int* n_frames; int* done; int* n_active;
     int G, H, max_tokens, eos, mask_eos;
@@ -2459,11 +2513,13 @@ __global__ void q3_code_frames_kernel(const bf16* codec_emb, int codec_rows, con
     const long long r = blockIdx.x;
     for (int i = threadIdx.x; i < H; i += blockDim.x) out[r * H + i] = q3_frame_sum(codec_emb, codec_rows, cp_emb, cp_rows, codes + r * G, G, H, i);
 }
-__global__ void q3_init_rows_kernel(int B, int L, int* talker_pos, int* row_frame, int* n_frames, int* done, int* n_active, unsigned* seen, int words) {
+// rows: the handle's row capacity (every row's state is reset; rows >= B start done)
+__global__ void q3_init_rows_kernel(int B, int L, int* talker_pos, int* row_frame, int* n_frames, int* done, int* n_active, unsigned* seen, int words,
+                                    int rows) {
     const int b = threadIdx.x;
     if (b == 0) *n_active = B;
-    if (b < 8) { talker_pos[b] = L - 1; row_frame[b] = 0; n_frames[b] = 0; done[b] = b < B ? 0 : 1; }
-    for (int i = threadIdx.x; i < 8 * words; i += blockDim.x) seen[i] = 0u;
+    if (b < rows) { talker_pos[b] = L - 1; row_frame[b] = 0; n_frames[b] = 0; done[b] = b < B ? 0 : 1; }
+    for (int i = threadIdx.x; i < rows * words; i += blockDim.x) seen[i] = 0u;
 }
 // bench only: the talker never emits EOS -- its logit is dropped before the sampler sees the row
 __global__ void q3_mask_eos_kernel(float* logits, int V, int eos) {
@@ -2509,6 +2565,7 @@ struct b2a_qwen3_talker {
         delete talker;
     }
     int G() const { return cfg.num_code_groups; }
+    int rows() const { return talker->rows_cap(); }   // rows of the per-row state buffers
     int H() const { return cfg.hidden_size; }
     int PH() const { return cfg.cp_hidden_size; }
     bool projected() const { return cfg.cp_hidden_size != cfg.hidden_size; }
@@ -2543,7 +2600,7 @@ struct b2a_qwen3_talker {
         B2A_CHECK(c.vocab_size >= 1 && c.vocab_size <= q3s::SLOTS && c.cp_vocab_size >= 1 && c.cp_vocab_size <= q3s::SLOTS, B2A_ERR_INVALID_INPUT,
                   "qwen3 talker: codec vocabularies must be <= 4096");
         B2A_CHECK(c.num_code_groups >= 2 && c.num_code_groups <= 32, B2A_ERR_INVALID_INPUT, "qwen3 talker: num_code_groups must be in 2..32");
-        B2A_CHECK(c.max_batch >= 1 && c.max_batch <= 8, B2A_ERR_INVALID_INPUT, "qwen3 talker: max_batch must be in 1..8");
+        B2A_CHECK(c.max_batch >= 1 && c.max_batch <= 32, B2A_ERR_INVALID_INPUT, "qwen3 talker: max_batch must be in 1..32");
     }
     // proj_tab: every table row through the projection, once.  The tables are bf16, so the GEMM reads them without a lo half
     // (hilo = 0); each row is the same linear map the reference applies per position (Qwen3TTS.swift:433-451), to fp32 rounding
@@ -2566,19 +2623,19 @@ struct b2a_qwen3_talker {
     }
     void alloc_state() {
         stream = talker->stream;
-        const int Hh = H(), P = PH();
-        x_in.alloc((size_t)8 * Hh); hid.alloc((size_t)8 * Hh); px.alloc((size_t)8 * P); pad.alloc(Hh);
-        B2A_CUDA(cudaMemset(x_in.p, 0, (size_t)8 * Hh * sizeof(float)));
-        B2A_CUDA(cudaMemset(hid.p, 0, (size_t)8 * Hh * sizeof(float)));
-        B2A_CUDA(cudaMemset(px.p, 0, (size_t)8 * P * sizeof(float)));
+        const int Hh = H(), P = PH(), RC = rows();
+        x_in.alloc((size_t)RC * Hh); hid.alloc((size_t)RC * Hh); px.alloc((size_t)RC * P); pad.alloc(Hh);
+        B2A_CUDA(cudaMemset(x_in.p, 0, (size_t)RC * Hh * sizeof(float)));
+        B2A_CUDA(cudaMemset(hid.p, 0, (size_t)RC * Hh * sizeof(float)));
+        B2A_CUDA(cudaMemset(px.p, 0, (size_t)RC * P * sizeof(float)));
         if (projected()) {
             build_proj_tables();
             proj_rows = b2a_tts::pick_tile_rows(P, talker->num_sms);
             tm_proj = tc::make_tmap_bf16(proj_w.p, P, Hh, proj_rows);
         }
-        codes.alloc((size_t)8 * G()); n_frames.alloc(8); done.alloc(8); n_active.alloc(1); row_frame.alloc(8); n_trailing.alloc(8);
-        B2A_CUDA(cudaMemset(codes.p, 0, (size_t)8 * G() * sizeof(int)));
-        seen.alloc((size_t)8 * cdiv(cfg.vocab_size, 32));
+        codes.alloc((size_t)RC * G()); n_frames.alloc(RC); done.alloc(RC); n_active.alloc(1); row_frame.alloc(RC); n_trailing.alloc(RC);
+        B2A_CUDA(cudaMemset(codes.p, 0, (size_t)RC * G() * sizeof(int)));
+        seen.alloc((size_t)RC * cdiv(cfg.vocab_size, 32));
         h_flag.alloc(16);
         std::vector<const bf16*> ptrs;
         for (auto& e : cp_emb) ptrs.push_back(e.p);
@@ -2588,7 +2645,6 @@ struct b2a_qwen3_talker {
         for (auto& hd : cp_head) tm_cp_head.push_back(tc::make_tmap_bf16(hd.p, cfg.cp_vocab_size, P, cp_head_rows));
         talker->x_ext = x_in.p; talker->normed_out = hid.p;
         pred->x_ext = px.p;
-        talker->set_batch(8); pred->set_batch(8);
         B2A_CUDA(cudaDeviceSynchronize());
     }
 
@@ -2859,7 +2915,7 @@ int32_t b2a_qwen3_talker_generate(b2a_qwen3_talker* h, const float* input_embeds
         h->talker->drop_graphs();
         h->embeds.upload(input_embeds, (size_t)B * L * Hh, s);
         h->trailing.alloc((size_t)B * nmax * Hh);
-        std::vector<int> nt(8, 0);
+        std::vector<int> nt(h->rows(), 0);
         if (n_trailing_max > 0) {
             B2A_CUDA(cudaMemcpyAsync(h->trailing.p, trailing_text_hidden, (size_t)B * n_trailing_max * Hh * sizeof(float), cudaMemcpyHostToDevice, s));
             for (int b = 0; b < B; ++b) {
@@ -2867,23 +2923,23 @@ int32_t b2a_qwen3_talker_generate(b2a_qwen3_talker* h, const float* input_embeds
                 nt[b] = n_trailing[b];
             }
         }
-        h->n_trailing.upload(nt.data(), 8, s);
+        h->n_trailing.upload(nt.data(), nt.size(), s);
         h->pad.upload(tts_pad_embed, Hh, s);
         h->out_codes.alloc((size_t)B * MT * G);
         B2A_CUDA(cudaStreamSynchronize(s));       // nt goes out of scope with the lambda only, but keep uploads ordered before capture
         h->capture_frame(B, *gp, MT, nmax);
         const double t0 = now_s();
         q3_init_rows_kernel<<<1, 256, 0, s>>>(B, L, h->talker->pos.p, h->row_frame.p, h->n_frames.p, h->done.p, h->n_active.p, h->seen.p,
-                                              cdiv(h->cfg.vocab_size, 32));
+                                              cdiv(h->cfg.vocab_size, 32), h->rows());
         count_launch();
         h->prefill(B, L, s);
         B2A_CUDA(cudaStreamSynchronize(s));
         const double t1 = now_s();
         int steps = 0, emitted = 0;
         bool cancelled = false;
-        std::vector<int> hn(8), hc;
+        std::vector<int> hn(h->rows()), hc;
         auto emit = [&]() {          // frames emitted since the last poll -> on_frame
-            B2A_CUDA(cudaMemcpy(hn.data(), h->n_frames.p, 8 * sizeof(int), cudaMemcpyDeviceToHost));
+            B2A_CUDA(cudaMemcpy(hn.data(), h->n_frames.p, hn.size() * sizeof(int), cudaMemcpyDeviceToHost));
             hc.resize((size_t)B * MT * G);
             B2A_CUDA(cudaMemcpy(hc.data(), h->out_codes.p, hc.size() * sizeof(int), cudaMemcpyDeviceToHost));
             for (int b = 0; b < B; ++b)
@@ -2902,7 +2958,7 @@ int32_t b2a_qwen3_talker_generate(b2a_qwen3_talker* h, const float* input_embeds
         }
         const double t2 = now_s();
         B2A_CHECK(!cancelled, B2A_ERR_CANCELLED, "generation cancelled");
-        B2A_CUDA(cudaMemcpy(hn.data(), h->n_frames.p, 8 * sizeof(int), cudaMemcpyDeviceToHost));
+        B2A_CUDA(cudaMemcpy(hn.data(), h->n_frames.p, hn.size() * sizeof(int), cudaMemcpyDeviceToHost));
         B2A_CUDA(cudaMemcpy(codes_out, h->out_codes.p, (size_t)B * MT * G * sizeof(int), cudaMemcpyDeviceToHost));
         int total = 0;
         for (int b = 0; b < B; ++b) { n_frames_out[b] = std::min(hn[b], MT); total += n_frames_out[b]; }

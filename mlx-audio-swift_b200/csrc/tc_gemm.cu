@@ -71,33 +71,56 @@ CUtensorMap make_tmap_planes(const void* base, int C, long long Ttot, int B, int
 }
 
 template <int BN>
-void launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const Args& a, int ctas, int n_tiles, cudaStream_t s) {
+void launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const Args& a, int ctas, int n_tiles, cudaStream_t s, bool share_sm) {
     B2A_CHECK(a.stages >= 1 && a.stages <= Smem<BN>::max_stages(), B2A_ERR_INVALID_INPUT, "tc_gemm: ring depth does not fit in shared memory");
     B2A_CHECK(a.epi_partial < 0 || (a.part_ws && a.part_cnt && a.part_slots >= stream_k_slots(a.m_tiles, a.k_blocks, ctas)),
               B2A_ERR_INVALID_INPUT, "tc_gemm: stream-K workspace missing or too small");
-    launch_pdl(tc_gemm_kernel<BN>, dim3(ctas, n_tiles), dim3(Cfg<BN>::NTHREADS), Smem<BN>::bytes(a.stages), s, tmA, tmB, a);
+    if (!share_sm) {
+        launch_pdl(tc_gemm_kernel<BN>, dim3(ctas, n_tiles), dim3(Cfg<BN>::NTHREADS), Smem<BN>::bytes(a.stages), s, tmA, tmB, a);
+        return;
+    }
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = dim3(ctas, n_tiles); cfg.blockDim = dim3(Cfg<BN>::NTHREADS); cfg.dynamicSmemBytes = Smem<BN>::bytes(a.stages); cfg.stream = s;
+    cudaLaunchAttribute at[2];
+    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    at[0].val.programmaticStreamSerializationAllowed = pdl_enabled() ? 1 : 0;
+    at[1].id = cudaLaunchAttributePreferredSharedMemoryCarveout;
+    at[1].val.sharedMemCarveout = cudaSharedmemCarveoutMaxShared;
+    cfg.attrs = at; cfg.numAttrs = 2;
+    B2A_CUDA(cudaLaunchKernelEx(&cfg, tc_gemm_kernel<BN>, tmA, tmB, a));
+    count_launch();
 }
-template void launch<16>(const CUtensorMap&, const CUtensorMap&, const Args&, int, int, cudaStream_t);
-template void launch<32>(const CUtensorMap&, const CUtensorMap&, const Args&, int, int, cudaStream_t);
-template void launch<128>(const CUtensorMap&, const CUtensorMap&, const Args&, int, int, cudaStream_t);
+template void launch<16>(const CUtensorMap&, const CUtensorMap&, const Args&, int, int, cudaStream_t, bool);
+template void launch<32>(const CUtensorMap&, const CUtensorMap&, const Args&, int, int, cudaStream_t, bool);
+template void launch<64>(const CUtensorMap&, const CUtensorMap&, const Args&, int, int, cudaStream_t, bool);
+template void launch<128>(const CUtensorMap&, const CUtensorMap&, const Args&, int, int, cudaStream_t, bool);
 
+template <int T>
 void launch_splitk(const CUtensorMap& tmA, const CUtensorMap& tmB, const SplitArgs& a, int m_tiles, int cluster, cudaStream_t s) {
-    B2A_CHECK(SmemSplit::bytes(a.stages, cluster) <= 227 * 1024, B2A_ERR_INVALID_INPUT, "tc_gemm: split-K ring does not fit in shared memory");
+    using SS = SmemSplit<T>;
+    B2A_CHECK(SS::bytes(a.stages, cluster) <= 227 * 1024, B2A_ERR_INVALID_INPUT, "tc_gemm: split-K ring does not fit in shared memory");
+    B2A_CHECK(a.stages >= SS::ACC_STAGES && a.stages <= SS::MAX_STAGES, B2A_ERR_INVALID_INPUT,
+              "tc_gemm: split-K ring too shallow for the staged accumulator or too deep for the barrier scratch");
+    B2A_CHECK(a.N >= 1 && a.N <= T, B2A_ERR_INVALID_INPUT, "tc_gemm: split-K token count exceeds the width");
     B2A_CHECK(a.sk_ctas <= 0 || (!a.h && cluster >= stream_k_slots(m_tiles, a.k_blocks, a.sk_ctas)), B2A_ERR_INVALID_INPUT,
               "tc_gemm: the stream-K cut is a store-mode option and needs a CTA per piece of a tile");
     cudaLaunchConfig_t cfg{};
     cfg.gridDim = dim3((unsigned)(m_tiles * cluster)); cfg.blockDim = dim3(THREADS);
-    cfg.dynamicSmemBytes = SmemSplit::bytes(a.stages, cluster); cfg.stream = s;
+    cfg.dynamicSmemBytes = SS::bytes(a.stages, cluster); cfg.stream = s;
     cudaLaunchAttribute at[2];
     at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     at[0].val.programmaticStreamSerializationAllowed = pdl_enabled() ? 1 : 0;
     at[1].id = cudaLaunchAttributeClusterDimension;
     at[1].val.clusterDim.x = (unsigned)cluster; at[1].val.clusterDim.y = 1; at[1].val.clusterDim.z = 1;
     cfg.attrs = at; cfg.numAttrs = 2;
-    B2A_CUDA(cudaLaunchKernelEx(&cfg, tc_gemm_splitk_kernel, tmA, tmB, a));
+    B2A_CUDA(cudaLaunchKernelEx(&cfg, tc_gemm_splitk_kernel<T>, tmA, tmB, a));
     count_launch();
 }
+template void launch_splitk<8>(const CUtensorMap&, const CUtensorMap&, const SplitArgs&, int, int, cudaStream_t);
+template void launch_splitk<16>(const CUtensorMap&, const CUtensorMap&, const SplitArgs&, int, int, cudaStream_t);
+template void launch_splitk<32>(const CUtensorMap&, const CUtensorMap&, const SplitArgs&, int, int, cudaStream_t);
 
+template <int T>
 int splitk_active_clusters(int cluster, size_t smem_bytes) {
     B2A_CHECK(cluster >= 1 && cluster <= SPLIT_MAX_CLUSTER, B2A_ERR_INVALID_INPUT, "tc_gemm: split-K cluster size must be in [1, 8]");
     cudaLaunchConfig_t cfg{};
@@ -108,17 +131,26 @@ int splitk_active_clusters(int cluster, size_t smem_bytes) {
     at[0].val.clusterDim.x = (unsigned)cluster; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
     cfg.attrs = at; cfg.numAttrs = 1;
     int n = 0;
-    B2A_CUDA(cudaOccupancyMaxActiveClusters(&n, tc_gemm_splitk_kernel, &cfg));
+    B2A_CUDA(cudaOccupancyMaxActiveClusters(&n, tc_gemm_splitk_kernel<T>, &cfg));
     return n;
 }
+template int splitk_active_clusters<8>(int, size_t);
+template int splitk_active_clusters<16>(int, size_t);
+template int splitk_active_clusters<32>(int, size_t);
 
 void set_attributes() {
-    B2A_CUDA(cudaFuncSetAttribute(tc_gemm_splitk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    B2A_CUDA(cudaFuncSetAttribute(tc_gemm_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     // the decode-step kernels are sized to share an SM with their neighbours in the step (Smem / SmemSplit): ask for the largest
     // shared-memory carve-out, or an SM configured for one kernel's footprint alone cannot take the next kernel's CTA beside it
-    B2A_CUDA(cudaFuncSetAttribute(tc_gemm_splitk_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
-    B2A_CUDA(cudaFuncSetAttribute(tc_gemm_kernel<16>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+    for (auto k : {tc_gemm_splitk_kernel<8>, tc_gemm_splitk_kernel<16>, tc_gemm_splitk_kernel<32>}) {
+        B2A_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+        B2A_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+    }
+    for (auto k : {tc_gemm_kernel<16>, tc_gemm_kernel<64>}) {
+        B2A_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+        B2A_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+    }
+    // tc_gemm_kernel<32> also serves Whisper's decoder, which keeps the default carve-out: the 16-row decode step asks for the largest
+    // one per launch (launch(..., share_sm))
     B2A_CUDA(cudaFuncSetAttribute(tc_gemm_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     B2A_CUDA(cudaFuncSetAttribute(tc_gemm_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
 }
@@ -213,7 +245,7 @@ extern "C" int32_t b2a_tc_gemm_splitk_test(const void* W, const void* X, float* 
         SplitArgs a{};
         a.M = M; a.N = N; a.K = K; a.k_blocks = K / BK; a.stages = stages;
         a.h = h; a.gain = gain; a.xn = (__nv_bfloat16*)xn; a.ss = ss;
-        launch_splitk(ta, tb, a, cdiv(M, BM), cluster, (cudaStream_t)stream);
+        launch_splitk<8>(ta, tb, a, cdiv(M, BM), cluster, (cudaStream_t)stream);
         B2A_CUDA(cudaGetLastError());
         B2A_CUDA(cudaStreamSynchronize((cudaStream_t)stream));
     });
@@ -239,7 +271,7 @@ extern "C" int32_t b2a_tc_gemm_splitk_store_test(const void* W, const void* X, f
         a.M = M; a.N = N; a.K = K; a.k_blocks = K / BK; a.stages = stages; a.sk_ctas = sk_ctas;
         a.out = out;
         a.rstd_ss = rstd_ss; a.rstd_parts = rstd_parts; a.rstd_inv_h = 1.0f / (float)K; a.rstd_eps = rstd_eps;
-        launch_splitk(ta, tb, a, cdiv(M, BM), cluster, (cudaStream_t)stream);
+        launch_splitk<8>(ta, tb, a, cdiv(M, BM), cluster, (cudaStream_t)stream);
         B2A_CUDA(cudaGetLastError());
         B2A_CUDA(cudaStreamSynchronize((cudaStream_t)stream));
     });

@@ -42,8 +42,8 @@ struct Args {
                              // have this many rows).  fewer rows per tile spread a GEMM whose 128-row tiles
                              // would leave SMs idle over all of them.  The MMA still multiplies 128
                              // shared-memory rows; rows past tile_rows are stale and their accumulator rows are never stored.
-    const float* rstd_ss;    // nullable [rstd_parts, 8]: the X rows are UN-normalised (h * gain); every accumulator column t is
-    int rstd_parts;          // multiplied by rsqrt(sum_p rstd_ss[p, t] * rstd_inv_h + rstd_eps) first (fused RMSNorm, BN = 16 only)
+    const float* rstd_ss;    // nullable [rstd_parts, BN / 2]: the X rows are UN-normalised (h * gain); every accumulator column t is
+    int rstd_parts;          // multiplied by rsqrt(sum_p rstd_ss[p, t] * rstd_inv_h + rstd_eps) first (fused RMSNorm, hi/lo, BN = 16, 32, 64)
     float rstd_inv_h, rstd_eps;
     int lo_rows;             // != 0: bf16 outputs are written as hi/lo pairs in the same tile-interleaved row layout the
                              // kernel reads X in: token t -> hi row (t / (BN/2)) * BN + t % (BN/2), lo row = hi row + BN/2
@@ -248,6 +248,36 @@ struct Cfg {
     static constexpr int NTHREADS = 32 * EPI_WARPS + 32;
 };
 
+// The decode step runs R = 8, 16 or 32 token rows as hi/lo pairs: X is [2R, K] with hi(x_t) in row t and lo(x_t) in row R + t, and the
+// GEMM tiles are BN = 2R columns wide.  One rule, here, turns a row count into that width; every kernel that writes or reads the
+// layout takes its lo-row offset R from it.
+constexpr int DECODE_WIDTHS[3] = {8, 16, 32};
+__host__ __device__ constexpr int decode_width(int rows) { return rows <= 8 ? 8 : rows <= 16 ? 16 : 32; }
+__host__ __device__ constexpr int decode_width_index(int width) { return width == 8 ? 0 : width == 16 ? 1 : 2; }
+template <int BN>
+struct DecodeWidth {
+    static constexpr bool OK = BN == 16 || BN == 32 || BN == 64;   // tc_gemm_kernel<BN> is a decode-step GEMM
+    static constexpr int TOKENS = OK ? BN / 2 : 8;
+};
+
+// rstd[t] = rsqrt(sum_p ss[p, t] * inv_h + eps) for the T tokens of a [parts, T] sum-of-squares array, by the whole warp: rs[g] holds
+// rstd[8 g + (lane & 7)].  Each group of 8 tokens is reduced as the 8-token step always was: lane = part * 8 + token loads one partial
+// per step, then xor 8 and xor 16, so a token's rstd does not depend on how many tokens the step runs.
+template <int T>
+__device__ __forceinline__ void rstd_lanes(float (&rs)[T / 8], const float* ss, int parts, float inv_h, float eps, int lane) {
+#pragma unroll
+    for (int g = 0; g < T / 8; ++g) {
+        float t = 0.f;
+        for (int p0 = 0; p0 < parts; p0 += 4) {
+            const int p = p0 + (lane >> 3);
+            if (p < parts) t += ss[p * T + 8 * g + (lane & 7)];
+        }
+        t += __shfl_xor_sync(0xffffffffu, t, 8);
+        t += __shfl_xor_sync(0xffffffffu, t, 16);
+        rs[g] = rsqrtf(t * inv_h + eps);
+    }
+}
+
 // Dynamic shared memory of tc_gemm_kernel<BN>: the ring, the staged accumulator, 256 bytes of barriers.  The decode step runs BN = 16
 // with 6 stages: 6 x 18 432 + 10 240 + 256 = 121 088 bytes, which leaves room on the SM (233 472 bytes, 1 KB of it reserved per
 // resident CTA) for one CTA of either neighbour in the step, the split-K GEMM or the attention kernel, so that the neighbour's
@@ -344,24 +374,30 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 #pragma unroll
             for (int i = 0; i < C::WN / 2; ++i) acc[rb][i] = 0.f;
         long long u = u0;
-        float rstd[8];
+        constexpr int NR = DecodeWidth<BN>::TOKENS;   // tokens per tile of a decode-step width (8 for the prefill tile: unused)
+        float rstd[8];                                // BN = 16: every token's rstd; wider: rsg[g] = rstd[8 g + (lane & 7)]
+        float rsg[NR / 8];
         bool have_rstd = false;
-        if (BN == 16 && a.rstd_ss) {
-            // fused RMSNorm: the producer of X left h * gain un-normalised plus per-m-tile sums of squares (SplitArgs::ss); the
-            // accumulator column of token t is scaled by rstd[t].  Computed while the main loop streams weights: these warps are
+        if (DecodeWidth<BN>::OK && a.rstd_ss) {
+            // fused RMSNorm: the producer of X left h * gain un-normalised plus per-m-tile sums of squares (SplitArgs::ss, [parts, NR]);
+            // the accumulator column of token t is scaled by rstd[t].  Computed while the main loop streams weights: these warps are
             // idle until the first accumulator is ready, so they wait for the previous kernel themselves and reduce the partial
-            // sums with one independent load per lane and step (lane = part * 8 + token).
+            // sums with one independent load per lane and step (lane = part * 8 + token), one group of 8 tokens at a time.
             asm volatile("griddepcontrol.wait;" ::: "memory");
-            float t = 0.f;
-            for (int p0 = 0; p0 < a.rstd_parts; p0 += 4) {
-                const int p = p0 + (lane >> 3);
-                if (p < a.rstd_parts) t += a.rstd_ss[p * 8 + (lane & 7)];
-            }
-            t += __shfl_xor_sync(0xffffffffu, t, 8);
-            t += __shfl_xor_sync(0xffffffffu, t, 16);
-            const float rs = rsqrtf(t * a.rstd_inv_h + a.rstd_eps);
+            if constexpr (BN == 16) {
+                float t = 0.f;
+                for (int p0 = 0; p0 < a.rstd_parts; p0 += 4) {
+                    const int p = p0 + (lane >> 3);
+                    if (p < a.rstd_parts) t += a.rstd_ss[p * 8 + (lane & 7)];
+                }
+                t += __shfl_xor_sync(0xffffffffu, t, 8);
+                t += __shfl_xor_sync(0xffffffffu, t, 16);
+                const float rs = rsqrtf(t * a.rstd_inv_h + a.rstd_eps);
 #pragma unroll
-            for (int j = 0; j < 8; ++j) rstd[j] = __shfl_sync(0xffffffffu, rs, j);
+                for (int j = 0; j < 8; ++j) rstd[j] = __shfl_sync(0xffffffffu, rs, j);
+            } else {
+                rstd_lanes<NR>(rsg, a.rstd_ss, a.rstd_parts, a.rstd_inv_h, a.rstd_eps, lane);
+            }
             have_rstd = true;
         }
         while (u < u1) {
@@ -427,6 +463,16 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                         ld_acc16(arow + c0 + HALF, w);
 #pragma unroll
                         for (int j = 0; j < 16; ++j) v[j] += w[j];
+                    }
+                    if constexpr (DecodeWidth<BN>::OK) {
+                        if (have_rstd) {   // hi/lo only: c0 is a multiple of 16 below NR (a constant index into rsg per branch)
+#pragma unroll
+                            for (int cc = 0; cc < NR; cc += 16)
+                                if (cc == c0) {
+#pragma unroll
+                                    for (int j = 0; j < 16; ++j) v[j] *= __shfl_sync(0xffffffffu, rsg[(cc + j) / 8], j % 8);
+                                }
+                        }
                     }
                 }
                 const int jn = (BN == 16 && !a.hilo) ? 16 : CH;
@@ -542,11 +588,11 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 }
 
 // ----------------------------------------------------------------------------------------------- cluster split-K
-// D[M, 8 tokens] = W[M, K] X^T for the two GEMMs of a decoder layer whose output feeds the residual stream (o_proj, down_proj),
-// with the residual add, the NEXT RMSNorm's gain, its hi/lo split and its sum of squares fused into the epilogue, so the step
-// has no stand-alone norm kernel.  One thread-block CLUSTER per 128-row m-tile: CTA r of the cluster streams k-blocks
-// [kb * r / C, kb * (r + 1) / C) of the tile (same TMA ring / wgmma warpgroup as tc_gemm_kernel<16>), then every
-// non-leader writes its 128 x 8 fp32 partial into the leader's shared memory (distributed shared memory, st.shared::cluster),
+// D[M, T tokens] = W[M, K] X^T (T = 8, 16 or 32: the decode width) for the two GEMMs of a decoder layer whose output feeds the residual
+// stream (o_proj, down_proj), with the residual add, the NEXT RMSNorm's gain, its hi/lo split and its sum of squares fused into the
+// epilogue, so the step has no stand-alone norm kernel.  One thread-block CLUSTER per 128-row m-tile: CTA r of the cluster streams
+// k-blocks [kb * r / C, kb * (r + 1) / C) of the tile (same TMA ring / wgmma warpgroup as tc_gemm_kernel<2T>), then every
+// non-leader writes its 128 x T fp32 partial into the leader's shared memory (distributed shared memory, st.shared::cluster),
 // one cluster barrier, and the leader adds the partials IN RANK ORDER (bit-reproducible) and runs
 //     h[t, m] += acc          (fp32 residual stream, updated in place)
 //     xn[t, m] = hi / lo of  h[t, m] * gain[m]        (UN-normalised: the consumer GEMM scales its accumulator by rstd[t])
@@ -556,16 +602,17 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 // P_r the partial of CTA r and rstd of the norm the input went through (rstd_ss; 1 without).  With sk_ctas > 0 CTA r streams the
 // r-th piece of the tile as tc_gemm_kernel's stream-K over sk_ctas CTAs cuts it (split_range), so out is bit-identical to that
 // launch: the same wgmma accumulation per piece, each piece scaled before the pieces are summed in slot order from 0.
+// Every per-token operation is the same at every T, so a token's output does not depend on the width it ran at.
 struct SplitArgs {
-    int M, N, K;                 // N = tokens (<= 8)
+    int M, N, K;                 // N = tokens (<= T)
     int k_blocks, stages;
     int sk_ctas;                 // > 0: k-blocks cut as stream-K over this many CTAs (cluster >= stream_k_slots); 0: evenly
-    float* h;                    // [8, M] residual stream (read-modify-write by the leader); nullptr: store mode
+    float* h;                    // [T, M] residual stream (read-modify-write by the leader); nullptr: store mode
     const float* gain;           // [M] the next norm's weight
-    __nv_bfloat16* xn;           // [16, M] hi rows 0..7 / lo rows 8..15
-    float* ss;                   // [m_tiles, 8] partial sums of squares
-    float* out;                  // store mode: [8, M] fp32, rows t < N written
-    const float* rstd_ss;        // nullable: partial sums [rstd_parts, 8] of the norm this GEMM's INPUT went through
+    __nv_bfloat16* xn;           // [2T, M] hi rows 0..T-1 / lo rows T..2T-1
+    float* ss;                   // [m_tiles, T] partial sums of squares
+    float* out;                  // store mode: [T, M] fp32, rows t < N written
+    const float* rstd_ss;        // nullable: partial sums [rstd_parts, T] of the norm this GEMM's INPUT went through
     int rstd_parts;
     float rstd_inv_h, rstd_eps;
 };
@@ -601,30 +648,36 @@ __host__ __device__ __forceinline__ void split_range(const SplitArgs& a, int mt,
 }
 
 constexpr int SPLIT_MAX_CLUSTER = 8;
-// Dynamic shared memory of tc_gemm_splitk_kernel: the ring, the peers' partials (written remotely while the leader may still be
-// streaming, so they have a buffer of their own), 512 bytes of barriers and reduction scratch.  A CTA streams ONE tile, so its ring
-// is idle once the main loop ends and the 128 x 16 accumulator is staged in ring stage 0.  The decode step runs 5 stages in clusters
-// of 5: 5 x 18 432 + 4 x 4096 + 512 = 109 056 bytes; with tc_gemm_kernel<16>'s 121 088 and 1 KB reserved per CTA that is
-// 232 192 of an SM's 233 472 bytes.
+// Dynamic shared memory of tc_gemm_splitk_kernel<T>: the ring, the peers' partials (written remotely while the leader may still be
+// streaming, so they have a buffer of their own), then barriers and the s_red reduction scratch.  A CTA streams ONE tile, so its ring
+// is idle once the main loop ends and the 128 x 2T accumulator is staged over its first ACC_STAGES stages.  The 8-token step runs 5
+// stages in clusters of 5: 5 x 18 432 + 4 x 4096 + 512 = 109 056 bytes; with tc_gemm_kernel<16>'s 121 088 and 1 KB reserved per CTA
+// that is 232 192 of an SM's 233 472 bytes.  DESIGN.md section 3.3 gives the wider widths' footprints.
+template <int T>
 struct SmemSplit {
-    static constexpr int STAGE = Smem<16>::STAGE;
-    static constexpr int PART_BYTES = BM * 8 * 4;                      // one CTA's 128 x 8 fp32 partial
-    static_assert(Smem<16>::ACC_BYTES <= STAGE, "the staged accumulator lives in ring stage 0");
-    static size_t bytes(int stages, int cluster) { return (size_t)stages * STAGE + (size_t)(cluster - 1) * PART_BYTES + 512; }
+    static constexpr int BN = 2 * T;
+    static constexpr int STAGE = Smem<BN>::STAGE;
+    static constexpr int PART_BYTES = BM * T * 4;                      // one CTA's 128 x T fp32 partial
+    static constexpr int SCRATCH = 16 * T + 128 > 512 ? 16 * T + 128 : 512;   // up to 8 stages of barriers + s_red [4][T]
+    static constexpr int MAX_STAGES = (SCRATCH - 16 * T) / 16;
+    static constexpr int ACC_STAGES = (Smem<BN>::ACC_BYTES + STAGE - 1) / STAGE;   // ring stages the staged accumulator covers
+    static size_t bytes(int stages, int cluster) { return (size_t)stages * STAGE + (size_t)(cluster - 1) * PART_BYTES + SCRATCH; }
 };
 
-#ifdef B2A_TC_GEMM_IMPL   // the kernel body lives in tc_gemm.cu only (a non-template __global__ cannot be defined in every translation unit)
+#ifdef B2A_TC_GEMM_IMPL   // the kernel body lives in tc_gemm.cu only
+template <int T>
 __global__ void __launch_bounds__(THREADS, 2)
 tc_gemm_splitk_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, SplitArgs a) {
-    using S = Smem<16>;
-    constexpr int BN = 16;
+    constexpr int BN = 2 * T;
+    using S = Smem<BN>;
+    constexpr int LD = Cfg<BN>::LD;
     extern __shared__ __align__(1024) uint8_t smem[];
     const uint32_t C = cluster_nctarank(), rank = cluster_ctarank();
-    float* part = reinterpret_cast<float*>(smem + (size_t)a.stages * S::STAGE);                 // [C - 1][128][8]
-    float* sacc = reinterpret_cast<float*>(smem);                                                // [128][LD], over ring stage 0
-    uint64_t* full = reinterpret_cast<uint64_t*>(part + (size_t)(C - 1) * BM * 8);
+    float* part = reinterpret_cast<float*>(smem + (size_t)a.stages * S::STAGE);                 // [C - 1][128][T]
+    float* sacc = reinterpret_cast<float*>(smem);                                                // [128][LD], over the ring
+    uint64_t* full = reinterpret_cast<uint64_t*>(part + (size_t)(C - 1) * BM * T);
     uint64_t* empty = full + a.stages;
-    float* s_red = reinterpret_cast<float*>(empty + a.stages);                                   // [4][8]
+    float* s_red = reinterpret_cast<float*>(empty + a.stages);                                   // [4][T]
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int mt = blockIdx.x / C, m_tiles = gridDim.x / C;
@@ -664,7 +717,7 @@ tc_gemm_splitk_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
         }
     }
     // ---- epilogue part 1 (warps 0..3): this CTA's partial = hi + lo columns; non-leaders hand it to the leader
-    float acc[8], hold[8], rstd[8];
+    float acc[T], hold[T], rstd[T];
     float g = 0.f;
     const int q = warp & 3, row = q * 32 + lane;
     const int m = mt * BM + row;
@@ -677,28 +730,31 @@ tc_gemm_splitk_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
             if (a.h) {
                 g = m_ok ? a.gain[m] : 0.f;
 #pragma unroll
-                for (int j = 0; j < 8; ++j) hold[j] = (j < a.N && m_ok) ? a.h[(long long)j * a.M + m] : 0.f;
+                for (int j = 0; j < T; ++j) hold[j] = (j < a.N && m_ok) ? a.h[(long long)j * a.M + m] : 0.f;
             }
             if (a.rstd_ss) {
                 // rstd of the norm this GEMM's input went through (its producer wrote un-normalised hi/lo rows), reduced as
-                // tc_gemm_kernel does: one independent load per lane and step (lane = part * 8 + token)
-                float t = 0.f;
-                for (int p0 = 0; p0 < a.rstd_parts; p0 += 4) {
-                    const int p = p0 + (lane >> 3);
-                    if (p < a.rstd_parts) t += a.rstd_ss[p * 8 + (lane & 7)];
-                }
-                t += __shfl_xor_sync(0xffffffffu, t, 8);
-                t += __shfl_xor_sync(0xffffffffu, t, 16);
-                const float rs = rsqrtf(t * a.rstd_inv_h + a.rstd_eps);
+                // tc_gemm_kernel does: one independent load per lane and step (lane = part * 8 + token), per group of 8 tokens
 #pragma unroll
-                for (int j = 0; j < 8; ++j) rstd[j] = __shfl_sync(0xffffffffu, rs, j);
+                for (int g0 = 0; g0 < T; g0 += 8) {
+                    float t = 0.f;
+                    for (int p0 = 0; p0 < a.rstd_parts; p0 += 4) {
+                        const int p = p0 + (lane >> 3);
+                        if (p < a.rstd_parts) t += a.rstd_ss[p * T + g0 + (lane & 7)];
+                    }
+                    t += __shfl_xor_sync(0xffffffffu, t, 8);
+                    t += __shfl_xor_sync(0xffffffffu, t, 16);
+                    const float rs = rsqrtf(t * a.rstd_inv_h + a.rstd_eps);
+#pragma unroll
+                    for (int j = 0; j < 8; ++j) rstd[g0 + j] = __shfl_sync(0xffffffffu, rs, j);
+                }
             }
         }
-        float d[2][8];
+        float d[2][T];
 #pragma unroll
         for (int rb = 0; rb < 2; ++rb)
 #pragma unroll
-            for (int i = 0; i < 8; ++i) d[rb][i] = 0.f;
+            for (int i = 0; i < T; ++i) d[rb][i] = 0.f;
         int stage = 0; uint32_t phase = 0;
         for (int kb = kb0; kb < kb1; ++kb) {
             mbar_wait(&full[stage], phase);
@@ -717,21 +773,35 @@ tc_gemm_splitk_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
             if (lane == 0) mbar_arrive(&empty[stage]);
             if (++stage == a.stages) { stage = 0; phase ^= 1; }
         }
-        named_sync(3, 128);                                      // every warp's last wgmma has read the ring: stage 0 is free
+        named_sync(3, 128);                                      // every warp's last wgmma has read the ring: it is free
 #pragma unroll
         for (int rb = 0; rb < 2; ++rb) {
             wg_fence_operand(d[rb]);
-            store_frag<BN>(sacc, Cfg<BN>::LD, d[rb], rb * 64, 0);
+            store_frag<BN>(sacc, LD, d[rb], rb * 64, 0);
         }
         named_sync(3, 128);
-        float v[16];
-        ld_acc16(sacc + (size_t)row * Cfg<BN>::LD, v);
+        if constexpr (T == 8) {
+            float v[16];
+            ld_acc16(sacc + (size_t)row * LD, v);
 #pragma unroll
-        for (int j = 0; j < 8; ++j) acc[j] = v[j] + v[j + 8];
+            for (int j = 0; j < 8; ++j) acc[j] = v[j] + v[j + 8];
+        } else {
+#pragma unroll
+        for (int j0 = 0; j0 < T; j0 += 8) {                      // hi column j0 + j pairs with lo column T + j0 + j
+            float hi[8], lo[8];
+            const float4* ph = reinterpret_cast<const float4*>(sacc + (size_t)row * LD + j0);
+            const float4* pl = reinterpret_cast<const float4*>(sacc + (size_t)row * LD + T + j0);
+            const float4 h0 = ph[0], h1 = ph[1], l0 = pl[0], l1 = pl[1];
+            hi[0] = h0.x; hi[1] = h0.y; hi[2] = h0.z; hi[3] = h0.w; hi[4] = h1.x; hi[5] = h1.y; hi[6] = h1.z; hi[7] = h1.w;
+            lo[0] = l0.x; lo[1] = l0.y; lo[2] = l0.z; lo[3] = l0.w; lo[4] = l1.x; lo[5] = l1.y; lo[6] = l1.z; lo[7] = l1.w;
+#pragma unroll
+            for (int j = 0; j < 8; ++j) acc[j0 + j] = hi[j] + lo[j];
+        }
+        }
         if (rank != 0) {
-            const uint32_t dst = map_to_rank(smem_u32(part + ((size_t)(rank - 1) * BM + row) * 8), 0);
-            st_cluster_f4(dst, acc[0], acc[1], acc[2], acc[3]);
-            st_cluster_f4(dst + 16, acc[4], acc[5], acc[6], acc[7]);
+            const uint32_t dst = map_to_rank(smem_u32(part + ((size_t)(rank - 1) * BM + row) * T), 0);
+#pragma unroll
+            for (int j = 0; j < T; j += 4) st_cluster_f4(dst + 4 * j, acc[j], acc[j + 1], acc[j + 2], acc[j + 3]);
         }
     }
     __syncwarp();
@@ -740,36 +810,38 @@ tc_gemm_splitk_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
         if (!a.h) {
             // store mode: each CTA's piece scaled by rstd, the pieces added to 0 in rank order, with no fused multiply-add -- the
             // arithmetic of tc_gemm_kernel's stream-K epilogue and slot reduction (a CTA with an empty piece has no slot there)
-            float sum[8];
+            float sum[T];
 #pragma unroll
-            for (int j = 0; j < 8; ++j) sum[j] = __fadd_rn(0.f, a.rstd_ss ? __fmul_rn(acc[j], rstd[j]) : acc[j]);
+            for (int j = 0; j < T; ++j) sum[j] = __fadd_rn(0.f, a.rstd_ss ? __fmul_rn(acc[j], rstd[j]) : acc[j]);
             for (uint32_t r = 1; r < C; ++r) {
                 int r0, r1;
                 split_range(a, mt, m_tiles, (int)r, (int)C, r0, r1);
                 if (r0 == r1) continue;
-                const float* p = part + ((size_t)(r - 1) * BM + row) * 8;
+                const float* p = part + ((size_t)(r - 1) * BM + row) * T;
 #pragma unroll
-                for (int j = 0; j < 8; ++j) sum[j] = __fadd_rn(sum[j], a.rstd_ss ? __fmul_rn(p[j], rstd[j]) : p[j]);
+                for (int j = 0; j < T; ++j) sum[j] = __fadd_rn(sum[j], a.rstd_ss ? __fmul_rn(p[j], rstd[j]) : p[j]);
             }
 #pragma unroll
-            for (int j = 0; j < 8; ++j)
+            for (int j = 0; j < T; ++j)
                 if (j < a.N && m_ok) a.out[(long long)j * a.M + m] = sum[j];
             return;
         }
         for (uint32_t r = 1; r < C; ++r) {                       // fixed order: deterministic sums
-            const float4 p0 = *reinterpret_cast<const float4*>(part + ((size_t)(r - 1) * BM + row) * 8);
-            const float4 p1 = *reinterpret_cast<const float4*>(part + ((size_t)(r - 1) * BM + row) * 8 + 4);
-            acc[0] += p0.x; acc[1] += p0.y; acc[2] += p0.z; acc[3] += p0.w;
-            acc[4] += p1.x; acc[5] += p1.y; acc[6] += p1.z; acc[7] += p1.w;
+            const float4* p = reinterpret_cast<const float4*>(part + ((size_t)(r - 1) * BM + row) * T);
+#pragma unroll
+            for (int j = 0; j < T; j += 4) {
+                const float4 pv = p[j / 4];
+                acc[j] += pv.x; acc[j + 1] += pv.y; acc[j + 2] += pv.z; acc[j + 3] += pv.w;
+            }
         }
         if (a.rstd_ss) {
 #pragma unroll
-            for (int j = 0; j < 8; ++j) acc[j] *= rstd[j];
+            for (int j = 0; j < T; ++j) acc[j] *= rstd[j];
         }
         const int w4 = warp;                                     // 0..3 (s_red rows)
-        float sq[8];
+        float sq[T];
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {
+        for (int j = 0; j < T; ++j) {
             float hv = 0.f;
             if (j < a.N && m_ok) {
                 hv = hold[j] + acc[j];
@@ -777,21 +849,21 @@ tc_gemm_splitk_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
                 const float t = hv * g;
                 const __nv_bfloat16 hi = __float2bfloat16_rn(t);
                 a.xn[(long long)j * a.M + m] = hi;
-                a.xn[(long long)(8 + j) * a.M + m] = __float2bfloat16_rn(t - __bfloat162float(hi));
+                a.xn[(long long)(T + j) * a.M + m] = __float2bfloat16_rn(t - __bfloat162float(hi));
             }
             sq[j] = hv * hv;
         }
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {
+        for (int j = 0; j < T; ++j) {
 #pragma unroll
             for (int o = 16; o; o >>= 1) sq[j] += __shfl_xor_sync(0xffffffffu, sq[j], o);
         }
         if (lane == 0) {
 #pragma unroll
-            for (int j = 0; j < 8; ++j) s_red[w4 * 8 + j] = sq[j];
+            for (int j = 0; j < T; ++j) s_red[w4 * T + j] = sq[j];
         }
         asm volatile("bar.sync 2, 128;" ::: "memory");
-        if (w4 == 0 && lane < 8) a.ss[mt * 8 + lane] = s_red[lane] + s_red[8 + lane] + s_red[16 + lane] + s_red[24 + lane];
+        if (w4 == 0 && lane < T) a.ss[mt * T + lane] = s_red[lane] + s_red[T + lane] + s_red[2 * T + lane] + s_red[3 * T + lane];
     }
 }
 #endif  // B2A_TC_GEMM_IMPL
@@ -803,12 +875,16 @@ CUtensorMap make_tmap_f16_3d(const void* base, long long d0, long long d1, long 
 // planar hi/lo activations [2][B][Ttot][C], bf16 (f16 != 0: fp16) -> rank-4 map {C, Ttot, B, 2}, box {64, box_frames, 1, 2}, 128-byte swizzle
 CUtensorMap make_tmap_planes(const void* base, int C, long long Ttot, int B, int box_frames, int f16);
 
+// share_sm: ask for the largest shared-memory carve-out at this launch (a decode-step GEMM whose neighbours share its SM)
 template <int BN>
-void launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const Args& a, int ctas, int n_tiles, cudaStream_t s);
+void launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const Args& a, int ctas, int n_tiles, cudaStream_t s, bool share_sm = false);
 
+// tc_gemm_splitk_kernel<T>: T = the decode width (8, 16 or 32), X a [2T, K] hi/lo map with 2T-row boxes
+template <int T>
 void launch_splitk(const CUtensorMap& tmA, const CUtensorMap& tmB, const SplitArgs& a, int m_tiles, int cluster, cudaStream_t s);
-// clusters of `cluster` tc_gemm_splitk_kernel CTAs of smem_bytes dynamic shared memory the current device can hold at once
+// clusters of `cluster` tc_gemm_splitk_kernel<T> CTAs of smem_bytes dynamic shared memory the current device can hold at once
 // (cudaOccupancyMaxActiveClusters: the clusters' GPC placement is part of the answer).  Needs set_attributes().
+template <int T>
 int splitk_active_clusters(int cluster, size_t smem_bytes);
 
 void set_attributes();   // cudaFuncSetAttribute for every instantiation (call once, outside graph capture)

@@ -7,7 +7,7 @@ HBM3 bandwidth (3.35 TB/s).  The card's name and power limit are read in the sam
 Weight bytes per frame: the talker's layers and codec head once, the predictor's layers 16 times (position 0 + 15 code positions),
 its 15 lm heads once each, and at 1.7B the small_to_mtp_projection once (the projected embedding rows are gathers).
 
-    python tools/bench_qwen3_talker.py --geometry 1.7b --batch 1,4,8 [--frames 512] [--warmup 1] [--iters 3]"""
+    python tools/bench_qwen3_talker.py --geometry 1.7b --batch 1,4,8,16,32 [--frames 512] [--warmup 1] [--iters 3]"""
 import argparse
 import json
 import sys
@@ -77,7 +77,7 @@ def run(cfg, name, B, frames, warmup, iters):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--geometry", default="1.7b", choices=["0.6b", "1.7b"])
-    ap.add_argument("--batch", default="1,4,8", help="comma-separated batch sizes (<= 8)")
+    ap.add_argument("--batch", default="1,4,8", help="comma-separated batch sizes (<= 32)")
     ap.add_argument("--frames", type=int, default=512)
     ap.add_argument("--warmup", type=int, default=1)
     ap.add_argument("--iters", type=int, default=3)

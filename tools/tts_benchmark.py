@@ -68,7 +68,7 @@ def soprano_benchmark(a):
 
 ap = argparse.ArgumentParser()
 ap.add_argument("--model", default="orpheus", choices=["orpheus", "qwen3", "soprano"])
-ap.add_argument("--batch", type=int, default=1)
+ap.add_argument("--batch", type=int, default=1, help="utterances per call, 1..32")
 ap.add_argument("--prompt", type=int, default=64)
 ap.add_argument("--max-tokens", type=int, default=512)
 ap.add_argument("--model-dir", default=None, help="checkpoint directory (config.json + *.safetensors); default: random init")
@@ -91,8 +91,9 @@ if a.model_dir:
 else:
     tts = Model.random_init(geometry, snac=codec, max_batch=a.batch, max_context=ctx)
 # the untruncated make_prompts rows are [SOH] body [EOT, EOH, SOS]: a body of prompt - 4 tokens keeps the framed prompt at --prompt
-body = [r[1:-3][:max(a.prompt - 4, 1)].tolist() for r in make_prompts(0)[:a.batch]]
-ids = make_prompts(0)[:a.batch, :a.prompt]
+prompts = make_prompts(0, max(a.batch, 8))[:a.batch]      # up to 32 rows; the first 8 are bench.py's
+body = [r[1:-3][:max(a.prompt - 4, 1)].tolist() for r in prompts]
+ids = prompts[:, :a.prompt]
 if a.model == "qwen3":
     ids, _ = tts.prepare_input_ids(body)
     ids = np.concatenate([ids, np.full((ids.shape[0], 1), sos, dtype=np.int32)], axis=1)
